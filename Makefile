@@ -1,6 +1,6 @@
-# Builds the in-tree native library (sm_100a only) and the CPU oracle.
+# Builds the in-tree native library (sm_90a only) and the CPU oracle.
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 EXTRA     ?=
 NVCCFLAGS := $(EXTRA) -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 CSRC      := parsec_b200/csrc

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json metric on its config: tasks/s (+ tile GB/s) of a 2D-block-cyclic tile DAG on B200.
+"""bench.py -- BASELINE.json metric on its config: tasks/s (+ tile GB/s) of a 2D-block-cyclic tile DAG on H100.
 
 Workload at N=1 = BASELINE configs[1]: Ex05_Broadcast dataflow, 256x256 fp32 tiles (262 144 B), K = 4096 broadcast
 groups, fan-out F = 8 (NB = 14): 36 864 tasks, 9.66 GB of algorithmic tile traffic per step.  A "step" is one complete
@@ -14,9 +14,9 @@ pass of that DAG.
                parsec_context_add_taskpool .. parsec_context_wait, measured inside the application.
   e2e_standalone  the same DAG through this repository's own C-ABI host runtime (include/pb2_parsec.h), which knows the
                whole pool up front and releases successors on the device.
-  roofline     dominant kernel pb2_engine_hbm_kernel: algorithmic bytes / CUDA-event time vs the measured HBM peak, plus
-               the DRAM traffic ncu measured (`traffic`, `dram_frac`) and the measured L2 read ceiling (`l2_frac`): 7 of
-               the 8 readers of a tile hit the 126 MB L2, so the algorithmic figure can exceed the HBM peak.
+  roofline     dominant kernel pb2_engine_hbm_kernel: algorithmic bytes / CUDA-event time vs the HBM peak (MEASURED_PEAKS.json
+               where present, else the H100 SXM data sheet): readers of a tile that is still in the 50 MB L2 do not touch
+               HBM, so the algorithmic figure can exceed the HBM peak.
   cpu_baseline / --impl reference
                the reference's OWN CPU implementation: the same generated task pool restricted to its CPU incarnations,
                scheduled by the reference runtime on all host cores (cpu_baseline.kind = "reference").
@@ -31,8 +31,11 @@ collection on a 1 x N block-cyclic grid (kp = 1: tile k on rank k mod N, the map
 NVLink and tiles are pulled by the consumers (NCCL is only the per-step barrier).  e2e at N > 1 is the SAME path as at
 N = 1: the reference runtime driving N b200 device modules from one process, run by rank 0 after the process group is gone.
 --impl reference: the reference's CPU implementation of the WHOLE job of the N-GPU arm (K*N groups) on the host cores.
+--dump-outputs DIR (N = 1): after the timed steps, what the last timed step computed -- per-task body results, the flow
+versions every task saw, the final tile versions and a fixed sample of the tile data -- as float64 .npy files.
 """
 import argparse
+import atexit
 import ctypes as C
 import json
 import os
@@ -51,8 +54,8 @@ K_GROUPS = 4096
 NB = 14
 F = NB // 2 + 1
 REF_BIN = os.path.join(ROOT, "oracle", "_ref", "bin")
-NVLINK_GBS = 770.0          # per direction per GPU: the MEASURED peer copy B200_PROFILING.md gives as the NVLink denominator
-NVLINK_NOMINAL_GBS = 900.0  # nominal, for context
+NVLINK_GBS = 450.0          # H100 SXM NVLink 4, per direction per GPU (data sheet: 900 GB/s both directions)
+DUMP_SAMPLE = 1 << 20       # tile elements kept by --dump-outputs (fixed, seeded positions)
 
 
 def measured(key, fallback):
@@ -61,11 +64,11 @@ def measured(key, fallback):
         d = json.load(open(p))
         if key in d:
             return float(d[key]), "measured (MEASURED_PEAKS.json %s)" % key
-    return fallback, "fallback (B200_PROFILING.md)"
+    return fallback, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries; the sampler ends with the run)."""
 
     def __init__(self, index=0):
         self.index, self.rows, self.proc = index, [], None
@@ -76,6 +79,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", f"--id={self.index}", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-lms", "20"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
             threading.Thread(target=self._read, daemon=True).start()
+            atexit.register(self._kill)
         except Exception:
             self.proc = None
         return self
@@ -84,9 +88,13 @@ class ClockSampler:
         for line in self.proc.stdout:
             self.rows.append([x.strip() for x in line.split(",")])
 
-    def stop(self):
-        if self.proc:
+    def _kill(self):
+        if self.proc and self.proc.poll() is None:
             self.proc.terminate()
+            self.proc.wait()
+
+    def stop(self):
+        self._kill()
         sm = sorted(int(r[0]) for r in self.rows if r and r[0].isdigit())
         mx = [int(r[1]) for r in self.rows if len(r) > 1 and r[1].isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -286,13 +294,12 @@ def secondary_gemm(clock_index):
         w.close()
     med = ms[len(ms) // 2]
     flops = 2.0 * (NT * T) ** 3
-    peak, how = measured("bf16_tflops", 1686.0)
-    sus, _ = measured("bf16_tflops_sustained", 1435.5)
+    peak, how = measured("bf16_tflops", 989.0)
     return {"config": "DTD tile-GEMM DAG, 512x512 bf16 tiles, N=16384, NT=32, 32768 tasks (configs[2])", "kernel": "pb2_engine_gemm2_kernel",
             "data": "reference LCG (dtd_test_simple_gemm.c:154-196, seeds 1789/1805/1901) cast to bf16", "ms_per_run_median": med,
             "ms_per_run_min": ms[0], "tasks_per_s": NT ** 3 / med * 1e3, "tflops": flops / med / 1e9,
             "roofline": {"bound": "tensor", "achieved": flops / med / 1e9, "peak": peak, "unit": "TFLOP/s", "frac": flops / med / 1e9 / peak,
-                         "frac_of_sustained": flops / med / 1e9 / sus, "peak_source": how},
+                         "peak_source": how},
             "parity": {"dependency_order_ok": order_ok, "tiles_checked": checked, "max_rel_err": worst,
                        "tolerance": 2.0 ** -7, "values_ok": bool(worst <= 2.0 ** -7)},
             "clocks": clocks}
@@ -396,12 +403,29 @@ def secondary_cholesky(rank, world, local, torch, dist):
     okf = tot[1:].clone(); dist.all_reduce(okf, op=dist.ReduceOp.MIN)
     t = float(ms.item()) / 1e3
     ngemm = int((tasks["body"] == 16).sum())
-    peak, _ = measured("bf16_tflops_sustained", 1435.5)
+    peak, _ = measured("bf16_tflops", 989.0)
     return {"config": "tile-Cholesky-shaped DAG, 1024x1024 bf16, N=65536 (NT=64), %dx%d grid (configs[4])" % (P, Q), "tasks": len(tasks),
             "ms_per_run": t * 1e3, "tasks_per_s": len(tasks) / t, "tflops": ngemm * 2.0 * nb ** 3 / t / 1e12,
-            "tensor_frac_of_sustained": ngemm * 2.0 * nb ** 3 / t / 1e12 / (peak * world), "d2d_bytes_per_run": float(d2d[0].item()),
+            "tensor_frac_of_peak": ngemm * 2.0 * nb ** 3 / t / 1e12 / (peak * world), "d2d_bytes_per_run": float(d2d[0].item()),
             "parity": {"all_tasks_retired_once": bool(okf[0].item() > 0.5),
                        "note": "values and versions of this DAG are checked against the oracle at NT=3/8 in the `cholesky` parity case"}}
+
+
+def dump_outputs(path, w, eng, slab, K):
+    """What the last timed step computed, as a caller of the window receives it: per-task body results (CHECK bodies:
+    mismatches << 32 | first element), the flow versions each task saw, the final tile versions, and DUMP_SAMPLE elements
+    of the tile data at fixed, seeded positions.  Scheduling-dependent arrays (retire order, sequence numbers, worker ids)
+    are left out: they differ from run to run."""
+    os.makedirs(path, exist_ok=True)
+    res = w.results()
+    data = np.empty(K * TILE // 4, np.int32)
+    eng.d2h(data, slab)
+    pos = np.sort(np.random.default_rng(0).choice(data.size, min(DUMP_SAMPLE, data.size), replace=False))
+    arrays = {"task_result": res["result"].astype(np.float64), "task_seen_version": res["seen_version"].astype(np.float64),
+              "tile_version": res["tiles"]["version"].astype(np.float64), "tile_data_sample": data[pos].astype(np.float64),
+              "tile_data_sample_index": pos.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -418,6 +442,7 @@ def main():
     ap.add_argument("--kp", type=int, default=1, help="N>1: k-cyclic factor of the 1xN collection (1: the map of examples/Ex05_Broadcast)")
     ap.add_argument("--mgpu", default="direct", choices=["direct", "exchange"],
                     help="N>1: device-released cross-GPU edges (default) or two windows + one NCCL exchange")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="N=1: write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -429,15 +454,14 @@ def main():
     algo_bytes = K * (1 + F) * TILE
     cfg = {"workload": "Ex05_Broadcast dataflow (BASELINE configs[1]), 256x256 fp32 tiles, K=%d groups/GPU, fan-out %d" % (K, F),
            "tile_bytes": TILE, "groups_per_gpu": K, "tasks_per_gpu_step": ntasks, "distribution": "two_dim_block_cyclic 1x%d, kp = 1 (tile k on rank k mod N: the map of mydata in examples/Ex05_Broadcast)" % world,
-           "l2": "inputs larger than L2: %.2f GiB of tiles per GPU vs 126 MB L2, FIFO ready order" % (K * TILE / 2 ** 30),
+           "l2": "inputs larger than L2: %.2f GiB of tiles per GPU vs 50 MB L2, FIFO ready order" % (K * TILE / 2 ** 30),
            "value_path": "device-resident: the window the host runtime builds for the pool, run by the raw engine (tiles VALID in HBM); the device module's LRU stage-in is inside e2e"}
 
     if args.impl == "reference":
         if rank != 0:
             return
-        # capped so that the arm ends within minutes whatever --steps says: a step is the FULL workload of the N-GPU arm
-        # (K groups per GPU x N) on all host cores
-        steps = min(args.steps, max(3, 20 // max(args.gpus, 1)))
+        # a step is the FULL workload of the N-GPU arm (K groups per GPU x N) on all host cores
+        steps = args.steps
         Kref = K * max(args.gpus, 1)
         cfg["reference_workload"] = "%d groups (%d tasks) per step: the whole job of the %d-GPU arm" % (Kref, Kref * (1 + F), max(args.gpus, 1))
         r = reference_cpu_arm(Kref, steps, args.warmup) or port_cpu_arm(Kref, steps, args.warmup)
@@ -457,6 +481,8 @@ def main():
 
     if not torch.cuda.is_available():
         raise SystemExit("bench.py: no CUDA device; parsec_b200 has no CPU fallback")
+    if args.dump_outputs and world > 1:
+        raise SystemExit("bench.py: --dump-outputs is only supported with one GPU")
     torch.cuda.set_device(local_rank)
     if world > 1:
         import datetime
@@ -550,6 +576,7 @@ def main():
         from parsec_b200.engine import Engine
         eng = Engine(local_rank)
         slab = eng.malloc(K * TILE)
+        eng.h2d(slab, host)                                       # the same (zero) tile contents in every run
         tiles = win["tiles"].copy()
         order = np.argsort(tiles["src_ptr"])
         tiles["dev_ptr"][order] = slab + np.arange(K, dtype=np.uint64) * np.uint64(TILE)
@@ -621,24 +648,16 @@ def main():
            "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "i32",
            "data": "synthetic", "config": cfg, "tile_gbs": world * algo_bytes / (ms_per_step / 1e3) / 1e9,
            "gpu_launches": launches_per_step * args.steps, "clocks": clocks,
-           "engine": {"hbm_worker": "64 threads x 12 per SM (80 registers, no spills), 16 x 16-byte loads per thread in flight in read-only bodies, TMA bulk tile mover", "gemm_worker": "CTA pair, cta_group::2, fused k-chains"}}
+           "engine": {"hbm_worker": "64 threads x 12 per SM, 16 x 16-byte loads per thread in flight in read-only bodies, TMA bulk tile mover", "gemm_worker": "one CTA per SM, TMA ring + two wgmma consumer warpgroups, fused k-chains"}}
     if world == 1:
-        peak, how = measured("hbm_gbs", 6650.0)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, w, eng, slab, K)
+        peak, how = measured("hbm_gbs", 3350.0)
         ach = algo_bytes / (only_kernel_ms / 1e3) / 1e9
-        traffic, l2_peak = None, None
-        for name in ("r02_ex05_traffic.json", "r01_ex05_traffic.json"):      # from the committed ncu --set full capture
-            tpath = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(tpath):
-                tj = json.load(open(tpath))
-                traffic = tj.get("dram_bytes_per_launch")
-                l2_peak = tj.get("l2_read_gbs_measured")
-                break
-        out["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": traffic,
+        out["roofline"] = {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
                            "kernel": "pb2_engine_hbm_kernel", "kernel_ms": only_kernel_ms, "algorithmic_bytes": algo_bytes,
                            "peak_source": how, "workers": nworkers,
-                           "dram_frac": (traffic / (only_kernel_ms / 1e3) / 1e9 / peak) if traffic else None,
-                           "l2_frac": (ach / l2_peak) if l2_peak else None, "l2_peak": l2_peak,
-                           "note": "frac is ALGORITHMIC bytes (K*(1+F)*262144) over the HBM copy peak and exceeds 1 because 7 of 8 reads of a tile hit the 126 MB L2; dram_frac is the ncu-measured DRAM traffic of the same launch over the same peak; l2_frac is the algorithmic rate over the L2 read rate tools/l2_probe measured on this GPU type"}
+                           "note": "frac is ALGORITHMIC bytes (K*(1+F)*262144) over the HBM peak; it can exceed 1 because reads of a tile that is still in L2 do not reach HBM"}
         base = reference_cpu_arm(K, 3, 1) or port_cpu_arm(K, 3, 1)
         out["cpu_baseline"] = {"value": base["value"], "unit": "tasks/s", "cores": base["cores"], "kind": base["kind"], "sample": base["sample"]}
         if not args.no_secondary:
@@ -686,8 +705,7 @@ def main():
         ingress = float(tot.item())
         out["roofline"] = {"bound": "nvlink", "achieved": ingress / (ms_per_step / 1e3) / 1e9, "peak": NVLINK_GBS, "unit": "GB/s",
                            "frac": ingress / (ms_per_step / 1e3) / 1e9 / NVLINK_GBS, "traffic": ingress,
-                           "frac_of_nominal_900": ingress / (ms_per_step / 1e3) / 1e9 / NVLINK_NOMINAL_GBS,
-                           "note": "bytes the busiest rank pulls from its peers per step (counted by the kernel) over the measured peer-copy rate of 770 GB/s per direction (B200_PROFILING.md; 900 nominal); the step cannot be shorter than traffic / peak"}
+                           "note": "bytes the busiest rank pulls from its peers per step (counted by the kernel) over the H100 SXM data-sheet NVLink rate of 450 GB/s per direction; the step cannot be shorter than traffic / peak"}
     if e2e_standalone is not None:
         out["e2e_standalone"] = e2e_standalone
     if secondary:

@@ -1,5 +1,5 @@
 /*
- * pb2_engine.h -- C ABI of the B200 device-side DAG execution engine (layer L0).
+ * pb2_engine.h -- C ABI of the H100 device-side DAG execution engine (layer L0).
  *
  * One engine instance drives one GPU.  It replaces, for tasks whose incarnation
  * is GPU, the host-driven stream pipeline of the reference
@@ -9,7 +9,7 @@
  * and the host dependency release of
  *   parsec/parsec.c:1609/1656/1749/1836 (update_deps_with_counter / _with_mask,
  *   release_local_OUT_dependencies, release_dep_fct)
- * by ONE persistent sm_100a kernel per "window" of the DAG: workers (CTAs) pop
+ * by ONE persistent sm_90a kernel per "window" of the DAG: workers (CTAs) pop
  * ready task descriptors from a device-resident ring, stage tiles in from
  * host-pinned / peer memory, run the body, release successors with device
  * atomics and append to a retire log.  No host round trip per task or per edge.
@@ -50,7 +50,7 @@ extern "C" {
 #define PB2_FLOW_PUSHOUT       0x40   /* engine-private: D2H the flow after the body (gpu_task->pushout bit) */
 
 /* Task bodies the persistent kernel can run in place (the "incarnations").
- * HBM-bound bodies are coalesced 16-byte vector loops; GEMM is tcgen05. */
+ * HBM-bound bodies are coalesced 16-byte vector loops; GEMM is wgmma. */
 enum pb2_body_e {
     PB2_BODY_NOP        = 0,  /* empty body: tests/runtime/scheduling/ep.jdf:36-40                       */
     PB2_BODY_FILL_I32   = 1,  /* flow0[:] = iparam[0]          (Ex05 TaskBcast: "*Aint = k", tile-wide)   */
@@ -68,7 +68,7 @@ enum pb2_body_e {
     PB2_BODY_ADD_AT_I32 = 13, /* flow0[iparam[0]] += iparam[1]  (ping_kernel.cu:13-21 pong_kernel <<<1,1>>>,
                                *                                 ptg_pingpong.jdf:72-73 TOKEN_CPU)          */
     PB2_BODY_GEMM_BF16  = 16, /* flow2 (C, M x N row-major bf16) += flow0 (A, M x K row-major) *
-                               * flow1 (B, N x K row-major == K x N column-major), fp32 accumulate in TMEM
+                               * flow1 (B, N x K row-major == K x N column-major), fp32 accumulate in registers
                                * iparam[0]=M, iparam[1]=N, iparam[2]=K (each tile edge)                     */
     PB2_BODY_USER       = 31, /* host-side only: the chore is a user `submit` callback that enqueues its own CUDA work
                                * on a stream (device_gpu.h:49-51); such tasks never enter an engine window           */
@@ -134,8 +134,8 @@ typedef struct pb2_engine_params_s {
     int32_t  queue_policy;     /* 0 = FIFO ring, 1 = successors-first (hot ring before FIFO ring)             */
     int32_t  timeout_ms;       /* device-side watchdog: a window that makes no progress for this long aborts
                                 * (default 20000); a malformed DAG must never hang the GPU                   */
-    int32_t  gemm_mode;        /* 0 = CTA pairs (cta_group::2) + fused k-chains (default), 1 = v1 single-CTA kernel,
-                                * 2 = CTA pairs, every task flushes C (per-task bf16 rounding, as the oracle)       */
+    int32_t  gemm_mode;        /* 0 = fused k-chains (default), 1 = v1 kernel (one task at a time),
+                                * 2 = chain kernel, every task flushes C (per-task bf16 rounding, as the oracle)       */
     int32_t  part_bytes;       /* HBM bodies: a task whose largest tile exceeds this many bytes is run as up to 512
                                 * parts (byte slices) by different workers (default 256 KiB, <0 = never split);
                                 * pb2_engine_set_part_bytes changes it for the windows created afterwards       */

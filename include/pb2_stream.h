@@ -1,6 +1,6 @@
 /*
  * pb2_stream.h -- C ABI of the STREAMING side of the engine: a host-written descriptor ring and ONE persistent
- * sm_100a kernel per GPU that pulls task descriptors from it (BASELINE north_star; SURVEY.md 7 step 4).
+ * sm_90a kernel per GPU that pulls task descriptors from it (BASELINE north_star; SURVEY.md 7 step 4).
  *
  * What it replaces in the reference, for one GPU:
  *   - the three stream rings (H2D / exec / D2H) with four CUDA events each that parsec_device_progress_stream

@@ -1,8 +1,8 @@
 """ctypes loader for the in-tree native library ``libparsec_b200.so``.
 
-The library is built by ``make`` / ``__graft_entry__.build()`` with nvcc for sm_100a only.
+The library is built by ``make`` / ``__graft_entry__.build()`` with nvcc for sm_90a only.
 There is no Python or CPU fallback: if the shared object is missing, or the machine has no
-B200-class GPU, the product path fails loudly (``pb2_engine_create`` returns PB2_ERR_DEVICE).
+H100-class GPU, the product path fails loudly (``pb2_engine_create`` returns PB2_ERR_DEVICE).
 """
 import ctypes as C
 import os

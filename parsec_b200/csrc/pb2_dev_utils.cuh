@@ -1,4 +1,4 @@
-// pb2_dev_utils.cuh -- small sm_100a device helpers shared by the engine kernels.
+// pb2_dev_utils.cuh -- small sm_90a device helpers shared by the engine kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

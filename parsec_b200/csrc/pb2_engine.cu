@@ -1,4 +1,4 @@
-// pb2_engine.cu -- the persistent sm_100a DAG-execution kernel and its C ABI (include/pb2_engine.h).
+// pb2_engine.cu -- the persistent sm_90a DAG-execution kernel and its C ABI (include/pb2_engine.h).
 //
 // What it replaces in the reference (file:line in /root/reference):
 //   * the manager thread's check_in_deps / exec / get_data_out / complete_task loop,
@@ -232,7 +232,7 @@ static int dev_alloc_copy(pb2_window_t* w, T** dptr, const T* host, size_t n) {
     pb2_engine_t* e = w->e;
     void* p = nullptr;
     // stream-ordered pool allocation: after the first window of a size class this costs microseconds, whereas
-    // cudaMalloc/cudaFree next to a 170 GB slab cost hundreds of microseconds each and synchronise the device
+    // cudaMalloc/cudaFree next to a slab that fills the device cost hundreds of microseconds each and synchronise the device
     if (w->shared) { PB2_CUDA(e, cudaMalloc(&p, (n ? n : 1) * sizeof(T))); }     // IPC needs cudaMalloc memory
     else PB2_CUDA(e, cudaMallocAsync(&p, (n ? n : 1) * sizeof(T), e->up_stream));
     w->allocs.push_back(p);
@@ -269,7 +269,7 @@ static int validate_window(pb2_engine_t* e, int kind, const pb2_task_t* tasks, i
 
 // One tensor map per tile used as a GEMM operand: global tensor [rows][inner] bf16, row pitch inner*2 bytes,
 // box {64 (inner, 128 bytes), 128 rows}, 128-byte swizzle: exactly the K-major SWIZZLE_128B smem layout the
-// UMMA descriptors in pb2_gemm.cuh describe.  OOB rows/columns of ragged tiles are zero-filled by TMA.
+// wgmma descriptors in pb2_gemm.cuh describe.  OOB rows/columns of ragged tiles are zero-filled by TMA.
 typedef CUresult (*pb2_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -360,8 +360,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         const bool g = is_gemm(h);
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
-        u.nparts = g ? ((u.M + 255) / 256) * ((u.N + 511) / 512) : 1;       // 256-row x 512-column blocks of C (TMEM: 512 columns)
-        if (g && ((u.N % 16) || u.nparts > 16)) return PB2_ERR_NOT_SUPPORTED;       // caller falls back to the v1 kernel
+        u.nparts = g ? ((u.M + gemm2::kPartRows - 1) / gemm2::kPartRows) * ((u.N + gemm2::kPartCols - 1) / gemm2::kPartCols) : 1;
+        if (g && ((u.N % 16) || u.nparts > gemm2::kMaxParts)) return PB2_ERR_NOT_SUPPORTED;       // caller falls back to the v1 kernel
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
             segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});
@@ -386,7 +386,7 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     std::vector<int32_t> entries;
     uint32_t total_parts = 0;
     for (const GUnit& u : units) total_parts += (uint32_t)u.nparts;
-    // Ready GEMM units enter the ring in Z-order of their (locals[0], locals[1]) = C(i,j) coordinates: the ~37 units
+    // Ready GEMM units enter the ring in Z-order of their (locals[0], locals[1]) = C(i,j) coordinates: the units
     // that run concurrently then form a compact block of C tiles that shares A rows and B columns in L2 (a FIFO
     // ring keeps whatever order the host gives it; the reference's priority hint mt*nt*kt - i*nt + j plays the
     // same role for its sorted pending list, device_gpu.c:2169-2174).
@@ -439,8 +439,8 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     e->cuda_device = cuda_device;
     PB2_CUDA(e, cudaSetDevice(cuda_device));
     PB2_CUDA(e, cudaGetDeviceProperties(&e->prop, cuda_device));
-    if (e->prop.major != 10) {
-        fprintf(stderr, "pb2_engine_create: device %d is sm_%d%d; this library only carries sm_100a code\n",
+    if (e->prop.major != 9 || e->prop.minor != 0) {
+        fprintf(stderr, "pb2_engine_create: device %d is sm_%d%d; this library only carries sm_90a code\n",
                 cuda_device, e->prop.major, e->prop.minor);
         delete e;
         return PB2_ERR_NOT_SUPPORTED;
@@ -475,7 +475,6 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     if (p.max_workers > 0 && p.max_workers < e->nworkers) e->nworkers = p.max_workers;
     e->nworkers_gemm = pb2_gemm_nworkers(e->prop.multiProcessorCount);
     if (p.max_workers > 0 && p.max_workers < e->nworkers_gemm) e->nworkers_gemm = p.max_workers;
-    if (p.gemm_mode != 1 && e->nworkers_gemm < 2) e->nworkers_gemm = 2;      // v2 workers are CTA pairs
     *engine = e;
     return PB2_SUCCESS;
 }
@@ -651,7 +650,7 @@ int pb2_body_launch(void* cuda_stream, int body, int nb_args, void* const* ptrs,
     if (body == PB2_BODY_NOP) return PB2_SUCCESS;
     int grid = (int)((widest + 32767) / 32768);             // 32 KiB per CTA
     if (grid < 1) grid = 1;
-    if (grid > 1184) grid = 1184;
+    if (grid > 1056) grid = 1056;                        // 8 CTAs per SM of an H100 SXM (132 SMs)
     if (body == PB2_BODY_ADD_AT_I32) grid = 1;
     pb2_body_launch_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(cuda_stream)>>>(la);
     return cudaGetLastError() == cudaSuccess ? PB2_SUCCESS : PB2_ERR_DEVICE;

@@ -1,19 +1,19 @@
-// pb2_gemm.cuh -- tensor-core (tcgen05 / TMEM / TMA) engine kernel for PB2_BODY_GEMM_BF16 windows.
+// pb2_gemm.cuh -- tensor-core (wgmma / TMA / mbarrier) engine kernel for PB2_BODY_GEMM_BF16 windows.
 //
 // The task body restates what the reference reaches through `dyld=cublasDgemm` / cublasDgemm_v2
 // (tests/dsl/dtd/dtd_test_simple_gemm.c:450,527; tests/runtime/cuda/nvlink.jdf:136-152): one tile
-// GEMM per task, C(M x N) += A(M x K) * B(K x N).  Here in bf16 with fp32 accumulation in TMEM
+// GEMM per task, C(M x N) += A(M x K) * B(K x N).  Here in bf16 with fp32 accumulation in registers
 // (BASELINE config 3); tiles are K-contiguous for both operands: A row-major [M][K], B stored
 // [N][K] (== column-major K x N, what a "TN" cuBLAS call consumes), C row-major [M][N].
 //
-// One CTA per SM is one worker.  Warp roles (192 threads):
-//   warp 0      : scheduler (ring pop / dependency release / retire) + TMA producer (one lane)
-//   warp 1      : TMEM allocator + tcgen05.mma issuer (one lane)
-//   warps 2..5  : epilogue: tcgen05.ld accumulators, C += acc in fp32, bf16 store
-// A task is executed as ceil(M/128) x ceil(N/256) accumulator sub-tiles of 128 x 256 fp32 (256 TMEM
-// columns); two accumulator buffers (512 columns) let the epilogue of sub-tile s overlap the MMAs
-// of sub-tile s+1.  Operands stream through a 4-stage smem ring of {A 128x64, B 256x64} bf16
-// 128B-swizzled boxes filled by TMA (`cp.async.bulk.tensor.2d`) from per-tile tensor maps.
+// One CTA per SM is one worker.  Three warpgroups (384 threads):
+//   warpgroup 0 : warp 0 is the scheduler (ring pop / dependency release / retire) and, one lane, the TMA producer
+//   warpgroups 1, 2 : consumers; each issues `wgmma.mma_async` m64n256k16 for its 64 rows of the sub-tile and keeps
+//                 the 64 x 256 fp32 accumulator in registers, then adds it into C (bf16) itself
+// A task is executed as ceil(M/128) x ceil(N/256) accumulator sub-tiles of 128 x 256 fp32.  Operands stream
+// through a 4-stage smem ring of {A 128x64, B 256x64} bf16 128B-swizzled boxes filled by TMA
+// (`cp.async.bulk.tensor.2d`) from per-tile tensor maps; the producer fills the next sub-tile's stages while the
+// consumers run the epilogue of the current one.
 #pragma once
 #include <cuda.h>
 #include "pb2_sched.cuh"
@@ -27,10 +27,9 @@ constexpr int kStages = 4;
 constexpr int kAStageBytes = BM * BK * 2;          // 16 KiB
 constexpr int kBStageBytes = BN * BK * 2;          // 32 KiB
 constexpr int kStageBytes = kAStageBytes + kBStageBytes;
-constexpr int kThreads = 192;
-constexpr int kEpiWarp0 = 2;
-constexpr int kTmemCols = 512;
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int kThreads = 384;
+constexpr int kConsumers = 2;                      // warpgroups 1 and 2, 64 rows of A each
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align*/;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -62,43 +61,54 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
         :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                 :: "r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], M=128, N=256, K=16, bf16 x bf16 -> fp32
-__device__ __forceinline__ void tc_mma(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+
+// D(64 x 256, fp32 registers) (+)= A[smem, 64 x 16] * B[smem, 256 x 16]^T, both K-major bf16.  Register d[4c + i] of
+// thread (warp w, lane l) of the warpgroup holds row 16w + l/4 + 8*(i/2), column 8c + 2*(l%4) + i%2.
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" :: "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %130, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+        "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+        "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+          "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+          "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+          "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+          "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+          "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+          "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+          "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+          "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 [0,14) | LBO=1 [16,30) | SBO=1024>>4 [32,46) | version=1 [46,48) | SWIZZLE_128B=2 [61,64)
+// K-major, 128B-swizzled wgmma operand descriptor: start>>4 [0,14) | LBO=1 [16,30) (unused with this swizzle) |
+// SBO = 1024>>4 [32,46) (eight 128-byte rows) | layout SWIZZLE_128B = 1 [62,64).  Stepping K by 16 elements inside
+// the 128-byte swizzle atom adds 32 bytes to the start address.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// kind::f16 instruction descriptor (InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-// A,B K-major (bits 15,16 = 0), N>>3 [17,23), M>>4 [24,29)
-__device__ __forceinline__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
 
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
@@ -109,13 +119,66 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     return r;
 }
 
+// Consumer warpgroup `cw` (0 or 1): run `n` k-blocks of the smem ring into acc (zeroed by the first one when `zero`).
+// A k-block's stage goes back to the producer once the wgmma group of the NEXT k-block has been issued and the
+// group reading it has retired, so one group is always in flight.
+__device__ __forceinline__ void mma_kblocks(float (&acc)[128], uint8_t* smem, uint64_t* full, uint64_t* empty,
+                                            uint32_t& stage, uint32_t& phase, int n, bool zero, int cw) {
+    int prev = -1;
+    for (int i = 0; i < n; ++i) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+        const uint64_t da = make_desc(sa + cw * 64 * 128), db = make_desc(sa + kAStageBytes);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < BK / UK; ++k)
+            wgmma_m64n256k16(acc, da + (uint64_t)(k * UK * 2 >> 4), db + (uint64_t)(k * UK * 2 >> 4),
+                             (zero && i == 0 && k == 0) ? 0u : 1u);
+        wg_commit();
+        wg_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+        prev = (int)stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wg_wait<0>();
+    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[prev]);
+}
+
+// C(row0.., col0..) += acc for this warpgroup's 64 x 256 block, rows < row_end and columns < col_end (bf16, ldc
+// elements per row).  C is read and written at L2: it may have been written by another SM earlier in the window.
+__device__ __forceinline__ void epilogue_add(const float (&acc)[128], uint8_t* Cbase, int ldc, int row0, int col0,
+                                             int row_end, int col_end) {
+    const int t = threadIdx.x & 127, l = t & 31;
+    const int r0 = row0 + 16 * (t >> 5) + (l >> 2), r1 = r0 + 8;
+    const int c0 = col0 + 2 * (l & 3);
+#pragma unroll
+    for (int g = 0; g < 32; g += 4) {           // four column blocks at a time: loads in flight before the stores
+        uint32_t v0[4], v1[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int col = c0 + 8 * (g + c);
+            v0[c] = (r0 < row_end && col < col_end) ? __ldcg(reinterpret_cast<const unsigned int*>(Cbase + ((size_t)r0 * ldc + col) * 2)) : 0u;
+            v1[c] = (r1 < row_end && col < col_end) ? __ldcg(reinterpret_cast<const unsigned int*>(Cbase + ((size_t)r1 * ldc + col) * 2)) : 0u;
+        }
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            const int col = c0 + 8 * (g + c), j = 4 * (g + c);
+            if (col < col_end) {
+                if (r0 < row_end)
+                    __stcg(reinterpret_cast<unsigned int*>(Cbase + ((size_t)r0 * ldc + col) * 2),
+                           pack_bf16(bf16_lo(v0[c]) + acc[j], bf16_hi(v0[c]) + acc[j + 1]));
+                if (r1 < row_end)
+                    __stcg(reinterpret_cast<unsigned int*>(Cbase + ((size_t)r1 * ldc + col) * 2),
+                           pack_bf16(bf16_lo(v1[c]) + acc[j + 2], bf16_hi(v1[c]) + acc[j + 3]));
+            }
+        }
+    }
+}
+
 struct Shared {
     alignas(16) pb2_task_t task;    // filled with four 16-byte loads
     uint64_t full[kStages];
     uint64_t empty[kStages];
-    uint64_t tmem_full[2];
-    uint64_t tmem_empty[2];
-    uint32_t tmem_base;
     int32_t  id;
     int32_t  need;
     int32_t  decide;
@@ -133,27 +196,17 @@ pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
     __shared__ Shared sh;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&sh.tmem_full[a], 1); mbar_init(&sh.tmem_empty[a], 4); }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], kConsumers); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     :: "r"(smem_u32(&sh.tmem_base)), "r"(kTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = sh.tmem_base;
 
     // pipeline state persists across tasks
     uint32_t p_stage = 0, p_phase = 0;     // producer
-    uint32_t c_stage = 0, c_phase = 0;     // MMA consumer
-    uint32_t m_acc = 0, m_acc_phase = 0;   // MMA accumulator buffer
-    uint32_t e_acc = 0, e_acc_phase = 0;   // epilogue accumulator buffer
+    uint32_t c_stage = 0, c_phase = 0;     // consumers
 
     for (;;) {
         if (threadIdx.x == 0) {
@@ -231,73 +284,23 @@ pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
                         mbar_expect_tx(&sh.full[p_stage], kStageBytes);
                         tma_load_2d(sa, mapA, &sh.full[p_stage], kb * BK, mb * BM);
                         tma_load_2d(sb, mapB, &sh.full[p_stage], kb * BK, nb * BN);
-                        tma_load_2d(sb + kAStageBytes, mapB, &sh.full[p_stage], kb * BK, nb * BN + 128);
+                        tma_load_2d(sb + kBStageBytes / 2, mapB, &sh.full[p_stage], kb * BK, nb * BN + 128);
                         if (++p_stage == kStages) { p_stage = 0; p_phase ^= 1; }
                     }
                 }
             }
-        } else if (warp == 1) {
-            // ===== MMA issuer =====
-            if (lane == 0 && nsub > 0) {
-                constexpr uint32_t idesc = make_idesc(BM, BN);
-                for (int sub = 0; sub < nsub; ++sub) {
-                    mbar_wait(&sh.tmem_empty[m_acc], m_acc_phase ^ 1);
-                    tc_fence_after();
-                    const uint32_t d = tmem_base + m_acc * BN;
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        mbar_wait(&sh.full[c_stage], c_phase);
-                        tc_fence_after();
-                        const uint32_t sa = smem_u32(smem + c_stage * kStageBytes);
-                        const uint64_t da = make_desc(sa), db = make_desc(sa + kAStageBytes);
-#pragma unroll
-                        for (int k = 0; k < BK / UK; ++k)
-                            tc_mma(d, da + (uint64_t)(k * UK * 2 >> 4), db + (uint64_t)(k * UK * 2 >> 4), idesc,
-                                   (kb | k) != 0 ? 1u : 0u);
-                        tc_commit(&sh.empty[c_stage]);         // smem slot free once these MMAs retire
-                        if (++c_stage == kStages) { c_stage = 0; c_phase ^= 1; }
-                    }
-                    tc_commit(&sh.tmem_full[m_acc]);           // accumulator ready for the epilogue
-                    if (++m_acc == 2) { m_acc = 0; m_acc_phase ^= 1; }
-                }
-            }
-        } else {
-            // ===== epilogue warps: TMEM -> registers -> C += acc -> bf16 =====
+        } else if (wg >= 1) {
+            // ===== consumer warpgroups: wgmma into registers, then C += acc -> bf16 =====
             if (nsub > 0) {
-                const int q = warp & 3;                         // TMEM lane quadrant this warp may access
+                const int cw = wg - 1;
                 uint8_t* Cbase = reinterpret_cast<uint8_t*>(w.tiles[t.tile[2]].dev_ptr);
+                float acc[128];
+#pragma unroll
+                for (int i = 0; i < 128; ++i) acc[i] = 0.f;
                 for (int sub = 0; sub < nsub; ++sub) {
                     const int mb = sub / nblocks, nb = sub % nblocks;
-                    mbar_wait(&sh.tmem_full[e_acc], e_acc_phase);
-                    tc_fence_after();
-                    const int row = mb * BM + q * 32 + lane;
-                    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + e_acc * BN;
-#pragma unroll 1
-                    for (int c = 0; c < BN / 32; ++c) {
-                        uint32_t acc[32];
-                        tc_ld_32x32b_x32(taddr + c * 32, acc);
-                        tc_wait_ld();
-                        const int col0 = nb * BN + c * 32;
-                        if (row < M && col0 < N) {
-                            uint4* cp = reinterpret_cast<uint4*>(Cbase + ((size_t)row * N + col0) * 2);
-                            const int nv = (N - col0 >= 32) ? 4 : (N - col0) / 8;
-#pragma unroll
-                            for (int v = 0; v < 4; ++v) {
-                                if (v < nv) {
-                                    uint4 cv = ld_stream(cp + v);
-                                    uint4 o;
-                                    o.x = pack_bf16(bf16_lo(cv.x) + __uint_as_float(acc[v * 8 + 0]), bf16_hi(cv.x) + __uint_as_float(acc[v * 8 + 1]));
-                                    o.y = pack_bf16(bf16_lo(cv.y) + __uint_as_float(acc[v * 8 + 2]), bf16_hi(cv.y) + __uint_as_float(acc[v * 8 + 3]));
-                                    o.z = pack_bf16(bf16_lo(cv.z) + __uint_as_float(acc[v * 8 + 4]), bf16_hi(cv.z) + __uint_as_float(acc[v * 8 + 5]));
-                                    o.w = pack_bf16(bf16_lo(cv.w) + __uint_as_float(acc[v * 8 + 6]), bf16_hi(cv.w) + __uint_as_float(acc[v * 8 + 7]));
-                                    st_stream(cp + v, o);
-                                }
-                            }
-                        }
-                    }
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&sh.tmem_empty[e_acc]);
-                    if (++e_acc == 2) { e_acc = 0; e_acc_phase ^= 1; }
+                    mma_kblocks(acc, smem, sh.full, sh.empty, c_stage, c_phase, kblocks, true, cw);
+                    epilogue_add(acc, Cbase, N, mb * BM + cw * 64, nb * BN, M, N);
                 }
                 fence_proxy_async();   // C may be consumed through TMA by a later task on another SM
             }
@@ -340,12 +343,6 @@ pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
             }
         }
         __syncthreads();
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_base), "r"(kTmemCols) : "memory");
     }
 }
 

@@ -310,11 +310,11 @@ int pb2_device_cuda_module_init(pb2_context_t* ctx, int cuda_index, int dry_run,
         d->major = info.cc_major; d->minor = info.cc_minor;
         total = info.total_mem; freeb = info.free_mem;
     } else {
-        d->major = 10; d->minor = 0;
+        d->major = 9; d->minor = 0;
         total = freeb = (size_t)1 << 30;
     }
-    // sm_100 rates the reference lacks (device_cuda_module.c:45-142 stops at sm_90): dense GFLOP/s of one B200
-    d->st.gflops_fp16 = 2250000; d->st.gflops_tf32 = 1100000; d->st.gflops_fp32 = 75000; d->st.gflops_fp64 = 37000;
+    // dense GFLOP/s of one H100 SXM (data sheet), the sm_90 rates of the reference's table (device_cuda_module.c:45-142)
+    d->st.gflops_fp16 = 989000; d->st.gflops_tf32 = 495000; d->st.gflops_fp32 = 67000; d->st.gflops_fp64 = 34000;
     // parsec_device_memory_reserve, device_gpu.c:866-991
     int64_t nblocks = ctx->mca["device_cuda_memory_number_of_blocks"];
     if (nblocks <= 0) nblocks = (int64_t)((double)freeb * (double)ctx->mca["device_cuda_memory_use"] / 100.0 / (double)d->mem_block_size);

@@ -1,4 +1,4 @@
-// pb2_stream.cu -- the streaming engine: host-written command ring, ONE persistent sm_100a kernel per GPU, retire ring
+// pb2_stream.cu -- the streaming engine: host-written command ring, ONE persistent sm_90a kernel per GPU, retire ring
 // back to the host (include/pb2_stream.h).  Original design; what it stands in for in the reference:
 //   parsec_device_progress_stream + the exec-stream rings            parsec/mca/device/device_gpu.c:2592-2731
 //   parsec_device_kernel_push / _exec / _pop (per task, per stream)  device_gpu.c:2745, :2873, :2943
@@ -46,7 +46,7 @@ struct alignas(64) Cmd {
 };
 static_assert(sizeof(Cmd) == 64, "Cmd must be one 64-byte line");
 
-// 32 bytes, written by a worker into pinned host memory; the 16 bytes holding `stamp` are stored last.
+// 32 bytes, written by a worker into pinned host memory; `stamp` is stored last, with release semantics.
 struct alignas(32) Retire {
     uint32_t seen[PB2_MAX_FLOWS];
     uint64_t result;
@@ -92,12 +92,11 @@ struct StreamDev {
 };
 
 __device__ __forceinline__ uint32_t ld_volatile_u32(const volatile uint32_t* p) { return *p; }
-__device__ __forceinline__ void st_volatile_v8(void* p, const uint4& a, const uint4& b) {      // 32-byte aligned
-    asm volatile("st.volatile.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-                 :: "l"(p), "r"(a.x), "r"(a.y), "r"(a.z), "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w) : "memory");
-}
 __device__ __forceinline__ void st_volatile_v4(void* p, const uint4& v) {
     asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ void st_volatile_v2(void* p, uint32_t a, uint32_t b) {
+    asm volatile("st.volatile.global.v2.u32 [%0], {%1,%2};" :: "l"(p), "r"(a), "r"(b) : "memory");
 }
 
 // One thread: push the ring entries of ready task `slot`.
@@ -340,12 +339,15 @@ pb2_stream_kernel(StreamDev sd) {
                 hi.w = (gen & 0x7fffffffu) | (r == ~0ull ? 0x80000000u : 0u);
                 // What the host must see BEFORE the record -- bytes this task pushed out to host memory, its trace entry --
                 // is ordered by one system-scope fence; a task that wrote nothing the host reads skips it.  The record
-                // itself is ONE 32-byte store (a single sector write over PCIe): the host, which reads the stamp first,
-                // never sees half of it, and the record is visible one posted write after the task ended.
+                // goes out as three stores, the stamp last as a system-scope release: the host, which reads the stamp
+                // first, never sees half of a record.
                 bool host_reads = sd.trace != nullptr;
                 for (int f = 0; f < (int)t.nb_flows; ++f) host_reads |= (t.access[f] & PB2_FLOW_PUSHOUT) != 0;
                 if (host_reads) __threadfence_system();
-                st_volatile_v8(rec, lo, hi);
+                st_volatile_v4(rec, lo);
+                st_volatile_v2(&rec->result, hi.x, hi.y);
+                *reinterpret_cast<volatile int32_t*>(&rec->ticket) = (int32_t)hi.z;
+                st_release_sys(reinterpret_cast<int32_t*>(&rec->stamp), (int32_t)hi.w);
                 __threadfence_system();
                 atomicAdd(&sd.sctl->published.v, 1ull);
             }

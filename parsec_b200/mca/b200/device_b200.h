@@ -1,5 +1,5 @@
 /*
- * device_b200.h -- public interface of the B200 device component (parsec/mca/device/b200).
+ * device_b200.h -- public interface of the b200 device component (parsec/mca/device/b200).
  *
  * The component fills the reference's own plug-in contract: one parsec_device_module_t (parsec/mca/device/device.h:145-189)
  * per GPU, type PARSEC_DEV_CUDA so that BODY [type=CUDA] chores emitted by parsec-ptgpp (jdf2c.c:6832-6969) and DTD

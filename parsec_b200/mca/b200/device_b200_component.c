@@ -1,5 +1,5 @@
 /*
- * device_b200_component.c -- MCA glue of the B200 device component (parsec/mca/device/b200).
+ * device_b200_component.c -- MCA glue of the b200 device component (parsec/mca/device/b200).
  *
  * Fills parsec_device_base_component_t the way every PaRSEC device component has to (device.h:54-58; the contract is
  * spelled out in SURVEY.md 8b; the reference's CUDA component is parsec/mca/device/cuda/device_cuda_component.c):
@@ -77,7 +77,7 @@ static int device_b200_component_register(void)
 {
     parsec_device_b200_enabled_index =
         parsec_mca_param_reg_int_name("device_b200", "enabled",
-                                      "Number of GPUs driven by the B200 engine (-1: all available, 0: component off)",
+                                      "Number of GPUs driven by the b200 engine (-1: all available, 0: component off)",
                                       false, false, 0, &parsec_device_b200_enabled);
     (void)parsec_mca_param_reg_int_name("device_b200", "mask", "Bit mask of the CUDA devices the component may use",
                                         false, false, -1, &b200_mask);
@@ -128,7 +128,7 @@ static int device_b200_component_open(void)
     } else {
         ndev = parsec_b200_device_count();
         if( ndev <= 0 ) {
-            parsec_warning("device_b200: enabled but no sm_100 CUDA device is usable on %s; component disabled", parsec_hostname);
+            parsec_warning("device_b200: enabled but no sm_90 CUDA device is usable on %s; component disabled", parsec_hostname);
             parsec_device_b200_enabled = 0;
             return MCA_ERROR;
         }

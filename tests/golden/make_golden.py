@@ -32,7 +32,27 @@ def run(app, args):
     return p.returncode, json.loads(line)
 
 
+def record_reference_pieces():
+    """tests/golden/reference_pieces.json.gz: the answers of the reference pieces of oracle/_ref (zone_malloc.c, data.c,
+    the 2D block-cyclic collection, device selection) to the call sequences of tests/test_oracle.py, which replays them
+    where oracle/_ref is not built."""
+    import gzip
+    import sys
+    sys.path.insert(0, ROOT)
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_oracle as T
+    assert T.HAVE_REF_ZONE and T.HAVE_REF_DATA and T.HAVE_REF_TWODBC and T.HAVE_REF_SELECT, "build oracle/_ref first"
+    T.test_zone_oracle_equals_reference_build()
+    T.test_coherency_oracle_equals_reference_build()
+    T.test_twodbc_oracle_and_product_equal_reference_build()
+    T.test_select_oracle_equals_reference_build()
+    with gzip.GzipFile(T.GOLDEN_PIECES, "wb", mtime=0) as f:
+        f.write(json.dumps(T.RECORDED, separators=(",", ":")).encode())
+    print("wrote", T.GOLDEN_PIECES)
+
+
 if __name__ == "__main__":
+    record_reference_pieces()
     out = {}
     for name, (app, args, fields) in CASES.items():
         rc, d = run(app, CPU_FLAG[app] + args)

@@ -58,7 +58,7 @@ def test_dtd_gemm_chain(mode, NT, T):
     ref = exact if mode == 0 else per_task
     # tolerance: one bf16 ulp (at most 2^-7 relative) of the largest magnitude along the chain PER ROUNDING: the tensor
     # core's fp32 accumulation order differs from numpy's, which can flip a rounding to the neighbouring bf16 value.
-    # Mode 0 keeps the accumulator in TMEM for the whole chain (one rounding, compared with the singly-rounded exact
+    # Mode 0 keeps the accumulator in registers for the whole chain (one rounding, compared with the singly-rounded exact
     # sum); the per-task modes round once per task of the k-chain, so NT flips can add up.
     tol = (1 if mode == 0 else NT) * 2.0 ** -7 * np.maximum(mag, 1.0)
     bad = np.abs(got - ref) > tol

@@ -1,7 +1,7 @@
 """The real drop-in boundary: parsec/mca/device/b200 compiled INTO the reference runtime (oracle/build_ref_runtime.sh),
 driven by task pools the reference's own parsec-ptgpp generated from .jdf files with BODY [type=CUDA] incarnations
 (tests/parsec/*.jdf).  CPU tests: the reference runtime alone (CPU bodies: the oracle), and the component in dry-run mode
-(scheduling, ownership hand-over, concurrent callers; no bodies run).  GPU tests: the same binaries on a B200, and the
+(scheduling, ownership hand-over, concurrent callers; no bodies run).  GPU tests: the same binaries on an H100, and the
 reference's own cuda component on the same task pools as a cross-check."""
 import json
 import os

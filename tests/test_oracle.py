@@ -1,7 +1,10 @@
 """Pins the CPU oracle (oracle/) against the reference: known answers of the reference's own tests and
-examples, and -- when oracle/_ref was built from /root/reference -- the reference's own compiled code.
+examples, and the reference's own compiled code -- live where oracle/_ref was built from the reference's sources,
+replayed from its recorded answers (tests/golden/reference_pieces.json.gz) everywhere else.
 No GPU needed."""
 import ctypes as C
+import gzip
+import json
 import os
 import random
 
@@ -14,6 +17,52 @@ HAVE_REF_ZONE = os.path.exists(orc.REF_ZONE_PATH)
 HAVE_REF_DATA = os.path.exists(orc.REF_DATA_PATH)
 HAVE_REF_TWODBC = os.path.exists(orc.REF_TWODBC_PATH)
 HAVE_REF_SELECT = os.path.exists(orc.REF_SELECT_PATH)
+GOLDEN_PIECES = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pieces.json.gz")
+RECORDED = {}           # piece -> answers of the live library, in call order (tests/golden/make_golden.py writes them out)
+_VOID = {"ref_twodbc_free", "ref_sel_init", "ref_sel_set_load", "zone_free", "ref_data_add_copy", "ref_data_set", "ref_end_transfer"}
+
+
+def _is_out(a):
+    return isinstance(a, C.Array) or type(a).__name__ == "CArgObject"
+
+
+class Reference:
+    """One piece of the reference compiled from its own sources (oracle/Makefile.ref), seen through its answers in call
+    order: return values and out-parameters (ctypes arrays, byref).  With the library (`lib`) the calls go to it and are
+    recorded; without it they are replayed from the golden file, so the oracle is held to the same answers.  zone_malloc
+    answers are kept relative to `base`, the arena the test hands the allocator."""
+
+    def __init__(self, piece, lib, base=0):
+        self.piece, self.lib, self.base = piece, lib, base
+        if lib is not None:
+            self.log = RECORDED.setdefault(piece, [])
+            del self.log[:]
+        else:
+            with gzip.open(GOLDEN_PIECES, "rt") as f:
+                self.log = json.load(f)[piece][::-1]
+
+    def __getattr__(self, fn):
+        def call(*args):
+            outs = [a._obj if type(a).__name__ == "CArgObject" else a for a in args if _is_out(a)]
+            if self.lib is not None:
+                r = getattr(self.lib, fn)(*args)
+                if fn not in _VOID:
+                    rec = (-1 if not r else r - self.base) if fn == "zone_malloc" else r
+                    self.log.append([fn, rec] + [list(o) if isinstance(o, C.Array) else o.value for o in outs])
+                return r
+            if fn in _VOID:
+                return None
+            e = self.log.pop()
+            assert e[0] == fn, ("replay out of step", e[0], fn)
+            for o, v in zip(outs, e[2:]):
+                if isinstance(o, C.Array):
+                    o[:] = v
+                else:
+                    o.value = v
+            if fn == "zone_malloc":
+                return None if e[1] < 0 else self.base + e[1]
+            return e[1]
+        return call
 
 
 def tiles_for(dag, valid=False):
@@ -173,13 +222,12 @@ def test_twodbc_owner_and_slots(P, Q, kp, kq, ip, jq):
                 assert L.orc_twodbc_rank_of(C.byref(d), m, n) == (m % P) * Q + (n % Q)   # SURVEY 8(e)
 
 
-@pytest.mark.skipif(not HAVE_REF_TWODBC, reason="oracle/_ref/libtwodbc_ref.so not built (needs /root/reference)")
 def test_twodbc_oracle_and_product_equal_reference_build():
-    """The reference's own two_dim_rectangle_cyclic.c (compiled from /root/reference) vs the oracle's restatement vs
-    the product's pb2_matrix_block_cyclic_new: owner, key, derived sizes, for plain, k-cyclic and offset grids, full
+    """The reference's own two_dim_rectangle_cyclic.c (compiled from the reference's sources) vs the oracle's restatement
+    vs the product's pb2_matrix_block_cyclic_new: owner, key, derived sizes, for plain, k-cyclic and offset grids, full
     and sub-matrices, every rank."""
     from parsec_b200 import runtime as R
-    ref = orc.ref_twodbc()
+    ref = Reference("twodbc", orc.ref_twodbc() if HAVE_REF_TWODBC else None)
     L = orc.lib()
     rl = R.lib()
     rng = random.Random(2026)
@@ -261,13 +309,12 @@ def _sel(devs, access, present, pref, owner, skew=20, allow_cpu=0):
     return orc.lib().orc_select_best_device(arr, len(devs), len(access), *[x.ctypes.data_as(C.c_void_p) for x in a], skew, allow_cpu)
 
 
-@pytest.mark.skipif(not HAVE_REF_SELECT, reason="oracle/_ref/libselect_ref.so not built (needs /root/reference)")
 def test_select_oracle_equals_reference_build():
-    """The reference's own parsec_select_best_device (device.c:100-310, compiled from /root/reference, driven with fake
+    """The reference's own parsec_select_best_device (device.c:100-310, compiled from its sources, driven with fake
     device modules and tasks) vs the oracle: 4000 random tasks over a CPU, the recursive device and four GPUs --
     affinity by preferred/owner device, ETA with the 20 % skew, taskpool device masks, CPU incarnations with and
     without load_balance_allow_cpu."""
-    ref = orc.ref_select()
+    ref = Reference("select", orc.ref_select() if HAVE_REF_SELECT else None)
     CPU, REC, CUDA = 1, 2, 4
     types = [CPU, REC, CUDA, CUDA, CUDA, CUDA]
     rng = random.Random(77)
@@ -357,19 +404,20 @@ def test_zone_reference_scenario():
     L.orc_zone_fini(z)
 
 
-@pytest.mark.skipif(not HAVE_REF_ZONE, reason="oracle/_ref/libzone_ref.so not built (needs /root/reference)")
 def test_zone_oracle_equals_reference_build():
     """Same malloc/free sequences through the REAL parsec/utils/zone_malloc.c (compiled by oracle/Makefile.ref)
     and through the restatement: identical addresses and in-use bytes at every step."""
-    ref = C.CDLL(orc.REF_ZONE_PATH)
+    lib = C.CDLL(orc.REF_ZONE_PATH) if HAVE_REF_ZONE else None
     L = orc.lib()
-    ref.zone_malloc_init.restype = C.c_void_p; ref.zone_malloc_init.argtypes = [C.c_void_p, C.c_int, C.c_size_t]
-    ref.zone_malloc.restype = C.c_void_p; ref.zone_malloc.argtypes = [C.c_void_p, C.c_size_t]
-    ref.zone_free.argtypes = [C.c_void_p, C.c_void_p]
-    ref.zone_in_use.restype = C.c_size_t; ref.zone_in_use.argtypes = [C.c_void_p]
+    if lib is not None:
+        lib.zone_malloc_init.restype = C.c_void_p; lib.zone_malloc_init.argtypes = [C.c_void_p, C.c_int, C.c_size_t]
+        lib.zone_malloc.restype = C.c_void_p; lib.zone_malloc.argtypes = [C.c_void_p, C.c_size_t]
+        lib.zone_free.argtypes = [C.c_void_p, C.c_void_p]
+        lib.zone_in_use.restype = C.c_size_t; lib.zone_in_use.argtypes = [C.c_void_p]
     NSEG, UNIT = 96, 512
     buf = (C.c_char * (NSEG * UNIT))()
     base = C.addressof(buf)
+    ref = Reference("zone", lib, base)
     for seed in range(25):
         rnd = random.Random(seed)
         zr, zo = ref.zone_malloc_init(base, NSEG, UNIT), L.orc_zone_init(NSEG, UNIT)
@@ -389,16 +437,17 @@ def test_zone_oracle_equals_reference_build():
 
 
 # ------------------------------------------------------------------ coherency protocol
-@pytest.mark.skipif(not HAVE_REF_DATA, reason="oracle/_ref/libdata_ref.so not built (needs /root/reference)")
 def test_coherency_oracle_equals_reference_build():
     """Random start/end_transfer_ownership sequences through the REAL parsec/data.c (compiled by
     oracle/Makefile.ref) and the restatement leave identical host-visible state and return values."""
-    ref = C.CDLL(orc.REF_DATA_PATH)
+    lib = C.CDLL(orc.REF_DATA_PATH) if HAVE_REF_DATA else None
     L = orc.lib()
-    ref.ref_data_new.restype = C.c_void_p
-    for fn in (ref.ref_data_add_copy, ref.ref_data_set, ref.ref_data_get, ref.ref_data_owner, ref.ref_start_transfer,
-               ref.ref_end_transfer, ref.ref_data_set_owner):
-        fn.argtypes = None
+    if lib is not None:
+        lib.ref_data_new.restype = C.c_void_p
+        for fn in (lib.ref_data_add_copy, lib.ref_data_set, lib.ref_data_get, lib.ref_data_owner, lib.ref_start_transfer,
+                   lib.ref_end_transfer, lib.ref_data_set_owner):
+            fn.argtypes = None
+    ref = Reference("data", lib)
     NDEV = 6
     assert ref.ref_data_setup(NDEV) == 0
     R, W = 0x04, 0x08

@@ -1,6 +1,6 @@
 // batch_probe.cu -- what moves 4096 tiles of 256 KiB from registered host memory to the device fastest:
 // one cudaMemcpyAsync per tile, cudaMemcpyBatchAsync of 128 tiles, or one copy of everything.
-// nvcc -arch=sm_100a tools/batch_probe.cu -o tools/batch_probe && tools/batch_probe
+// nvcc -arch=sm_90a tools/batch_probe.cu -o tools/batch_probe && tools/batch_probe
 #include <cuda_runtime.h>
 #include <chrono>
 #include <cstdio>
