@@ -126,12 +126,12 @@ typedef struct pb2_tile_s {
 #define PB2_TILE_VALID     2   /* SHARED/OWNED + COMPLETE_TRANSFER                                           */
 
 typedef struct pb2_engine_params_s {
-    int32_t  workers_per_sm;   /* CTAs per SM for HBM-body windows (default 4)                               */
-    int32_t  threads;          /* threads per CTA for HBM-body windows (default 256)                         */
+    int32_t  workers_per_sm;   /* CTAs per SM for HBM-body windows (default 12, at most what the kernel's occupancy allows) */
+    int32_t  threads;          /* threads per CTA for HBM-body windows (default and maximum 64)               */
     int32_t  max_workers;      /* 0 = all; 1 = single worker => deterministic FIFO order (tests)             */
     int32_t  stage_mode;       /* tile mover of the HBM-body kernels: 0 = TMA bulk copy (cp.async.bulk through a
                                 * shared-memory ring, default), 1 = SIMT 16-byte LDG/STG loops                      */
-    int32_t  queue_policy;     /* 0 = FIFO ring, 1 = successors-first (hot ring before FIFO ring)             */
+    int32_t  queue_policy;     /* accepted and ignored: every kernel runs one FIFO ready ring                 */
     int32_t  timeout_ms;       /* device-side watchdog: a window that makes no progress for this long aborts
                                 * (default 20000); a malformed DAG must never hang the GPU                   */
     int32_t  gemm_mode;        /* 0 = fused k-chains (default), 1 = v1 kernel (one task at a time),
@@ -139,6 +139,9 @@ typedef struct pb2_engine_params_s {
     int32_t  part_bytes;       /* HBM bodies: a task whose largest tile exceeds this many bytes is run as up to 512
                                 * parts (byte slices) by different workers (default 256 KiB, <0 = never split);
                                 * pb2_engine_set_part_bytes changes it for the windows created afterwards       */
+    int32_t  read_groups;      /* HBM windows that are not shared: 0 = a run of consecutive out-edges of one task into
+                                * CHECK readers of the same tile (that edge their only input) is executed as one group
+                                * that streams the tile once for all its members (default); < 0 = every task alone  */
 } pb2_engine_params_t;
 
 typedef struct pb2_engine_info_s {

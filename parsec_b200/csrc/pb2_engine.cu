@@ -71,8 +71,11 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
 // ---------------------------------------------------------------------------------------------
 // 64-thread workers, 12 per SM (<= 80 registers, no spills): a worker keeps PB2_CHECK_UNROLL = 16 (read-only bodies) or
 // PB2_UNROLL = 4 (read-modify-write bodies) 16-byte requests per thread in flight -- bytes in flight per SM are what
-// the L2-bound Ex05 window responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms, 12 x 16 0.60 ms),
-// while many small workers still overlap the serial pop / release sections of one task with the streaming of the others.
+// a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
+// 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
+// streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
+// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times, and the step
+// takes what F = 1 takes (DESIGN.md §8).
 // What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
 #ifndef PB2_HBM_MINB
 #define PB2_HBM_MINB 12
@@ -80,10 +83,44 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
 #ifndef PB2_HBM_THREADS
 #define PB2_HBM_THREADS 64
 #endif
+// A read group in flight on one worker: its members (the leader first), their CHECK constants, this part's results.
+struct GroupSmem {
+    int32_t n;                              // members; 0: the popped task runs alone
+    int32_t mem[PB2_GROUP_MAX];
+    uint32_t k[PB2_GROUP_MAX];
+    unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
+};
+
+// All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
+// bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
+//  - k equal to the leader's: the leader's result;
+//  - the slice held nothing but the leader's constant: every element mismatches (the first element is the same);
+//  - otherwise the member's slice is counted again, exactly, as a failing CHECK counts it.
+static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const unsigned long long r0 = g.res[0];
+#pragma unroll 1
+    for (int i = 1; i < g.n; ++i) {
+        const uint32_t k = g.k[i];
+        if (k == g.k[0] || !(r0 >> 32)) {
+            if (threadIdx.x == 0) g.res[i] = k == g.k[0] ? r0 : ((unsigned long long)(s.args.bytes[0] >> 2) << 32) | (uint32_t)r0;
+            continue;
+        }
+        if (threadIdx.x == 0) s.args.iparam[0] = (int32_t)k;
+        __syncthreads();
+        const unsigned long long r = run_hbm_body(PB2_BODY_CHECK_I32, s.args, s.red);
+        if (threadIdx.x == 0) g.res[i] = r;
+        __syncthreads();
+    }
+    __syncthreads();
+}
+
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
 pb2_engine_hbm_kernel(WinDev w) {
     __shared__ TaskSmem s;
     __shared__ BulkSmem bulk;
+    __shared__ GroupSmem g;
     if (threadIdx.x == 0) bulk_init(bulk);
     __syncthreads();
 
@@ -100,25 +137,68 @@ pb2_engine_hbm_kernel(WinDev w) {
         const int part = w.nparts ? PB2_ENT_PART(entry) : 0;
         if (threadIdx.x < 4) reinterpret_cast<uint4*>(&s.task)[threadIdx.x] =
             __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
-        if (threadIdx.x == 0 && part == 0) {
-            w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
-            w.worker[id] = (int32_t)blockIdx.x;
+        {
+            const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
+            const int gn = (int)(gd & 15u);
+            if ((int)threadIdx.x < gn) {
+                const int32_t m = __ldg(&w.group_mem[(gd >> 4) + threadIdx.x]);
+                const pb2_task_t& mt = w.tasks[m];
+                g.mem[threadIdx.x] = m;
+                g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
+            }
+            if (threadIdx.x == 0) {
+                g.n = gn;
+                if (part == 0 && gn) {
+                    // the members start together: consecutive event numbers, one worker
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
+                    for (int i = 0; i < gn; ++i) {
+                        const int32_t m = __ldg(&w.group_mem[(gd >> 4) + i]);
+                        w.start_seq[m] = seq + (uint32_t)i;
+                        w.worker[m] = (int32_t)blockIdx.x;
+                    }
+                } else if (part == 0) {
+                    w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
+                    w.worker[id] = (int32_t)blockIdx.x;
+                }
+            }
         }
         __syncthreads();
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts);
+        if (g.n) {
+            // the leader's part stored the version it saw; every member saw the same one
+            if (threadIdx.x == 0) {
+                g.res[0] = r;
+                if (part == 0) {
+                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.seen_version[(size_t)id * PB2_MAX_FLOWS]);
+                    for (int i = 1; i < g.n; ++i) w.seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
+                }
+            }
+            __syncthreads();
+            group_results(&s, &g);
+        }
 
         if (threadIdx.x < 32) {
             __threadfence();   // release side: the body's stores (all threads, ordered by the barrier) become
                                // visible before any successor can observe its dependency word / ring slot
             if (threadIdx.x == 0) {
                 const pb2_task_t& t = s.task;
-                store_result(w, t, id, part, nparts, r);
+                const int gn = g.n;
+                if (gn) for (int i = 0; i < gn; ++i) store_result(w, t, g.mem[i], part, nparts, g.res[i]);
+                else store_result(w, t, id, part, nparts, r);
                 // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
                 int last = 1;
                 if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
                 s.window_done = 0; s.last = last;
-                if (last) {
+                if (last && gn) {
+                    // members only read their tile: no written flows; they retire back to back, in member order
+                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
+                    for (int i = 0; i < gn; ++i) { w.end_seq[g.mem[i]] = ev + (uint32_t)i; w.retire_log[seq + (uint32_t)i] = g.mem[i]; }
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    s.window_done = (int32_t)(seq + (uint32_t)gn) == w.ntasks ? 1 : 0;
+                    __threadfence();
+                } else if (last) {
                     epilog_written_flows(w, t);
                     w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
                     // the retire log is written before the out-edges are released, so that it is a linear
@@ -135,7 +215,8 @@ pb2_engine_hbm_kernel(WinDev w) {
             if (s.last && w.ps_begin[id + 1] > w.ps_begin[id]) push_written_tiles(w.tiles, w.ctl, w.ps_begin, w.ps, id, &bulk);
         }
         if (threadIdx.x < 32) {
-            if (s.last) { release_successors_warp(w, s.task); release_remote_warp(w, id); }
+            if (s.last && g.n) { for (int i = 0; i < g.n; ++i) release_successors_warp(w, w.tasks[g.mem[i]]); }
+            else if (s.last) { release_successors_warp(w, s.task); release_remote_warp(w, id); }
             if (threadIdx.x == 0 && s.window_done) {
                 __threadfence();
                 st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
@@ -420,6 +501,63 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     w->g.units = d_units; w->g.segs = d_segs; w->g.usucc = d_usucc; w->g.nunits = (int32_t)units.size();
     w->nentries = (int32_t)entries.size();
     return PB2_SUCCESS;
+}
+
+// ---------------------------------------------------------------------------------------------
+// read groups of HBM windows
+// ---------------------------------------------------------------------------------------------
+// A run of >= 2 consecutive out-edges of one task whose targets all
+//   - have that edge as their only input (in-degree 1, not ready at start; counter goal 1, or the edge's one mask bit),
+//   - run a CHECK body over exactly one data flow, flow 0, READ only, on the same tile,
+// becomes one edge to the run's first target (the leader) in the device CSR, and the leader's worker streams the tile
+// once for all the members (pb2_engine_hbm_kernel).  Without groups F readers of a tile each pull it through L2 into
+// their own SM, F passes where one carries the same bytes.  The members become ready together and would have entered
+// the FIFO ring back to back: with one worker the retire order is the ungrouped one.  Runs longer than PB2_GROUP_MAX
+// are split.  O(ntasks + nsucc); tasks keep their own out-edges.  Returns false when no group formed.
+static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
+                             std::vector<uint32_t>& gsucc, std::vector<uint32_t>& group, std::vector<int32_t>& gmem) {
+    const size_t n = tasks.size();
+    std::vector<uint8_t> indeg(n, 0);                        // saturates at 2
+    for (size_t u = 0; u < n; ++u)
+        for (int32_t j = 0; j < tasks[u].succ_count; ++j) {
+            uint8_t& d = indeg[(size_t)PB2_SUCC_TASK(succ[tasks[u].succ_begin + j])];
+            if (d < 2) ++d;
+        }
+    for (int32_t i = 0; i < nready; ++i) indeg[(size_t)ready[i]] = 2;
+    auto reader = [&](uint32_t s) {
+        const pb2_task_t& t = tasks[(size_t)PB2_SUCC_TASK(s)];
+        if (indeg[(size_t)PB2_SUCC_TASK(s)] != 1) return false;
+        if (t.dep_goal != ((t.flags & PB2_TASK_DEPS_MASK) ? (int32_t)(1u << PB2_SUCC_FLOW(s)) : 1)) return false;
+        if (t.body != PB2_BODY_CHECK_I32 && t.body != PB2_BODY_CHECK_F32) return false;
+        if (t.nb_flows < 1 || t.tile[0] < 0 || (t.access[0] & (PB2_FLOW_ACCESS_RW | PB2_FLOW_PUSHOUT)) != PB2_FLOW_ACCESS_READ) return false;
+        for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
+        return true;
+    };
+    std::vector<int32_t> begin(n), count(n);
+    group.assign(n, 0u);
+    gsucc.clear(); gmem.clear();
+    for (size_t u = 0; u < n; ++u) {
+        const uint32_t* out = succ + tasks[u].succ_begin;
+        const int32_t c = tasks[u].succ_count;
+        begin[u] = (int32_t)gsucc.size();
+        for (int32_t j = 0; j < c;) {
+            int32_t r = j + 1;
+            if (reader(out[j])) {
+                const int32_t tile = tasks[(size_t)PB2_SUCC_TASK(out[j])].tile[0];
+                while (r < c && r - j < PB2_GROUP_MAX && reader(out[r]) && tasks[(size_t)PB2_SUCC_TASK(out[r])].tile[0] == tile) ++r;
+            }
+            gsucc.push_back(out[j]);
+            if (r - j >= 2) {
+                group[(size_t)PB2_SUCC_TASK(out[j])] = ((uint32_t)gmem.size() << 4) | (uint32_t)(r - j);
+                for (int32_t q = j; q < r; ++q) gmem.push_back(PB2_SUCC_TASK(out[q]));
+            }
+            j = r;
+        }
+        count[u] = (int32_t)gsucc.size() - begin[u];
+    }
+    if (gmem.empty()) return false;
+    for (size_t u = 0; u < n; ++u) { tasks[u].succ_begin = begin[u]; tasks[u].succ_count = count[u]; }
+    return true;
 }
 
 extern "C" {
@@ -741,8 +879,14 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
         for (int p = 0; p < (int)nparts[(size_t)ready[i]]; ++p) entries.push_back(PB2_ENT_MAKE(ready[i], p));
     w->task_entry.resize((size_t)ntasks);
     for (int32_t i = 0; i < ntasks; ++i) w->task_entry[(size_t)i] = PB2_ENT_MAKE(i, (int)nparts[(size_t)i] - 1);
+    // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
+    std::vector<uint32_t> gsucc, group;
+    std::vector<int32_t> gmem;
+    const bool grouped = kind == 0 && !w->shared && e->params.read_groups >= 0 &&
+                         form_read_groups(dtasks, succ, ready, nready, gsucc, group, gmem);
     TRY(dev_alloc_copy(w, &w->d_tasks, dtasks.data(), (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &w->d_succ, succ, (size_t)nsucc));
+    if (grouped) TRY(dev_alloc_copy(w, &w->d_succ, gsucc.data(), gsucc.size()));
+    else TRY(dev_alloc_copy(w, &w->d_succ, succ, (size_t)nsucc));
     TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
     TRY(dev_alloc_copy(w, &w->d_tiles, (const pb2_tile_t*)nullptr, (size_t)ntiles));
     TRY(dev_alloc_copy(w, &w->d_ready, entries.data(), entries.size()));
@@ -775,6 +919,13 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     d.ps_begin = nullptr; d.ps = nullptr;
     d.slice_claim = nullptr; d.slice_done = nullptr; d.part_bytes = e->params.part_bytes;
     d.nparts = nullptr; d.remote_units = 0;
+    d.group = nullptr; d.group_mem = nullptr;
+    if (grouped) {
+        uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
+        TRY(dev_alloc_copy(w, &d_group, group.data(), group.size()));
+        TRY(dev_alloc_copy(w, &d_gmem, gmem.data(), gmem.size()));
+        d.group = d_group; d.group_mem = d_gmem;
+    }
     if (kind == 0 && extra_parts) {
         uint16_t* d_np = nullptr;
         TRY(dev_alloc_copy(w, &d_np, nparts.data(), (size_t)ntasks));
