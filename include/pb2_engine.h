@@ -134,8 +134,8 @@ typedef struct pb2_engine_params_s {
     int32_t  queue_policy;     /* accepted and ignored: every kernel runs one FIFO ready ring                 */
     int32_t  timeout_ms;       /* device-side watchdog: a window that makes no progress for this long aborts
                                 * (default 20000); a malformed DAG must never hang the GPU                   */
-    int32_t  gemm_mode;        /* 0 = fused k-chains (default), 1 = v1 kernel (one task at a time),
-                                * 2 = chain kernel, every task flushes C (per-task bf16 rounding, as the oracle)       */
+    int32_t  gemm_mode;        /* 0 = fused k-chains (default), 2 = every task is its own unit and flushes C
+                                * (per-task bf16 rounding, as the oracle); 1 is accepted as an alias of 2        */
     int32_t  part_bytes;       /* HBM bodies: a task whose largest tile exceeds this many bytes is run as up to 512
                                 * parts (byte slices) by different workers (default 256 KiB, <0 = never split);
                                 * pb2_engine_set_part_bytes changes it for the windows created afterwards       */

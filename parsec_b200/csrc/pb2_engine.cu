@@ -29,7 +29,6 @@
 #include "pb2_sched.cuh"
 #include "pb2_worker.cuh"
 #include "pb2_gemm.cuh"
-#include "pb2_gemm2.cuh"
 
 namespace pb2 {
 
@@ -226,7 +225,7 @@ pb2_engine_hbm_kernel(WinDev w) {
     }
 }
 
-// re-arm the unit-level scheduling state of a v2 GEMM window (after pb2_window_reset_kernel re-armed the rest)
+// re-arm the unit-level scheduling state of a GEMM window (after pb2_window_reset_kernel re-armed the rest)
 __global__ void pb2_window2_reset_kernel(Win2Dev g, const int32_t* ready_entries, int32_t nentries) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
@@ -295,8 +294,7 @@ struct pb2_window_s {
     int32_t* d_ready = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
     CUtensorMap* d_tmaps = nullptr;     // kind 1: one 2-D bf16 tensor map per tile (box 64 x 128, 128B swizzle)
-    bool v2 = false;                    // kind 1 executed by the CTA-pair kernel on units
-    Win2Dev g{};
+    Win2Dev g{};                        // kind 1: the unit-level state of pb2_engine_gemm2_kernel
     int32_t* d_ready_entries = nullptr;
     int32_t nentries = 0;
     bool launched = false;
@@ -326,6 +324,7 @@ static int validate_window(pb2_engine_t* e, int kind, const pb2_task_t* tasks, i
                            const uint32_t* succ, int32_t nsucc, int32_t ntiles,
                            const int32_t* ready, int32_t nready) {
     if (ntasks < 0 || nsucc < 0 || ntiles < 0 || nready < 0) return PB2_ERR_BAD_PARAM;
+    if (kind != 0 && kind != 1) { e->last_error = "window kind must be 0 (HBM bodies) or 1 (GEMM bodies)"; return PB2_ERR_BAD_PARAM; }
     if (ntasks >= (1 << 27)) return PB2_ERR_VALUE_OUT_OF_BOUNDS;
     // ready-ring entries of the HBM kernel carry the task id in 22 bits (PB2_ENT_MAKE: part << 22 | task)
     if (kind == 0 && ntasks >= (1 << 22)) { e->last_error = "an HBM window holds at most 4194303 tasks (22-bit task id in the ready ring)"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
@@ -401,7 +400,7 @@ static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
 
 
 // ---------------------------------------------------------------------------------------------
-// v2 GEMM windows: group tasks into units (fused k-chains), see pb2_gemm2.cuh
+// GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
 static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
                              const int32_t* ready, int32_t nready, bool fuse, uint32_t* ring_cap_needed,
@@ -441,8 +440,9 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         const bool g = is_gemm(h);
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
-        u.nparts = g ? ((u.M + gemm2::kPartRows - 1) / gemm2::kPartRows) * ((u.N + gemm2::kPartCols - 1) / gemm2::kPartCols) : 1;
-        if (g && ((u.N % 16) || u.nparts > gemm2::kMaxParts)) return PB2_ERR_NOT_SUPPORTED;       // caller falls back to the v1 kernel
+        // a part runs every nparts-th 128 x 256 sub-tile of C
+        const int nsub = g ? ((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN) : 1;
+        u.nparts = std::min(nsub, gemm::kMaxParts);
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
             segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});
@@ -611,7 +611,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     if (per_sm < 1) per_sm = 1;
     e->nworkers = e->prop.multiProcessorCount * per_sm;
     if (p.max_workers > 0 && p.max_workers < e->nworkers) e->nworkers = p.max_workers;
-    e->nworkers_gemm = pb2_gemm_nworkers(e->prop.multiProcessorCount);
+    e->nworkers_gemm = e->prop.multiProcessorCount;      // one CTA per SM
     if (p.max_workers > 0 && p.max_workers < e->nworkers_gemm) e->nworkers_gemm = p.max_workers;
     *engine = e;
     return PB2_SUCCESS;
@@ -894,12 +894,8 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     uint32_t parts_needed = 0;
     if (kind == 1) {
         TRY(build_tensor_maps(w, tasks, ntasks, tiles, ntiles));
-        if (e->params.gemm_mode != 1) {
-            rc = build_gemm2_units(w, tasks, ntasks, succ, ready, nready, e->params.gemm_mode == 0, &parts_needed,
-                                   w->shared ? e->next_rs_begin : nullptr);
-            if (rc == PB2_SUCCESS) w->v2 = true;
-            else if (rc != PB2_ERR_NOT_SUPPORTED) { pb2_window_destroy(w); return rc; }     // NOT_SUPPORTED: v1 kernel
-        }
+        TRY(build_gemm2_units(w, tasks, ntasks, succ, ready, nready, e->params.gemm_mode == 0, &parts_needed,
+                              w->shared ? e->next_rs_begin : nullptr));
     }
     const int maxw = e->nworkers > e->nworkers_gemm ? e->nworkers : e->nworkers_gemm;
     uint32_t cap = 1024;
@@ -947,9 +943,9 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
             TRY(dev_alloc_copy(w, &d.slice_done, (const uint32_t*)nullptr, (size_t)ntiles * (PB2_SLICE_WORDS + 1)));
         }
     }
-    if (kind == 1 && w->v2) {
-        // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every CTA pair
-        // that needs them (the parts of one unit, the units that share an operand) instead of by one CTA alone
+    if (kind == 1) {
+        // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every worker
+        // that needs them (the parts of one unit, the units that share an operand) instead of by one worker alone
         d.part_bytes = 64 * 1024;
         TRY(dev_alloc_copy(w, &d.slice_claim, (const uint32_t*)nullptr, (size_t)ntiles * PB2_SLICE_WORDS));
         TRY(dev_alloc_copy(w, &d.slice_done, (const uint32_t*)nullptr, (size_t)ntiles * (PB2_SLICE_WORDS + 1)));
@@ -957,7 +953,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
 #undef TRY
     d.cap_mask = cap - 1; d.ntasks = ntasks; d.ntiles = ntiles; d.stage_mode = e->params.stage_mode;
     d.timeout_ns = (unsigned long long)e->params.timeout_ms * 1000000ull;
-    if (w->v2) { w->g.w = d; w->g.tmaps = w->d_tmaps; w->g.debug = getenv("PB2_GEMM_DEBUG") ? atoi(getenv("PB2_GEMM_DEBUG")) : 0; }
+    if (kind == 1) { w->g.w = d; w->g.tmaps = w->d_tmaps; w->g.fresh_tmaps = 1; }
     PB2_CUDA(e, cudaEventCreate(&w->ev0));
     PB2_CUDA(e, cudaEventCreate(&w->ev1));
     PB2_CUDA(e, cudaEventCreate(&w->ev2));
@@ -1001,7 +997,7 @@ int pb2_window_arm(pb2_window_t* w) {
         pb2_window_reset_kernel<<<blocks, threads, 0, e->stream>>>(w->d, w->d_tiles_init, w->d_ready, w->nready_entries);
         PB2_CUDA(e, cudaGetLastError());
     }
-    if (w->ntasks > 0 && w->kind == 1 && w->v2) {
+    if (w->ntasks > 0 && w->kind == 1) {
         pb2_window2_reset_kernel<<<64, 256, 0, e->stream>>>(w->g, w->d_ready_entries, w->nentries);
         PB2_CUDA(e, cudaGetLastError());
     }
@@ -1017,12 +1013,10 @@ int pb2_window_start(pb2_window_t* w) {
         if (w->kind == 0) {
             pb2_engine_hbm_kernel<<<e->nworkers, e->params.threads, 0, e->stream>>>(w->d);
             PB2_CUDA(e, cudaGetLastError());
-        } else if (w->v2) {
-            int rc = pb2_gemm2_launch(w->g, e->nworkers_gemm, e->stream);
-            if (rc != PB2_SUCCESS) { e->last_error = "gemm v2 window launch failed"; return rc; }
         } else {
-            int rc = pb2_gemm_launch(w->d, w->d_tmaps, e->nworkers_gemm, e->stream);
+            int rc = pb2_gemm2_launch(w->g, e->nworkers_gemm, e->stream);
             if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
+            w->g.fresh_tmaps = 0;
         }
     }
     PB2_CUDA(e, cudaEventRecord(w->ev2, e->stream));
@@ -1042,18 +1036,18 @@ int pb2_window_export(pb2_window_t* w, pb2_window_handle_t* h) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     memset(h, 0, sizeof *h);
     cudaIpcMemHandle_t ih;
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->v2 ? w->g.udep : w->d.dep));  memcpy(h->dep, &ih, 64);   // fused-GEMM windows: unit words
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->kind == 1 ? w->g.udep : w->d.dep));  memcpy(h->dep, &ih, 64);   // GEMM windows: unit words
     PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.ring)); memcpy(h->ring, &ih, 64);
     PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.ctl));  memcpy(h->ctl, &ih, 64);
     if (w->d.tiles && w->ntiles > 0) { PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.tiles)); memcpy(h->tiles, &ih, 64); h->ntiles = w->ntiles; }
-    h->cap_mask = w->d.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->v2 ? 1 : 0;
+    h->cap_mask = w->d.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->kind == 1 ? 1 : 0;
     return PB2_SUCCESS;
 }
 
 int pb2_window_set_push(pb2_window_t* w, const int32_t* ps_begin, const pb2_push_t* push, int32_t npush) {
     if (!w || !ps_begin || npush < 0 || (npush && !push)) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
-    if (w->v2 || !w->d.peers) { e->last_error = "pushes need an HBM window whose remote edges are set (pb2_window_set_remote)"; return PB2_ERR_NOT_SUPPORTED; }
+    if (w->kind == 1 || !w->d.peers) { e->last_error = "pushes need an HBM window whose remote edges are set (pb2_window_set_remote)"; return PB2_ERR_NOT_SUPPORTED; }
     if (ps_begin[w->ntasks] != npush) return PB2_ERR_BAD_PARAM;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     std::vector<PushDev> pd((size_t)npush);
@@ -1080,7 +1074,7 @@ int pb2_window_set_remote(pb2_window_t* w, int32_t my_rank, int32_t nranks, cons
     if (!w || nranks <= 0 || my_rank < 0 || my_rank >= nranks || !peers || !rs_begin || nrs < 0) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
-    const int32_t my_kind = w->v2 ? 1 : 0;
+    const int32_t my_kind = w->kind == 1 ? 1 : 0;
     for (int32_t r = 0; r < nranks; ++r)
         if (r != my_rank && peers[r].entry_kind != my_kind) { e->last_error = "peers run a different kind of window (fused GEMM units vs tasks)"; return PB2_ERR_NOT_SUPPORTED; }
     for (int32_t i = 0; i < nrs; ++i) {
@@ -1119,7 +1113,7 @@ int pb2_window_set_remote(pb2_window_t* w, int32_t my_rank, int32_t nranks, cons
     if ((rc = dev_alloc_copy(w, &d_t, rs_target, (size_t)nrs)) != PB2_SUCCESS) return rc;
     PB2_CUDA(e, cudaStreamSynchronize(e->up_stream));
     w->d.peers = d_pw; w->d.rs_begin = d_b; w->d.rs_rank = d_r; w->d.rs_target = d_t; w->d.remote_units = my_kind;
-    if (w->v2) w->g.w = w->d;
+    if (w->kind == 1) w->g.w = w->d;
     return PB2_SUCCESS;
 }
 

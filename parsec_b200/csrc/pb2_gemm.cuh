@@ -1,4 +1,4 @@
-// pb2_gemm.cuh -- tensor-core (wgmma / TMA / mbarrier) engine kernel for PB2_BODY_GEMM_BF16 windows.
+// pb2_gemm.cuh -- the tensor-core (wgmma / TMA / mbarrier) engine kernel of PB2_BODY_GEMM_BF16 windows.
 //
 // The task body restates what the reference reaches through `dyld=cublasDgemm` / cublasDgemm_v2
 // (tests/dsl/dtd/dtd_test_simple_gemm.c:450,527; tests/runtime/cuda/nvlink.jdf:136-152): one tile
@@ -6,12 +6,23 @@
 // (BASELINE config 3); tiles are K-contiguous for both operands: A row-major [M][K], B stored
 // [N][K] (== column-major K x N, what a "TN" cuBLAS call consumes), C row-major [M][N].
 //
+// The host groups GEMM tasks into UNITS (build_gemm2_units): a maximal chain of tasks that accumulate into the same C
+// tile and whose only missing dependency is the previous link (the C(i,j) k-chain of dtd_test_simple_gemm.c:675-696,
+// the k-chains of a tile Cholesky); with gemm_mode 1 or 2 every task is a unit of its own.  A unit's C is cut into
+// sub-tiles of 128 rows x 256 columns, run by nparts = min(sub-tiles, kMaxParts) independent parts: part p runs
+// sub-tiles p, p + nparts, p + 2 nparts, ...  For each sub-tile the worker keeps the 128 x 256 fp32 accumulator in the
+// registers of its two consumer warpgroups across ALL the members of the chain and touches C once:
+// C_out = bf16(C_in + sum_k A_k B_k^T).  This is the reference's "keep the released successor for the same execution
+// stream" (es->next_task, scheduling.c:517-530) taken to its conclusion: 32 dependent tasks become one accumulation.
+// Members still retire one by one, in chain order, with their own sequence numbers, versions and out-edges (the
+// dependency trace is unchanged); only the intermediate bf16 roundings of C disappear.  Scheduling entities on the
+// device are units (counter-mode dependency words), ring entries are (part, unit).
+//
 // One CTA per SM is one worker.  Three warpgroups (384 threads):
-//   warpgroup 0 : warp 0 is the scheduler (ring pop / dependency release / retire) and, one lane, the TMA producer
+//   warpgroup 0 : warp 0 retires a unit and releases its out-edges; one lane of warp 1 is the TMA producer
 //   warpgroups 1, 2 : consumers; each issues `wgmma.mma_async` m64n256k16 for its 64 rows of the sub-tile and keeps
 //                 the 64 x 256 fp32 accumulator in registers, then adds it into C (bf16) itself
-// A task is executed as ceil(M/128) x ceil(N/256) accumulator sub-tiles of 128 x 256 fp32.  Operands stream
-// through a 4-stage smem ring of {A 128x64, B 256x64} bf16 128B-swizzled boxes filled by TMA
+// Operands stream through a 4-stage smem ring of {A 128x64, B 256x64} bf16 128B-swizzled boxes filled by TMA
 // (`cp.async.bulk.tensor.2d`) from per-tile tensor maps; the producer fills the next sub-tile's stages while the
 // consumers run the epilogue of the current one.
 #pragma once
@@ -61,6 +72,11 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
         :: "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// Acquire a tensor map the host wrote into global memory (system scope: the writer is the host), so that the TMA unit
+// does not use a descriptor it cached when an earlier, since destroyed window had its maps at that address.
+__device__ __forceinline__ void tmap_acquire(const CUtensorMap* m) {
+    asm volatile("fence.proxy.tensormap::generic.acquire.sys [%0], 128;" :: "l"(m) : "memory");
+}
 
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -175,22 +191,133 @@ __device__ __forceinline__ void epilogue_add(const float (&acc)[128], uint8_t* C
     }
 }
 
+}  // namespace gemm
+
+struct GUnit {                  // 48 bytes, read-only
+    int32_t seg_begin, seg_count;   // members, in chain order
+    int32_t succ_begin, succ_count; // out-edges of all members (chain links removed): target unit ids
+    int32_t dep_goal;               // in-edges from other units
+    int32_t nparts;                 // ring entries: min(sub-tiles of C, kMaxParts) for GEMM units, 1 otherwise
+    int32_t tileC;                  // GEMM units: the C tile; -1 otherwise
+    int32_t M, N, K;
+    int32_t flags;                  // bit0 is_gemm, bit1 pushout C
+    int32_t pad;
+};
+struct GSeg { int32_t task, tileA, tileB, pad; };
+
+struct Win2Dev {
+    WinDev w;                       // task-level arrays (descriptors, tiles, outputs, ctl, ring)
+    const GUnit* units;
+    const GSeg*  segs;
+    const int32_t* usucc;
+    int32_t* udep;
+    int32_t* parts_left;
+    const CUtensorMap* tmaps;       // one per tile (w.ntiles)
+    int32_t nunits;
+    int32_t fresh_tmaps;            // first launch since tmaps were written: every producer acquires all of them first
+};
+
+namespace gemm {
+
+constexpr int kMaxParts = 32;      // the part index travels in the 5-bit flow field of a ring entry
+
+struct Job {
+    int32_t unit, part, stop, is_gemm;
+    int32_t seg_begin, seg_count, tileC, nparts;
+    int32_t M, N, K, pushout;
+    int32_t mblocks, nsub;          // GEMM units: sub-tiles of C, ceil(M / BM) per column block; nsub = 0 otherwise
+};
+
 struct Shared {
-    alignas(16) pb2_task_t task;    // filled with four 16-byte loads
+    alignas(16) Job job;
+    alignas(16) pb2_task_t task;    // non-GEMM units: the single member's descriptor
     uint64_t full[kStages];
     uint64_t empty[kStages];
-    int32_t  id;
-    int32_t  need;
-    int32_t  decide;
-    int32_t  last;
+    int32_t  need, decide;
     uint32_t red[32];
 };
+
+// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges
+__device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u, int unit_id) {
+    const WinDev& w = g.w;
+    const int lane = threadIdx.x & 31;
+    const int L = u.seg_count;
+    unsigned long long ebase = 0, rbase = 0;
+    if (lane == 0) {
+        ebase = atomicAdd(&w.ctl->evt.v, (unsigned long long)(2 * L));
+        rbase = atomicAdd(&w.ctl->retired.v, (unsigned long long)L);
+        *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+    }
+    ebase = __shfl_sync(0xffffffffu, ebase, 0);
+    rbase = __shfl_sync(0xffffffffu, rbase, 0);
+    const uint32_t cver = (u.flags & 1) ? *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) : 0u;
+    for (int i = lane; i < L; i += 32) {
+        const GSeg s = g.segs[u.seg_begin + i];
+        const pb2_task_t& t = w.tasks[s.task];
+        w.start_seq[s.task] = (uint32_t)(ebase + 2 * i);
+        w.end_seq[s.task] = (uint32_t)(ebase + 2 * i + 1);
+        w.retire_log[rbase + i] = s.task;
+        w.worker[s.task] = (int32_t)blockIdx.x;
+        if (u.flags & 1) {
+            w.seen_version[s.task * PB2_MAX_FLOWS + 0] = *reinterpret_cast<volatile uint32_t*>(&w.tiles[s.tileA].version);
+            w.seen_version[s.task * PB2_MAX_FLOWS + 1] = *reinterpret_cast<volatile uint32_t*>(&w.tiles[s.tileB].version);
+            w.seen_version[s.task * PB2_MAX_FLOWS + 2] = cver + (uint32_t)i;
+            w.result[s.task] = 0;
+        } else {
+            for (int f = 0; f < t.nb_flows; ++f)
+                if (t.tile[f] >= 0) {
+                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
+                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&tile->version);
+                    w.seen_version[s.task * PB2_MAX_FLOWS + f] = v;
+                    if (t.access[f] & PB2_FLOW_ACCESS_WRITE) {
+                        *reinterpret_cast<volatile uint32_t*>(&tile->version) = v + 1;
+                        st_relaxed_gpu(&tile->state, PB2_TILE_VALID);
+                    }
+                }
+        }
+    }
+    if (lane == 0 && (u.flags & 1)) {
+        *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) = cver + (uint32_t)L;
+        st_relaxed_gpu(&w.tiles[u.tileC].state, PB2_TILE_VALID);
+    }
+    __threadfence();
+    __syncwarp();
+    // release: parsec_update_deps_with_counter on the successor units; a ready unit contributes nparts ring entries
+    for (int e0 = 0; e0 < u.succ_count; e0 += 32) {
+        const int e = e0 + lane;
+        int nparts = 0, sid = -1;
+        if (e < u.succ_count) {
+            sid = g.usucc[u.succ_begin + e];
+            if (atomicSub(&g.udep[sid], 1) == 1) nparts = g.units[sid].nparts;
+        }
+        // exclusive scan of nparts over the warp
+        int incl = nparts;
+        for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        if (total) {
+            unsigned long long base = 0;
+            if (lane == 0) base = atomicAdd(&w.ctl->tail.v, (unsigned long long)total);
+            base = __shfl_sync(0xffffffffu, base, 0);
+            for (int p = 0; p < nparts; ++p)
+                st_release_gpu(&w.ring[((uint32_t)base + (uint32_t)(incl - nparts + p)) & w.cap_mask], (int32_t)PB2_SUCC_MAKE(sid, p));
+        }
+    }
+    // out-edges into other GPUs' windows, member by member (a member with remote successors is always the last of
+    // its unit: build_gemm2_units does not fuse across it)
+    if (w.rs_begin) for (int i = 0; i < L; ++i) release_remote_warp(w, g.segs[u.seg_begin + i].task);
+    if (lane == 0 && (int32_t)(rbase + L) == w.ntasks) {
+        __threadfence();
+        st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
+    }
+    (void)unit_id;
+}
 
 }  // namespace gemm
 
 __global__ void __launch_bounds__(gemm::kThreads, 1)
-pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
+pb2_engine_gemm2_kernel(Win2Dev g) {
     using namespace gemm;
+    const WinDev& w = g.w;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ Shared sh;
@@ -202,55 +329,124 @@ pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
         for (int s = 0; s < kStages; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], kConsumers); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    // The maps of a live window stay at their addresses and never change, so what a launch caches stays valid for the
+    // next launches of the window; only the first one has to drop what an earlier window left at those addresses.
+    if (g.fresh_tmaps && warp == 1 && lane == 0)
+        for (int i = 0; i < w.ntiles; ++i) tmap_acquire(&g.tmaps[i]);
     __syncthreads();
 
-    // pipeline state persists across tasks
-    uint32_t p_stage = 0, p_phase = 0;     // producer
-    uint32_t c_stage = 0, c_phase = 0;     // consumers
+    uint32_t p_stage = 0, p_phase = 0, c_stage = 0, c_phase = 0;
 
     for (;;) {
+        // ---------------- pop the next (part, unit), stage its tiles in
         if (threadIdx.x == 0) {
-            const int32_t id = pop_task(w);
-            if (id != kEmpty) {
+            Job j; memset(&j, 0, sizeof j);
+            const int32_t e = pop_task(w);
+            if (e == kEmpty) { j.stop = 1; }
+            else {
                 __threadfence();
-                w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
-                w.worker[id] = (int32_t)blockIdx.x;
+                j.unit = PB2_SUCC_TASK((uint32_t)e); j.part = PB2_SUCC_FLOW((uint32_t)e);
+                const GUnit u = g.units[j.unit];
+                j.is_gemm = u.flags & 1; j.pushout = (u.flags >> 1) & 1;
+                j.seg_begin = u.seg_begin; j.seg_count = u.seg_count; j.tileC = u.tileC; j.nparts = u.nparts;
+                j.M = u.M; j.N = u.N; j.K = u.K;
+                if (j.is_gemm) { j.mblocks = (u.M + BM - 1) / BM; j.nsub = j.mblocks * ((u.N + BN - 1) / BN); }
             }
-            sh.id = id;
+            sh.job = j;
         }
         __syncthreads();
-        const int32_t id = sh.id;
-        if (id == kEmpty) break;
-        if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.task)[threadIdx.x] =
-            __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
-        __syncthreads();
-        const pb2_task_t& t = sh.task;
-
-        // ---- stage in (same protocol as the HBM kernel) ----
-        if (threadIdx.x == 0) {
-            int need = 0;
-            for (int f = 0; f < t.nb_flows; ++f)
-                if (t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_ACCESS_READ) &&
-                    ld_acquire_gpu(&w.tiles[t.tile[f]].state) != PB2_TILE_VALID) need |= 1 << f;
-            sh.need = need;
-        }
-        __syncthreads();
+        if (sh.job.stop) break;
         {
-            const int need = sh.need;
-            for (int f = 0; f < t.nb_flows; ++f) {
-                if (t.tile[f] < 0) continue;
-                pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                if ((need >> f) & 1) stage_in_flow(stage_ctx(w), tile, t.access[f], &sh.decide);
-                if (threadIdx.x == 0)
-                    w.seen_version[id * PB2_MAX_FLOWS + f] = *reinterpret_cast<volatile uint32_t*>(&tile->version);
+            // stage in every INVALID tile the job reads (same protocol as the other kernels)
+            const int nseg = sh.job.is_gemm ? sh.job.seg_count : 0;
+            for (int i = -1; i < 2 * nseg; ++i) {
+                int tile_id; uint8_t acc;
+                if (i < 0) { if (!sh.job.is_gemm) break; tile_id = sh.job.tileC; acc = PB2_FLOW_ACCESS_RW; }
+                else { const GSeg s = g.segs[sh.job.seg_begin + (i >> 1)]; tile_id = (i & 1) ? s.tileB : s.tileA; acc = PB2_FLOW_ACCESS_READ; }
+                pb2_tile_t* tile = &w.tiles[tile_id];
+                if (threadIdx.x == 0) sh.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
+                __syncthreads();
+                if (sh.need) {
+                    const int ns = tile_slices(w, tile->bytes);
+                    if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.decide);
+                    else stage_in_slices(stage_ctx(w), tile_id, ns, 0, ns, &sh.decide);     // take what nobody has claimed, wait for the rest
+                    fence_proxy_async();
+                }
+                __syncthreads();
             }
-            if (need) { fence_proxy_async(); __syncthreads(); }
+            if (!sh.job.is_gemm) {
+                const GSeg s = g.segs[sh.job.seg_begin];
+                if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.task)[threadIdx.x] =
+                    __ldg(reinterpret_cast<const uint4*>(&w.tasks[s.task]) + threadIdx.x);
+                __syncthreads();
+                const pb2_task_t& t = sh.task;
+                for (int f = 0; f < t.nb_flows; ++f) {
+                    if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_ACCESS_READ)) continue;
+                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
+                    if (threadIdx.x == 0) sh.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
+                    __syncthreads();
+                    if (sh.need) { stage_in_flow(stage_ctx(w), tile, t.access[f], &sh.decide); fence_proxy_async(); }
+                    __syncthreads();
+                }
+            }
         }
+        const Job& job = sh.job;       // read from shared memory, not held in registers across the wgmma loop
 
-        const bool is_gemm = (t.body == PB2_BODY_GEMM_BF16);
-        unsigned long long hbm_result = 0;
-        if (!is_gemm && t.body != PB2_BODY_NOP) {
-            // GEMM windows may carry a few HBM-bound tasks of the same DAG (e.g. a panel task): run them in place
+        // The part's sub-tiles are job.part, job.part + nparts, ...: sub-tile `sub` is rows m0 .. m0 + 127 and columns
+        // n0 .. n0 + Nj - 1 of C.  The producer and the consumers walk the same sequence, so the ring's stage and phase
+        // carry over from one sub-tile to the next.
+        if (job.is_gemm) {
+            const int kblocks = (job.K + BK - 1) / BK;
+            if (warp == 1) {
+                // ===== TMA producer: 128 rows of A, 256 rows of B per k-block, every member of the chain
+                if (lane == 0) {
+                    fence_proxy_async();
+                    for (int sub = job.part; sub < job.nsub; sub += job.nparts) {
+                        const int m0 = (sub % job.mblocks) * BM, n0 = (sub / job.mblocks) * BN;
+                        for (int s = 0; s < job.seg_count; ++s) {
+                            const GSeg sg = g.segs[job.seg_begin + s];
+                            const CUtensorMap* mapA = &g.tmaps[sg.tileA];
+                            const CUtensorMap* mapB = &g.tmaps[sg.tileB];
+                            if (s + 1 < job.seg_count) {        // the next member's descriptors: fetch them now, not on first use
+                                const GSeg nx = g.segs[job.seg_begin + s + 1];
+                                asm volatile("prefetch.tensormap [%0];" :: "l"(&g.tmaps[nx.tileA]) : "memory");
+                                asm volatile("prefetch.tensormap [%0];" :: "l"(&g.tmaps[nx.tileB]) : "memory");
+                            }
+                            for (int kb = 0; kb < kblocks; ++kb) {
+                                mbar_wait(&sh.empty[p_stage], p_phase ^ 1);
+                                uint8_t* sa = smem + p_stage * kStageBytes;
+                                mbar_expect_tx(&sh.full[p_stage], kStageBytes);
+                                tma_load_2d(sa, mapA, &sh.full[p_stage], kb * BK, m0);
+                                tma_load_2d(sa + kAStageBytes, mapB, &sh.full[p_stage], kb * BK, n0);
+                                tma_load_2d(sa + kAStageBytes + kBStageBytes / 2, mapB, &sh.full[p_stage], kb * BK, n0 + 128);
+                                if (++p_stage == kStages) { p_stage = 0; p_phase ^= 1; }
+                            }
+                        }
+                    }
+                }
+            } else if (wg >= 1) {
+                // ===== consumers: rows m0 + 64 * cw .. of each sub-tile, the whole chain into one accumulator
+                const int cw = wg - 1;
+                uint8_t* Cbase = reinterpret_cast<uint8_t*>(w.tiles[job.tileC].dev_ptr);
+                float acc[128];
+#pragma unroll
+                for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+                for (int sub = job.part; sub < job.nsub; sub += job.nparts) {
+                    const int m0 = (sub % job.mblocks) * BM, n0 = (sub / job.mblocks) * BN, Nj = min(BN, job.N - n0);
+                    {   // pull the sub-tile's C rows into L2 now, so that the read-modify-write after the chain does not pay DRAM latency
+                        const int t = threadIdx.x - 128, row = m0 + (t >> 1);
+                        if (row < job.M)
+                            for (int b = (t & 1) * 128; b < Nj * 2; b += 256)
+                                asm volatile("prefetch.global.L2 [%0];" :: "l"(Cbase + ((size_t)row * job.N + n0) * 2 + b));
+                    }
+                    mma_kblocks(acc, smem, sh.full, sh.empty, c_stage, c_phase, job.seg_count * kblocks, true, cw);
+                    epilogue_add(acc, Cbase, job.N, m0 + cw * 64, n0, job.M, n0 + Nj);
+                }
+                fence_proxy_async();
+            }
+        } else {
+            // ---------------- a non-GEMM member of the DAG (e.g. a panel stand-in): the whole CTA runs it in place
+            const pb2_task_t& t = sh.task;
             BodyArgs a;
             for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
                 const bool has = f < t.nb_flows && t.tile[f] >= 0;
@@ -259,103 +455,62 @@ pb2_engine_gemm_kernel(WinDev w, const CUtensorMap* __restrict__ tmaps) {
             }
             a.elem0 = 0; a.part = 0;
             a.iparam[0] = t.iparam[0]; a.iparam[1] = t.iparam[1]; a.iparam[2] = t.iparam[2]; a.fparam = t.fparam;
-            hbm_result = run_hbm_body(t.body, a, sh.red);
+            const unsigned long long r = run_hbm_body(t.body, a, sh.red);
+            if (threadIdx.x == 0) {
+                w.result[g.segs[job.seg_begin].task] = r;
+                if ((t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) && (r >> 32)) atomicAdd(&w.ctl->body_errors.v, r >> 32);
+            }
             fence_proxy_async();
+            for (int f = 0; f < t.nb_flows; ++f)
+                if (t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
+                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
+                    cta_copy<false>(tile->src_ptr, tile->dev_ptr, tile->bytes);
+                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)tile->bytes);
+                }
+        }
+        __threadfence();
+        __syncthreads();             // every store of the part is done and visible
+
+        // ---------------- part complete: pushout of its sub-tiles' C rows, then unit retirement by the last part
+        if (job.is_gemm && job.pushout) {
+            pb2_tile_t* tile = &w.tiles[job.tileC];
+            const size_t row_bytes = (size_t)job.N * 2;
+            for (int sub = job.part; sub < job.nsub; sub += job.nparts) {
+                const int m0 = (sub % job.mblocks) * BM, n0 = (sub / job.mblocks) * BN, Nj = min(BN, job.N - n0);
+                const int rows = min(BM, job.M - m0);
+                if (Nj == job.N) {
+                    cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + (size_t)m0 * row_bytes,
+                                    reinterpret_cast<const uint8_t*>(tile->dev_ptr) + (size_t)m0 * row_bytes, (size_t)rows * row_bytes);
+                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)rows * row_bytes);
+                } else {
+                    // a column block of a tile wider than one sub-tile: row segments
+                    for (int r = 0; r < rows; ++r) {
+                        const size_t o = (size_t)(m0 + r) * row_bytes + (size_t)n0 * 2;
+                        cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + o, reinterpret_cast<const uint8_t*>(tile->dev_ptr) + o, (size_t)Nj * 2);
+                    }
+                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)rows * (unsigned long long)Nj * 2ull);
+                }
+            }
             __syncthreads();
         }
-        const int M = t.iparam[0], N = t.iparam[1], K = t.iparam[2];
-        const int mblocks = is_gemm ? (M + BM - 1) / BM : 0;
-        const int nblocks = is_gemm ? (N + BN - 1) / BN : 0;
-        const int kblocks = (K + BK - 1) / BK;
-        const int nsub = mblocks * nblocks;
-
         if (warp == 0) {
-            // ===== TMA producer =====
-            if (lane == 0 && nsub > 0) {
-                fence_proxy_async();    // operand tiles may have been written by generic-proxy stores
-                const CUtensorMap* mapA = &tmaps[t.tile[0]];
-                const CUtensorMap* mapB = &tmaps[t.tile[1]];
-                for (int sub = 0; sub < nsub; ++sub) {
-                    const int mb = sub / nblocks, nb = sub % nblocks;
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        mbar_wait(&sh.empty[p_stage], p_phase ^ 1);
-                        uint8_t* sa = smem + p_stage * kStageBytes;
-                        uint8_t* sb = sa + kAStageBytes;
-                        mbar_expect_tx(&sh.full[p_stage], kStageBytes);
-                        tma_load_2d(sa, mapA, &sh.full[p_stage], kb * BK, mb * BM);
-                        tma_load_2d(sb, mapB, &sh.full[p_stage], kb * BK, nb * BN);
-                        tma_load_2d(sb + kBStageBytes / 2, mapB, &sh.full[p_stage], kb * BK, nb * BN + 128);
-                        if (++p_stage == kStages) { p_stage = 0; p_phase ^= 1; }
-                    }
-                }
-            }
-        } else if (wg >= 1) {
-            // ===== consumer warpgroups: wgmma into registers, then C += acc -> bf16 =====
-            if (nsub > 0) {
-                const int cw = wg - 1;
-                uint8_t* Cbase = reinterpret_cast<uint8_t*>(w.tiles[t.tile[2]].dev_ptr);
-                float acc[128];
-#pragma unroll
-                for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-                for (int sub = 0; sub < nsub; ++sub) {
-                    const int mb = sub / nblocks, nb = sub % nblocks;
-                    mma_kblocks(acc, smem, sh.full, sh.empty, c_stage, c_phase, kblocks, true, cw);
-                    epilogue_add(acc, Cbase, N, mb * BM + cw * 64, nb * BN, M, N);
-                }
-                fence_proxy_async();   // C may be consumed through TMA by a later task on another SM
-            }
+            int last = 0;
+            if (lane == 0) { __threadfence(); last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
+            last = __shfl_sync(0xffffffffu, last, 0);
+            if (last) { __threadfence(); retire_unit_warp(g, g.units[job.unit], job.unit); }
         }
-        __syncthreads();
-
-        // ---- pushout (PARSEC_PUSHOUT on the last k, dtd_test_simple_gemm.c:687) ----
-        for (int f = 0; f < t.nb_flows; ++f) {
-            if (t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
-                pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                cta_copy<false>(tile->src_ptr, tile->dev_ptr, tile->bytes);
-                if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)tile->bytes);
-            }
-        }
-        __syncthreads();
-
-        if (threadIdx.x < 32) {
-            __threadfence();
-            if (threadIdx.x == 0) {
-                w.result[id] = hbm_result;
-                if ((t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) && (hbm_result >> 32))
-                    atomicAdd(&w.ctl->body_errors.v, hbm_result >> 32);
-                for (int f = 0; f < t.nb_flows; ++f) {
-                    if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_ACCESS_WRITE)) continue;
-                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                    *reinterpret_cast<volatile uint32_t*>(&tile->version) =
-                        *reinterpret_cast<volatile uint32_t*>(&tile->version) + 1;
-                    if (!(t.access[f] & PB2_FLOW_ACCESS_READ)) st_relaxed_gpu(&tile->state, PB2_TILE_VALID);
-                }
-                w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
-                sh.last = retire_task(w, id) ? 1 : 0;
-                __threadfence();
-            }
-            __syncwarp();
-            release_successors_warp(w, t);
-            release_remote_warp(w, id);
-            if (threadIdx.x == 0 && sh.last) {
-                __threadfence();
-                st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
-            }
-        }
-        __syncthreads();
+        __syncthreads();             // sh.job is rewritten by the next pop
     }
 }
 
-static inline int pb2_gemm_nworkers(int sm_count) { return sm_count; }
-
-static inline int pb2_gemm_launch(const WinDev& w, const CUtensorMap* tmaps, int nworkers, cudaStream_t stream) {
+static inline int pb2_gemm2_launch(const Win2Dev& g, int nworkers, cudaStream_t stream) {
     static bool attr_set = false;
     if (!attr_set) {
-        if (cudaFuncSetAttribute(pb2_engine_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
+        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
         attr_set = true;
     }
-    pb2_engine_gemm_kernel<<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(w, tmaps);
+    if (nworkers < 1) return PB2_ERR_BAD_PARAM;
+    pb2_engine_gemm2_kernel<<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
     return cudaGetLastError() == cudaSuccess ? PB2_SUCCESS : PB2_ERR_DEVICE;
 }
 

@@ -268,3 +268,14 @@ def test_hbm_window_larger_than_the_ring_entry_id_is_rejected(engine):
     with pytest.raises(L.Pb2Error) as ei:
         engine.window(0, tasks, np.zeros(0, np.uint32), tiles, np.arange(n, dtype=np.int32))
     assert ei.value.rc == L.PB2_ERR_VALUE_OUT_OF_BOUNDS
+
+
+def test_unknown_window_kind_is_rejected(engine):
+    """Kinds other than 0 (HBM bodies) and 1 (GEMM bodies) name no kernel: refused at creation."""
+    tasks = np.zeros(1, L.TASK_DTYPE)
+    tasks["tile"][:] = -1
+    tiles = np.zeros(1, L.TILE_DTYPE)
+    tiles["bytes"], tiles["state"] = 64, L.TILE_VALID
+    with pytest.raises(L.Pb2Error) as ei:
+        engine.window(2, tasks, np.zeros(0, np.uint32), tiles, np.zeros(1, np.int32))
+    assert ei.value.rc == L.PB2_ERR_BAD_PARAM

@@ -1,4 +1,5 @@
-"""GPU tests of the tensor-core GEMM windows (BASELINE config 3 shape, reduced NT), all three kernel modes."""
+"""GPU tests of the tensor-core GEMM windows (BASELINE config 3 shape, reduced NT): fused k-chains (mode 0), every
+task its own unit (mode 2) and its alias (mode 1)."""
 import numpy as np
 import pytest
 
@@ -27,7 +28,9 @@ def chain_references(A, B, C, NT):
 
 
 @pytest.mark.parametrize("mode", [0, 2, 1])
-@pytest.mark.parametrize("NT,T", [(1, 128), (2, 256), (3, 512), (2, 320), (4, 512), (2, 768), (2, 1024)])
+# 264: N % 16 == 8; 1152: 45 sub-tiles of 128 x 256 over 32 parts (13 parts run two); 1160: both
+@pytest.mark.parametrize("NT,T", [(1, 128), (2, 256), (3, 512), (2, 320), (4, 512), (2, 768), (2, 1024),
+                                  (2, 264), (2, 1152), (2, 1160)])
 def test_dtd_gemm_chain(mode, NT, T):
     rng = np.random.default_rng(1789 + NT * 1000 + T)
     rnd = lambda shape: round_to_bf16(rng.uniform(-0.5, 0.5, shape).astype(np.float32))

@@ -8,7 +8,7 @@ from parsec_b200.engine import Engine
 
 NT = int(sys.argv[1]) if len(sys.argv) > 1 else 16
 T = int(sys.argv[2]) if len(sys.argv) > 2 else 512
-modes = [int(x) for x in sys.argv[3].split(",")] if len(sys.argv) > 3 else [0, 2, 1]
+modes = [int(x) for x in sys.argv[3].split(",")] if len(sys.argv) > 3 else [0, 2]
 tb = T * T * 2
 for mode in modes:
     with Engine(0, gemm_mode=mode) as e:
