@@ -142,6 +142,10 @@ typedef struct pb2_engine_params_s {
     int32_t  read_groups;      /* HBM windows that are not shared: 0 = a run of consecutive out-edges of one task into
                                 * CHECK readers of the same tile (that edge their only input) is executed as one group
                                 * that streams the tile once for all its members (default); < 0 = every task alone  */
+    int32_t  fuse_readers;     /* HBM windows that are not shared, with read groups on and more than one worker:
+                                * 0 = a producer that writes the tile its first read group checks runs with that
+                                * group as one unit, each chunk written and then checked while it is still in L2
+                                * (default); < 0 = the producer and the group run one after the other            */
 } pb2_engine_params_t;
 
 typedef struct pb2_engine_info_s {

@@ -68,7 +68,8 @@ def succ_make(task, flow=0):
 class EngineParams(C.Structure):
     _fields_ = [("workers_per_sm", C.c_int32), ("threads", C.c_int32), ("max_workers", C.c_int32),
                 ("stage_mode", C.c_int32), ("queue_policy", C.c_int32), ("timeout_ms", C.c_int32),
-                ("gemm_mode", C.c_int32), ("part_bytes", C.c_int32), ("read_groups", C.c_int32)]
+                ("gemm_mode", C.c_int32), ("part_bytes", C.c_int32), ("read_groups", C.c_int32),
+                ("fuse_readers", C.c_int32)]
 
 
 class EngineInfo(C.Structure):

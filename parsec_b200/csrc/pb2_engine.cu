@@ -73,8 +73,9 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
 // a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
 // 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
 // streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
-// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times, and the step
-// takes what F = 1 takes (DESIGN.md §8).
+// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
+// producer runs with its group as one unit (run_fused_part) that checks each 16 KiB chunk right after writing it, so
+// the CHECK reads hit L2 and DRAM carries the write-back of the tiles alone (DESIGN.md §5, §8).
 // What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
 #ifndef PB2_HBM_MINB
 #define PB2_HBM_MINB 12
@@ -85,9 +86,18 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
 // A read group in flight on one worker: its members (the leader first), their CHECK constants, this part's results.
 struct GroupSmem {
     int32_t n;                              // members; 0: the popped task runs alone
+    int32_t fused;                          // the popped task is a producer that runs with this group as one unit
+    int32_t tile;                           // the tile the members read
+    int32_t fx;                             // fused: the producer's written flow on that tile
     int32_t mem[PB2_GROUP_MAX];
     uint32_t k[PB2_GROUP_MAX];
     unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
+    // fused: the producer's slice of every flow for this part, and the members' view of the current chunk
+    void* base[PB2_MAX_FLOWS];
+    uint32_t len[PB2_MAX_FLOWS];
+    uint32_t e0;
+    unsigned long long r0;                  // the leader's result on the current chunk
+    BodyArgs c;
 };
 
 // All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
@@ -115,6 +125,76 @@ static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
     __syncthreads();
 }
 
+// Results of a body run chunk by chunk: the mismatch counts add up, the first element is the first chunk's.
+__device__ __forceinline__ unsigned long long chunk_sum(unsigned long long acc, unsigned long long r, uint32_t c0) {
+    if (c0 == 0 || acc == ~0ull || r == ~0ull) return c0 == 0 ? r : ~0ull;
+    return acc + (r & 0xffffffff00000000ull);
+}
+
+// All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
+// producer's slice of every flow for this part.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, the
+// last chunk ragged): the producer's body writes a chunk, then the members read it back while it is still in L2.  Run
+// as separate tasks, the readers of a tile come long after its writer: every other worker writes its own tile in
+// between, and that is far more than L2 holds.  Member results follow group_results chunk by chunk, summed.
+// Returns the producer's result (thread 0).
+static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, uint32_t chunk) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    if (threadIdx.x == 0) {
+        int fx = 0;
+        for (int f = PB2_MAX_FLOWS - 1; f >= 0; --f) {
+            if (f < (int)s.task.nb_flows && s.task.tile[f] == g.tile && (s.task.access[f] & PB2_FLOW_ACCESS_WRITE)) fx = f;
+            g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f];
+        }
+        g.fx = fx;
+        g.e0 = s.args.elem0;
+        g.c = s.args;
+    }
+    __syncthreads();
+    const uint32_t len = g.len[g.fx];
+    unsigned long long acc = 0;
+#pragma unroll 1
+    for (uint32_t c0 = 0;; c0 += chunk) {
+        if (threadIdx.x == 0) {
+            // every flow at the same offset (they are cut alike, and the group's tile is the widest)
+            for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
+                const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
+                s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
+                s.args.bytes[f] = rest < chunk ? rest : chunk;
+            }
+            s.args.elem0 = g.e0 + (c0 >> 2);
+            g.c.flow[0] = s.args.flow[g.fx]; g.c.bytes[0] = s.args.bytes[g.fx]; g.c.iparam[0] = (int32_t)g.k[0];
+        }
+        __syncthreads();
+        const unsigned long long r = run_hbm_body(s.task.body, s.args, s.red);
+        __syncthreads();            // the chunk's stores are visible to the whole CTA before it reads them back
+        const unsigned long long r0 = run_hbm_body(PB2_BODY_CHECK_I32, g.c, s.red);
+        if (threadIdx.x == 0) { acc = chunk_sum(acc, r, c0); g.res[0] = chunk_sum(g.res[0], r0, c0); g.r0 = r0; }
+        __syncthreads();
+#pragma unroll 1
+        for (int i = 1; i < g.n; ++i) {
+            const uint32_t k = g.k[i];
+            if (k == g.k[0] || !(g.r0 >> 32)) {
+                if (threadIdx.x == 0)
+                    g.res[i] = chunk_sum(g.res[i], k == g.k[0] ? g.r0 : ((unsigned long long)(g.c.bytes[0] >> 2) << 32) | (uint32_t)g.r0, c0);
+                continue;
+            }
+            if (threadIdx.x == 0) g.c.iparam[0] = (int32_t)k;
+            __syncthreads();
+            const unsigned long long ri = run_hbm_body(PB2_BODY_CHECK_I32, g.c, s.red);
+            if (threadIdx.x == 0) g.res[i] = chunk_sum(g.res[i], ri, c0);
+            __syncthreads();
+        }
+        if (len - c0 <= chunk) break;
+    }
+    if (threadIdx.x == 0) {         // the pushout that follows works on the whole slice
+        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { s.args.flow[f] = g.base[f]; s.args.bytes[f] = g.len[f]; }
+        s.args.elem0 = g.e0;
+    }
+    __syncthreads();
+    return acc;
+}
+
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
 pb2_engine_hbm_kernel(WinDev w) {
     __shared__ TaskSmem s;
@@ -139,32 +219,39 @@ pb2_engine_hbm_kernel(WinDev w) {
         {
             const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
             const int gn = (int)(gd & 15u);
+            const uint32_t gb = (gd & ~PB2_GROUP_FUSED) >> 4;
+            const bool fused = (gd & PB2_GROUP_FUSED) != 0;
             if ((int)threadIdx.x < gn) {
-                const int32_t m = __ldg(&w.group_mem[(gd >> 4) + threadIdx.x]);
+                const int32_t m = __ldg(&w.group_mem[gb + threadIdx.x]);
                 const pb2_task_t& mt = w.tasks[m];
                 g.mem[threadIdx.x] = m;
                 g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
+                if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
             }
             if (threadIdx.x == 0) {
-                g.n = gn;
-                if (part == 0 && gn) {
+                g.n = gn; g.fused = fused;
+                if (part == 0 && gn && !fused) {
                     // the members start together: consecutive event numbers, one worker
                     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
                     for (int i = 0; i < gn; ++i) {
-                        const int32_t m = __ldg(&w.group_mem[(gd >> 4) + i]);
+                        const int32_t m = __ldg(&w.group_mem[gb + i]);
                         w.start_seq[m] = seq + (uint32_t)i;
                         w.worker[m] = (int32_t)blockIdx.x;
                     }
                 } else if (part == 0) {
                     w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
                     w.worker[id] = (int32_t)blockIdx.x;
+                    // a fused unit's members start when it retires (below); they run on the producer's worker
+                    for (int i = 0; i < gn; ++i) w.worker[__ldg(&w.group_mem[gb + i])] = (int32_t)blockIdx.x;
                 }
             }
         }
         __syncthreads();
         const int nparts = task_nparts(w, id);
-        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts);
-        if (g.n) {
+        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
+            return g.fused ? run_fused_part(&s, &g, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
+        });
+        if (g.n && !g.fused) {
             // the leader's part stored the version it saw; every member saw the same one
             if (threadIdx.x == 0) {
                 g.res[0] = r;
@@ -183,13 +270,33 @@ pb2_engine_hbm_kernel(WinDev w) {
             if (threadIdx.x == 0) {
                 const pb2_task_t& t = s.task;
                 const int gn = g.n;
-                if (gn) for (int i = 0; i < gn; ++i) store_result(w, t, g.mem[i], part, nparts, g.res[i]);
-                else store_result(w, t, id, part, nparts, r);
+                for (int i = 0; i < gn; ++i) store_result(w, w.tasks[g.mem[i]], g.mem[i], part, nparts, g.res[i]);
+                if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
                 // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
                 int last = 1;
                 if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
                 s.window_done = 0; s.last = last;
-                if (last && gn) {
+                if (last && gn && g.fused) {
+                    // the producer, then its members as if they had run right after it: they saw the version it
+                    // wrote; its end, their starts, their ends are consecutive events (end before start on every
+                    // edge); they retire right after it, in member order
+                    epilog_written_flows(w, t);
+                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.tiles[g.tile].version);
+                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)(1 + 2 * gn));
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)(1 + gn));
+                    w.end_seq[id] = ev;
+                    w.retire_log[seq] = id;
+                    for (int i = 0; i < gn; ++i) {
+                        const int32_t m = g.mem[i];
+                        w.seen_version[(size_t)m * PB2_MAX_FLOWS] = v;
+                        w.start_seq[m] = ev + 1u + (uint32_t)i;
+                        w.end_seq[m] = ev + 1u + (uint32_t)(gn + i);
+                        w.retire_log[seq + 1u + (uint32_t)i] = m;
+                    }
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    s.window_done = (int32_t)(seq + 1u + (uint32_t)gn) == w.ntasks ? 1 : 0;
+                    __threadfence();
+                } else if (last && gn) {
                     // members only read their tile: no written flows; they retire back to back, in member order
                     const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
                     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
@@ -214,8 +321,11 @@ pb2_engine_hbm_kernel(WinDev w) {
             if (s.last && w.ps_begin[id + 1] > w.ps_begin[id]) push_written_tiles(w.tiles, w.ctl, w.ps_begin, w.ps, id, &bulk);
         }
         if (threadIdx.x < 32) {
-            if (s.last && g.n) { for (int i = 0; i < g.n; ++i) release_successors_warp(w, w.tasks[g.mem[i]]); }
-            else if (s.last) { release_successors_warp(w, s.task); release_remote_warp(w, id); }
+            if (s.last) {
+                // a fused producer's own successors first (its edge to the group is not among them), then the members'
+                if (!g.n || g.fused) { release_successors_warp(w, s.task); release_remote_warp(w, id); }
+                for (int i = 0; i < g.n; ++i) release_successors_warp(w, w.tasks[g.mem[i]]);
+            }
             if (threadIdx.x == 0 && s.window_done) {
                 __threadfence();
                 st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
@@ -514,7 +624,15 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
 // their own SM, F passes where one carries the same bytes.  The members become ready together and would have entered
 // the FIFO ring back to back: with one worker the retire order is the ungrouped one.  Runs longer than PB2_GROUP_MAX
 // are split.  O(ntasks + nsucc); tasks keep their own out-edges.  Returns false when no group formed.
+//
+// With `fuse`, a task P also runs with the first group among its out-edges as one unit when P has a body, writes the
+// group's tile X without pushing it out, and X is P's widest tile (so P's parts cut X as the members' parts do): the
+// edge P -> leader leaves the device CSR and group[P] = PB2_GROUP_FUSED | the leader's group word.  The worker that
+// runs a part of P writes it chunk by chunk and the members check each chunk right after (run_fused_part).  The
+// caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
+// every task that was queued when P retired, and a fused unit runs them right after P.
 static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
+                             const pb2_tile_t* tiles, bool fuse,
                              std::vector<uint32_t>& gsucc, std::vector<uint32_t>& group, std::vector<int32_t>& gmem) {
     const size_t n = tasks.size();
     std::vector<uint8_t> indeg(n, 0);                        // saturates at 2
@@ -533,6 +651,19 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
         for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
         return true;
     };
+    auto fusable = [&](const pb2_task_t& p, int32_t x) {
+        if (p.body == PB2_BODY_NOP || p.body == PB2_BODY_GEMM_BF16) return false;
+        bool writes = false;
+        for (int f = 0; f < p.nb_flows; ++f) {
+            if (p.tile[f] < 0) continue;
+            if (tiles[p.tile[f]].bytes > tiles[x].bytes) return false;
+            if (p.tile[f] == x && (p.access[f] & PB2_FLOW_ACCESS_WRITE)) {
+                if (p.access[f] & PB2_FLOW_PUSHOUT) return false;
+                writes = true;
+            }
+        }
+        return writes;
+    };
     std::vector<int32_t> begin(n), count(n);
     group.assign(n, 0u);
     gsucc.clear(); gmem.clear();
@@ -540,17 +671,24 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
         const uint32_t* out = succ + tasks[u].succ_begin;
         const int32_t c = tasks[u].succ_count;
         begin[u] = (int32_t)gsucc.size();
+        bool first_group = true;
         for (int32_t j = 0; j < c;) {
             int32_t r = j + 1;
+            int32_t tile = -1;
             if (reader(out[j])) {
-                const int32_t tile = tasks[(size_t)PB2_SUCC_TASK(out[j])].tile[0];
+                tile = tasks[(size_t)PB2_SUCC_TASK(out[j])].tile[0];
                 while (r < c && r - j < PB2_GROUP_MAX && reader(out[r]) && tasks[(size_t)PB2_SUCC_TASK(out[r])].tile[0] == tile) ++r;
             }
-            gsucc.push_back(out[j]);
+            bool fused = false;
             if (r - j >= 2) {
-                group[(size_t)PB2_SUCC_TASK(out[j])] = ((uint32_t)gmem.size() << 4) | (uint32_t)(r - j);
+                const uint32_t gw = ((uint32_t)gmem.size() << 4) | (uint32_t)(r - j);
+                group[(size_t)PB2_SUCC_TASK(out[j])] = gw;
                 for (int32_t q = j; q < r; ++q) gmem.push_back(PB2_SUCC_TASK(out[q]));
+                fused = fuse && first_group && fusable(tasks[u], tile);
+                if (fused) group[u] = PB2_GROUP_FUSED | gw;
+                first_group = false;
             }
+            if (!fused) gsucc.push_back(out[j]);
             j = r;
         }
         count[u] = (int32_t)gsucc.size() - begin[u];
@@ -592,6 +730,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     if (p.part_bytes == 0) p.part_bytes = 256 * 1024;
     e->params = p;
     if (const char* sl = getenv("PB2_STAGE_SLICE_BYTES")) e->stage_slice_bytes = atoi(sl);
+    if (const char* fc = getenv("PB2_FUSE_CHUNK_BYTES")) e->fuse_chunk_bytes = atoi(fc);       // development aid
     if (const char* sm = getenv("PB2_STAGE_MODE")) e->params.stage_mode = atoi(sm);      // 1: SIMT mover (development aid)
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->up_stream, cudaStreamNonBlocking));
@@ -883,7 +1022,8 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     std::vector<uint32_t> gsucc, group;
     std::vector<int32_t> gmem;
     const bool grouped = kind == 0 && !w->shared && e->params.read_groups >= 0 &&
-                         form_read_groups(dtasks, succ, ready, nready, gsucc, group, gmem);
+                         form_read_groups(dtasks, succ, ready, nready, tiles, e->params.fuse_readers >= 0 && e->nworkers > 1,
+                                          gsucc, group, gmem);
     TRY(dev_alloc_copy(w, &w->d_tasks, dtasks.data(), (size_t)ntasks));
     if (grouped) TRY(dev_alloc_copy(w, &w->d_succ, gsucc.data(), gsucc.size()));
     else TRY(dev_alloc_copy(w, &w->d_succ, succ, (size_t)nsucc));
@@ -916,6 +1056,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     d.slice_claim = nullptr; d.slice_done = nullptr; d.part_bytes = e->params.part_bytes;
     d.nparts = nullptr; d.remote_units = 0;
     d.group = nullptr; d.group_mem = nullptr;
+    d.fuse_chunk = e->fuse_chunk_bytes > 16 ? ((uint32_t)e->fuse_chunk_bytes + 15u) & ~15u : 16u;
     if (grouped) {
         uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
         TRY(dev_alloc_copy(w, &d_group, group.data(), group.size()));

@@ -60,12 +60,15 @@ struct WinDev {
     int32_t           remote_units;   // remote targets are (parts-1) << 27 | unit of a fused-GEMM window, not << 22 | task
     // read groups of HBM windows (form_read_groups in pb2_engine.cu; null: none): task id leads the members
     // group_mem[group[id] >> 4 .. + (group[id] & 15)), itself first; a count of 0 means the task runs alone.  The other
-    // members are never released or popped on their own.
+    // members are never released or popped on their own.  A producer fused with a group (PB2_GROUP_FUSED set in its
+    // group word) names that group's members, the leader included, and its edge to the leader is gone from succ[].
     const uint32_t*   group;
     const int32_t*    group_mem;
+    uint32_t          fuse_chunk;     // bytes a fused producer writes before its group checks them (multiple of 16)
 };
 
 #define PB2_GROUP_MAX 8     // members per read group (at most 15: the count is 4 bits of group[])
+#define PB2_GROUP_FUSED 0x80000000u   // group[] of a producer that runs with its group as one unit
 
 struct PeerWin { int32_t* dep; int32_t* ring; Ctl* ctl; uint32_t cap_mask; int32_t pad; pb2_tile_t* tiles; };
 struct alignas(32) PushDev { void* dst; int32_t* dst_state; uint32_t bytes; int32_t src_tile; int32_t pad[2]; };

@@ -300,7 +300,8 @@ pb2_stream_kernel(StreamDev sd) {
             __ldcg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
         __syncthreads();
         const int nparts = (int)__ldcg(&w.nparts[id]);
-        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts);
+        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts,
+                                                   [&] { return run_hbm_body(s.task.body, s.args, s.red); });
 
         if (threadIdx.x == 0) {
             __threadfence();

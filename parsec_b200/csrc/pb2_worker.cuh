@@ -50,9 +50,11 @@ static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, Task
     }
 }
 
-// All threads.  On entry s.task holds the descriptor (published by a barrier).  Returns the body result (thread 0).
+// All threads.  On entry s.task holds the descriptor (published by a barrier).  exec() runs the body over s.args (all
+// threads) and returns its result in thread 0.  Returns the body result (thread 0).
+template <class Exec>
 __device__ __forceinline__ unsigned long long
-run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts) {
+run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts, Exec exec) {
     const pb2_task_t& t = s.task;
     // ---- push: one thread per flow works out its slice and whether the tile has to be staged in -----------------
     if (threadIdx.x < 32) {
@@ -91,7 +93,7 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     if (s.need) stage_in_needed_flows(stage_ctx(w), &s, bulk);
 
     // ---- exec: the body (parsec_device_kernel_exec -> submit) ----
-    const unsigned long long r = run_hbm_body(t.body, s.args, s.red);
+    const unsigned long long r = exec();
     __syncthreads();
 
     // ---- pop: pushout of written flows to their home copy (parsec_device_kernel_pop stage_out) ----

@@ -26,11 +26,12 @@ class Engine:
     """One engine per GPU (the reference's parsec_device_cuda_module_t, device_cuda.h:43-48)."""
 
     def __init__(self, cuda_device=0, workers_per_sm=0, threads=0, max_workers=0, stage_mode=0,
-                 queue_policy=0, timeout_ms=0, gemm_mode=0, part_bytes=0, read_groups=0):
+                 queue_policy=0, timeout_ms=0, gemm_mode=0, part_bytes=0, read_groups=0,
+                 fuse_readers=0):
         self._lib = L.load()
         self._h = C.c_void_p()
         p = L.EngineParams(workers_per_sm, threads, max_workers, stage_mode, queue_policy, timeout_ms, gemm_mode, part_bytes,
-                           read_groups)
+                           read_groups, fuse_readers)
         rc = self._lib.pb2_engine_create(C.byref(self._h), cuda_device, C.byref(p))
         if rc != L.PB2_SUCCESS:
             self._h = C.c_void_p()

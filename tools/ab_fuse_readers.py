@@ -1,0 +1,101 @@
+"""Where the resident Ex05 window spends its time, and what fusing each producer with its read group changes
+(development aid, not the bench).
+
+1. the card: name, power limit and maximum SM clock (read-only nvidia-smi query);
+2. tools/l2_probe (compiled into a temporary directory): the L2 read rate and the DRAM rates of this GPU;
+3. a FILL-only window (the K producers of the Ex05 window, no readers): the write floor of the fused window;
+4. the resident Ex05 window (dags.ex05_broadcast(K, 14, 262144), tiles VALID) with fusion off, and on at chunk sizes
+   4 .. 256 KiB (PB2_FUSE_CHUNK_BYTES; 256 KiB is the whole tile: the producer writes it all before the group reads it);
+5. --ab: the same window with fusion off and on (default chunk), alternated run by run.
+Each row: median / min / max / spread of reset_ms + kernel_ms.
+
+    python tools/ab_fuse_readers.py [--runs 30] [--ab]
+"""
+import argparse
+import json
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
+from parsec_b200 import _lib as L
+from oracle import orc_dags as dags
+from parsec_b200.engine import Engine
+from ab_read_groups import TB, card, l2_probe, summary
+
+
+class Window:
+    """One engine and one resident window of the Ex05 DAG (or of its producers alone) on it."""
+
+    def __init__(self, K, fuse_readers=0, chunk=None, fill_only=False):
+        if chunk is not None:
+            os.environ["PB2_FUSE_CHUNK_BYTES"] = str(chunk)       # read when the engine is created
+        try:
+            self.e = Engine(0, fuse_readers=fuse_readers)
+        finally:
+            os.environ.pop("PB2_FUSE_CHUNK_BYTES", None)
+        dag = dags.ex05_broadcast(K, 14, TB)
+        tasks, succ = dag.tasks, dag.succ
+        if fill_only:
+            tasks = tasks[:K].copy()
+            tasks["succ_begin"], tasks["succ_count"] = 0, 0
+            succ = np.zeros(0, np.uint32)
+        self.ntasks = len(tasks)
+        self.slab = self.e.malloc(K * TB)
+        self.e.h2d(self.slab, np.zeros(K * TB // 4, np.int32))
+        tiles = np.zeros(K, L.TILE_DTYPE)
+        tiles["dev_ptr"] = self.slab + np.arange(K, dtype=np.uint64) * np.uint64(TB)
+        tiles["bytes"] = TB
+        tiles["state"] = L.TILE_VALID
+        self.w = self.e.window(0, tasks, succ, tiles, dag.ready)
+
+    def run(self):
+        st = self.w.run()
+        assert st["body_errors"] == 0 and st["tasks_retired"] == self.ntasks
+        return st["reset_ms"] + st["kernel_ms"]
+
+    def close(self):
+        self.w.close()
+        self.e.close()
+
+
+def measure(x, warmup, runs):
+    for _ in range(warmup):
+        x.run()
+    s = summary([x.run() for _ in range(runs)])
+    x.close()
+    return s
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--K", type=int, default=4096)
+    ap.add_argument("--runs", type=int, default=30)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--ab", action="store_true", help="also alternate fusion off / on (default chunk)")
+    args = ap.parse_args()
+    print(json.dumps({"card": card()}), flush=True)
+    print(json.dumps({"l2_probe": l2_probe()}), flush=True)
+    print(json.dumps({"fill_only": measure(Window(args.K, fill_only=True), args.warmup, args.runs)}), flush=True)
+    print(json.dumps({"sweep": "fusion_off", **measure(Window(args.K, -1), args.warmup, args.runs)}), flush=True)
+    for kib in (4, 8, 16, 32, 64, 256):
+        print(json.dumps({"sweep": "fusion_on", "chunk_kib": kib, **measure(Window(args.K, 0, kib * 1024), args.warmup, args.runs)}), flush=True)
+
+    if args.ab:
+        xs = {"fusion_off": Window(args.K, -1), "fusion_on": Window(args.K, 0)}
+        for x in xs.values():
+            for _ in range(args.warmup):
+                x.run()
+        ms = {k: [] for k in xs}
+        for _ in range(args.runs):
+            for k, x in xs.items():
+                ms[k].append(x.run())
+        res = {k: summary(v) for k, v in ms.items()}
+        res["speedup_median"] = res["fusion_off"]["median_ms"] / res["fusion_on"]["median_ms"]
+        print(json.dumps({"ab": res}), flush=True)
+        for x in xs.values():
+            x.close()
+
+
+if __name__ == "__main__":
+    main()
