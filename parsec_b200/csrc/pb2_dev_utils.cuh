@@ -99,6 +99,32 @@ struct alignas(128) BulkSmem {
 
 __device__ __forceinline__ uint32_t smem_addr_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
+// Where a body's payload lives: a tile in global memory (the streaming accesses above), or a staging slot in this CTA's
+// shared memory (a fused unit stages each chunk in a BulkSmem slot, pb2_engine.cu).  Shared accesses go through the
+// shared window explicitly: the slot reaches the bodies as a generic pointer.
+enum Space { kGlobal, kShared };
+template <Space S> __device__ __forceinline__ uint4 ld_v4(const uint4* p) {
+    if (S == kGlobal) return ld_stream(p);
+    uint4 r;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(smem_addr_u32(p)) : "memory");
+    return r;
+}
+template <Space S> __device__ __forceinline__ void st_v4(uint4* p, const uint4& v) {
+    if (S == kGlobal) { st_stream(p, v); return; }
+    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" :: "r"(smem_addr_u32(p)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+template <Space S> __device__ __forceinline__ uint32_t ld_u32(const uint32_t* p) {
+    if (S == kGlobal) return __ldcg(p);
+    uint32_t r;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(smem_addr_u32(p)) : "memory");
+    return r;
+}
+template <Space S> __device__ __forceinline__ void st_u32(uint32_t* p, uint32_t v) {
+    if (S == kGlobal) { __stcg(p, v); return; }
+    asm volatile("st.shared.u32 [%0], %1;" :: "r"(smem_addr_u32(p)), "r"(v) : "memory");
+}
+
 __device__ __forceinline__ void bulk_init(BulkSmem& b) {     // thread 0, once per kernel, followed by a barrier
     for (int s = 0; s < kBulkDepth; ++s)
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_addr_u32(&b.bar[s])) : "memory");
@@ -115,8 +141,12 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint3
                  :: "l"(gdst), "r"(smem_addr_u32(smem_src)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
-__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+// at most N bulk groups may still be reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all0()  { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// every thread that wrote a shared-memory buffer with generic stores, before the barrier after which a bulk store reads it
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_bar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok = 0;
     while (!ok) {
@@ -148,7 +178,7 @@ __device__ __forceinline__ void cta_bulk_copy(void* dst, const void* src, size_t
             if (i >= 1 && issued < n) {
                 // the slot of chunk i-1: its store is the second most recent group, and it has finished READING the
                 // buffer once at most one group (the store just issued) still has reads pending
-                bulk_wait_read1();
+                bulk_wait_read<1>();
                 const int fs = (int)((i - 1) % kBulkDepth);           // == issued % depth
                 const size_t noff = issued * kBulkChunk;
                 bulk_g2s(b.buf[fs], s + noff, (uint32_t)(bytes - noff < kBulkChunk ? bytes - noff : kBulkChunk), &b.bar[fs]);

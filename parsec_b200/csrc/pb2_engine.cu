@@ -74,8 +74,9 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
 // 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
 // streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
 // (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
-// producer runs with its group as one unit (run_fused_part) that checks each 16 KiB chunk right after writing it, so
-// the CHECK reads hit L2 and DRAM carries the write-back of the tiles alone (DESIGN.md §5, §8).
+// producer runs with its group as one unit (run_fused_part) that computes each 4 KiB chunk into a slot of the bulk
+// ring, checks it there and writes it to HBM with one TMA bulk store: the tile goes SM -> L2 -> DRAM once and never
+// comes back to the SM (DESIGN.md §5, §8).
 // What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
 #ifndef PB2_HBM_MINB
 #define PB2_HBM_MINB 12
@@ -88,16 +89,14 @@ struct GroupSmem {
     int32_t n;                              // members; 0: the popped task runs alone
     int32_t fused;                          // the popped task is a producer that runs with this group as one unit
     int32_t tile;                           // the tile the members read
-    int32_t fx;                             // fused: the producer's written flow on that tile
+    int32_t fx;                             // fused: the producer's output flow, on that tile
     int32_t mem[PB2_GROUP_MAX];
     uint32_t k[PB2_GROUP_MAX];
     unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
-    // fused: the producer's slice of every flow for this part, and the members' view of the current chunk
+    // fused: the producer's slice of every flow for this part
     void* base[PB2_MAX_FLOWS];
     uint32_t len[PB2_MAX_FLOWS];
     uint32_t e0;
-    unsigned long long r0;                  // the leader's result on the current chunk
-    BodyArgs c;
 };
 
 // All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
@@ -131,63 +130,91 @@ __device__ __forceinline__ unsigned long long chunk_sum(unsigned long long acc, 
     return acc + (r & 0xffffffff00000000ull);
 }
 
+// Thread 0: point s.args at the chunk of every flow that starts c0 bytes into this part's slice (the flows are cut
+// alike, and the group's tile is the widest).
+static __device__ __forceinline__ void set_chunk(TaskSmem& s, const GroupSmem& g, uint32_t c0, uint32_t chunk) {
+    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
+        const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
+        s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
+        s.args.bytes[f] = rest < chunk ? rest : chunk;
+    }
+    s.args.elem0 = g.e0 + (c0 >> 2);
+}
+
 // All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
-// producer's slice of every flow for this part.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, the
-// last chunk ragged): the producer's body writes a chunk, then the members read it back while it is still in L2.  Run
-// as separate tasks, the readers of a tile come long after its writer: every other worker writes its own tile in
-// between, and that is far more than L2 holds.  Member results follow group_results chunk by chunk, summed.
-// Returns the producer's result (thread 0).
-static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, uint32_t chunk) {
+// producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
+// writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
+// while they are still on the SM.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, at most kBulkChunk,
+// the last one ragged), and chunk i is staged in slot i % kBulkDepth of the bulk ring, which is idle while a body runs:
+//  1. the producer's staged body computes the chunk of its output flow into the slot (it reads its flows from global);
+//  2. the members check the slot, by group_results' rules, while one bulk store writes it to the tile;
+//  3. before the barrier that ends the chunk, thread 0 waits until the store that read the next chunk's slot is done.
+// So a chunk costs two barriers and no round trip through L2.  Member results are summed over the chunks (chunk_sum).
+// Tile slices are 16-byte aligned, as every body assumes; only the end of a slice (< 16 bytes) takes SIMT stores.
+// Returns the producer's result (thread 0) once every bulk store has completed and is ordered before the caller's
+// __threadfence(): successors on other SMs read the tile with generic loads.
+static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, BulkSmem* bulk, uint32_t chunk) {
     TaskSmem& s = *sp;
     GroupSmem& g = *gp;
+    const int body = s.task.body;
     if (threadIdx.x == 0) {
-        int fx = 0;
-        for (int f = PB2_MAX_FLOWS - 1; f >= 0; --f) {
-            if (f < (int)s.task.nb_flows && s.task.tile[f] == g.tile && (s.task.access[f] & PB2_FLOW_ACCESS_WRITE)) fx = f;
-            g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f];
-        }
-        g.fx = fx;
+        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f]; }
+        g.fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
         g.e0 = s.args.elem0;
-        g.c = s.args;
+        set_chunk(s, g, 0, chunk);
     }
     __syncthreads();
     const uint32_t len = g.len[g.fx];
+    uint8_t* const dst = static_cast<uint8_t*>(g.base[g.fx]);
+    const uint32_t k0 = g.k[0];
     unsigned long long acc = 0;
+    int slot_i = 0;
 #pragma unroll 1
     for (uint32_t c0 = 0;; c0 += chunk) {
+        const uint32_t n = len - c0 < chunk ? len - c0 : chunk;       // bytes of the output flow in this chunk
+        const bool last = len - c0 <= chunk;
+        uint8_t* const slot = bulk->buf[slot_i];
+        const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, slot);
+        fence_proxy_async_smem();
+        __syncthreads();
+        // the bytes the body wrote: a tail of < 4 bytes keeps what the tile holds, except for the bodies that write bytes
+        const uint32_t nw = (body == PB2_BODY_MEMSET_U8 || body == PB2_BODY_COPY) ? n : n & ~3u;
+        const uint32_t nb = nw & ~15u;
+        if (threadIdx.x == 0 && nb) bulk_s2g(dst + c0, slot, nb);
+        if (threadIdx.x < nw - nb) __stcg(dst + c0 + nb + threadIdx.x, slot[nb + threadIdx.x]);
+        const uint32_t diff = cta_xor_scan<kShared>(slot, n, k0);
         if (threadIdx.x == 0) {
-            // every flow at the same offset (they are cut alike, and the group's tile is the widest)
-            for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-                const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
-                s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
-                s.args.bytes[f] = rest < chunk ? rest : chunk;
-            }
-            s.args.elem0 = g.e0 + (c0 >> 2);
-            g.c.flow[0] = s.args.flow[g.fx]; g.c.bytes[0] = s.args.bytes[g.fx]; g.c.iparam[0] = (int32_t)g.k[0];
+            bulk_wait_read<kBulkDepth - 1>();
+            if (!last) set_chunk(s, g, c0 + chunk, chunk);
         }
-        __syncthreads();
-        const unsigned long long r = run_hbm_body(s.task.body, s.args, s.red);
-        __syncthreads();            // the chunk's stores are visible to the whole CTA before it reads them back
-        const unsigned long long r0 = run_hbm_body(PB2_BODY_CHECK_I32, g.c, s.red);
-        if (threadIdx.x == 0) { acc = chunk_sum(acc, r, c0); g.res[0] = chunk_sum(g.res[0], r0, c0); g.r0 = r0; }
-        __syncthreads();
+        const bool mismatch = __syncthreads_or(diff != 0u) != 0;
+        const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && n >= 4 ? *reinterpret_cast<const uint32_t*>(slot) : 0u;
+        if (!mismatch) {
+            // the chunk holds nothing but the leader's constant: every element mismatches any other constant
+            if (threadIdx.x == 0) {
+                acc = chunk_sum(acc, r, c0);
+                for (int m = 0; m < g.n; ++m)
+                    g.res[m] = chunk_sum(g.res[m], g.k[m] == k0 ? first : ((unsigned long long)(n >> 2) << 32) | first, c0);
+            }
+        } else {
+            // count again, exactly, for every constant but the leader's repeated
+            unsigned long long r0 = 0;
 #pragma unroll 1
-        for (int i = 1; i < g.n; ++i) {
-            const uint32_t k = g.k[i];
-            if (k == g.k[0] || !(g.r0 >> 32)) {
-                if (threadIdx.x == 0)
-                    g.res[i] = chunk_sum(g.res[i], k == g.k[0] ? g.r0 : ((unsigned long long)(g.c.bytes[0] >> 2) << 32) | (uint32_t)g.r0, c0);
-                continue;
+            for (int m = 0; m < g.n; ++m) {
+                const uint32_t k = g.k[m];
+                unsigned long long rm = r0;
+                if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne<kShared>(slot, n, k, s.red) << 32) | first;
+                if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = chunk_sum(g.res[m], rm, c0); }
             }
-            if (threadIdx.x == 0) g.c.iparam[0] = (int32_t)k;
-            __syncthreads();
-            const unsigned long long ri = run_hbm_body(PB2_BODY_CHECK_I32, g.c, s.red);
-            if (threadIdx.x == 0) g.res[i] = chunk_sum(g.res[i], ri, c0);
-            __syncthreads();
+            if (threadIdx.x == 0) acc = chunk_sum(acc, r, c0);
         }
-        if (len - c0 <= chunk) break;
+        if (last) break;
+        slot_i = slot_i + 1 == kBulkDepth ? 0 : slot_i + 1;
     }
-    if (threadIdx.x == 0) {         // the pushout that follows works on the whole slice
+    if (threadIdx.x == 0) {
+        bulk_wait_all0();
+        asm volatile("fence.proxy.async;" ::: "memory");
+        // the pushout that follows works on the whole slice
         for (int f = 0; f < PB2_MAX_FLOWS; ++f) { s.args.flow[f] = g.base[f]; s.args.bytes[f] = g.len[f]; }
         s.args.elem0 = g.e0;
     }
@@ -249,7 +276,7 @@ pb2_engine_hbm_kernel(WinDev w) {
         __syncthreads();
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
-            return g.fused ? run_fused_part(&s, &g, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
+            return g.fused ? run_fused_part(&s, &g, &bulk, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
         });
         if (g.n && !g.fused) {
             // the leader's part stored the version it saw; every member saw the same one
@@ -628,7 +655,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
 // With `fuse`, a task P also runs with the first group among its out-edges as one unit when P has a body, writes the
 // group's tile X without pushing it out, and X is P's widest tile (so P's parts cut X as the members' parts do): the
 // edge P -> leader leaves the device CSR and group[P] = PB2_GROUP_FUSED | the leader's group word.  The worker that
-// runs a part of P writes it chunk by chunk and the members check each chunk right after (run_fused_part).  The
+// runs a part of P stages it chunk by chunk in shared memory, the members check each chunk there, and a bulk store
+// writes it to X (run_fused_part); so P's body must have a staged form that writes X (fusable).  The
 // caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
 // every task that was queued when P retired, and a fused unit runs them right after P.
 static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
@@ -651,18 +679,24 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
         for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
         return true;
     };
+    // the bodies with a staged form (run_hbm_body<true>), whose output flow `out` writes X
     auto fusable = [&](const pb2_task_t& p, int32_t x) {
-        if (p.body == PB2_BODY_NOP || p.body == PB2_BODY_GEMM_BF16) return false;
-        bool writes = false;
+        int out = 0;
+        switch (p.body) {
+        case PB2_BODY_FILL_I32: case PB2_BODY_FILL_F32: case PB2_BODY_MEMSET_U8: case PB2_BODY_INCR_I32:
+        case PB2_BODY_SCALE_I32: case PB2_BODY_ADD_IOTA_I32: case PB2_BODY_IOTA_I32: case PB2_BODY_INCR_F32: break;
+        case PB2_BODY_COPY: case PB2_BODY_AXPY_F32: out = 1; break;
+        default: return false;
+        }
+        if (p.nb_flows <= out || p.tile[out] != x || !(p.access[out] & PB2_FLOW_ACCESS_WRITE)) return false;
+        // the staged COPY / AXPY writes every byte of the chunk: the tile they read is as long as X
+        if (out == 1 && (p.tile[0] < 0 || tiles[p.tile[0]].bytes != tiles[x].bytes)) return false;
         for (int f = 0; f < p.nb_flows; ++f) {
             if (p.tile[f] < 0) continue;
             if (tiles[p.tile[f]].bytes > tiles[x].bytes) return false;
-            if (p.tile[f] == x && (p.access[f] & PB2_FLOW_ACCESS_WRITE)) {
-                if (p.access[f] & PB2_FLOW_PUSHOUT) return false;
-                writes = true;
-            }
+            if (p.tile[f] == x && (p.access[f] & PB2_FLOW_ACCESS_WRITE) && (p.access[f] & PB2_FLOW_PUSHOUT)) return false;
         }
-        return writes;
+        return true;
     };
     std::vector<int32_t> begin(n), count(n);
     group.assign(n, 0u);
@@ -1056,7 +1090,8 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     d.slice_claim = nullptr; d.slice_done = nullptr; d.part_bytes = e->params.part_bytes;
     d.nparts = nullptr; d.remote_units = 0;
     d.group = nullptr; d.group_mem = nullptr;
-    d.fuse_chunk = e->fuse_chunk_bytes > 16 ? ((uint32_t)e->fuse_chunk_bytes + 15u) & ~15u : 16u;
+    // a fused unit stages each chunk in one slot of the bulk ring
+    d.fuse_chunk = e->fuse_chunk_bytes > 16 ? std::min(((uint32_t)e->fuse_chunk_bytes + 15u) & ~15u, kBulkChunk) : 16u;
     if (grouped) {
         uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
         TRY(dev_alloc_copy(w, &d_group, group.data(), group.size()));

@@ -5,15 +5,18 @@
 2. tools/l2_probe (compiled into a temporary directory): the L2 read rate and the DRAM rates of this GPU;
 3. a FILL-only window (the K producers of the Ex05 window, no readers): the write floor of the fused window;
 4. the resident Ex05 window (dags.ex05_broadcast(K, 14, 262144), tiles VALID) with fusion off, and on at chunk sizes
-   4 .. 256 KiB (PB2_FUSE_CHUNK_BYTES; 256 KiB is the whole tile: the producer writes it all before the group reads it);
-5. --ab: the same window with fusion off and on (default chunk), alternated run by run.
+   1, 2 and 4 KiB (PB2_FUSE_CHUNK_BYTES; a fused unit stages each chunk in one 4 KiB slot of the bulk ring);
+5. --ab LIB: the fused window (default chunk) on library LIB (another build of libparsec_b200.so, e.g. the parent
+   commit's) and on this tree's library, alternated: --rounds child processes per build, each with PB2_LIB_PATH set,
+   --warmup and --runs runs each.
 Each row: median / min / max / spread of reset_ms + kernel_ms.
 
-    python tools/ab_fuse_readers.py [--runs 30] [--ab]
+    python tools/ab_fuse_readers.py [--runs 30] [--ab /path/to/parent/libparsec_b200.so]
 """
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -59,12 +62,34 @@ class Window:
         self.e.close()
 
 
-def measure(x, warmup, runs):
+def runs_of(x, warmup, runs):
     for _ in range(warmup):
         x.run()
-    s = summary([x.run() for _ in range(runs)])
+    ms = [x.run() for _ in range(runs)]
     x.close()
-    return s
+    return ms
+
+
+def measure(x, warmup, runs):
+    return summary(runs_of(x, warmup, runs))
+
+
+def ab_libraries(args):
+    """The fused window on two library builds, one child process at a time, alternated."""
+    libs = {"lib_a": os.path.abspath(args.ab), "lib_b": L.LIB_PATH}
+    ms = {k: [] for k in libs}
+    medians = {k: [] for k in libs}
+    for _ in range(args.rounds):
+        for k, lib in libs.items():
+            out = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--K", str(args.K),
+                                  "--runs", str(args.runs), "--warmup", str(args.warmup)],
+                                 env=dict(os.environ, PB2_LIB_PATH=lib), capture_output=True, text=True, check=True).stdout
+            got = json.loads([l for l in out.splitlines() if l.startswith("{")][-1])["child_ms"]
+            ms[k] += got
+            medians[k].append(summary(got)["median_ms"])
+    res = {k: dict(summary(v), lib=libs[k], round_medians_ms=medians[k]) for k, v in ms.items()}
+    res["b_over_a_median"] = res["lib_b"]["median_ms"] / res["lib_a"]["median_ms"]
+    return res
 
 
 def main():
@@ -72,29 +97,21 @@ def main():
     ap.add_argument("--K", type=int, default=4096)
     ap.add_argument("--runs", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--ab", action="store_true", help="also alternate fusion off / on (default chunk)")
+    ap.add_argument("--ab", metavar="LIB", help="alternate the fused window on library LIB (lib_a) and on this tree's (lib_b)")
+    ap.add_argument("--rounds", type=int, default=4, help="--ab: child processes per library")
+    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.child:
+        print(json.dumps({"child_ms": runs_of(Window(args.K, 0), args.warmup, args.runs)}), flush=True)
+        return
     print(json.dumps({"card": card()}), flush=True)
     print(json.dumps({"l2_probe": l2_probe()}), flush=True)
     print(json.dumps({"fill_only": measure(Window(args.K, fill_only=True), args.warmup, args.runs)}), flush=True)
     print(json.dumps({"sweep": "fusion_off", **measure(Window(args.K, -1), args.warmup, args.runs)}), flush=True)
-    for kib in (4, 8, 16, 32, 64, 256):
+    for kib in (1, 2, 4):
         print(json.dumps({"sweep": "fusion_on", "chunk_kib": kib, **measure(Window(args.K, 0, kib * 1024), args.warmup, args.runs)}), flush=True)
-
     if args.ab:
-        xs = {"fusion_off": Window(args.K, -1), "fusion_on": Window(args.K, 0)}
-        for x in xs.values():
-            for _ in range(args.warmup):
-                x.run()
-        ms = {k: [] for k in xs}
-        for _ in range(args.runs):
-            for k, x in xs.items():
-                ms[k].append(x.run())
-        res = {k: summary(v) for k, v in ms.items()}
-        res["speedup_median"] = res["fusion_off"]["median_ms"] / res["fusion_on"]["median_ms"]
-        print(json.dumps({"ab": res}), flush=True)
-        for x in xs.values():
-            x.close()
+        print(json.dumps({"ab": ab_libraries(args)}), flush=True)
 
 
 if __name__ == "__main__":
