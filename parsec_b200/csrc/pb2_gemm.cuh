@@ -491,6 +491,14 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                     if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)rows * (unsigned long long)Nj * 2ull);
                 }
             }
+            // a pushout writes the whole tile back, as every other body's does: the part that runs the last sub-tile also
+            // copies the bytes of the tile past C
+            const size_t c_bytes = (size_t)job.M * row_bytes;
+            if (job.part == (job.nsub - 1) % job.nparts && tile->bytes > c_bytes) {
+                cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + c_bytes,
+                                reinterpret_cast<const uint8_t*>(tile->dev_ptr) + c_bytes, tile->bytes - c_bytes);
+                if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)(tile->bytes - c_bytes));
+            }
             __syncthreads();
         }
         if (warp == 0) {
