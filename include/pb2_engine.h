@@ -85,7 +85,8 @@ typedef struct pb2_task_s {
                              * mask mode: tc->dependencies_goal (parsec.c:1656-1720)                        */
     int32_t  succ_begin;    /* first entry in succ[]                                                         */
     int32_t  succ_count;    /* number of out-edges (iterate_successors fan-out)                              */
-    int32_t  priority;      /* task priority (larger first when a priority lane is used)                      */
+    int32_t  priority;      /* task priority: with queue_policy 1 a larger value is popped first (see
+                             * pb2_engine_params_t::queue_policy); ignored with the default FIFO policy        */
     uint8_t  body;          /* enum pb2_body_e                                                                */
     uint8_t  nb_flows;
     uint8_t  flags;         /* PB2_TASK_* */
@@ -131,7 +132,17 @@ typedef struct pb2_engine_params_s {
     int32_t  max_workers;      /* 0 = all; 1 = single worker => deterministic FIFO order (tests)             */
     int32_t  stage_mode;       /* tile mover of the HBM-body kernels: 0 = TMA bulk copy (cp.async.bulk through a
                                 * shared-memory ring, default), 1 = SIMT 16-byte LDG/STG loops                      */
-    int32_t  queue_policy;     /* accepted and ignored: every kernel runs one FIFO ready ring                 */
+    int32_t  queue_policy;     /* order in which the workers of HBM and GEMM windows pop ready tasks:
+                                *   0 = one FIFO ready ring (default);
+                                *   1 = priority, the reference's rule (device_gpu.c:2169-2174): higher
+                                *       pb2_task_t::priority first, FIFO among equal priorities.  The ring is cut into
+                                *       16 FIFO lanes; the distinct priorities of a window's tasks are ranked highest
+                                *       first and rank r goes to lane r when there are at most 16 of them (exact
+                                *       order), to lane floor(r * 16 / ndistinct) otherwise.  A read group or a fused
+                                *       unit runs in its leader's / producer's lane, a GEMM unit in its first task's.
+                                *       Not with shared windows (pb2_window_create: PB2_ERR_NOT_SUPPORTED).
+                                * pb2_engine_create refuses any other value (PB2_ERR_BAD_PARAM).  The streaming kernel
+                                * (pb2_stream.h) always pops in submission order.                                 */
     int32_t  timeout_ms;       /* device-side watchdog: a window that makes no progress for this long aborts
                                 * (default 20000); a malformed DAG must never hang the GPU                   */
     int32_t  gemm_mode;        /* 0 = fused k-chains (default), 2 = every task is its own unit and flushes C

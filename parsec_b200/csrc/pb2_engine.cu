@@ -24,10 +24,11 @@
 #include <mutex>
 #include <map>
 #include <algorithm>
+#include <functional>
 
 #include "../../include/pb2_engine.h"
 #include "pb2_sched.cuh"
-#include "pb2_worker.cuh"
+#include "pb2_hbm.cuh"
 #include "pb2_gemm.cuh"
 
 namespace pb2 {
@@ -35,6 +36,16 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // reset: (re)arm one window.  dep words, ring, counters, tile table.
 // ---------------------------------------------------------------------------------------------
+// queue_policy 1: every lane starts with its initial entries, which the ring image `ready` holds at the start of the
+// lane's segment (empty slots kEmpty).
+__device__ __forceinline__ void reset_lanes(Lanes* lanes, size_t gid) {
+    if (lanes && gid < PB2_PRIO_LANES) {
+        lanes->head[gid].v = lanes->begin[gid];
+        lanes->tail[gid].v = (unsigned long long)lanes->begin[gid] + lanes->ninit[gid];
+        lanes->avail[gid].v = lanes->ninit[gid];
+    }
+}
+
 __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -56,6 +67,7 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
             for (int k = 0; k <= PB2_SLICE_WORDS; ++k) w.slice_done[i * (PB2_SLICE_WORDS + 1) + k] = 0;
         }
     }
+    reset_lanes(w.lanes, gid);
     if (gid == 0) {
         w.ctl->head.v = 0; w.ctl->tail.v = (unsigned long long)nready; w.ctl->evt.v = 0;
         w.ctl->retired.v = 0; w.ctl->done.v = (w.ntasks == 0) ? kDoneOK : 0;
@@ -65,309 +77,13 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
     }
 }
 
-// ---------------------------------------------------------------------------------------------
-// the persistent engine kernel, HBM-bound bodies
-// ---------------------------------------------------------------------------------------------
-// 64-thread workers, 12 per SM (<= 80 registers, no spills): a worker keeps PB2_CHECK_UNROLL = 16 (read-only bodies) or
-// PB2_UNROLL = 4 (read-modify-write bodies) 16-byte requests per thread in flight -- bytes in flight per SM are what
-// a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
-// 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
-// streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
-// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
-// producer runs with its group as one unit (run_fused_part) that computes each 4 KiB chunk into a slot of the bulk
-// ring, checks it there and writes it to HBM with one TMA bulk store: the tile goes SM -> L2 -> DRAM once and never
-// comes back to the SM (DESIGN.md §5, §8).
-// What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
-#ifndef PB2_HBM_MINB
-#define PB2_HBM_MINB 12
-#endif
-#ifndef PB2_HBM_THREADS
-#define PB2_HBM_THREADS 64
-#endif
-// A read group in flight on one worker: its members (the leader first), their CHECK constants, this part's results.
-struct GroupSmem {
-    int32_t n;                              // members; 0: the popped task runs alone
-    int32_t fused;                          // the popped task is a producer that runs with this group as one unit
-    int32_t tile;                           // the tile the members read
-    int32_t fx;                             // fused: the producer's output flow, on that tile
-    int32_t mem[PB2_GROUP_MAX];
-    uint32_t k[PB2_GROUP_MAX];
-    unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
-    // fused: the producer's slice of every flow for this part
-    void* base[PB2_MAX_FLOWS];
-    uint32_t len[PB2_MAX_FLOWS];
-    uint32_t e0;
-};
-
-// All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
-// bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
-//  - k equal to the leader's: the leader's result;
-//  - the slice held nothing but the leader's constant: every element mismatches (the first element is the same);
-//  - otherwise the member's slice is counted again, exactly, as a failing CHECK counts it.
-static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
-    TaskSmem& s = *sp;
-    GroupSmem& g = *gp;
-    const unsigned long long r0 = g.res[0];
-#pragma unroll 1
-    for (int i = 1; i < g.n; ++i) {
-        const uint32_t k = g.k[i];
-        if (k == g.k[0] || !(r0 >> 32)) {
-            if (threadIdx.x == 0) g.res[i] = k == g.k[0] ? r0 : ((unsigned long long)(s.args.bytes[0] >> 2) << 32) | (uint32_t)r0;
-            continue;
-        }
-        if (threadIdx.x == 0) s.args.iparam[0] = (int32_t)k;
-        __syncthreads();
-        const unsigned long long r = run_hbm_body(PB2_BODY_CHECK_I32, s.args, s.red);
-        if (threadIdx.x == 0) g.res[i] = r;
-        __syncthreads();
-    }
-    __syncthreads();
-}
-
-// Results of a body run chunk by chunk: the mismatch counts add up, the first element is the first chunk's.
-__device__ __forceinline__ unsigned long long chunk_sum(unsigned long long acc, unsigned long long r, uint32_t c0) {
-    if (c0 == 0 || acc == ~0ull || r == ~0ull) return c0 == 0 ? r : ~0ull;
-    return acc + (r & 0xffffffff00000000ull);
-}
-
-// Thread 0: point s.args at the chunk of every flow that starts c0 bytes into this part's slice (the flows are cut
-// alike, and the group's tile is the widest).
-static __device__ __forceinline__ void set_chunk(TaskSmem& s, const GroupSmem& g, uint32_t c0, uint32_t chunk) {
-    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-        const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
-        s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
-        s.args.bytes[f] = rest < chunk ? rest : chunk;
-    }
-    s.args.elem0 = g.e0 + (c0 >> 2);
-}
-
-// All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
-// producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
-// writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
-// while they are still on the SM.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, at most kBulkChunk,
-// the last one ragged), and chunk i is staged in slot i % kBulkDepth of the bulk ring, which is idle while a body runs:
-//  1. the producer's staged body computes the chunk of its output flow into the slot (it reads its flows from global);
-//  2. the members check the slot, by group_results' rules, while one bulk store writes it to the tile;
-//  3. before the barrier that ends the chunk, thread 0 waits until the store that read the next chunk's slot is done.
-// So a chunk costs two barriers and no round trip through L2.  Member results are summed over the chunks (chunk_sum).
-// Tile slices are 16-byte aligned, as every body assumes; only the end of a slice (< 16 bytes) takes SIMT stores.
-// Returns the producer's result (thread 0) once every bulk store has completed and is ordered before the caller's
-// __threadfence(): successors on other SMs read the tile with generic loads.
-static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, BulkSmem* bulk, uint32_t chunk) {
-    TaskSmem& s = *sp;
-    GroupSmem& g = *gp;
-    const int body = s.task.body;
-    if (threadIdx.x == 0) {
-        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f]; }
-        g.fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
-        g.e0 = s.args.elem0;
-        set_chunk(s, g, 0, chunk);
-    }
-    __syncthreads();
-    const uint32_t len = g.len[g.fx];
-    uint8_t* const dst = static_cast<uint8_t*>(g.base[g.fx]);
-    const uint32_t k0 = g.k[0];
-    unsigned long long acc = 0;
-    int slot_i = 0;
-#pragma unroll 1
-    for (uint32_t c0 = 0;; c0 += chunk) {
-        const uint32_t n = len - c0 < chunk ? len - c0 : chunk;       // bytes of the output flow in this chunk
-        const bool last = len - c0 <= chunk;
-        uint8_t* const slot = bulk->buf[slot_i];
-        const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, slot);
-        fence_proxy_async_smem();
-        __syncthreads();
-        // the bytes the body wrote: a tail of < 4 bytes keeps what the tile holds, except for the bodies that write bytes
-        const uint32_t nw = (body == PB2_BODY_MEMSET_U8 || body == PB2_BODY_COPY) ? n : n & ~3u;
-        const uint32_t nb = nw & ~15u;
-        if (threadIdx.x == 0 && nb) bulk_s2g(dst + c0, slot, nb);
-        if (threadIdx.x < nw - nb) __stcg(dst + c0 + nb + threadIdx.x, slot[nb + threadIdx.x]);
-        const uint32_t diff = cta_xor_scan<kShared>(slot, n, k0);
-        if (threadIdx.x == 0) {
-            bulk_wait_read<kBulkDepth - 1>();
-            if (!last) set_chunk(s, g, c0 + chunk, chunk);
-        }
-        const bool mismatch = __syncthreads_or(diff != 0u) != 0;
-        const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && n >= 4 ? *reinterpret_cast<const uint32_t*>(slot) : 0u;
-        if (!mismatch) {
-            // the chunk holds nothing but the leader's constant: every element mismatches any other constant
-            if (threadIdx.x == 0) {
-                acc = chunk_sum(acc, r, c0);
-                for (int m = 0; m < g.n; ++m)
-                    g.res[m] = chunk_sum(g.res[m], g.k[m] == k0 ? first : ((unsigned long long)(n >> 2) << 32) | first, c0);
-            }
-        } else {
-            // count again, exactly, for every constant but the leader's repeated
-            unsigned long long r0 = 0;
-#pragma unroll 1
-            for (int m = 0; m < g.n; ++m) {
-                const uint32_t k = g.k[m];
-                unsigned long long rm = r0;
-                if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne<kShared>(slot, n, k, s.red) << 32) | first;
-                if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = chunk_sum(g.res[m], rm, c0); }
-            }
-            if (threadIdx.x == 0) acc = chunk_sum(acc, r, c0);
-        }
-        if (last) break;
-        slot_i = slot_i + 1 == kBulkDepth ? 0 : slot_i + 1;
-    }
-    if (threadIdx.x == 0) {
-        bulk_wait_all0();
-        asm volatile("fence.proxy.async;" ::: "memory");
-        // the pushout that follows works on the whole slice
-        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { s.args.flow[f] = g.base[f]; s.args.bytes[f] = g.len[f]; }
-        s.args.elem0 = g.e0;
-    }
-    __syncthreads();
-    return acc;
-}
-
-__global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
-pb2_engine_hbm_kernel(WinDev w) {
-    __shared__ TaskSmem s;
-    __shared__ BulkSmem bulk;
-    __shared__ GroupSmem g;
-    if (threadIdx.x == 0) bulk_init(bulk);
-    __syncthreads();
-
-    for (;;) {
-        if (threadIdx.x == 0) {
-            const int32_t e = pop_task(w);
-            if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
-            s.entry = e;
-        }
-        __syncthreads();
-        const int32_t entry = s.entry;
-        if (entry == kEmpty) break;
-        const int32_t id = w.nparts ? PB2_ENT_TASK(entry) : entry;
-        const int part = w.nparts ? PB2_ENT_PART(entry) : 0;
-        if (threadIdx.x < 4) reinterpret_cast<uint4*>(&s.task)[threadIdx.x] =
-            __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
-        {
-            const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
-            const int gn = (int)(gd & 15u);
-            const uint32_t gb = (gd & ~PB2_GROUP_FUSED) >> 4;
-            const bool fused = (gd & PB2_GROUP_FUSED) != 0;
-            if ((int)threadIdx.x < gn) {
-                const int32_t m = __ldg(&w.group_mem[gb + threadIdx.x]);
-                const pb2_task_t& mt = w.tasks[m];
-                g.mem[threadIdx.x] = m;
-                g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
-                if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
-            }
-            if (threadIdx.x == 0) {
-                g.n = gn; g.fused = fused;
-                if (part == 0 && gn && !fused) {
-                    // the members start together: consecutive event numbers, one worker
-                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
-                    for (int i = 0; i < gn; ++i) {
-                        const int32_t m = __ldg(&w.group_mem[gb + i]);
-                        w.start_seq[m] = seq + (uint32_t)i;
-                        w.worker[m] = (int32_t)blockIdx.x;
-                    }
-                } else if (part == 0) {
-                    w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
-                    w.worker[id] = (int32_t)blockIdx.x;
-                    // a fused unit's members start when it retires (below); they run on the producer's worker
-                    for (int i = 0; i < gn; ++i) w.worker[__ldg(&w.group_mem[gb + i])] = (int32_t)blockIdx.x;
-                }
-            }
-        }
-        __syncthreads();
-        const int nparts = task_nparts(w, id);
-        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
-            return g.fused ? run_fused_part(&s, &g, &bulk, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
-        });
-        if (g.n && !g.fused) {
-            // the leader's part stored the version it saw; every member saw the same one
-            if (threadIdx.x == 0) {
-                g.res[0] = r;
-                if (part == 0) {
-                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.seen_version[(size_t)id * PB2_MAX_FLOWS]);
-                    for (int i = 1; i < g.n; ++i) w.seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
-                }
-            }
-            __syncthreads();
-            group_results(&s, &g);
-        }
-
-        if (threadIdx.x < 32) {
-            __threadfence();   // release side: the body's stores (all threads, ordered by the barrier) become
-                               // visible before any successor can observe its dependency word / ring slot
-            if (threadIdx.x == 0) {
-                const pb2_task_t& t = s.task;
-                const int gn = g.n;
-                for (int i = 0; i < gn; ++i) store_result(w, w.tasks[g.mem[i]], g.mem[i], part, nparts, g.res[i]);
-                if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
-                // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
-                int last = 1;
-                if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
-                s.window_done = 0; s.last = last;
-                if (last && gn && g.fused) {
-                    // the producer, then its members as if they had run right after it: they saw the version it
-                    // wrote; its end, their starts, their ends are consecutive events (end before start on every
-                    // edge); they retire right after it, in member order
-                    epilog_written_flows(w, t);
-                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.tiles[g.tile].version);
-                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)(1 + 2 * gn));
-                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)(1 + gn));
-                    w.end_seq[id] = ev;
-                    w.retire_log[seq] = id;
-                    for (int i = 0; i < gn; ++i) {
-                        const int32_t m = g.mem[i];
-                        w.seen_version[(size_t)m * PB2_MAX_FLOWS] = v;
-                        w.start_seq[m] = ev + 1u + (uint32_t)i;
-                        w.end_seq[m] = ev + 1u + (uint32_t)(gn + i);
-                        w.retire_log[seq + 1u + (uint32_t)i] = m;
-                    }
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
-                    s.window_done = (int32_t)(seq + 1u + (uint32_t)gn) == w.ntasks ? 1 : 0;
-                    __threadfence();
-                } else if (last && gn) {
-                    // members only read their tile: no written flows; they retire back to back, in member order
-                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
-                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
-                    for (int i = 0; i < gn; ++i) { w.end_seq[g.mem[i]] = ev + (uint32_t)i; w.retire_log[seq + (uint32_t)i] = g.mem[i]; }
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
-                    s.window_done = (int32_t)(seq + (uint32_t)gn) == w.ntasks ? 1 : 0;
-                    __threadfence();
-                } else if (last) {
-                    epilog_written_flows(w, t);
-                    w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
-                    // the retire log is written before the out-edges are released, so that it is a linear
-                    // extension of the DAG's partial order (a successor can only retire after us)
-                    s.window_done = retire_task(w, id) ? 1 : 0;
-                    __threadfence();
-                }
-            }
-            __syncwarp();
-        }
-        if (w.ps_begin != nullptr) {
-            // tiles this task wrote for readers on other GPUs go out before those readers are released
-            __syncthreads();
-            if (s.last && w.ps_begin[id + 1] > w.ps_begin[id]) push_written_tiles(w.tiles, w.ctl, w.ps_begin, w.ps, id, &bulk);
-        }
-        if (threadIdx.x < 32) {
-            if (s.last) {
-                // a fused producer's own successors first (its edge to the group is not among them), then the members'
-                if (!g.n || g.fused) { release_successors_warp(w, s.task); release_remote_warp(w, id); }
-                for (int i = 0; i < g.n; ++i) release_successors_warp(w, w.tasks[g.mem[i]]);
-            }
-            if (threadIdx.x == 0 && s.window_done) {
-                __threadfence();
-                st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
-            }
-        }
-        __syncthreads();
-    }
-}
-
 // re-arm the unit-level scheduling state of a GEMM window (after pb2_window_reset_kernel re-armed the rest)
 __global__ void pb2_window2_reset_kernel(Win2Dev g, const int32_t* ready_entries, int32_t nentries) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
     for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
     for (size_t i = gid; i <= (size_t)g.w.cap_mask; i += gsz) g.w.ring[i] = (i < (size_t)nentries) ? ready_entries[i] : kEmpty;
+    reset_lanes(g.w.lanes, gid);
     if (gid == 0) g.w.ctl->tail.v = (unsigned long long)nentries;
 }
 
@@ -537,11 +253,59 @@ static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
 
 
 // ---------------------------------------------------------------------------------------------
+// queue_policy 1: priority lanes
+// ---------------------------------------------------------------------------------------------
+// The lane of every task: the distinct priorities of the window's tasks ranked highest first, lane = rank r with at most
+// PB2_PRIO_LANES of them, floor(r * PB2_PRIO_LANES / ndistinct) otherwise.  tests/priority_order.py restates it.
+static std::vector<uint8_t> task_priority_lanes(const pb2_task_t* tasks, int32_t ntasks, int32_t* nlanes) {
+    std::vector<int32_t> v((size_t)ntasks);
+    for (int32_t i = 0; i < ntasks; ++i) v[(size_t)i] = tasks[i].priority;
+    std::sort(v.begin(), v.end(), std::greater<int32_t>());
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    const int64_t nd = (int64_t)v.size();
+    std::vector<uint8_t> lane((size_t)ntasks, 0);
+    for (int32_t i = 0; i < ntasks; ++i) {
+        const int64_t r = std::lower_bound(v.begin(), v.end(), tasks[i].priority, std::greater<int32_t>()) - v.begin();
+        lane[(size_t)i] = (uint8_t)(nd <= PB2_PRIO_LANES ? r : r * PB2_PRIO_LANES / nd);
+    }
+    *nlanes = nd == 0 ? 1 : (int32_t)std::min<int64_t>(nd, PB2_PRIO_LANES);
+    return lane;
+}
+
+// Cut the ring into one segment per lane, as long as the entries the lane's owners can ever push (owner o: a task of an
+// HBM window or a unit of a GEMM window, in lane owner_lane[o], pushes at most owner_pushes[o] entries).  `entries`, the
+// initial ready entries in the order a FIFO ring would hold them, becomes the image of the whole ring that the reset
+// kernels write: each entry at the start of its lane's segment, in the same order within a lane.
+static int build_lane_ring(pb2_window_t* w, const std::vector<uint8_t>& owner_lane, const std::vector<uint32_t>& owner_pushes,
+                           std::vector<int32_t>& entries, bool unit_entries) {
+    Lanes h;
+    memset(&h, 0, sizeof h);
+    uint32_t size[PB2_PRIO_LANES] = {0};
+    for (size_t o = 0; o < owner_lane.size(); ++o) size[owner_lane[o]] += owner_pushes[o];
+    uint32_t b = 0;
+    for (int l = 0; l < PB2_PRIO_LANES; ++l) { h.begin[l] = b; b += size[l]; }
+    std::vector<int32_t> ring(b, kEmpty);
+    for (const int32_t e : entries) {
+        const int l = owner_lane[(size_t)(unit_entries ? PB2_SUCC_TASK((uint32_t)e) : PB2_ENT_TASK(e))];
+        ring[h.begin[l] + h.ninit[l]++] = e;
+    }
+    entries.swap(ring);
+    int rc;
+    Lanes* d_lanes = nullptr;
+    uint8_t* d_lane = nullptr;
+    if ((rc = dev_alloc_copy(w, &d_lanes, &h, 1)) != PB2_SUCCESS) return rc;
+    if ((rc = dev_alloc_copy(w, &d_lane, owner_lane.data(), owner_lane.size())) != PB2_SUCCESS) return rc;
+    w->d.lanes = d_lanes; w->d.lane = d_lane;
+    return PB2_SUCCESS;
+}
+
+// ---------------------------------------------------------------------------------------------
 // GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
+// task_lane (queue_policy 1, else null): a unit's lane is the lane of its first task.
 static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
                              const int32_t* ready, int32_t nready, bool fuse, uint32_t* ring_cap_needed,
-                             const int32_t* rs_begin) {
+                             const int32_t* rs_begin, const std::vector<uint8_t>* task_lane) {
     std::vector<int32_t> indeg((size_t)ntasks, 0), cpred((size_t)ntasks, -1), ccons((size_t)ntasks, 0), next((size_t)ntasks, -1);
     auto is_gemm = [&](int32_t t) { return tasks[t].body == PB2_BODY_GEMM_BF16; };
     for (int32_t u = 0; u < ntasks; ++u)
@@ -626,6 +390,15 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         for (int32_t p = 0; p < units[o.second].nparts; ++p) entries.push_back((int32_t)PB2_SUCC_MAKE(o.second, p));
     *ring_cap_needed = total_parts;
     int rc;
+    if (task_lane) {
+        std::vector<uint8_t> ulane(units.size());
+        std::vector<uint32_t> upush(units.size());
+        for (size_t u = 0; u < units.size(); ++u) {
+            ulane[u] = (*task_lane)[(size_t)segs[(size_t)units[u].seg_begin].task];
+            upush[u] = (uint32_t)units[u].nparts;
+        }
+        if ((rc = build_lane_ring(w, ulane, upush, entries, true)) != PB2_SUCCESS) return rc;
+    }
     GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
     if ((rc = dev_alloc_copy(w, &d_units, units.data(), units.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_segs, segs.data(), segs.size())) != PB2_SUCCESS) return rc;
@@ -737,6 +510,7 @@ extern "C" {
 int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_params_t* params) {
     if (!engine) return PB2_ERR_BAD_PARAM;
     *engine = nullptr;
+    if (params && params->queue_policy != 0 && params->queue_policy != 1) return PB2_ERR_BAD_PARAM;
     int ndev = 0;
     cudaError_t err = cudaGetDeviceCount(&ndev);
     if (err != cudaSuccess || ndev == 0) {
@@ -779,7 +553,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
         }
     }
     int occ = 0;
-    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb2_engine_hbm_kernel, p.threads, 0));
+    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb2_engine_hbm_kernel<false>, p.threads, 0));
     int per_sm = occ < p.workers_per_sm ? occ : p.workers_per_sm;
     if (per_sm < 1) per_sm = 1;
     e->nworkers = e->prop.multiProcessorCount * per_sm;
@@ -1028,6 +802,11 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     if ((ntasks && !tasks) || (nsucc && !succ) || (ntiles && !tiles) || (nready && !ready)) return PB2_ERR_BAD_PARAM;
     int rc = validate_window(e, kind, tasks, ntasks, succ, nsucc, ntiles, ready, nready);
     if (rc != PB2_SUCCESS) return rc;
+    const bool prio = e->params.queue_policy == 1;
+    if (prio && e->shared_windows) {
+        e->last_error = "queue_policy 1 (priority lanes) is not supported with shared windows: peers push into one FIFO ring";
+        return PB2_ERR_NOT_SUPPORTED;
+    }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     pb2_window_t* w = new pb2_window_s();
     w->shared = e->shared_windows;
@@ -1063,13 +842,17 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     else TRY(dev_alloc_copy(w, &w->d_succ, succ, (size_t)nsucc));
     TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
     TRY(dev_alloc_copy(w, &w->d_tiles, (const pb2_tile_t*)nullptr, (size_t)ntiles));
+    int32_t nlanes = 0;
+    std::vector<uint8_t> task_lane;
+    if (prio) task_lane = task_priority_lanes(tasks, ntasks, &nlanes);
+    if (prio && kind == 0) TRY(build_lane_ring(w, task_lane, std::vector<uint32_t>(nparts.begin(), nparts.end()), entries, false));
     TRY(dev_alloc_copy(w, &w->d_ready, entries.data(), entries.size()));
     w->nready_entries = (int32_t)entries.size();
     uint32_t parts_needed = 0;
     if (kind == 1) {
         TRY(build_tensor_maps(w, tasks, ntasks, tiles, ntiles));
         TRY(build_gemm2_units(w, tasks, ntasks, succ, ready, nready, e->params.gemm_mode == 0, &parts_needed,
-                              w->shared ? e->next_rs_begin : nullptr));
+                              w->shared ? e->next_rs_begin : nullptr, prio ? &task_lane : nullptr));
     }
     const int maxw = e->nworkers > e->nworkers_gemm ? e->nworkers : e->nworkers_gemm;
     uint32_t cap = 1024;
@@ -1090,6 +873,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     d.slice_claim = nullptr; d.slice_done = nullptr; d.part_bytes = e->params.part_bytes;
     d.nparts = nullptr; d.remote_units = 0;
     d.group = nullptr; d.group_mem = nullptr;
+    d.nlanes = nlanes;          // d.lanes / d.lane: build_lane_ring
     // a fused unit stages each chunk in one slot of the bulk ring
     d.fuse_chunk = e->fuse_chunk_bytes > 16 ? std::min(((uint32_t)e->fuse_chunk_bytes + 15u) & ~15u, kBulkChunk) : 16u;
     if (grouped) {
@@ -1187,10 +971,14 @@ int pb2_window_start(pb2_window_t* w) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
         if (w->kind == 0) {
-            pb2_engine_hbm_kernel<<<e->nworkers, e->params.threads, 0, e->stream>>>(w->d);
-            PB2_CUDA(e, cudaGetLastError());
+            if (w->d.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(w->d, e->nworkers, e->params.threads, e->stream));
+            else {
+                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(w->d);
+                PB2_CUDA(e, cudaGetLastError());
+            }
         } else {
-            int rc = pb2_gemm2_launch(w->g, e->nworkers_gemm, e->stream);
+            int rc = w->d.lanes ? pb2_gemm2_prio_launch(w->g, e->nworkers_gemm, e->stream)
+                                : pb2_gemm2_launch<false>(w->g, e->nworkers_gemm, e->stream);
             if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
             w->g.fresh_tmaps = 0;
         }

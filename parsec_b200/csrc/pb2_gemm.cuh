@@ -238,6 +238,7 @@ struct Shared {
 };
 
 // whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges
+template <bool PRIO>
 __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u, int unit_id) {
     const WinDev& w = g.w;
     const int lane = threadIdx.x & 31;
@@ -294,7 +295,10 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
         int incl = nparts;
         for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
         const int total = __shfl_sync(0xffffffffu, incl, 31);
-        if (total) {
+        if (total && PRIO) {
+            const uint32_t first = reserve_lane_slots(w.lanes, nparts ? (int)w.lane[sid] : 0, nparts);
+            for (int p = 0; p < nparts; ++p) st_release_gpu(&w.ring[first + (uint32_t)p], (int32_t)PB2_SUCC_MAKE(sid, p));
+        } else if (total) {
             unsigned long long base = 0;
             if (lane == 0) base = atomicAdd(&w.ctl->tail.v, (unsigned long long)total);
             base = __shfl_sync(0xffffffffu, base, 0);
@@ -314,6 +318,8 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
 
 }  // namespace gemm
 
+// PRIO: queue_policy 1 (priority lanes of units, pop_prio)
+template <bool PRIO>
 __global__ void __launch_bounds__(gemm::kThreads, 1)
 pb2_engine_gemm2_kernel(Win2Dev g) {
     using namespace gemm;
@@ -341,7 +347,7 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
         // ---------------- pop the next (part, unit), stage its tiles in
         if (threadIdx.x == 0) {
             Job j; memset(&j, 0, sizeof j);
-            const int32_t e = pop_task(w);
+            const int32_t e = pop_entry<PRIO>(w);
             if (e == kEmpty) { j.stop = 1; }
             else {
                 __threadfence();
@@ -505,21 +511,25 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             int last = 0;
             if (lane == 0) { __threadfence(); last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
             last = __shfl_sync(0xffffffffu, last, 0);
-            if (last) { __threadfence(); retire_unit_warp(g, g.units[job.unit], job.unit); }
+            if (last) { __threadfence(); retire_unit_warp<PRIO>(g, g.units[job.unit], job.unit); }
         }
         __syncthreads();             // sh.job is rewritten by the next pop
     }
 }
 
+template <bool PRIO>
 static inline int pb2_gemm2_launch(const Win2Dev& g, int nworkers, cudaStream_t stream) {
-    static bool attr_set = false;
+    static bool attr_set = false;       // one per instantiation
     if (!attr_set) {
-        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
+        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel<PRIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
         attr_set = true;
     }
     if (nworkers < 1) return PB2_ERR_BAD_PARAM;
-    pb2_engine_gemm2_kernel<<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
+    pb2_engine_gemm2_kernel<PRIO><<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
     return cudaGetLastError() == cudaSuccess ? PB2_SUCCESS : PB2_ERR_DEVICE;
 }
+
+// pb2_engine_prio.cu: launch the queue_policy 1 instantiation
+int pb2_gemm2_prio_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
 
 }  // namespace pb2

@@ -1,0 +1,314 @@
+// pb2_hbm.cuh -- the persistent engine kernel of HBM-body windows (pb2_engine_hbm_kernel) and what it runs besides
+// the shared worker code of pb2_worker.cuh: read groups and fused producer units.  Instantiated for the FIFO ready ring
+// in pb2_engine.cu and for priority lanes (queue_policy 1) in pb2_engine_prio.cu: each translation unit holds one
+// instantiation, because a second kernel calling the same __noinline__ helpers makes ptxas give them the standard call
+// ABI, which costs the kernel a stack frame and spills at its 80-register budget.
+#pragma once
+#include "pb2_sched.cuh"
+#include "pb2_worker.cuh"
+
+namespace pb2 {
+
+// ---------------------------------------------------------------------------------------------
+// the persistent engine kernel, HBM-bound bodies
+// ---------------------------------------------------------------------------------------------
+// 64-thread workers, 12 per SM (<= 80 registers, no spills): a worker keeps PB2_CHECK_UNROLL = 16 (read-only bodies) or
+// PB2_UNROLL = 4 (read-modify-write bodies) 16-byte requests per thread in flight -- bytes in flight per SM are what
+// a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
+// 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
+// streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
+// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
+// producer runs with its group as one unit (run_fused_part) that computes each 4 KiB chunk into a slot of the bulk
+// ring, checks it there and writes it to HBM with one TMA bulk store: the tile goes SM -> L2 -> DRAM once and never
+// comes back to the SM (DESIGN.md §5, §8).
+// What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
+#ifndef PB2_HBM_MINB
+#define PB2_HBM_MINB 12
+#endif
+#ifndef PB2_HBM_THREADS
+#define PB2_HBM_THREADS 64
+#endif
+// A read group in flight on one worker: its members (the leader first), their CHECK constants, this part's results.
+struct GroupSmem {
+    int32_t n;                              // members; 0: the popped task runs alone
+    int32_t fused;                          // the popped task is a producer that runs with this group as one unit
+    int32_t tile;                           // the tile the members read
+    int32_t fx;                             // fused: the producer's output flow, on that tile
+    int32_t mem[PB2_GROUP_MAX];
+    uint32_t k[PB2_GROUP_MAX];
+    unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
+    // fused: the producer's slice of every flow for this part
+    void* base[PB2_MAX_FLOWS];
+    uint32_t len[PB2_MAX_FLOWS];
+    uint32_t e0;
+};
+
+// All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
+// bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
+//  - k equal to the leader's: the leader's result;
+//  - the slice held nothing but the leader's constant: every element mismatches (the first element is the same);
+//  - otherwise the member's slice is counted again, exactly, as a failing CHECK counts it.
+static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const unsigned long long r0 = g.res[0];
+#pragma unroll 1
+    for (int i = 1; i < g.n; ++i) {
+        const uint32_t k = g.k[i];
+        if (k == g.k[0] || !(r0 >> 32)) {
+            if (threadIdx.x == 0) g.res[i] = k == g.k[0] ? r0 : ((unsigned long long)(s.args.bytes[0] >> 2) << 32) | (uint32_t)r0;
+            continue;
+        }
+        if (threadIdx.x == 0) s.args.iparam[0] = (int32_t)k;
+        __syncthreads();
+        const unsigned long long r = run_hbm_body(PB2_BODY_CHECK_I32, s.args, s.red);
+        if (threadIdx.x == 0) g.res[i] = r;
+        __syncthreads();
+    }
+    __syncthreads();
+}
+
+// Results of a body run chunk by chunk: the mismatch counts add up, the first element is the first chunk's.
+__device__ __forceinline__ unsigned long long chunk_sum(unsigned long long acc, unsigned long long r, uint32_t c0) {
+    if (c0 == 0 || acc == ~0ull || r == ~0ull) return c0 == 0 ? r : ~0ull;
+    return acc + (r & 0xffffffff00000000ull);
+}
+
+// Thread 0: point s.args at the chunk of every flow that starts c0 bytes into this part's slice (the flows are cut
+// alike, and the group's tile is the widest).
+static __device__ __forceinline__ void set_chunk(TaskSmem& s, const GroupSmem& g, uint32_t c0, uint32_t chunk) {
+    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
+        const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
+        s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
+        s.args.bytes[f] = rest < chunk ? rest : chunk;
+    }
+    s.args.elem0 = g.e0 + (c0 >> 2);
+}
+
+// All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
+// producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
+// writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
+// while they are still on the SM.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, at most kBulkChunk,
+// the last one ragged), and chunk i is staged in slot i % kBulkDepth of the bulk ring, which is idle while a body runs:
+//  1. the producer's staged body computes the chunk of its output flow into the slot (it reads its flows from global);
+//  2. the members check the slot, by group_results' rules, while one bulk store writes it to the tile;
+//  3. before the barrier that ends the chunk, thread 0 waits until the store that read the next chunk's slot is done.
+// So a chunk costs two barriers and no round trip through L2.  Member results are summed over the chunks (chunk_sum).
+// Tile slices are 16-byte aligned, as every body assumes; only the end of a slice (< 16 bytes) takes SIMT stores.
+// Returns the producer's result (thread 0) once every bulk store has completed and is ordered before the caller's
+// __threadfence(): successors on other SMs read the tile with generic loads.
+static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, BulkSmem* bulk, uint32_t chunk) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const int body = s.task.body;
+    if (threadIdx.x == 0) {
+        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f]; }
+        g.fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
+        g.e0 = s.args.elem0;
+        set_chunk(s, g, 0, chunk);
+    }
+    __syncthreads();
+    const uint32_t len = g.len[g.fx];
+    uint8_t* const dst = static_cast<uint8_t*>(g.base[g.fx]);
+    const uint32_t k0 = g.k[0];
+    unsigned long long acc = 0;
+    int slot_i = 0;
+#pragma unroll 1
+    for (uint32_t c0 = 0;; c0 += chunk) {
+        const uint32_t n = len - c0 < chunk ? len - c0 : chunk;       // bytes of the output flow in this chunk
+        const bool last = len - c0 <= chunk;
+        uint8_t* const slot = bulk->buf[slot_i];
+        const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, slot);
+        fence_proxy_async_smem();
+        __syncthreads();
+        // the bytes the body wrote: a tail of < 4 bytes keeps what the tile holds, except for the bodies that write bytes
+        const uint32_t nw = (body == PB2_BODY_MEMSET_U8 || body == PB2_BODY_COPY) ? n : n & ~3u;
+        const uint32_t nb = nw & ~15u;
+        if (threadIdx.x == 0 && nb) bulk_s2g(dst + c0, slot, nb);
+        if (threadIdx.x < nw - nb) __stcg(dst + c0 + nb + threadIdx.x, slot[nb + threadIdx.x]);
+        const uint32_t diff = cta_xor_scan<kShared>(slot, n, k0);
+        if (threadIdx.x == 0) {
+            bulk_wait_read<kBulkDepth - 1>();
+            if (!last) set_chunk(s, g, c0 + chunk, chunk);
+        }
+        const bool mismatch = __syncthreads_or(diff != 0u) != 0;
+        const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && n >= 4 ? *reinterpret_cast<const uint32_t*>(slot) : 0u;
+        if (!mismatch) {
+            // the chunk holds nothing but the leader's constant: every element mismatches any other constant
+            if (threadIdx.x == 0) {
+                acc = chunk_sum(acc, r, c0);
+                for (int m = 0; m < g.n; ++m)
+                    g.res[m] = chunk_sum(g.res[m], g.k[m] == k0 ? first : ((unsigned long long)(n >> 2) << 32) | first, c0);
+            }
+        } else {
+            // count again, exactly, for every constant but the leader's repeated
+            unsigned long long r0 = 0;
+#pragma unroll 1
+            for (int m = 0; m < g.n; ++m) {
+                const uint32_t k = g.k[m];
+                unsigned long long rm = r0;
+                if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne<kShared>(slot, n, k, s.red) << 32) | first;
+                if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = chunk_sum(g.res[m], rm, c0); }
+            }
+            if (threadIdx.x == 0) acc = chunk_sum(acc, r, c0);
+        }
+        if (last) break;
+        slot_i = slot_i + 1 == kBulkDepth ? 0 : slot_i + 1;
+    }
+    if (threadIdx.x == 0) {
+        bulk_wait_all0();
+        asm volatile("fence.proxy.async;" ::: "memory");
+        // the pushout that follows works on the whole slice
+        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { s.args.flow[f] = g.base[f]; s.args.bytes[f] = g.len[f]; }
+        s.args.elem0 = g.e0;
+    }
+    __syncthreads();
+    return acc;
+}
+
+// PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
+template <bool PRIO>
+__global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
+pb2_engine_hbm_kernel(WinDev w) {
+    __shared__ TaskSmem s;
+    __shared__ BulkSmem bulk;
+    __shared__ GroupSmem g;
+    if (threadIdx.x == 0) bulk_init(bulk);
+    __syncthreads();
+
+    for (;;) {
+        if (threadIdx.x == 0) {
+            const int32_t e = pop_entry<PRIO>(w);
+            if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
+            s.entry = e;
+        }
+        __syncthreads();
+        const int32_t entry = s.entry;
+        if (entry == kEmpty) break;
+        const int32_t id = w.nparts ? PB2_ENT_TASK(entry) : entry;
+        const int part = w.nparts ? PB2_ENT_PART(entry) : 0;
+        if (threadIdx.x < 4) reinterpret_cast<uint4*>(&s.task)[threadIdx.x] =
+            __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
+        {
+            const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
+            const int gn = (int)(gd & 15u);
+            const uint32_t gb = (gd & ~PB2_GROUP_FUSED) >> 4;
+            const bool fused = (gd & PB2_GROUP_FUSED) != 0;
+            if ((int)threadIdx.x < gn) {
+                const int32_t m = __ldg(&w.group_mem[gb + threadIdx.x]);
+                const pb2_task_t& mt = w.tasks[m];
+                g.mem[threadIdx.x] = m;
+                g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
+                if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
+            }
+            if (threadIdx.x == 0) {
+                g.n = gn; g.fused = fused;
+                if (part == 0 && gn && !fused) {
+                    // the members start together: consecutive event numbers, one worker
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
+                    for (int i = 0; i < gn; ++i) {
+                        const int32_t m = __ldg(&w.group_mem[gb + i]);
+                        w.start_seq[m] = seq + (uint32_t)i;
+                        w.worker[m] = (int32_t)blockIdx.x;
+                    }
+                } else if (part == 0) {
+                    w.start_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
+                    w.worker[id] = (int32_t)blockIdx.x;
+                    // a fused unit's members start when it retires (below); they run on the producer's worker
+                    for (int i = 0; i < gn; ++i) w.worker[__ldg(&w.group_mem[gb + i])] = (int32_t)blockIdx.x;
+                }
+            }
+        }
+        __syncthreads();
+        const int nparts = task_nparts(w, id);
+        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
+            return g.fused ? run_fused_part(&s, &g, &bulk, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
+        });
+        if (g.n && !g.fused) {
+            // the leader's part stored the version it saw; every member saw the same one
+            if (threadIdx.x == 0) {
+                g.res[0] = r;
+                if (part == 0) {
+                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.seen_version[(size_t)id * PB2_MAX_FLOWS]);
+                    for (int i = 1; i < g.n; ++i) w.seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
+                }
+            }
+            __syncthreads();
+            group_results(&s, &g);
+        }
+
+        if (threadIdx.x < 32) {
+            __threadfence();   // release side: the body's stores (all threads, ordered by the barrier) become
+                               // visible before any successor can observe its dependency word / ring slot
+            if (threadIdx.x == 0) {
+                const pb2_task_t& t = s.task;
+                const int gn = g.n;
+                for (int i = 0; i < gn; ++i) store_result(w, w.tasks[g.mem[i]], g.mem[i], part, nparts, g.res[i]);
+                if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
+                // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
+                int last = 1;
+                if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
+                s.window_done = 0; s.last = last;
+                if (last && gn && g.fused) {
+                    // the producer, then its members as if they had run right after it: they saw the version it
+                    // wrote; its end, their starts, their ends are consecutive events (end before start on every
+                    // edge); they retire right after it, in member order
+                    epilog_written_flows(w, t);
+                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.tiles[g.tile].version);
+                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)(1 + 2 * gn));
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)(1 + gn));
+                    w.end_seq[id] = ev;
+                    w.retire_log[seq] = id;
+                    for (int i = 0; i < gn; ++i) {
+                        const int32_t m = g.mem[i];
+                        w.seen_version[(size_t)m * PB2_MAX_FLOWS] = v;
+                        w.start_seq[m] = ev + 1u + (uint32_t)i;
+                        w.end_seq[m] = ev + 1u + (uint32_t)(gn + i);
+                        w.retire_log[seq + 1u + (uint32_t)i] = m;
+                    }
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    s.window_done = (int32_t)(seq + 1u + (uint32_t)gn) == w.ntasks ? 1 : 0;
+                    __threadfence();
+                } else if (last && gn) {
+                    // members only read their tile: no written flows; they retire back to back, in member order
+                    const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
+                    const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
+                    for (int i = 0; i < gn; ++i) { w.end_seq[g.mem[i]] = ev + (uint32_t)i; w.retire_log[seq + (uint32_t)i] = g.mem[i]; }
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    s.window_done = (int32_t)(seq + (uint32_t)gn) == w.ntasks ? 1 : 0;
+                    __threadfence();
+                } else if (last) {
+                    epilog_written_flows(w, t);
+                    w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
+                    // the retire log is written before the out-edges are released, so that it is a linear
+                    // extension of the DAG's partial order (a successor can only retire after us)
+                    s.window_done = retire_task(w, id) ? 1 : 0;
+                    __threadfence();
+                }
+            }
+            __syncwarp();
+        }
+        if (w.ps_begin != nullptr) {
+            // tiles this task wrote for readers on other GPUs go out before those readers are released
+            __syncthreads();
+            if (s.last && w.ps_begin[id + 1] > w.ps_begin[id]) push_written_tiles(w.tiles, w.ctl, w.ps_begin, w.ps, id, &bulk);
+        }
+        if (threadIdx.x < 32) {
+            if (s.last) {
+                // a fused producer's own successors first (its edge to the group is not among them), then the members'
+                if (!g.n || g.fused) { release_successors_warp<PRIO>(w, s.task); release_remote_warp(w, id); }
+                for (int i = 0; i < g.n; ++i) release_successors_warp<PRIO>(w, w.tasks[g.mem[i]]);
+            }
+            if (threadIdx.x == 0 && s.window_done) {
+                __threadfence();
+                st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// pb2_engine_prio.cu: launch the queue_policy 1 instantiation
+cudaError_t pb2_hbm_prio_launch(const WinDev& w, int nworkers, int threads, cudaStream_t stream);
+
+}  // namespace pb2

@@ -253,6 +253,8 @@ int pb2_init(pb2_context_t** pctx, int nb_cores) {
     ctx->mca["device_engine_max_workers"] = 0;
     ctx->mca["device_engine_timeout_ms"] = 0;
     ctx->mca["device_engine_gemm_mode"] = 0;
+    // 1: windows pop ready tasks by priority (JDF priority expressions, DTD insert priorities), FIFO among equals
+    ctx->mca["device_engine_queue_policy"] = 0;
     // a batch of at least _min_roots ready GPU tasks is cut into _pipeline windows of whole dependency closures:
     // while one window runs, the host builds the next one and replays the bookkeeping of the previous one
     // tiles a window has to read from pinned host memory: runs of at least this many contiguous bytes (host and
@@ -303,6 +305,7 @@ int pb2_device_cuda_module_init(pb2_context_t* ctx, int cuda_index, int dry_run,
         p.max_workers = (int32_t)ctx->mca["device_engine_max_workers"];
         p.timeout_ms = (int32_t)ctx->mca["device_engine_timeout_ms"];
         p.gemm_mode = (int32_t)ctx->mca["device_engine_gemm_mode"];
+        p.queue_policy = (int32_t)ctx->mca["device_engine_queue_policy"];
         int rc = pb2_engine_create(&d->engine, cuda_index, &p);
         if (rc != PB2_SUCCESS) { delete d; return rc; }                 // no GPU => loud failure, no fallback
         pb2_engine_info_t info;

@@ -1,5 +1,5 @@
 // pb2_sched.cuh -- device-resident scheduling state and primitives shared by the engine kernels
-// (HBM-body kernel in pb2_engine.cu, tensor-core kernel in pb2_gemm.cuh).
+// (HBM-body kernel in pb2_hbm.cuh, tensor-core kernel in pb2_gemm.cuh).
 #pragma once
 #include "../../include/pb2_engine.h"
 #include "pb2_dev_utils.cuh"
@@ -65,6 +65,25 @@ struct WinDev {
     const uint32_t*   group;
     const int32_t*    group_mem;
     uint32_t          fuse_chunk;     // bytes a fused producer writes before its group checks them (multiple of 16)
+    // queue_policy 1 (null / 0 otherwise): the ready ring is cut into priority lanes, see Lanes below
+    int32_t           nlanes;         // lanes in use (1 .. PB2_PRIO_LANES)
+    struct Lanes*     lanes;
+    const uint8_t*    lane;           // lane of each ring-entry owner: a task (HBM windows) or a unit (GEMM windows)
+};
+
+// Priority policy (queue_policy 1): PB2_PRIO_LANES FIFO lanes, lane 0 popped first.  pb2_window_create ranks the
+// distinct priorities of the window's tasks, highest first; with at most PB2_PRIO_LANES of them a value's lane is its
+// rank r (the reference's order exactly: higher priority first, FIFO among equals), otherwise floor(r * LANES / n).
+// Each lane owns a contiguous segment of the ring as long as the entries its owners can ever push, so nothing wraps
+// and head / tail are absolute ring indices.  avail counts the entries pushed and not yet claimed: a popper takes one
+// from it before it takes a head ticket, so a ticket never runs past the entries that exist.
+#define PB2_PRIO_LANES 16
+struct Lanes {
+    Line head[PB2_PRIO_LANES];        // next slot to pop
+    Line tail[PB2_PRIO_LANES];        // next slot to push
+    Line avail[PB2_PRIO_LANES];       // entries reserved by pushers and not claimed yet (may dip below 0 briefly)
+    uint32_t begin[PB2_PRIO_LANES];   // first slot of each lane's segment
+    uint32_t ninit[PB2_PRIO_LANES];   // initial ready entries at the start of each segment
 };
 
 #define PB2_GROUP_MAX 8     // members per read group (at most 15: the count is 4 bits of group[])
@@ -111,6 +130,23 @@ __device__ __forceinline__ void push_entries_warp(int32_t* ring, uint32_t cap_ma
 // scheduling primitives shared by the HBM and the GEMM engine kernels
 // ---------------------------------------------------------------------------------------------
 
+// One thread, while it finds nothing to pop: true when the window is finished (or aborted, or the watchdog trips),
+// otherwise back off.
+__device__ __forceinline__ bool pop_idle(const WinDev& w, uint32_t& spins) {
+    if (ld_relaxed_gpu(reinterpret_cast<const int32_t*>(&w.ctl->done.v)) != 0) return true;
+    if ((++spins & 1023u) == 0) {
+        // watchdog: a DAG whose dependency counts are wrong would spin forever
+        const unsigned long long last = *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v);
+        // signed: %globaltimer read on another SM can be slightly behind the value a retiring SM just stored
+        if ((long long)(globaltimer_ns() - last) > (long long)w.timeout_ns) {
+            st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneTimeout);
+            return true;
+        }
+    }
+    __nanosleep(spins < 64 ? 32 : 256);
+    return false;
+}
+
 // One thread: take the next pop ticket and wait for its slot.  Returns a task id, or kEmpty when the
 // window is finished (or aborted).  Ticket order == push order, i.e. a strict FIFO ready queue.
 __device__ __forceinline__ int32_t pop_task(const WinDev& w) {
@@ -123,23 +159,65 @@ __device__ __forceinline__ int32_t pop_task(const WinDev& w) {
 #else
     while ((id = (w.shared ? ld_acquire_sys(slot) : ld_acquire_gpu(slot))) == kEmpty) {
 #endif
-        if (ld_relaxed_gpu(reinterpret_cast<const int32_t*>(&w.ctl->done.v)) != 0) return kEmpty;
-        if ((++spins & 1023u) == 0) {
-            // watchdog: a DAG whose dependency counts are wrong would spin forever
-            const unsigned long long last = *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v);
-            // signed: %globaltimer read on another SM can be slightly behind the value a retiring SM just stored
-            if ((long long)(globaltimer_ns() - last) > (long long)w.timeout_ns) {
-                st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneTimeout);
-                return kEmpty;
-            }
-        }
-        __nanosleep(spins < 64 ? 32 : 256);
+        if (pop_idle(w, spins)) return kEmpty;
     }
     return id;
 }
 
+// One thread, queue_policy 1: claim the head entry of the first non-empty lane.  The claim is a decrement of the
+// lane's avail count that found it positive (a decrement that did not is given back), then a head ticket: the number
+// of tickets never exceeds the entries pushers have reserved, so the ticket's slot is below the tail.  The pusher
+// reserves before it stores the entry, so the slot may still have to be waited for.  (A CAS on the head while it is
+// below the tail claims the same slots, but a thousand workers polling one lane make it a retry round trip per claim:
+// 7x the FIFO time of the resident Ex05 window.)  Shared windows never get here: their peers push into one remote
+// ring (pb2_window_create refuses the combination).
+__device__ __forceinline__ int32_t pop_prio(const WinDev& w) {
+    uint32_t spins = 0;
+    for (;;) {
+        for (int l = 0; l < w.nlanes; ++l) {
+            unsigned long long* avail = &w.lanes->avail[l].v;
+            if (*reinterpret_cast<volatile long long*>(avail) <= 0) continue;
+            if ((long long)atomicAdd(avail, ~0ull) > 0) {
+                const unsigned long long h = atomicAdd(&w.lanes->head[l].v, 1ull);
+                int32_t id;
+                while ((id = ld_acquire_gpu(&w.ring[h])) == kEmpty) __nanosleep(32);
+                return id;
+            }
+            atomicAdd(avail, 1ull);
+        }
+        if (pop_idle(w, spins)) return kEmpty;
+    }
+}
+
+template <bool PRIO>
+__device__ __forceinline__ int32_t pop_entry(const WinDev& w) { return PRIO ? pop_prio(w) : pop_task(w); }
+
+// Whole warp, queue_policy 1: lanes with np > 0 push np entries into priority lane `ln`.  One tail reservation per
+// lane in use (the lanes of the warp that push into the same one are aggregated); returns this lane's first slot.
+// Out of line: inlined, it costs the HBM kernel spills at its 80-register budget.
+static __device__ __noinline__ uint32_t reserve_lane_slots(Lanes* lanes, int ln, int np) {
+    const int lane = threadIdx.x & 31;
+    const unsigned grp = __match_any_sync(0xffffffffu, np > 0 ? ln : -1);
+    const unsigned act = __ballot_sync(0xffffffffu, np > 0);
+    int pre = 0, tot = 0;
+    for (unsigned m = act; m; m &= m - 1) {
+        const int j = __ffs(m) - 1;
+        const int v = __shfl_sync(0xffffffffu, np, j);
+        if ((grp >> j) & 1u) { tot += v; if (j < lane) pre += v; }
+    }
+    const int leader = __ffs(grp) - 1;
+    unsigned long long base = 0;
+    if (np > 0 && lane == leader) {
+        base = atomicAdd(&lanes->tail[ln].v, (unsigned long long)tot);
+        atomicAdd(&lanes->avail[ln].v, (unsigned long long)tot);
+    }
+    base = __shfl_sync(0xffffffffu, base, leader);
+    return (uint32_t)base + (uint32_t)pre;
+}
+
 // Whole warp: release the out-edges of task t (parsec_release_dep_fct semantics), push the newly
 // ready successors.  Must be called after a __threadfence() that follows the body's stores.
+template <bool PRIO>
 __device__ __forceinline__ void release_successors_warp(const WinDev& w, const pb2_task_t& t) {
     const int lane = threadIdx.x & 31;
     for (int e0 = 0; e0 < t.succ_count; e0 += 32) {
@@ -166,7 +244,10 @@ __device__ __forceinline__ void release_successors_warp(const WinDev& w, const p
         int incl = nparts;
         for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
         const int total = __shfl_sync(0xffffffffu, incl, 31);
-        if (total) {
+        if (total && PRIO) {
+            const uint32_t first = reserve_lane_slots(w.lanes, nparts ? (int)w.lane[sid] : 0, nparts);
+            push_entries_warp<false>(w.ring, 0xffffffffu, sid, nparts, first);     // lanes never wrap
+        } else if (total) {
             unsigned long long base = 0;
             if (lane == 0) base = atomicAdd(&w.ctl->tail.v, (unsigned long long)total);
             base = __shfl_sync(0xffffffffu, base, 0);

@@ -175,7 +175,8 @@ def cholesky_global(NT, nb, P, Q, elem_bytes=2):
       SYRK(m,k)     READ A(m,k) x2, RW T(m,m)   m > k          <- TRSM(m,k), SYRK(m,k-1)
       GEMM(m,n,k)   READ A(m,k), B(n,k), RW C(m,n)  m > n > k  <- TRSM(m,k), TRSM(n,k), GEMM(m,n,k-1)
     GEMM-class bodies C += A * B^T on nb x nb bf16 tiles; owner of a task = rank_of(its RW tile) on a P x Q grid
-    (two_dim_rectangle_cyclic.c:281-283).  Tile id of (m,n), m >= n: m*(m+1)/2 + n.
+    (two_dim_rectangle_cyclic.c:281-283).  Tile id of (m,n), m >= n: m*(m+1)/2 + n.  Priorities as bound there:
+    POTRF 4(NT-k) > TRSM 3(NT-k) > SYRK 2(NT-k) > GEMM NT-k (used by queue_policy 1 only).
     Returns (tasks, succ, tiles, ready, task_rank, tile_rank)."""
     tid = lambda m, n: m * (m + 1) // 2 + n
     ntiles = NT * (NT + 1) // 2
@@ -214,6 +215,7 @@ def cholesky_global(NT, nb, P, Q, elem_bytes=2):
             t["tile"][i, f], t["access"][i, f] = tile, acc
         t["locals"][i, 0], t["locals"][i, 1] = m, n
         t["iparam"][i] = (nb, nb, nb) if body == L.BODY_GEMM_BF16 else (0, 0, 0)
+        t["priority"][i] = (4 * (NT - m), 3 * (NT - n), 2 * (NT - n), NT - k)[cls]     # as the PTG classes bind them
         if cls == 0:                                   # POTRF(k=m) -> TRSM(p, k) flows 0, 1
             for p in range(m + 1, NT):
                 edge(i, (1, p, m, 0), 0); edge(i, (1, p, m, 0), 1)
