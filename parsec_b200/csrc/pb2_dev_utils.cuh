@@ -141,6 +141,14 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint3
                  :: "l"(gdst), "r"(smem_addr_u32(smem_src)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
+// bulk_s2g for bytes nobody is expected to read back soon: the lines it writes are the first L2 evicts
+__device__ __forceinline__ void bulk_s2g_evict_first(void* gdst, const void* smem_src, uint32_t bytes) {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
+                 :: "l"(gdst), "r"(smem_addr_u32(smem_src)), "r"(bytes), "l"(pol) : "memory");
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+}
 // at most N bulk groups may still be reading their shared-memory source
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }

@@ -30,11 +30,11 @@ from ab_read_groups import TB, card, l2_probe, summary
 class Window:
     """One engine and one resident window of the Ex05 DAG (or of its producers alone) on it."""
 
-    def __init__(self, K, fuse_readers=0, chunk=None, fill_only=False):
+    def __init__(self, K, fuse_readers=0, chunk=None, fill_only=False, part_bytes=0):
         if chunk is not None:
             os.environ["PB2_FUSE_CHUNK_BYTES"] = str(chunk)       # read when the engine is created
         try:
-            self.e = Engine(0, fuse_readers=fuse_readers)
+            self.e = Engine(0, fuse_readers=fuse_readers, part_bytes=part_bytes)
         finally:
             os.environ.pop("PB2_FUSE_CHUNK_BYTES", None)
         dag = dags.ex05_broadcast(K, 14, TB)
