@@ -302,10 +302,13 @@ static int build_lane_ring(pb2_window_t* w, const std::vector<uint8_t>& owner_la
 // ---------------------------------------------------------------------------------------------
 // GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
-// task_lane (queue_policy 1, else null): a unit's lane is the lane of its first task.
+// task_lane (queue_policy 1, else null): a unit's lane is the lane of its first task, for all its parts.
+// part_bytes > 0: a unit that runs an HBM body (not NOP) over a tile wider than part_bytes is cut into
+// min(ceil(widest tile / part_bytes), kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.
 static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
                              const int32_t* ready, int32_t nready, bool fuse, uint32_t* ring_cap_needed,
-                             const int32_t* rs_begin, const std::vector<uint8_t>* task_lane) {
+                             const int32_t* rs_begin, const std::vector<uint8_t>* task_lane,
+                             const pb2_tile_t* tiles, int32_t part_bytes) {
     std::vector<int32_t> indeg((size_t)ntasks, 0), cpred((size_t)ntasks, -1), ccons((size_t)ntasks, 0), next((size_t)ntasks, -1);
     auto is_gemm = [&](int32_t t) { return tasks[t].body == PB2_BODY_GEMM_BF16; };
     for (int32_t u = 0; u < ntasks; ++u)
@@ -341,8 +344,16 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         const bool g = is_gemm(h);
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
-        // a part runs every nparts-th 128 x 256 sub-tile of C
-        const int nsub = g ? ((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN) : 1;
+        // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body
+        int nsub = 1;
+        if (g) nsub = ((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN);
+        else if (part_bytes > 0 && tasks[h].body != PB2_BODY_NOP) {
+            uint32_t big = 0;
+            for (int f = 0; f < tasks[h].nb_flows; ++f)
+                if (tasks[h].tile[f] >= 0) big = std::max(big, tiles[tasks[h].tile[f]].bytes);
+            nsub = (int)std::min<uint32_t>((big + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes, (uint32_t)gemm::kMaxParts);
+            nsub = std::max(nsub, 1);
+        }
         u.nparts = std::min(nsub, gemm::kMaxParts);
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
@@ -850,9 +861,13 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     w->nready_entries = (int32_t)entries.size();
     uint32_t parts_needed = 0;
     if (kind == 1) {
+        // HBM bodies of a GEMM window are cut into parts as HBM windows cut them.  Not in shared windows: their units
+        // are released by peers over NVLink, and the multi-GPU runs that check those releases cover single-part HBM
+        // units only, so shared windows keep one part per HBM unit.
+        const int32_t hbm_part_bytes = w->shared ? 0 : e->params.part_bytes;
         TRY(build_tensor_maps(w, tasks, ntasks, tiles, ntiles));
         TRY(build_gemm2_units(w, tasks, ntasks, succ, ready, nready, e->params.gemm_mode == 0, &parts_needed,
-                              w->shared ? e->next_rs_begin : nullptr, prio ? &task_lane : nullptr));
+                              w->shared ? e->next_rs_begin : nullptr, prio ? &task_lane : nullptr, tiles, hbm_part_bytes));
     }
     const int maxw = e->nworkers > e->nworkers_gemm ? e->nworkers : e->nworkers_gemm;
     uint32_t cap = 1024;

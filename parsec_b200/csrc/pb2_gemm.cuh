@@ -17,6 +17,9 @@
 // Members still retire one by one, in chain order, with their own sequence numbers, versions and out-edges (the
 // dependency trace is unchanged); only the intermediate bf16 roundings of C disappear.  Scheduling entities on the
 // device are units (counter-mode dependency words), ring entries are (part, unit).
+// The other tasks of the DAG (HBM bodies: FILL, SCALE, COPY, AXPY, CHECK, ... between the chains) are units of one
+// task; one wider than part_bytes is cut into byte-slice parts like a wide task of an HBM window, each run by a whole
+// CTA, and the last part to finish retires it.
 //
 // One CTA per SM is one worker.  Three warpgroups (384 threads):
 //   warpgroup 0 : warp 0 retires a unit and releases its out-edges; one lane of warp 1 is the TMA producer
@@ -28,6 +31,7 @@
 #pragma once
 #include <cuda.h>
 #include "pb2_sched.cuh"
+#include "pb2_worker.cuh"
 
 namespace pb2 {
 
@@ -197,7 +201,8 @@ struct GUnit {                  // 48 bytes, read-only
     int32_t seg_begin, seg_count;   // members, in chain order
     int32_t succ_begin, succ_count; // out-edges of all members (chain links removed): target unit ids
     int32_t dep_goal;               // in-edges from other units
-    int32_t nparts;                 // ring entries: min(sub-tiles of C, kMaxParts) for GEMM units, 1 otherwise
+    int32_t nparts;                 // ring entries: min(sub-tiles of C, kMaxParts) for GEMM units; for an HBM body
+                                    // min(ceil(widest tile / part_bytes), kMaxParts) byte slices (1 in shared windows)
     int32_t tileC;                  // GEMM units: the C tile; -1 otherwise
     int32_t M, N, K;
     int32_t flags;                  // bit0 is_gemm, bit1 pushout C
@@ -231,6 +236,8 @@ struct Job {
 struct Shared {
     alignas(16) Job job;
     alignas(16) pb2_task_t task;    // non-GEMM units: the single member's descriptor
+    uint32_t off[PB2_MAX_FLOWS];    // non-GEMM units: this part's byte slice of every flow
+    uint32_t len[PB2_MAX_FLOWS];
     uint64_t full[kStages];
     uint64_t empty[kStages];
     int32_t  need, decide;
@@ -386,12 +393,34 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                     __ldg(reinterpret_cast<const uint4*>(&w.tasks[s.task]) + threadIdx.x);
                 __syncthreads();
                 const pb2_task_t& t = sh.task;
+                if (threadIdx.x == 0) {
+                    // every flow is cut at the offsets of the widest one, as the HBM kernel cuts its parts (part_slice)
+                    uint32_t bytes[PB2_MAX_FLOWS], widest = 0;
+                    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
+                        bytes[f] = (f < t.nb_flows && t.tile[f] >= 0) ? w.tiles[t.tile[f]].bytes : 0u;
+                        widest = bytes[f] > widest ? bytes[f] : widest;
+                    }
+                    for (int f = 0; f < PB2_MAX_FLOWS; ++f)
+                        part_slice(widest, (uint32_t)sh.job.nparts, (uint32_t)sh.job.part, bytes[f], sh.off[f], sh.len[f]);
+                }
+                __syncthreads();
                 for (int f = 0; f < t.nb_flows; ++f) {
                     if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_ACCESS_READ)) continue;
                     pb2_tile_t* tile = &w.tiles[t.tile[f]];
                     if (threadIdx.x == 0) sh.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
                     __syncthreads();
-                    if (sh.need) { stage_in_flow(stage_ctx(w), tile, t.access[f], &sh.decide); fence_proxy_async(); }
+                    if (sh.need) {
+                        // a sliced tile (the rule the GEMM units stage by) is pulled slice by slice: this part takes
+                        // the slices over its bytes that nobody has claimed and waits for the others
+                        const int ns = tile_slices(w, tile->bytes);
+                        if (ns == 1) stage_in_flow(stage_ctx(w), tile, t.access[f], &sh.decide);
+                        else {
+                            int s0, s1;
+                            slices_over(tile->bytes, ns, sh.off[f], sh.len[f], s0, s1);
+                            stage_in_slices(stage_ctx(w), t.tile[f], ns, s0, s1, &sh.decide);
+                        }
+                        fence_proxy_async();
+                    }
                     __syncthreads();
                 }
             }
@@ -451,27 +480,30 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 fence_proxy_async();
             }
         } else {
-            // ---------------- a non-GEMM member of the DAG (e.g. a panel stand-in): the whole CTA runs it in place
+            // ---------------- an HBM body in the DAG (element-wise task, panel stand-in): the whole CTA runs this
+            // part's byte slice of its flows in place
             const pb2_task_t& t = sh.task;
             BodyArgs a;
             for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
                 const bool has = f < t.nb_flows && t.tile[f] >= 0;
-                a.flow[f] = has ? w.tiles[t.tile[f]].dev_ptr : nullptr;
-                a.bytes[f] = has ? w.tiles[t.tile[f]].bytes : 0;
+                a.flow[f] = has ? reinterpret_cast<uint8_t*>(w.tiles[t.tile[f]].dev_ptr) + sh.off[f] : nullptr;
+                a.bytes[f] = has ? sh.len[f] : 0u;
             }
-            a.elem0 = 0; a.part = 0;
+            a.elem0 = sh.off[0] >> 2; a.part = (uint32_t)job.part;
             a.iparam[0] = t.iparam[0]; a.iparam[1] = t.iparam[1]; a.iparam[2] = t.iparam[2]; a.fparam = t.fparam;
             const unsigned long long r = run_hbm_body(t.body, a, sh.red);
-            if (threadIdx.x == 0) {
-                w.result[g.segs[job.seg_begin].task] = r;
-                if ((t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) && (r >> 32)) atomicAdd(&w.ctl->body_errors.v, r >> 32);
-            }
+            // CHECK parts add their mismatch counts; the first element comes from part 0
+            if (threadIdx.x == 0) store_result(w, t, g.segs[job.seg_begin].task, job.part, job.nparts, r);
             fence_proxy_async();
+            // the pushout's threads do not read the bytes each wrote (a host copy that is only 4- or 1-byte aligned
+            // takes the narrow copy loops): every store of the body is done before any of them reads
+            __syncthreads();
             for (int f = 0; f < t.nb_flows; ++f)
                 if (t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
                     pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                    cta_copy<false>(tile->src_ptr, tile->dev_ptr, tile->bytes);
-                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)tile->bytes);
+                    cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + sh.off[f],
+                                    reinterpret_cast<const uint8_t*>(tile->dev_ptr) + sh.off[f], sh.len[f]);
+                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)sh.len[f]);
                 }
         }
         __threadfence();

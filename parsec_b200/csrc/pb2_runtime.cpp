@@ -905,17 +905,16 @@ static bool predicted_on_device(pb2_device_module_t* dev, pb2_htask_t* s) {
     return true;   // no affinity: stays with its predecessor's device
 }
 
-// Build the dependency-closed window reachable from the pending tasks of one taskpool.
+// Build the dependency-closed window reachable from the pending tasks of one taskpool.  An engine window takes tile
+// GEMMs and HBM bodies together, so that a GEMM chain and the element-wise tasks around it are released on the device
+// instead of through the host; its kind is decided by the closure: 1 (the GEMM kernel, which also runs HBM bodies) when
+// it holds a GEMM task, else 0.  User submit tasks never mix with engine tasks.
 static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu_task_t*>& taken, size_t max_roots) {
     if (dev->pending.empty()) return PB2_SUCCESS;
     w.tp = dev->pending.front()->ec->tp;
-    const bool want_gemm = dev->pending.front()->ec->body == PB2_BODY_GEMM_BF16;
     const bool want_user = dev->pending.front()->ec->body == PB2_BODY_USER;      // the host-driven stream lane
-    w.kind = want_user ? 2 : (want_gemm ? 1 : 0);
-    auto fits = [&](const pb2_htask_t* t) {
-        if (want_user || t->body == PB2_BODY_USER) return want_user && t->body == PB2_BODY_USER;
-        return (t->body == PB2_BODY_GEMM_BF16) == want_gemm || t->body == PB2_BODY_NOP;
-    };
+    auto fits = [&](const pb2_htask_t* t) { return (t->body == PB2_BODY_USER) == want_user; };
+    bool has_gemm = false;
     std::deque<pb2_htask_t*> queue;
     std::deque<pb2_gpu_task_t*> keep;
     for (pb2_gpu_task_t* g : dev->pending) {
@@ -927,8 +926,9 @@ static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu
     bool full = false;
     while (!queue.empty()) {
         pb2_htask_t* t = queue.front(); queue.pop_front();
-        // the ready-ring entries of an HBM window carry a 22-bit task id: a larger closure goes into the next window
-        if (w.kind == 0 && w.tasks.size() + 1 >= ((size_t)1 << 22)) full = true;
+        // the ready-ring entries of an HBM window carry a 22-bit task id: a larger closure without a GEMM task (which
+        // would make it a GEMM window, whose entries carry 27-bit unit ids) goes on in the next window
+        if (!want_user && !has_gemm && w.order.size() + 1 >= ((size_t)1 << 22)) full = true;
         bool ok = !full;
         std::vector<pb2_data_copy_t*> fresh;
         if (ok) {
@@ -958,6 +958,7 @@ static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu
         }
         t->window_index = (int32_t)w.order.size();
         w.order.push_back(t);
+        has_gemm |= t->body == PB2_BODY_GEMM_BF16;
         for (uint32_t s : t->succ) {
             pb2_htask_t* n = &w.tp->tasks[PB2_SUCC_TASK(s)];
             if (n->inwin_pred == 0) touched.push_back(n);
@@ -967,6 +968,7 @@ static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu
         }
     }
     for (pb2_htask_t* n : touched) n->inwin_pred = 0;
+    w.kind = want_user ? 2 : (has_gemm ? 1 : 0);
     if (full) {      // tasks that were handed over but did not fit stay pending, in their arrival order
         std::vector<pb2_gpu_task_t*> in;
         for (pb2_gpu_task_t* g : taken) { if (g->ec->window_index >= 0) in.push_back(g); else dev->pending.push_back(g); }

@@ -103,6 +103,27 @@ struct alignas(32) PushDev { void* dst; int32_t* dst_state; uint32_t bytes; int3
 
 __device__ __forceinline__ int task_nparts(const WinDev& w, int32_t id) { return w.nparts ? (int)w.nparts[id] : 1; }
 
+// The byte slice [off, off + len) of a flow of `bytes` bytes that part `part` of `nparts` runs.  Every flow of a task is
+// cut at the offsets of its widest flow (16-byte aligned, the last part takes the remainder), so two-flow bodies pair
+// equal offsets.  Both engine kernels cut their wide HBM bodies with it.
+__device__ __forceinline__ void part_slice(uint32_t widest, uint32_t nparts, uint32_t part, uint32_t bytes,
+                                           uint32_t& off, uint32_t& len) {
+    const uint32_t per = ((widest / nparts) + 15u) & ~15u;
+    off = per * part < bytes ? per * part : bytes;
+    len = (part == nparts - 1) ? bytes - off : (off + per <= bytes ? per : bytes - off);
+}
+
+// The stage-in slices [s0, s1) that cover the bytes [off, off + len) of a tile of `bytes` bytes cut into ns slices
+// (stage_in_slices cuts the same way).  A part may be cut differently from the tile when its widest flow is another tile.
+__device__ __forceinline__ void slices_over(uint32_t bytes, int ns, uint32_t off, uint32_t len, int& s0, int& s1) {
+    const uint32_t sper = ((bytes / (uint32_t)ns) + 15u) & ~15u;
+    s0 = (int)(off / sper);
+    s1 = (int)((off + len + sper - 1) / sper);
+    if (s0 > ns - 1) s0 = ns - 1;
+    if (s1 > ns) s1 = ns;
+    if (len == 0) s1 = s0;
+}
+
 // Whole warp: lanes with np > 0 own a ready task `sid` whose entries go to ring[first .. first + np).  Tasks with
 // hundreds of parts are written by all 32 lanes together.
 template <bool SYS>

@@ -37,14 +37,8 @@ static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, Task
         const int ns = tile_slices_of(c.part_bytes, c.slice_claim, bytes);
         if (ns == 1) stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, bulk);
         else {
-            // slices [s0, s1) of the tile cover this part's bytes (the task may be cut differently from the tile
-            // when its widest flow is another tile)
-            const uint32_t sper = ((bytes / (uint32_t)ns) + 15u) & ~15u;
-            const uint32_t off = s.off[f], len = s.args.bytes[f];
-            int s0 = (int)(off / sper), s1 = (int)((off + len + sper - 1) / sper);
-            if (s0 > ns - 1) s0 = ns - 1;
-            if (s1 > ns) s1 = ns;
-            if (len == 0) s1 = s0;
+            int s0, s1;
+            slices_over(bytes, ns, s.off[f], s.args.bytes[f], s0, s1);     // the slices under this part's bytes
             stage_in_slices(c, tid, ns, s0, s1, &s.decide, bulk);
         }
     }
@@ -62,16 +56,14 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
         const bool mine = f < PB2_MAX_FLOWS && f < (int)t.nb_flows && t.tile[f < PB2_MAX_FLOWS ? f : 0] >= 0;
         pb2_tile_t* tile = mine ? &w.tiles[t.tile[f]] : nullptr;
         const uint32_t bytes = mine ? tile->bytes : 0u;
-        // every flow is cut at the same byte offsets (those of the task's widest tile, 16-byte aligned, the last
-        // part takes the remainder), so two-flow bodies pair equal offsets
+        // every flow is cut at the offsets of the task's widest tile (part_slice)
         uint32_t widest = bytes;
         for (int o = 1; o < PB2_MAX_FLOWS; o <<= 1) {
             const uint32_t v = __shfl_xor_sync(0xffffffffu, widest, o);
             widest = v > widest ? v : widest;
         }
-        const uint32_t per = ((widest / (uint32_t)nparts) + 15u) & ~15u;
-        const uint32_t off = per * (uint32_t)part < bytes ? per * (uint32_t)part : bytes;
-        const uint32_t len = (part == nparts - 1) ? bytes - off : (off + per <= bytes ? per : bytes - off);
+        uint32_t off, len;
+        part_slice(widest, (uint32_t)nparts, (uint32_t)part, bytes, off, len);
         const bool need = mine && (t.access[f] & PB2_FLOW_ACCESS_READ) && ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
         const unsigned needmask = __ballot_sync(0xffffffffu, need);
         if (f < PB2_MAX_FLOWS) {
