@@ -127,7 +127,7 @@ typedef struct pb2_tile_s {
 #define PB2_TILE_VALID     2   /* SHARED/OWNED + COMPLETE_TRANSFER                                           */
 
 typedef struct pb2_engine_params_s {
-    int32_t  workers_per_sm;   /* CTAs per SM for HBM-body windows (default 12, at most what the kernel's occupancy allows) */
+    int32_t  workers_per_sm;   /* CTAs per SM for HBM-body windows (default 8, at most what the kernel's occupancy allows: 12) */
     int32_t  threads;          /* threads per CTA for HBM-body windows (default and maximum 64)               */
     int32_t  max_workers;      /* 0 = all; 1 = single worker => deterministic FIFO order (tests)             */
     int32_t  stage_mode;       /* tile mover of the HBM-body kernels: 0 = TMA bulk copy (cp.async.bulk through a

@@ -2,8 +2,8 @@
 //
 // Each body is executed by one whole CTA (the "worker") over one tile.  All payload
 // accesses are 16-byte, fully coalesced, L1-bypassing (ld.global.cg / st.global.cg) with
-// UNROLL independent requests in flight per thread (a staged body writes a shared-memory slot instead, see
-// run_hbm_body<true>); ragged tails (bytes % 16, bytes % 4)
+// UNROLL independent requests in flight per thread (the checked form of a producer, run_hbm_body<true>, also compares
+// every value it stores with a constant, and stores with an L2 evict-first policy); ragged tails (bytes % 16, bytes % 4)
 // are handled by scalar epilogues so empty and odd-sized tiles are legal.
 //
 // Reference bodies these restate (the reference ships them as toy <<<1,1>>> kernels or CPU code):
@@ -22,13 +22,28 @@ namespace pb2 {
 #endif
 constexpr int kUnroll = PB2_UNROLL;
 
+// What the checked form of a producer body (run_fused_part) does besides storing: every element it stores is compared
+// with the group leader's constant k, and the stores carry the L2 evict-first policy `pol` (the group never reads the
+// tile back).
+struct Checked {
+    uint32_t k;
+    uint32_t diff;      // OR of (element ^ k) over the elements this thread stored: 0 iff all of them equal k
+    uint64_t pol;
+};
+
 // f(uint4& v, uint32_t first_elem_index) ; elements are 4-byte lanes x,y,z,w, read from src (READ) and written to dst
-// (WRITE) at the same offsets; SRC / DST say which memory each is in.  Tiles are below 4 GiB (pb2_tile_t::bytes is
-// 32-bit), so all indices are 32-bit: half the address registers of a size_t loop.
-template <bool READ, bool WRITE, Space SRC = kGlobal, Space DST = kGlobal, class F>
-__device__ __forceinline__ void cta_vec_loop(const void* src, void* dst, uint32_t bytes, F f) {
+// (WRITE) at the same offsets.  CHECKED: the stores go through ck (WRITE implied).  Tiles are below 4 GiB
+// (pb2_tile_t::bytes is 32-bit), so all indices are 32-bit: half the address registers of a size_t loop.
+template <bool READ, bool WRITE, bool CHECKED = false, class F>
+__device__ __forceinline__ void cta_vec_loop(const void* src, void* dst, uint32_t bytes, F f, Checked* ck = nullptr) {
     const uint4* p = reinterpret_cast<const uint4*>(src);
     uint4* q = reinterpret_cast<uint4*>(dst);
+    auto store = [&](uint32_t i, const uint4& v) {
+        if (CHECKED) {
+            ck->diff |= ((v.x ^ ck->k) | (v.y ^ ck->k)) | ((v.z ^ ck->k) | (v.w ^ ck->k));
+            st_v4_policy(q + i, v, ck->pol);
+        } else if (WRITE) st_stream(q + i, v);
+    };
     const uint32_t nvec = bytes >> 4;
     const uint32_t tid = threadIdx.x, nt = blockDim.x;
     const uint32_t per_iter = nt * kUnroll;
@@ -37,30 +52,31 @@ __device__ __forceinline__ void cta_vec_loop(const void* src, void* dst, uint32_
         uint4 v[kUnroll];
 #pragma unroll
         for (int j = 0; j < kUnroll; ++j) {
-            if (READ) v[j] = ld_v4<SRC>(p + (base + j * nt + tid));
+            if (READ) v[j] = ld_stream(p + (base + j * nt + tid));
             else      v[j] = make_uint4(0, 0, 0, 0);
         }
 #pragma unroll
         for (int j = 0; j < kUnroll; ++j) {
             f(v[j], (base + j * nt + tid) * 4u);
-            if (WRITE) st_v4<DST>(q + (base + j * nt + tid), v[j]);
+            store(base + j * nt + tid, v[j]);
         }
     }
     for (uint32_t i = base + tid; i < nvec; i += nt) {
-        uint4 v = READ ? ld_v4<SRC>(p + i) : make_uint4(0, 0, 0, 0);
+        uint4 v = READ ? ld_stream(p + i) : make_uint4(0, 0, 0, 0);
         f(v, i * 4u);
-        if (WRITE) st_v4<DST>(q + i, v);
+        store(i, v);
     }
     // scalar 4-byte tail (bytes not a multiple of 16)
     const uint32_t nelem = bytes >> 2;
     const uint32_t* e = reinterpret_cast<const uint32_t*>(src);
     uint32_t* o = reinterpret_cast<uint32_t*>(dst);
     for (uint32_t i = (nvec << 2) + tid; i < nelem; i += nt) {
-        uint4 v = make_uint4(READ ? ld_u32<SRC>(e + i) : 0u, 0, 0, 0);
-        // present the single element in lane x only; f must treat y,z,w as don't-care here
+        uint4 v = make_uint4(READ ? __ldcg(e + i) : 0u, 0, 0, 0);
+        // present the single element in lane x only; f must treat y,z,w as don't-care here (and the check ignores them)
         uint4 w = v;
         f(w, i);
-        if (WRITE) st_u32<DST>(o + i, w.x);
+        if (CHECKED) { ck->diff |= w.x ^ ck->k; st_u32_policy(o + i, w.x, ck->pol); }
+        else if (WRITE) __stcg(o + i, w.x);
     }
 }
 
@@ -137,7 +153,6 @@ __device__ __forceinline__ void cta_copy(void* dst, const void* src, size_t byte
 #endif
 // OR over the slice of (element ^ k): zero iff every 4-byte element equals k.  Read-only, 16-byte loads,
 // PB2_CHECK_UNROLL independent requests per thread in flight.
-template <Space S = kGlobal>
 __device__ __forceinline__ uint32_t cta_xor_scan(const void* ptr, uint32_t bytes, uint32_t k) {
     const uint4* p = reinterpret_cast<const uint4*>(ptr);
     const uint32_t nvec = bytes >> 4, tid = threadIdx.x, nt = blockDim.x;
@@ -146,16 +161,16 @@ __device__ __forceinline__ uint32_t cta_xor_scan(const void* ptr, uint32_t bytes
     for (; i + (U - 1) * nt < nvec; i += U * nt) {
         uint4 v[U];
 #pragma unroll
-        for (uint32_t j = 0; j < U; ++j) v[j] = ld_v4<S>(p + i + j * nt);
+        for (uint32_t j = 0; j < U; ++j) v[j] = ld_stream(p + i + j * nt);
 #pragma unroll
         for (uint32_t j = 0; j < U; ++j) diff |= ((v[j].x ^ k) | (v[j].y ^ k)) | ((v[j].z ^ k) | (v[j].w ^ k));
     }
     for (; i < nvec; i += nt) {
-        const uint4 v = ld_v4<S>(p + i);
+        const uint4 v = ld_stream(p + i);
         diff |= ((v.x ^ k) | (v.y ^ k)) | ((v.z ^ k) | (v.w ^ k));
     }
     const uint32_t* e = reinterpret_cast<const uint32_t*>(ptr);
-    for (uint32_t j = (nvec << 2) + tid; j < (bytes >> 2); j += nt) diff |= ld_u32<S>(e + j) ^ k;
+    for (uint32_t j = (nvec << 2) + tid; j < (bytes >> 2); j += nt) diff |= __ldcg(e + j) ^ k;
     return diff;
 }
 
@@ -175,11 +190,10 @@ __device__ __forceinline__ uint32_t cta_reduce_sum(uint32_t v, uint32_t* smem) {
 }
 
 // The number of 4-byte elements of the slice that differ from k, counted exactly; result valid in thread 0.
-template <Space S = kGlobal>
 __device__ __forceinline__ uint32_t cta_count_ne(const void* ptr, uint32_t bytes, uint32_t k, uint32_t* red_smem) {
     uint32_t bad = 0;
     const uint32_t nvec_elems = (bytes >> 4) << 2;
-    cta_vec_loop<true, false, S, S>(ptr, nullptr, bytes, [&](uint4& v, uint32_t i) {
+    cta_vec_loop<true, false>(ptr, nullptr, bytes, [&](uint4& v, uint32_t i) {
         if (i < nvec_elems) bad += (v.x != k) + (v.y != k) + (v.z != k) + (v.w != k);
         else                bad += (v.x != k);
     });
@@ -196,38 +210,37 @@ struct BodyArgs {
 };
 
 // Returns the body result (only meaningful in thread 0): CHECK -> (mismatches << 32) | first element bits.
-// STAGED: the staged form of a producer that runs with its read group as one unit (run_fused_part, pb2_engine.cu).  The
-// body reads its flows from global memory as usual, but the bytes it would write to its output flow (flow 1 for COPY and
-// AXPY, else flow 0) go to `slot` in shared memory, at the same offsets.  Bodies without a staged form (NOP, CHECK,
-// ADD_AT) return ~0 there; form_read_groups fuses none of them.
-template <bool STAGED = false>
-__device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, uint32_t* red_smem, void* slot = nullptr) {
-    constexpr Space D = STAGED ? kShared : kGlobal;
-    void* const out = STAGED ? slot : a.flow[0];     // where flow 0's bytes are written
+// CHECKED: the checked form of a producer that runs with its read group as one unit (run_fused_part, pb2_hbm.cuh).  The
+// body writes its output flow (flow 1 for COPY and AXPY, else flow 0) as the unchecked form does, through ck: each
+// thread ORs (element ^ ck->k) of every whole 4-byte element it stores into ck->diff (a byte tail, MEMSET's or COPY's,
+// is stored but not checked, as cta_xor_scan does not check it).  Bodies without a checked form (NOP, CHECK, ADD_AT)
+// return ~0 there; form_read_groups fuses none of them.
+template <bool CHECKED = false>
+__device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, uint32_t* red_smem, Checked* ck = nullptr) {
     switch (body) {
     case PB2_BODY_NOP:
-        return STAGED ? ~0ull : 0;
+        return CHECKED ? ~0ull : 0;
     case PB2_BODY_FILL_I32: {
         const uint32_t k = (uint32_t)a.iparam[0];
-        cta_vec_loop<false, true, kGlobal, D>(out, out, a.bytes[0], [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); });
+        cta_vec_loop<false, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); }, ck);
         return 0;
     }
     case PB2_BODY_FILL_F32: {
         const uint32_t k = __float_as_uint(a.fparam);
-        cta_vec_loop<false, true, kGlobal, D>(out, out, a.bytes[0], [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); });
+        cta_vec_loop<false, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); }, ck);
         return 0;
     }
     case PB2_BODY_MEMSET_U8: {
         const uint32_t b = (uint32_t)a.iparam[0] & 0xffu;
         const uint32_t k = b | (b << 8) | (b << 16) | (b << 24);
-        cta_vec_loop<false, true, kGlobal, D>(out, out, a.bytes[0] & ~3u, [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); });
-        unsigned char* db = reinterpret_cast<unsigned char*>(out);
+        cta_vec_loop<false, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0] & ~3u, [k](uint4& v, uint32_t) { v = make_uint4(k, k, k, k); }, ck);
+        unsigned char* db = reinterpret_cast<unsigned char*>(a.flow[0]);
         for (size_t i = (a.bytes[0] & ~3u) + threadIdx.x; i < a.bytes[0]; i += blockDim.x) db[i] = (unsigned char)b;
         return 0;
     }
     case PB2_BODY_CHECK_I32:
     case PB2_BODY_CHECK_F32: {
-        if (STAGED) return ~0ull;
+        if (CHECKED) return ~0ull;
         const uint32_t k = (body == PB2_BODY_CHECK_I32) ? (uint32_t)a.iparam[0] : __float_as_uint(a.fparam);
         // Fast path: OR of (element ^ k) over the slice -- three LOP3 per 16 bytes, no predicates, no per-thread count.
         // A slice with a mismatch (the exception) is counted exactly by a second, slower pass.
@@ -239,43 +252,43 @@ __device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, ui
     }
     case PB2_BODY_INCR_I32: {
         const uint32_t k = (uint32_t)a.iparam[0];
-        cta_vec_loop<true, true, kGlobal, D>(a.flow[0], out, a.bytes[0], [k](uint4& v, uint32_t) { v.x += k; v.y += k; v.z += k; v.w += k; });
+        cta_vec_loop<true, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [k](uint4& v, uint32_t) { v.x += k; v.y += k; v.z += k; v.w += k; }, ck);
         return 0;
     }
     case PB2_BODY_SCALE_I32: {
         const int32_t k = a.iparam[0];
-        cta_vec_loop<true, true, kGlobal, D>(a.flow[0], out, a.bytes[0], [k](uint4& v, uint32_t) {
+        cta_vec_loop<true, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [k](uint4& v, uint32_t) {
             v.x = (uint32_t)((int32_t)v.x * k); v.y = (uint32_t)((int32_t)v.y * k);
             v.z = (uint32_t)((int32_t)v.z * k); v.w = (uint32_t)((int32_t)v.w * k);
-        });
+        }, ck);
         return 0;
     }
     case PB2_BODY_ADD_IOTA_I32: {
         const uint32_t e0 = a.elem0;
-        cta_vec_loop<true, true, kGlobal, D>(a.flow[0], out, a.bytes[0], [e0](uint4& v, uint32_t i) {
+        cta_vec_loop<true, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [e0](uint4& v, uint32_t i) {
             const uint32_t j = e0 + i;
             v.x += j; v.y += j + 1; v.z += j + 2; v.w += j + 3;
-        });
+        }, ck);
         return 0;
     }
     case PB2_BODY_IOTA_I32: {
         const uint32_t e0 = a.elem0;
-        cta_vec_loop<false, true, kGlobal, D>(out, out, a.bytes[0], [e0](uint4& v, uint32_t i) {
+        cta_vec_loop<false, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [e0](uint4& v, uint32_t i) {
             const uint32_t j = e0 + i;
             v = make_uint4(j, j + 1, j + 2, j + 3);
-        });
+        }, ck);
         return 0;
     }
     case PB2_BODY_INCR_F32: {
         const float k = a.fparam;
-        cta_vec_loop<true, true, kGlobal, D>(a.flow[0], out, a.bytes[0], [k](uint4& v, uint32_t) {
+        cta_vec_loop<true, true, CHECKED>(a.flow[0], a.flow[0], a.bytes[0], [k](uint4& v, uint32_t) {
             v.x = __float_as_uint(__uint_as_float(v.x) + k); v.y = __float_as_uint(__uint_as_float(v.y) + k);
             v.z = __float_as_uint(__uint_as_float(v.z) + k); v.w = __float_as_uint(__uint_as_float(v.w) + k);
-        });
+        }, ck);
         return 0;
     }
     case PB2_BODY_ADD_AT_I32: {
-        if (STAGED) return ~0ull;
+        if (CHECKED) return ~0ull;
         const long long rel = (long long)a.iparam[0] - (long long)a.elem0;     // the element may live in another part
         if (threadIdx.x == 0 && rel >= 0 && (size_t)rel * 4 + 4 <= a.bytes[0]) {
             uint32_t* e = reinterpret_cast<uint32_t*>(a.flow[0]) + rel;
@@ -285,12 +298,12 @@ __device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, ui
     }
     case PB2_BODY_COPY: {
         const uint32_t n = a.bytes[0] < a.bytes[1] ? a.bytes[0] : a.bytes[1];
-        if (!STAGED) { cta_copy<false>(a.flow[1], a.flow[0], n); return 0; }
-        // cta_copy would move the bytes through the bulk ring that holds the slot
-        cta_vec_loop<true, true, kGlobal, kShared>(a.flow[0], slot, n, [](uint4&, uint32_t) {});
+        if (!CHECKED) { cta_copy<false>(a.flow[1], a.flow[0], n); return 0; }
+        // through registers, where the check sees the bytes (cta_copy's bulk path never has them there)
+        cta_vec_loop<true, true, true>(a.flow[0], a.flow[1], n, [](uint4&, uint32_t) {}, ck);
         const unsigned char* sb = reinterpret_cast<const unsigned char*>(a.flow[0]);
-        unsigned char* db = reinterpret_cast<unsigned char*>(slot);
-        for (uint32_t i = (n & ~3u) + threadIdx.x; i < n; i += blockDim.x) db[i] = __ldcg(sb + i);
+        unsigned char* db = reinterpret_cast<unsigned char*>(a.flow[1]);
+        for (uint32_t i = (n & ~3u) + threadIdx.x; i < n; i += blockDim.x) __stcg(db + i, __ldcg(sb + i));
         return 0;
     }
     case PB2_BODY_AXPY_F32: {
@@ -299,7 +312,7 @@ __device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, ui
         const uint32_t* xe = reinterpret_cast<const uint32_t*>(a.flow[0]);
         const uint32_t n = a.bytes[0] < a.bytes[1] ? a.bytes[0] : a.bytes[1];
         const uint32_t nvec_elems = (n >> 4) << 2;
-        cta_vec_loop<true, true, kGlobal, D>(a.flow[1], STAGED ? slot : a.flow[1], n, [&](uint4& v, uint32_t i) {
+        cta_vec_loop<true, true, CHECKED>(a.flow[1], a.flow[1], n, [&](uint4& v, uint32_t i) {
             if (i < nvec_elems) {
                 const uint4 xv = ld_stream(x + (i >> 2));
                 v.x = __float_as_uint(fmaf(k, __uint_as_float(xv.x), __uint_as_float(v.x)));
@@ -309,7 +322,7 @@ __device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, ui
             } else {
                 v.x = __float_as_uint(fmaf(k, __uint_as_float(__ldcg(xe + i)), __uint_as_float(v.x)));
             }
-        });
+        }, ck);
         return 0;
     }
     default:

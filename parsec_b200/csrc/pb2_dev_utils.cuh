@@ -59,6 +59,21 @@ __device__ __forceinline__ uint4 ld_remote(const uint4* p) {
     return r;
 }
 
+// Stores of bytes nobody is expected to read back soon (a fused unit's tile, checked on the SM before it is stored):
+// with the policy of l2_evict_first() the lines they write are the first L2 evicts.
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void st_v4_policy(uint4* p, const uint4& v, uint64_t pol) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;"
+                 :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_u32_policy(uint32_t* p, uint32_t v, uint64_t pol) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.u32 [%0], %1, %2;" :: "l"(p), "r"(v), "l"(pol) : "memory");
+}
+
 __device__ __forceinline__ uint32_t lanemask_lt() {
     uint32_t m;
     asm volatile("mov.u32 %0, %lanemask_lt;" : "=r"(m));
@@ -99,32 +114,6 @@ struct alignas(128) BulkSmem {
 
 __device__ __forceinline__ uint32_t smem_addr_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// Where a body's payload lives: a tile in global memory (the streaming accesses above), or a staging slot in this CTA's
-// shared memory (a fused unit stages each chunk in a BulkSmem slot, pb2_engine.cu).  Shared accesses go through the
-// shared window explicitly: the slot reaches the bodies as a generic pointer.
-enum Space { kGlobal, kShared };
-template <Space S> __device__ __forceinline__ uint4 ld_v4(const uint4* p) {
-    if (S == kGlobal) return ld_stream(p);
-    uint4 r;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(smem_addr_u32(p)) : "memory");
-    return r;
-}
-template <Space S> __device__ __forceinline__ void st_v4(uint4* p, const uint4& v) {
-    if (S == kGlobal) { st_stream(p, v); return; }
-    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" :: "r"(smem_addr_u32(p)), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-template <Space S> __device__ __forceinline__ uint32_t ld_u32(const uint32_t* p) {
-    if (S == kGlobal) return __ldcg(p);
-    uint32_t r;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(r) : "r"(smem_addr_u32(p)) : "memory");
-    return r;
-}
-template <Space S> __device__ __forceinline__ void st_u32(uint32_t* p, uint32_t v) {
-    if (S == kGlobal) { __stcg(p, v); return; }
-    asm volatile("st.shared.u32 [%0], %1;" :: "r"(smem_addr_u32(p)), "r"(v) : "memory");
-}
-
 __device__ __forceinline__ void bulk_init(BulkSmem& b) {     // thread 0, once per kernel, followed by a barrier
     for (int s = 0; s < kBulkDepth; ++s)
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_addr_u32(&b.bar[s])) : "memory");
@@ -141,20 +130,10 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, uint3
                  :: "l"(gdst), "r"(smem_addr_u32(smem_src)), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
-// bulk_s2g for bytes nobody is expected to read back soon: the lines it writes are the first L2 evicts
-__device__ __forceinline__ void bulk_s2g_evict_first(void* gdst, const void* smem_src, uint32_t bytes) {
-    uint64_t pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
-                 :: "l"(gdst), "r"(smem_addr_u32(smem_src)), "r"(bytes), "l"(pol) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
 // at most N bulk groups may still be reading their shared-memory source
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
 __device__ __forceinline__ void bulk_wait_all0()  { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// every thread that wrote a shared-memory buffer with generic stores, before the barrier after which a bulk store reads it
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_bar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok = 0;
     while (!ok) {

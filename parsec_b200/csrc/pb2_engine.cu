@@ -439,8 +439,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
 // With `fuse`, a task P also runs with the first group among its out-edges as one unit when P has a body, writes the
 // group's tile X without pushing it out, and X is P's widest tile (so P's parts cut X as the members' parts do): the
 // edge P -> leader leaves the device CSR and group[P] = PB2_GROUP_FUSED | the leader's group word.  The worker that
-// runs a part of P stages it chunk by chunk in shared memory, the members check each chunk there, and a bulk store
-// writes it to X (run_fused_part); so P's body must have a staged form that writes X (fusable).  The
+// runs a part of P writes it to X and checks every value for the members in registers before it stores it
+// (run_fused_part); so P's body must have a checked form that writes X (fusable).  The
 // caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
 // every task that was queued when P retired, and a fused unit runs them right after P.
 static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
@@ -463,7 +463,7 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
         for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
         return true;
     };
-    // the bodies with a staged form (run_hbm_body<true>), whose output flow `out` writes X
+    // the bodies with a checked form (run_hbm_body<true>), whose output flow `out` writes X
     auto fusable = [&](const pb2_task_t& p, int32_t x) {
         int out = 0;
         switch (p.body) {
@@ -473,7 +473,7 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
         default: return false;
         }
         if (p.nb_flows <= out || p.tile[out] != x || !(p.access[out] & PB2_FLOW_ACCESS_WRITE)) return false;
-        // the staged COPY / AXPY writes every byte of the chunk: the tile they read is as long as X
+        // the checked COPY / AXPY writes every byte of the slice: the tile they read is as long as X
         if (out == 1 && (p.tile[0] < 0 || tiles[p.tile[0]].bytes != tiles[x].bytes)) return false;
         for (int f = 0; f < p.nb_flows; ++f) {
             if (p.tile[f] < 0) continue;
@@ -542,14 +542,13 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     }
     pb2_engine_params_t p{};
     if (params) p = *params;
-    if (p.workers_per_sm <= 0) p.workers_per_sm = PB2_HBM_MINB;
+    if (p.workers_per_sm <= 0) p.workers_per_sm = kHbmWorkersPerSm;
     if (p.threads <= 0 || p.threads > PB2_HBM_THREADS) p.threads = PB2_HBM_THREADS;     // the kernel is compiled for this CTA size
     p.threads = (p.threads + 31) & ~31;
     if (p.timeout_ms <= 0) p.timeout_ms = 20000;
     if (p.part_bytes == 0) p.part_bytes = 256 * 1024;
     e->params = p;
     if (const char* sl = getenv("PB2_STAGE_SLICE_BYTES")) e->stage_slice_bytes = atoi(sl);
-    if (const char* fc = getenv("PB2_FUSE_CHUNK_BYTES")) e->fuse_chunk_bytes = atoi(fc);       // development aid
     if (const char* sm = getenv("PB2_STAGE_MODE")) e->params.stage_mode = atoi(sm);      // 1: SIMT mover (development aid)
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->up_stream, cudaStreamNonBlocking));
@@ -889,8 +888,6 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     d.nparts = nullptr; d.remote_units = 0;
     d.group = nullptr; d.group_mem = nullptr;
     d.nlanes = nlanes;          // d.lanes / d.lane: build_lane_ring
-    // a fused unit stages each chunk in one slot of the bulk ring
-    d.fuse_chunk = e->fuse_chunk_bytes > 16 ? std::min(((uint32_t)e->fuse_chunk_bytes + 15u) & ~15u, kBulkChunk) : 16u;
     if (grouped) {
         uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
         TRY(dev_alloc_copy(w, &d_group, group.data(), group.size()));

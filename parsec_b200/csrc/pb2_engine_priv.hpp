@@ -21,8 +21,6 @@ struct pb2_engine_s {
     bool dma_pending = false;
     int nworkers = 0;
     int32_t stage_slice_bytes = 64 * 1024;   // stage-in granularity: every CTA that needs a tile pulls the slices nobody has claimed
-    int32_t fuse_chunk_bytes = 4096;         // fused producer + read group: bytes staged before the group checks them
-                                             // (clamped to one slot of the bulk ring, kBulkChunk)
     int nworkers_gemm = 0;
     std::string last_error;
     std::mutex mu;

@@ -12,19 +12,22 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // the persistent engine kernel, HBM-bound bodies
 // ---------------------------------------------------------------------------------------------
-// 64-thread workers, 12 per SM (<= 80 registers, no spills): a worker keeps PB2_CHECK_UNROLL = 16 (read-only bodies) or
+// 64-thread workers, up to 12 per SM (<= 80 registers, no spills; 8 by default, kHbmWorkersPerSm): a worker keeps PB2_CHECK_UNROLL = 16 (read-only bodies) or
 // PB2_UNROLL = 4 (read-modify-write bodies) 16-byte requests per thread in flight -- bytes in flight per SM are what
 // a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
 // 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
 // streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
 // (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
-// producer runs with its group as one unit (run_fused_part) that computes each 4 KiB chunk into a slot of the bulk
-// ring, checks it there and writes it to HBM with one TMA bulk store: the tile goes SM -> L2 -> DRAM once and never
-// comes back to the SM (DESIGN.md §5, §8).
+// producer runs with its group as one unit (run_fused_part) that checks every value in registers before it stores it:
+// the tile goes SM -> L2 -> DRAM once and never comes back to the SM (DESIGN.md §5, §8).
 // What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
 #ifndef PB2_HBM_MINB
 #define PB2_HBM_MINB 12
 #endif
+// Workers per SM of an HBM window unless pb2_engine_params_t::workers_per_sm says otherwise.  The kernel keeps the
+// 80-register budget of PB2_HBM_MINB = 12, but a fused unit is a plain streaming write loop, and the resident Ex05 step
+// is about 3.5 % shorter at 8 (or 6) workers per SM than at 12, with the fusion-off window unchanged (DESIGN.md §8).
+constexpr int kHbmWorkersPerSm = 8;
 #ifndef PB2_HBM_THREADS
 #define PB2_HBM_THREADS 64
 #endif
@@ -33,14 +36,9 @@ struct GroupSmem {
     int32_t n;                              // members; 0: the popped task runs alone
     int32_t fused;                          // the popped task is a producer that runs with this group as one unit
     int32_t tile;                           // the tile the members read
-    int32_t fx;                             // fused: the producer's output flow, on that tile
     int32_t mem[PB2_GROUP_MAX];
     uint32_t k[PB2_GROUP_MAX];
     unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
-    // fused: the producer's slice of every flow for this part
-    void* base[PB2_MAX_FLOWS];
-    uint32_t len[PB2_MAX_FLOWS];
-    uint32_t e0;
 };
 
 // All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
@@ -68,104 +66,45 @@ static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
     __syncthreads();
 }
 
-// Results of a body run chunk by chunk: the mismatch counts add up, the first element is the first chunk's.
-__device__ __forceinline__ unsigned long long chunk_sum(unsigned long long acc, unsigned long long r, uint32_t c0) {
-    if (c0 == 0 || acc == ~0ull || r == ~0ull) return c0 == 0 ? r : ~0ull;
-    return acc + (r & 0xffffffff00000000ull);
-}
-
-// Thread 0: point s.args at the chunk of every flow that starts c0 bytes into this part's slice (the flows are cut
-// alike, and the group's tile is the widest).
-static __device__ __forceinline__ void set_chunk(TaskSmem& s, const GroupSmem& g, uint32_t c0, uint32_t chunk) {
-    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-        const uint32_t rest = g.len[f] > c0 ? g.len[f] - c0 : 0u;
-        s.args.flow[f] = g.base[f] ? static_cast<uint8_t*>(g.base[f]) + c0 : nullptr;
-        s.args.bytes[f] = rest < chunk ? rest : chunk;
-    }
-    s.args.elem0 = g.e0 + (c0 >> 2);
-}
-
 // All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
 // producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
 // writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
-// while they are still on the SM.  The slice is cut into chunks of `chunk` bytes (a multiple of 16, at most kBulkChunk,
-// the last one ragged), and chunk i is staged in slot i % kBulkDepth of the bulk ring, which is idle while a body runs:
-//  1. the producer's staged body computes the chunk of its output flow into the slot (it reads its flows from global);
-//  2. the members check the slot, by group_results' rules, while one bulk store writes it to the tile;
-//  3. before the barrier that ends the chunk, thread 0 waits until the store that read the next chunk's slot is done.
-// So a chunk costs two barriers and no round trip through L2.  Member results are summed over the chunks (chunk_sum).
-// Tile slices are 16-byte aligned, as every body assumes; only the end of a slice (< 16 bytes) takes SIMT stores.
-// Returns the producer's result (thread 0) once every bulk store has completed and is ordered before the caller's
-// __threadfence(): successors on other SMs read the tile with generic loads.
-static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp, BulkSmem* bulk, uint32_t chunk) {
+// before they leave the SM: the producer's checked body (run_hbm_body<true>) writes its output flow as it would alone,
+// and every thread ORs (element ^ the leader's constant) of each value it stores while the value is still in registers.
+// Its stores carry an L2 evict-first policy: nobody reads the tile back here (the resident Ex05 step is about 3 %
+// shorter than with the default policy, DESIGN.md §8).  One barrier then tells every thread whether the slice held
+// anything but the leader's constant, and the members get group_results' rules:
+//  - nothing else: a member with the leader's constant counts no mismatch, any other member counts every element;
+//  - otherwise the slice is counted again, exactly, from the tile (the barrier made the CTA's stores visible to its
+//    threads, and the loads go through L2), for the leader and every member whose constant differs from the leader's.
+// Returns the producer's result (thread 0); the caller's barrier and __threadfence() order the stores before the release.
+static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp) {
     TaskSmem& s = *sp;
     GroupSmem& g = *gp;
     const int body = s.task.body;
-    if (threadIdx.x == 0) {
-        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { g.base[f] = s.args.flow[f]; g.len[f] = s.args.bytes[f]; }
-        g.fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
-        g.e0 = s.args.elem0;
-        set_chunk(s, g, 0, chunk);
-    }
-    __syncthreads();
-    const uint32_t len = g.len[g.fx];
-    uint8_t* const dst = static_cast<uint8_t*>(g.base[g.fx]);
     const uint32_t k0 = g.k[0];
-    unsigned long long acc = 0;
-    int slot_i = 0;
-#pragma unroll 1
-    for (uint32_t c0 = 0;; c0 += chunk) {
-        const uint32_t n = len - c0 < chunk ? len - c0 : chunk;       // bytes of the output flow in this chunk
-        const bool last = len - c0 <= chunk;
-        uint8_t* const slot = bulk->buf[slot_i];
-        const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, slot);
-        fence_proxy_async_smem();
-        __syncthreads();
-        // the bytes the body wrote: a tail of < 4 bytes keeps what the tile holds, except for the bodies that write bytes
-        const uint32_t nw = (body == PB2_BODY_MEMSET_U8 || body == PB2_BODY_COPY) ? n : n & ~3u;
-        const uint32_t nb = nw & ~15u;
-        // the group checks the chunk here and never reads it back, so its lines are the first L2 evicts
-        // (the resident Ex05 step is about 3 % shorter than with the default policy, DESIGN.md §8)
-        if (threadIdx.x == 0 && nb) bulk_s2g_evict_first(dst + c0, slot, nb);
-        if (threadIdx.x < nw - nb) __stcg(dst + c0 + nb + threadIdx.x, slot[nb + threadIdx.x]);
-        const uint32_t diff = cta_xor_scan<kShared>(slot, n, k0);
-        if (threadIdx.x == 0) {
-            bulk_wait_read<kBulkDepth - 1>();
-            if (!last) set_chunk(s, g, c0 + chunk, chunk);
-        }
-        const bool mismatch = __syncthreads_or(diff != 0u) != 0;
-        const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && n >= 4 ? *reinterpret_cast<const uint32_t*>(slot) : 0u;
-        if (!mismatch) {
-            // the chunk holds nothing but the leader's constant: every element mismatches any other constant
-            if (threadIdx.x == 0) {
-                acc = chunk_sum(acc, r, c0);
-                for (int m = 0; m < g.n; ++m)
-                    g.res[m] = chunk_sum(g.res[m], g.k[m] == k0 ? first : ((unsigned long long)(n >> 2) << 32) | first, c0);
-            }
-        } else {
-            // count again, exactly, for every constant but the leader's repeated
-            unsigned long long r0 = 0;
-#pragma unroll 1
-            for (int m = 0; m < g.n; ++m) {
-                const uint32_t k = g.k[m];
-                unsigned long long rm = r0;
-                if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne<kShared>(slot, n, k, s.red) << 32) | first;
-                if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = chunk_sum(g.res[m], rm, c0); }
-            }
-            if (threadIdx.x == 0) acc = chunk_sum(acc, r, c0);
-        }
-        if (last) break;
-        slot_i = slot_i + 1 == kBulkDepth ? 0 : slot_i + 1;
+    Checked ck{k0, 0u, l2_evict_first()};
+    const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, &ck);
+    const bool mismatch = __syncthreads_or(ck.diff != 0u) != 0;
+    const int fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
+    const uint32_t len = s.args.bytes[fx];
+    const uint32_t* const out = static_cast<const uint32_t*>(s.args.flow[fx]);
+    // the slice's first element: k0 if nothing mismatched, else what thread 0 stored there
+    const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && len >= 4 ? (mismatch ? __ldcg(out) : k0) : 0u;
+    if (!mismatch) {
+        if (threadIdx.x == 0)
+            for (int m = 0; m < g.n; ++m) g.res[m] = g.k[m] == k0 ? first : ((unsigned long long)(len >> 2) << 32) | first;
+        return r;
     }
-    if (threadIdx.x == 0) {
-        bulk_wait_all0();
-        asm volatile("fence.proxy.async;" ::: "memory");
-        // the pushout that follows works on the whole slice
-        for (int f = 0; f < PB2_MAX_FLOWS; ++f) { s.args.flow[f] = g.base[f]; s.args.bytes[f] = g.len[f]; }
-        s.args.elem0 = g.e0;
+    unsigned long long r0 = 0;
+#pragma unroll 1
+    for (int m = 0; m < g.n; ++m) {
+        const uint32_t k = g.k[m];
+        unsigned long long rm = r0;
+        if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne(out, len, k, s.red) << 32) | first;
+        if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = rm; }
     }
-    __syncthreads();
-    return acc;
+    return r;
 }
 
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
@@ -224,7 +163,7 @@ pb2_engine_hbm_kernel(WinDev w) {
         __syncthreads();
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
-            return g.fused ? run_fused_part(&s, &g, &bulk, w.fuse_chunk) : run_hbm_body(s.task.body, s.args, s.red);
+            return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         });
         if (g.n && !g.fused) {
             // the leader's part stored the version it saw; every member saw the same one

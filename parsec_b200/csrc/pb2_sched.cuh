@@ -64,7 +64,6 @@ struct WinDev {
     // group word) names that group's members, the leader included, and its edge to the leader is gone from succ[].
     const uint32_t*   group;
     const int32_t*    group_mem;
-    uint32_t          fuse_chunk;     // bytes a fused producer writes before its group checks them (multiple of 16)
     // queue_policy 1 (null / 0 otherwise): the ready ring is cut into priority lanes, see Lanes below
     int32_t           nlanes;         // lanes in use (1 .. PB2_PRIO_LANES)
     struct Lanes*     lanes;

@@ -4,7 +4,7 @@
 //
 // Reference: parsec_device_kernel_push / _exec / _pop, parsec/mca/device/device_gpu.c:2745, :2873, :2943.
 //
-// Register discipline: the kernels run 12 CTAs of 64 threads per SM (<= 80 registers per thread).  Everything that is
+// Register discipline: the kernels are built for 12 CTAs of 64 threads per SM (<= 80 registers per thread).  Everything that is
 // indexed by a run-time flow number lives in shared memory (TaskSmem), filled by one thread per flow, so that no
 // array is demoted to local memory; tile payloads move through TMA (no payload registers) or 4 x 16-byte loads.
 #pragma once

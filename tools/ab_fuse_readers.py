@@ -4,9 +4,8 @@
 1. the card: name, power limit and maximum SM clock (read-only nvidia-smi query);
 2. tools/l2_probe (compiled into a temporary directory): the L2 read rate and the DRAM rates of this GPU;
 3. a FILL-only window (the K producers of the Ex05 window, no readers): the write floor of the fused window;
-4. the resident Ex05 window (dags.ex05_broadcast(K, 14, 262144), tiles VALID) with fusion off, and on at chunk sizes
-   1, 2 and 4 KiB (PB2_FUSE_CHUNK_BYTES; a fused unit stages each chunk in one 4 KiB slot of the bulk ring);
-5. --ab LIB: the fused window (default chunk) on library LIB (another build of libparsec_b200.so, e.g. the parent
+4. the resident Ex05 window (dags.ex05_broadcast(K, 14, 262144), tiles VALID) with fusion off and on;
+5. --ab LIB: the fused window on library LIB (another build of libparsec_b200.so, e.g. the parent
    commit's) and on this tree's library, alternated: --rounds child processes per build, each with PB2_LIB_PATH set,
    --warmup and --runs runs each.
 Each row: median / min / max / spread of reset_ms + kernel_ms.
@@ -30,13 +29,8 @@ from ab_read_groups import TB, card, l2_probe, summary
 class Window:
     """One engine and one resident window of the Ex05 DAG (or of its producers alone) on it."""
 
-    def __init__(self, K, fuse_readers=0, chunk=None, fill_only=False, part_bytes=0):
-        if chunk is not None:
-            os.environ["PB2_FUSE_CHUNK_BYTES"] = str(chunk)       # read when the engine is created
-        try:
-            self.e = Engine(0, fuse_readers=fuse_readers, part_bytes=part_bytes)
-        finally:
-            os.environ.pop("PB2_FUSE_CHUNK_BYTES", None)
+    def __init__(self, K, fuse_readers=0, fill_only=False, part_bytes=0, workers_per_sm=0):
+        self.e = Engine(0, workers_per_sm=workers_per_sm, fuse_readers=fuse_readers, part_bytes=part_bytes)
         dag = dags.ex05_broadcast(K, 14, TB)
         tasks, succ = dag.tasks, dag.succ
         if fill_only:
@@ -108,8 +102,7 @@ def main():
     print(json.dumps({"l2_probe": l2_probe()}), flush=True)
     print(json.dumps({"fill_only": measure(Window(args.K, fill_only=True), args.warmup, args.runs)}), flush=True)
     print(json.dumps({"sweep": "fusion_off", **measure(Window(args.K, -1), args.warmup, args.runs)}), flush=True)
-    for kib in (1, 2, 4):
-        print(json.dumps({"sweep": "fusion_on", "chunk_kib": kib, **measure(Window(args.K, 0, kib * 1024), args.warmup, args.runs)}), flush=True)
+    print(json.dumps({"sweep": "fusion_on", **measure(Window(args.K, 0), args.warmup, args.runs)}), flush=True)
     if args.ab:
         print(json.dumps({"ab": ab_libraries(args)}), flush=True)
 
