@@ -303,8 +303,8 @@ static int build_lane_ring(pb2_window_t* w, const std::vector<uint8_t>& owner_la
 // GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
 // task_lane (queue_policy 1, else null): a unit's lane is the lane of its first task, for all its parts.
-// part_bytes > 0: a unit that runs an HBM body (not NOP) over a tile wider than part_bytes is cut into
-// min(ceil(widest tile / part_bytes), kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.
+// A unit that runs an HBM body is cut into task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide
+// tasks.
 static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
                              const int32_t* ready, int32_t nready, bool fuse, uint32_t* ring_cap_needed,
                              const int32_t* rs_begin, const std::vector<uint8_t>* task_lane,
@@ -345,16 +345,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
         // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body
-        int nsub = 1;
-        if (g) nsub = ((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN);
-        else if (part_bytes > 0 && tasks[h].body != PB2_BODY_NOP) {
-            uint32_t big = 0;
-            for (int f = 0; f < tasks[h].nb_flows; ++f)
-                if (tasks[h].tile[f] >= 0) big = std::max(big, tiles[tasks[h].tile[f]].bytes);
-            nsub = (int)std::min<uint32_t>((big + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes, (uint32_t)gemm::kMaxParts);
-            nsub = std::max(nsub, 1);
-        }
-        u.nparts = std::min(nsub, gemm::kMaxParts);
+        u.nparts = g ? std::min(((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN), gemm::kMaxParts)
+                     : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
             segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});
@@ -546,7 +538,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     if (p.threads <= 0 || p.threads > PB2_HBM_THREADS) p.threads = PB2_HBM_THREADS;     // the kernel is compiled for this CTA size
     p.threads = (p.threads + 31) & ~31;
     if (p.timeout_ms <= 0) p.timeout_ms = 20000;
-    if (p.part_bytes == 0) p.part_bytes = 256 * 1024;
+    if (p.part_bytes == 0) p.part_bytes = kDefaultPartBytes;
     e->params = p;
     if (const char* sl = getenv("PB2_STAGE_SLICE_BYTES")) e->stage_slice_bytes = atoi(sl);
     if (const char* sm = getenv("PB2_STAGE_MODE")) e->params.stage_mode = atoi(sm);      // 1: SIMT mover (development aid)
@@ -766,7 +758,7 @@ int pb2_engine_set_stage_slice_bytes(pb2_engine_t* e, int32_t bytes) {
 }
 int pb2_engine_set_part_bytes(pb2_engine_t* e, int32_t part_bytes) {
     if (!e) return PB2_ERR_BAD_PARAM;
-    e->params.part_bytes = part_bytes == 0 ? 256 * 1024 : part_bytes;
+    e->params.part_bytes = part_bytes == 0 ? kDefaultPartBytes : part_bytes;
     return PB2_SUCCESS;
 }
 int pb2_engine_set_shared_windows(pb2_engine_t* e, int on, const int32_t* next_rs_begin) {
@@ -822,7 +814,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     w->shared = e->shared_windows;
     w->e = e; w->kind = kind; w->ntasks = ntasks; w->nsucc = nsucc; w->ntiles = ntiles; w->nready = nready;
 #define TRY(x) do { rc = (x); if (rc != PB2_SUCCESS) { pb2_window_destroy(w); return rc; } } while (0)
-    // wide tasks (HBM windows): parts per task = ceil(widest tile / part_bytes), at most PB2_MAX_PARTS
+    // wide tasks (HBM windows): at most PB2_MAX_PARTS parts per task
     std::vector<pb2_task_t> dtasks(tasks, tasks + ntasks);
     std::vector<uint16_t> nparts((size_t)ntasks, 1);
     std::vector<int32_t> entries;
@@ -830,12 +822,9 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     for (int32_t i = 0; i < ntasks; ++i) {
         pb2_task_t& t = dtasks[i];
         t.flags &= 0x07;
-        if (kind != 0 || t.body == PB2_BODY_NOP || e->params.part_bytes < 0 || ntasks >= (1 << 22)) continue;
-        uint32_t big = 0;
-        for (int f = 0; f < t.nb_flows; ++f) if (t.tile[f] >= 0 && tiles[t.tile[f]].bytes > big) big = tiles[t.tile[f]].bytes;
-        uint32_t np = (big + (uint32_t)e->params.part_bytes - 1) / (uint32_t)e->params.part_bytes;
-        if (np > PB2_MAX_PARTS) np = PB2_MAX_PARTS;
-        if (np > 1) { nparts[(size_t)i] = (uint16_t)np; extra_parts += np - 1; }
+        if (kind != 0) continue;
+        const int np = task_parts(t, [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
+        nparts[(size_t)i] = (uint16_t)np; extra_parts += (uint32_t)np - 1;
     }
     for (int32_t i = 0; i < nready; ++i)
         for (int p = 0; p < (int)nparts[(size_t)ready[i]]; ++p) entries.push_back(PB2_ENT_MAKE(ready[i], p));

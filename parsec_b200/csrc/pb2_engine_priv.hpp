@@ -1,4 +1,4 @@
-// pb2_engine_priv.hpp -- host-side engine object shared by the translation units of libparsec_b200.so
+// pb2_engine_priv.hpp -- host-side engine object and part rule shared by the translation units of libparsec_b200.so
 // (pb2_engine.cu: windows; pb2_stream.cu: the streaming ring + persistent kernel).
 #pragma once
 #include <cuda_runtime.h>
@@ -28,6 +28,21 @@ struct pb2_engine_s {
     const int32_t* next_rs_begin = nullptr;   // remote out-degree CSR of the next shared window (not owned)
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
 };
+
+// part_bytes of engines and streams whose parameters leave it 0
+constexpr int32_t kDefaultPartBytes = 256 * 1024;
+
+// The parts a task runs as: min(ceil(widest tile / part_bytes), cap) byte slices; one for a NOP body or part_bytes <= 0.
+// tile_bytes(id) is the byte count of tile id.  The device cuts the slices of a tile by the same rule (tile_slices_of).
+template <class TileBytes>
+static inline int task_parts(const pb2_task_t& t, TileBytes tile_bytes, int32_t part_bytes, int cap) {
+    if (part_bytes <= 0 || t.body == PB2_BODY_NOP) return 1;
+    uint32_t big = 0;
+    for (int f = 0; f < t.nb_flows; ++f)
+        if (t.tile[f] >= 0 && tile_bytes(t.tile[f]) > big) big = tile_bytes(t.tile[f]);
+    const uint32_t np = (big + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes;
+    return np < 1 ? 1 : (np > (uint32_t)cap ? cap : (int)np);
+}
 
 #define PB2_CUDA(e, call)                                                                        \
     do {                                                                                         \

@@ -18,8 +18,8 @@
 // dependency trace is unchanged); only the intermediate bf16 roundings of C disappear.  Scheduling entities on the
 // device are units (counter-mode dependency words), ring entries are (part, unit).
 // The other tasks of the DAG (HBM bodies: FILL, SCALE, COPY, AXPY, CHECK, ... between the chains) are units of one
-// task; one wider than part_bytes is cut into byte-slice parts like a wide task of an HBM window, each run by a whole
-// CTA, and the last part to finish retires it.
+// task; one wider than part_bytes is cut into byte-slice parts like a wide task of an HBM window.  A whole CTA runs each
+// part with the HBM workers' run_task_part (pb2_worker.cuh), and the last part to finish retires the unit.
 //
 // One CTA per SM is one worker.  Three warpgroups (384 threads):
 //   warpgroup 0 : warp 0 retires a unit and releases its out-edges; one lane of warp 1 is the TMA producer
@@ -235,13 +235,9 @@ struct Job {
 
 struct Shared {
     alignas(16) Job job;
-    alignas(16) pb2_task_t task;    // non-GEMM units: the single member's descriptor
-    uint32_t off[PB2_MAX_FLOWS];    // non-GEMM units: this part's byte slice of every flow
-    uint32_t len[PB2_MAX_FLOWS];
+    TaskSmem ts;                    // non-GEMM units: run_task_part's state; GEMM units stage in with its need / decide
     uint64_t full[kStages];
     uint64_t empty[kStages];
-    int32_t  need, decide;
-    uint32_t red[32];
 };
 
 // whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges
@@ -261,7 +257,6 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
     const uint32_t cver = (u.flags & 1) ? *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) : 0u;
     for (int i = lane; i < L; i += 32) {
         const GSeg s = g.segs[u.seg_begin + i];
-        const pb2_task_t& t = w.tasks[s.task];
         w.start_seq[s.task] = (uint32_t)(ebase + 2 * i);
         w.end_seq[s.task] = (uint32_t)(ebase + 2 * i + 1);
         w.retire_log[rbase + i] = s.task;
@@ -272,16 +267,7 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
             w.seen_version[s.task * PB2_MAX_FLOWS + 2] = cver + (uint32_t)i;
             w.result[s.task] = 0;
         } else {
-            for (int f = 0; f < t.nb_flows; ++f)
-                if (t.tile[f] >= 0) {
-                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&tile->version);
-                    w.seen_version[s.task * PB2_MAX_FLOWS + f] = v;
-                    if (t.access[f] & PB2_FLOW_ACCESS_WRITE) {
-                        *reinterpret_cast<volatile uint32_t*>(&tile->version) = v + 1;
-                        st_relaxed_gpu(&tile->state, PB2_TILE_VALID);
-                    }
-                }
+            epilog_written_flows(w, w.tasks[s.task]);      // part 0 stored seen_version (run_task_part)
         }
     }
     if (lane == 0 && (u.flags & 1)) {
@@ -370,59 +356,22 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
         __syncthreads();
         if (sh.job.stop) break;
         {
-            // stage in every INVALID tile the job reads (same protocol as the other kernels)
+            // GEMM units: stage in every INVALID tile the job reads (same protocol as the other kernels)
             const int nseg = sh.job.is_gemm ? sh.job.seg_count : 0;
             for (int i = -1; i < 2 * nseg; ++i) {
                 int tile_id; uint8_t acc;
                 if (i < 0) { if (!sh.job.is_gemm) break; tile_id = sh.job.tileC; acc = PB2_FLOW_ACCESS_RW; }
                 else { const GSeg s = g.segs[sh.job.seg_begin + (i >> 1)]; tile_id = (i & 1) ? s.tileB : s.tileA; acc = PB2_FLOW_ACCESS_READ; }
                 pb2_tile_t* tile = &w.tiles[tile_id];
-                if (threadIdx.x == 0) sh.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
+                if (threadIdx.x == 0) sh.ts.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
                 __syncthreads();
-                if (sh.need) {
+                if (sh.ts.need) {
                     const int ns = tile_slices(w, tile->bytes);
-                    if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.decide);
-                    else stage_in_slices(stage_ctx(w), tile_id, ns, 0, ns, &sh.decide);     // take what nobody has claimed, wait for the rest
+                    if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.ts.decide);
+                    else stage_in_slices(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide);     // take what nobody has claimed, wait for the rest
                     fence_proxy_async();
                 }
                 __syncthreads();
-            }
-            if (!sh.job.is_gemm) {
-                const GSeg s = g.segs[sh.job.seg_begin];
-                if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.task)[threadIdx.x] =
-                    __ldg(reinterpret_cast<const uint4*>(&w.tasks[s.task]) + threadIdx.x);
-                __syncthreads();
-                const pb2_task_t& t = sh.task;
-                if (threadIdx.x == 0) {
-                    // every flow is cut at the offsets of the widest one, as the HBM kernel cuts its parts (part_slice)
-                    uint32_t bytes[PB2_MAX_FLOWS], widest = 0;
-                    for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-                        bytes[f] = (f < t.nb_flows && t.tile[f] >= 0) ? w.tiles[t.tile[f]].bytes : 0u;
-                        widest = bytes[f] > widest ? bytes[f] : widest;
-                    }
-                    for (int f = 0; f < PB2_MAX_FLOWS; ++f)
-                        part_slice(widest, (uint32_t)sh.job.nparts, (uint32_t)sh.job.part, bytes[f], sh.off[f], sh.len[f]);
-                }
-                __syncthreads();
-                for (int f = 0; f < t.nb_flows; ++f) {
-                    if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_ACCESS_READ)) continue;
-                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                    if (threadIdx.x == 0) sh.need = ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
-                    __syncthreads();
-                    if (sh.need) {
-                        // a sliced tile (the rule the GEMM units stage by) is pulled slice by slice: this part takes
-                        // the slices over its bytes that nobody has claimed and waits for the others
-                        const int ns = tile_slices(w, tile->bytes);
-                        if (ns == 1) stage_in_flow(stage_ctx(w), tile, t.access[f], &sh.decide);
-                        else {
-                            int s0, s1;
-                            slices_over(tile->bytes, ns, sh.off[f], sh.len[f], s0, s1);
-                            stage_in_slices(stage_ctx(w), t.tile[f], ns, s0, s1, &sh.decide);
-                        }
-                        fence_proxy_async();
-                    }
-                    __syncthreads();
-                }
             }
         }
         const Job& job = sh.job;       // read from shared memory, not held in registers across the wgmma loop
@@ -481,30 +430,20 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             }
         } else {
             // ---------------- an HBM body in the DAG (element-wise task, panel stand-in): the whole CTA runs this
-            // part's byte slice of its flows in place
-            const pb2_task_t& t = sh.task;
-            BodyArgs a;
-            for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-                const bool has = f < t.nb_flows && t.tile[f] >= 0;
-                a.flow[f] = has ? reinterpret_cast<uint8_t*>(w.tiles[t.tile[f]].dev_ptr) + sh.off[f] : nullptr;
-                a.bytes[f] = has ? sh.len[f] : 0u;
-            }
-            a.elem0 = sh.off[0] >> 2; a.part = (uint32_t)job.part;
-            a.iparam[0] = t.iparam[0]; a.iparam[1] = t.iparam[1]; a.iparam[2] = t.iparam[2]; a.fparam = t.fparam;
-            const unsigned long long r = run_hbm_body(t.body, a, sh.red);
-            // CHECK parts add their mismatch counts; the first element comes from part 0
-            if (threadIdx.x == 0) store_result(w, t, g.segs[job.seg_begin].task, job.part, job.nparts, r);
-            fence_proxy_async();
-            // the pushout's threads do not read the bytes each wrote (a host copy that is only 4- or 1-byte aligned
-            // takes the narrow copy loops): every store of the body is done before any of them reads
+            // part's byte slice of its flows in place, as a worker of an HBM window does.  Later units read the tiles
+            // through TMA: the generic stores of a stage-in and of the body are followed by fence.proxy.async.
+            const int32_t id = g.segs[job.seg_begin].task;
+            if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.ts.task)[threadIdx.x] =
+                __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
             __syncthreads();
-            for (int f = 0; f < t.nb_flows; ++f)
-                if (t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
-                    pb2_tile_t* tile = &w.tiles[t.tile[f]];
-                    cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + sh.off[f],
-                                    reinterpret_cast<const uint8_t*>(tile->dev_ptr) + sh.off[f], sh.len[f]);
-                    if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)sh.len[f]);
-                }
+            const unsigned long long r = run_task_part<false>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
+                if (sh.ts.need) fence_proxy_async();
+                const unsigned long long body_r = run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
+                fence_proxy_async();
+                return body_r;
+            });
+            // CHECK parts add their mismatch counts; the first element comes from part 0
+            if (threadIdx.x == 0) store_result(w, sh.ts.task, id, job.part, job.nparts, r);
         }
         __threadfence();
         __syncthreads();             // every store of the part is done and visible

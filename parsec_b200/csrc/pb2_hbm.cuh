@@ -20,7 +20,8 @@ namespace pb2 {
 // (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
 // producer runs with its group as one unit (run_fused_part) that checks every value in registers before it stores it:
 // the tile goes SM -> L2 -> DRAM once and never comes back to the SM (DESIGN.md §5, §8).
-// What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu).
+// What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu and the
+// HBM-body units of the GEMM kernel).
 #ifndef PB2_HBM_MINB
 #define PB2_HBM_MINB 12
 #endif
@@ -162,7 +163,7 @@ pb2_engine_hbm_kernel(WinDev w) {
         }
         __syncthreads();
         const int nparts = task_nparts(w, id);
-        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts, [&] {
+        const unsigned long long r = run_task_part<true>(w, s, &bulk, id, part, nparts, [&] {
             return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         });
         if (g.n && !g.fused) {

@@ -300,8 +300,8 @@ pb2_stream_kernel(StreamDev sd) {
             __ldcg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
         __syncthreads();
         const int nparts = (int)__ldcg(&w.nparts[id]);
-        const unsigned long long r = run_task_part(w, s, &bulk, id, part, nparts,
-                                                   [&] { return run_hbm_body(s.task.body, s.args, s.red); });
+        const unsigned long long r = run_task_part<true>(w, s, &bulk, id, part, nparts,
+                                                         [&] { return run_hbm_body(s.task.body, s.args, s.red); });
 
         if (threadIdx.x == 0) {
             __threadfence();
@@ -460,7 +460,7 @@ int pb2_stream_create(pb2_engine_t* e, const pb2_stream_params_t* params, pb2_st
     if (p.max_tiles <= 0) p.max_tiles = 65536;
     if (p.idle_us <= 0) p.idle_us = 2000;
     if (p.timeout_ms <= 0) p.timeout_ms = 20000;
-    if (p.part_bytes == 0) p.part_bytes = 256 * 1024;
+    if (p.part_bytes == 0) p.part_bytes = kDefaultPartBytes;
     pb2_stream_t* s = new pb2_stream_s();
     s->e = e; s->p = p; s->dry = p.dry_run != 0;
     s->slots = round_pow2((uint32_t)p.cmd_slots, 1024u, 1u << 21);
@@ -628,16 +628,8 @@ int pb2_stream_submit(pb2_stream_t* s, const pb2_task_t* task, uint64_t cookie, 
         s->freed_head.store(h, std::memory_order_release);
         if (s->free_tickets.empty()) return PB2_ERR_OUT_OF_RESOURCE;
     }
-    // parts: ceil(widest tile / part_bytes), the rule the device applies to the slices of a tile (tile_slices)
-    uint32_t np = 1;
-    if (s->p.part_bytes > 0 && task->body != PB2_BODY_NOP) {
-        uint32_t big = 0;
-        for (int f = 0; f < task->nb_flows; ++f)
-            if (task->tile[f] >= 0 && s->tile_bytes[(size_t)task->tile[f]] > big) big = s->tile_bytes[(size_t)task->tile[f]];
-        np = (big + (uint32_t)s->p.part_bytes - 1) / (uint32_t)s->p.part_bytes;
-        if (np > PB2_MAX_PARTS) np = PB2_MAX_PARTS;
-        if (np < 1) np = 1;
-    }
+    const uint32_t np = (uint32_t)task_parts(*task, [&](int32_t id) { return s->tile_bytes[(size_t)id]; },
+                                             s->p.part_bytes, PB2_MAX_PARTS);
     {   // ready-ring capacity: entries in flight, with a view of the poll side's counter that is refreshed only when needed
         const uint64_t sub = s->sub_entries.load(std::memory_order_relaxed);
         if (sub - s->ret_entries_seen + np + 64 > (uint64_t)s->ring_cap / 2) {

@@ -1,12 +1,14 @@
 // pb2_worker.cuh -- what one worker CTA does with one (part of a) task: push (stage-in), exec (body), pop (pushout).
-// Shared by the window kernel (pb2_engine.cu) and the streaming kernel (pb2_stream.cu); the two differ only in where
-// ready tasks come from and in how a finished task is retired and its successors are released.
+// Shared by the HBM window kernel (pb2_hbm.cuh), the streaming kernel (pb2_stream.cu) and the HBM-body units of the
+// GEMM window kernel (pb2_gemm.cuh); they differ only in where ready tasks come from, in what runs as the body and in
+// how a finished task is retired and its successors are released.
 //
 // Reference: parsec_device_kernel_push / _exec / _pop, parsec/mca/device/device_gpu.c:2745, :2873, :2943.
 //
-// Register discipline: the kernels are built for 12 CTAs of 64 threads per SM (<= 80 registers per thread).  Everything that is
-// indexed by a run-time flow number lives in shared memory (TaskSmem), filled by one thread per flow, so that no
-// array is demoted to local memory; tile payloads move through TMA (no payload registers) or 4 x 16-byte loads.
+// Register discipline: the HBM and streaming kernels are built for 12 CTAs of 64 threads per SM (<= 80 registers per
+// thread).  Everything that is indexed by a run-time flow number lives in shared memory (TaskSmem), filled by one thread
+// per flow, so that no array is demoted to local memory; tile payloads move through TMA (no payload registers) or
+// 4 x 16-byte loads.  The GEMM kernel (384 threads, no bulk ring) runs the same code with BULK = false.
 #pragma once
 #include "pb2_sched.cuh"
 
@@ -26,6 +28,10 @@ struct alignas(16) TaskSmem {
 };
 
 // All threads (uniform): stage in every flow whose bit is set in s.need.  One CTA-wide call per task at most.
+// BULK: the calling kernel has a TMA bulk ring (without one the copies take the SIMT loops).  Each instantiation has
+// one caller kernel per translation unit: a second caller kernel makes ptxas give this helper the standard call ABI,
+// which costs the HBM kernels a stack frame and spills at their 80-register budget (see pb2_hbm.cuh).
+template <bool BULK>
 static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, TaskSmem* sp, BulkSmem* bulk) {
     TaskSmem& s = *sp;
     const int need = s.need;
@@ -35,18 +41,19 @@ static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, Task
         const int32_t tid = s.task.tile[f];
         const uint32_t bytes = s.tbytes[f];
         const int ns = tile_slices_of(c.part_bytes, c.slice_claim, bytes);
-        if (ns == 1) stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, bulk);
+        if (ns == 1) stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr);
         else {
             int s0, s1;
             slices_over(bytes, ns, s.off[f], s.args.bytes[f], s0, s1);     // the slices under this part's bytes
-            stage_in_slices(c, tid, ns, s0, s1, &s.decide, bulk);
+            stage_in_slices(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr);
         }
     }
 }
 
 // All threads.  On entry s.task holds the descriptor (published by a barrier).  exec() runs the body over s.args (all
-// threads) and returns its result in thread 0.  Returns the body result (thread 0).
-template <class Exec>
+// threads) and returns its result in thread 0.  Returns the body result (thread 0).  BULK as for
+// stage_in_needed_flows; without it `bulk` is not used.
+template <bool BULK, class Exec>
 __device__ __forceinline__ unsigned long long
 run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts, Exec exec) {
     const pb2_task_t& t = s.task;
@@ -82,7 +89,7 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     __syncthreads();
     // the cold path, out of line and called once: everything it needs is in shared memory, nothing of the caller's
     // has to survive the call in registers
-    if (s.need) stage_in_needed_flows(stage_ctx(w), &s, bulk);
+    if (s.need) stage_in_needed_flows<BULK>(stage_ctx(w), &s, bulk);
 
     // ---- exec: the body (parsec_device_kernel_exec -> submit) ----
     const unsigned long long r = exec();
@@ -93,7 +100,8 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
         if (f < (int)t.nb_flows && t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
             const pb2_tile_t* tile = &w.tiles[t.tile[f]];
-            cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + s.off[f], s.args.flow[f], s.args.bytes[f], bulk);
+            cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + s.off[f], s.args.flow[f], s.args.bytes[f],
+                            BULK ? bulk : nullptr);
             if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)s.args.bytes[f]);
         }
     }
