@@ -34,7 +34,7 @@
 namespace pb2 {
 
 // ---------------------------------------------------------------------------------------------
-// reset: (re)arm one window.  dep words, ring, counters, tile table.
+// reset: (re)arm one window.  dep words, ring, counters, tile table; the units of a GEMM window.
 // ---------------------------------------------------------------------------------------------
 // queue_policy 1: every lane starts with its initial entries, which the ring image `ready` holds at the start of the
 // lane's segment (empty slots kEmpty).
@@ -46,10 +46,13 @@ __device__ __forceinline__ void reset_lanes(Lanes* lanes, size_t gid) {
     }
 }
 
-__global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
+// `ready` is the window's image of its first nready ring slots.  A GEMM window never has more units than tasks.
+__global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
+    const WinDev& w = g.w;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
     for (size_t i = gid; i < (size_t)w.ntasks; i += gsz) {
         const pb2_task_t& t = w.tasks[i];
         // counter mode counts down from the goal (parsec.c:1625-1633); mask mode ORs up from 0 (:1693-1703)
@@ -75,16 +78,6 @@ __global__ void pb2_window_reset_kernel(WinDev w, const pb2_tile_t* tiles_init,
         w.ctl->bytes_h2d.v = 0; w.ctl->bytes_d2d.v = 0; w.ctl->bytes_d2h.v = 0;
         w.ctl->stage_ins.v = 0; w.ctl->body_errors.v = 0;
     }
-}
-
-// re-arm the unit-level scheduling state of a GEMM window (after pb2_window_reset_kernel re-armed the rest)
-__global__ void pb2_window2_reset_kernel(Win2Dev g, const int32_t* ready_entries, int32_t nentries) {
-    const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const size_t gsz = (size_t)gridDim.x * blockDim.x;
-    for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
-    for (size_t i = gid; i <= (size_t)g.w.cap_mask; i += gsz) g.w.ring[i] = (i < (size_t)nentries) ? ready_entries[i] : kEmpty;
-    reset_lanes(g.w.lanes, gid);
-    if (gid == 0) g.w.ctl->tail.v = (unsigned long long)nentries;
 }
 
 // The same bodies as a stand-alone kernel on a caller's stream: what a BODY [type=CUDA] enqueues when it runs under a
@@ -138,18 +131,11 @@ using namespace pb2;
 struct pb2_window_s {
     pb2_engine_t* e = nullptr;
     int kind = 0;
-    int32_t ntasks = 0, nsucc = 0, ntiles = 0, nready = 0, nready_entries = 0;
-    WinDev d{};
-    pb2_task_t* d_tasks = nullptr;
-    uint32_t* d_succ = nullptr;
-    pb2_tile_t* d_tiles = nullptr;
+    int32_t ntasks = 0, ntiles = 0, nready_entries = 0;
+    Win2Dev g{};                        // g.w: the window's device descriptor; the rest: kind 1's units and tensor maps
     pb2_tile_t* d_tiles_init = nullptr;
-    int32_t* d_ready = nullptr;
+    int32_t* d_ready = nullptr;         // image of the first nready_entries ring slots
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
-    CUtensorMap* d_tmaps = nullptr;     // kind 1: one 2-D bf16 tensor map per tile (box 64 x 128, 128B swizzle)
-    Win2Dev g{};                        // kind 1: the unit-level state of pb2_engine_gemm2_kernel
-    int32_t* d_ready_entries = nullptr;
-    int32_t nentries = 0;
     bool launched = false;
     bool shared = false;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
@@ -157,6 +143,18 @@ struct pb2_window_s {
     std::vector<void*> peer_ptrs;
     std::vector<pb2_tile_t*> peer_tiles;     // per rank: its tile table as mapped here (nullptr: none / self)
     std::vector<int32_t> peer_ntiles;
+};
+
+// What the plan of a window kind (plan_hbm_window, build_gemm2_units) hands to pb2_window_create.  An entry owner is a
+// task of an HBM window or a unit of a GEMM window.
+struct WindowPlan {
+    std::vector<int32_t> entries;         // the initial ready-ring entries, in FIFO order
+    std::vector<int32_t> entry_owner;     // the owner of each of them
+    std::vector<uint8_t> owner_lane;      // queue_policy 1: per owner, its lane
+    std::vector<uint32_t> owner_pushes;   // queue_policy 1: per owner, the entries it can ever push
+    uint32_t ring_slots = 0;              // ring slots the window needs besides the workers' slack
+    int32_t slice_bytes = 0;              // stage-in slice size (WinDev::part_bytes)
+    bool claims = false;                  // stage-in is sliced: allocate the claim arrays
 };
 
 template <class T>
@@ -248,7 +246,10 @@ static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { e->last_error = "cuTensorMapEncodeTiled failed"; return PB2_ERR_DEVICE; }
     }
-    return dev_alloc_copy(w, &w->d_tmaps, maps.data(), maps.size());
+    CUtensorMap* d_tmaps = nullptr;
+    const int rc = dev_alloc_copy(w, &d_tmaps, maps.data(), maps.size());
+    w->g.tmaps = d_tmaps; w->g.fresh_tmaps = 1;
+    return rc;
 }
 
 
@@ -272,43 +273,41 @@ static std::vector<uint8_t> task_priority_lanes(const pb2_task_t* tasks, int32_t
     return lane;
 }
 
-// Cut the ring into one segment per lane, as long as the entries the lane's owners can ever push (owner o: a task of an
-// HBM window or a unit of a GEMM window, in lane owner_lane[o], pushes at most owner_pushes[o] entries).  `entries`, the
-// initial ready entries in the order a FIFO ring would hold them, becomes the image of the whole ring that the reset
-// kernels write: each entry at the start of its lane's segment, in the same order within a lane.
-static int build_lane_ring(pb2_window_t* w, const std::vector<uint8_t>& owner_lane, const std::vector<uint32_t>& owner_pushes,
-                           std::vector<int32_t>& entries, bool unit_entries) {
+// Cut the ring into one segment per lane, as long as the entries the lane's owners can ever push (owner o, in lane
+// p.owner_lane[o], pushes at most p.owner_pushes[o] entries).  p.entries becomes the image of the whole ring that the
+// reset kernel writes: each entry at the start of its owner's lane's segment, in the same order within a lane.
+static int build_lane_ring(pb2_window_t* w, WindowPlan& p) {
     Lanes h;
     memset(&h, 0, sizeof h);
     uint32_t size[PB2_PRIO_LANES] = {0};
-    for (size_t o = 0; o < owner_lane.size(); ++o) size[owner_lane[o]] += owner_pushes[o];
+    for (size_t o = 0; o < p.owner_lane.size(); ++o) size[p.owner_lane[o]] += p.owner_pushes[o];
     uint32_t b = 0;
     for (int l = 0; l < PB2_PRIO_LANES; ++l) { h.begin[l] = b; b += size[l]; }
     std::vector<int32_t> ring(b, kEmpty);
-    for (const int32_t e : entries) {
-        const int l = owner_lane[(size_t)(unit_entries ? PB2_SUCC_TASK((uint32_t)e) : PB2_ENT_TASK(e))];
-        ring[h.begin[l] + h.ninit[l]++] = e;
+    for (size_t i = 0; i < p.entries.size(); ++i) {
+        const int l = p.owner_lane[(size_t)p.entry_owner[i]];
+        ring[h.begin[l] + h.ninit[l]++] = p.entries[i];
     }
-    entries.swap(ring);
+    p.entries.swap(ring);
     int rc;
     Lanes* d_lanes = nullptr;
     uint8_t* d_lane = nullptr;
     if ((rc = dev_alloc_copy(w, &d_lanes, &h, 1)) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &d_lane, owner_lane.data(), owner_lane.size())) != PB2_SUCCESS) return rc;
-    w->d.lanes = d_lanes; w->d.lane = d_lane;
+    if ((rc = dev_alloc_copy(w, &d_lane, p.owner_lane.data(), p.owner_lane.size())) != PB2_SUCCESS) return rc;
+    w->g.w.lanes = d_lanes; w->g.w.lane = d_lane;
     return PB2_SUCCESS;
 }
 
 // ---------------------------------------------------------------------------------------------
 // GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
-// task_lane (queue_policy 1, else null): a unit's lane is the lane of its first task, for all its parts.
-// A unit that runs an HBM body is cut into task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide
-// tasks.
-static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
-                             const int32_t* ready, int32_t nready, bool fuse, uint32_t* ring_cap_needed,
-                             const int32_t* rs_begin, const std::vector<uint8_t>* task_lane,
-                             const pb2_tile_t* tiles, int32_t part_bytes) {
+// The plan of a GEMM window: its units are the ring-entry owners.  task_lane (queue_policy 1, else empty): a unit's
+// lane is the lane of its first task, for all its parts.  A unit that runs an HBM body is cut into
+// task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.  Uploads the CSR and the unit arrays.
+static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ, int32_t nsucc,
+                             const int32_t* ready, int32_t nready, bool fuse, const int32_t* rs_begin,
+                             const std::vector<uint8_t>& task_lane, const pb2_tile_t* tiles, int32_t part_bytes,
+                             WindowPlan& plan) {
     std::vector<int32_t> indeg((size_t)ntasks, 0), cpred((size_t)ntasks, -1), ccons((size_t)ntasks, 0), next((size_t)ntasks, -1);
     auto is_gemm = [&](int32_t t) { return tasks[t].body == PB2_BODY_GEMM_BF16; };
     for (int32_t u = 0; u < ntasks; ++u)
@@ -368,7 +367,6 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         }
         u.succ_count = (int32_t)usucc.size() - u.succ_begin;
     }
-    std::vector<int32_t> entries;
     uint32_t total_parts = 0;
     for (const GUnit& u : units) total_parts += (uint32_t)u.nparts;
     // Ready GEMM units enter the ring in Z-order of their (locals[0], locals[1]) = C(i,j) coordinates: the units
@@ -390,29 +388,32 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     }
     std::stable_sort(order.begin(), order.end(), [](const std::pair<uint64_t, int32_t>& a, const std::pair<uint64_t, int32_t>& b) { return a.first < b.first; });
     for (auto& o : order)
-        for (int32_t p = 0; p < units[o.second].nparts; ++p) entries.push_back((int32_t)PB2_SUCC_MAKE(o.second, p));
-    *ring_cap_needed = total_parts;
-    int rc;
-    if (task_lane) {
-        std::vector<uint8_t> ulane(units.size());
-        std::vector<uint32_t> upush(units.size());
-        for (size_t u = 0; u < units.size(); ++u) {
-            ulane[u] = (*task_lane)[(size_t)segs[(size_t)units[u].seg_begin].task];
-            upush[u] = (uint32_t)units[u].nparts;
+        for (int32_t p = 0; p < units[o.second].nparts; ++p) {
+            plan.entries.push_back((int32_t)PB2_SUCC_MAKE(o.second, p));
+            plan.entry_owner.push_back(o.second);
         }
-        if ((rc = build_lane_ring(w, ulane, upush, entries, true)) != PB2_SUCCESS) return rc;
-    }
-    GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
+    if (!task_lane.empty())
+        for (const GUnit& u : units) {
+            plan.owner_lane.push_back(task_lane[(size_t)segs[(size_t)u.seg_begin].task]);
+            plan.owner_pushes.push_back((uint32_t)u.nparts);
+        }
+    plan.ring_slots = (uint32_t)ntasks + total_parts;
+    // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every worker
+    // that needs them (the parts of one unit, the units that share an operand) instead of by one worker alone
+    plan.slice_bytes = 64 * 1024;
+    plan.claims = true;
+    w->task_entry.resize((size_t)ntasks);
+    for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
+    int rc;
+    uint32_t* d_succ = nullptr; GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
+    if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_units, units.data(), units.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_segs, segs.data(), segs.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_usucc, usucc.data(), usucc.size())) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &w->d_ready_entries, entries.data(), entries.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &w->g.udep, (const int32_t*)nullptr, units.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &w->g.parts_left, (const int32_t*)nullptr, units.size())) != PB2_SUCCESS) return rc;
-    w->task_entry.assign((size_t)ntasks, -1);
-    for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
+    w->g.w.succ = d_succ;
     w->g.units = d_units; w->g.segs = d_segs; w->g.usucc = d_usucc; w->g.nunits = (int32_t)units.size();
-    w->nentries = (int32_t)entries.size();
     return PB2_SUCCESS;
 }
 
@@ -506,6 +507,62 @@ static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* suc
     if (gmem.empty()) return false;
     for (size_t u = 0; u < n; ++u) { tasks[u].succ_begin = begin[u]; tasks[u].succ_count = count[u]; }
     return true;
+}
+
+// The plan of an HBM window: its tasks are the ring-entry owners, each cut into task_parts(..., PB2_MAX_PARTS) parts.
+// task_lane: as for build_gemm2_units.  Forms the read groups (which rewrites the out-edges of dtasks) and uploads the
+// CSR, the group arrays and, with wide tasks, the part counts.
+static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, const uint32_t* succ, int32_t nsucc,
+                           const pb2_tile_t* tiles, int32_t ntiles, const int32_t* ready, int32_t nready,
+                           const std::vector<uint8_t>& task_lane, WindowPlan& plan) {
+    pb2_engine_t* e = w->e;
+    WinDev& d = w->g.w;
+    const int32_t ntasks = (int32_t)dtasks.size();
+    std::vector<uint16_t> nparts((size_t)ntasks);
+    uint32_t extra_parts = 0;
+    w->task_entry.resize((size_t)ntasks);
+    for (int32_t i = 0; i < ntasks; ++i) {
+        const int np = task_parts(dtasks[(size_t)i], [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
+        nparts[(size_t)i] = (uint16_t)np; extra_parts += (uint32_t)np - 1;
+        w->task_entry[(size_t)i] = PB2_ENT_MAKE(i, np - 1);
+    }
+    for (int32_t i = 0; i < nready; ++i)
+        for (int p = 0; p < (int)nparts[(size_t)ready[i]]; ++p) {
+            plan.entries.push_back(PB2_ENT_MAKE(ready[i], p));
+            plan.entry_owner.push_back(ready[i]);
+        }
+    if (!task_lane.empty()) { plan.owner_lane = task_lane; plan.owner_pushes.assign(nparts.begin(), nparts.end()); }
+    plan.ring_slots = (uint32_t)ntasks + extra_parts;
+    // Stage-in is cut finer than tasks are: a tile that has to come from the host or a peer GPU is pulled in slices
+    // by EVERY worker that needs it (claim bit per slice), so the readers of a tile share the transfer instead of one
+    // moving it while the others wait.
+    plan.slice_bytes = stage_slice(e->stage_slice_bytes, e->params.part_bytes);
+    plan.claims = extra_parts > 0;
+    for (int32_t i = 0; i < ntiles && !plan.claims; ++i)
+        plan.claims = plan.slice_bytes > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)plan.slice_bytes;
+    // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
+    std::vector<uint32_t> gsucc, group;
+    std::vector<int32_t> gmem;
+    const bool grouped = !w->shared && e->params.read_groups >= 0 &&
+                         form_read_groups(dtasks, succ, ready, nready, tiles, e->params.fuse_readers >= 0 && e->nworkers > 1,
+                                          gsucc, group, gmem);
+    int rc;
+    uint32_t* d_succ = nullptr;
+    if (grouped) {
+        uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
+        if ((rc = dev_alloc_copy(w, &d_succ, gsucc.data(), gsucc.size())) != PB2_SUCCESS) return rc;
+        if ((rc = dev_alloc_copy(w, &d_group, group.data(), group.size())) != PB2_SUCCESS) return rc;
+        if ((rc = dev_alloc_copy(w, &d_gmem, gmem.data(), gmem.size())) != PB2_SUCCESS) return rc;
+        d.group = d_group; d.group_mem = d_gmem;
+    } else if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
+    d.succ = d_succ;
+    if (extra_parts) {
+        uint16_t* d_np = nullptr;
+        if ((rc = dev_alloc_copy(w, &d_np, nparts.data(), nparts.size())) != PB2_SUCCESS) return rc;
+        if ((rc = dev_alloc_copy(w, &d.parts_left, (const int32_t*)nullptr, (size_t)ntasks)) != PB2_SUCCESS) return rc;
+        d.nparts = d_np;
+    }
+    return PB2_SUCCESS;
 }
 
 extern "C" {
@@ -812,56 +869,36 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     pb2_window_t* w = new pb2_window_s();
     w->shared = e->shared_windows;
-    w->e = e; w->kind = kind; w->ntasks = ntasks; w->nsucc = nsucc; w->ntiles = ntiles; w->nready = nready;
+    w->e = e; w->kind = kind; w->ntasks = ntasks; w->ntiles = ntiles;
 #define TRY(x) do { rc = (x); if (rc != PB2_SUCCESS) { pb2_window_destroy(w); return rc; } } while (0)
-    // wide tasks (HBM windows): at most PB2_MAX_PARTS parts per task
+    WinDev& d = w->g.w;
     std::vector<pb2_task_t> dtasks(tasks, tasks + ntasks);
-    std::vector<uint16_t> nparts((size_t)ntasks, 1);
-    std::vector<int32_t> entries;
-    uint32_t extra_parts = 0;
-    for (int32_t i = 0; i < ntasks; ++i) {
-        pb2_task_t& t = dtasks[i];
-        t.flags &= 0x07;
-        if (kind != 0) continue;
-        const int np = task_parts(t, [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
-        nparts[(size_t)i] = (uint16_t)np; extra_parts += (uint32_t)np - 1;
-    }
-    for (int32_t i = 0; i < nready; ++i)
-        for (int p = 0; p < (int)nparts[(size_t)ready[i]]; ++p) entries.push_back(PB2_ENT_MAKE(ready[i], p));
-    w->task_entry.resize((size_t)ntasks);
-    for (int32_t i = 0; i < ntasks; ++i) w->task_entry[(size_t)i] = PB2_ENT_MAKE(i, (int)nparts[(size_t)i] - 1);
-    // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
-    std::vector<uint32_t> gsucc, group;
-    std::vector<int32_t> gmem;
-    const bool grouped = kind == 0 && !w->shared && e->params.read_groups >= 0 &&
-                         form_read_groups(dtasks, succ, ready, nready, tiles, e->params.fuse_readers >= 0 && e->nworkers > 1,
-                                          gsucc, group, gmem);
-    TRY(dev_alloc_copy(w, &w->d_tasks, dtasks.data(), (size_t)ntasks));
-    if (grouped) TRY(dev_alloc_copy(w, &w->d_succ, gsucc.data(), gsucc.size()));
-    else TRY(dev_alloc_copy(w, &w->d_succ, succ, (size_t)nsucc));
-    TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
-    TRY(dev_alloc_copy(w, &w->d_tiles, (const pb2_tile_t*)nullptr, (size_t)ntiles));
+    for (pb2_task_t& t : dtasks) t.flags &= 0x07;
     int32_t nlanes = 0;
     std::vector<uint8_t> task_lane;
     if (prio) task_lane = task_priority_lanes(tasks, ntasks, &nlanes);
-    if (prio && kind == 0) TRY(build_lane_ring(w, task_lane, std::vector<uint32_t>(nparts.begin(), nparts.end()), entries, false));
-    TRY(dev_alloc_copy(w, &w->d_ready, entries.data(), entries.size()));
-    w->nready_entries = (int32_t)entries.size();
-    uint32_t parts_needed = 0;
-    if (kind == 1) {
+    WindowPlan plan;
+    if (kind == 0) TRY(plan_hbm_window(w, dtasks, succ, nsucc, tiles, ntiles, ready, nready, task_lane, plan));
+    else {
         // HBM bodies of a GEMM window are cut into parts as HBM windows cut them.  Not in shared windows: their units
         // are released by peers over NVLink, and the multi-GPU runs that check those releases cover single-part HBM
         // units only, so shared windows keep one part per HBM unit.
         const int32_t hbm_part_bytes = w->shared ? 0 : e->params.part_bytes;
         TRY(build_tensor_maps(w, tasks, ntasks, tiles, ntiles));
-        TRY(build_gemm2_units(w, tasks, ntasks, succ, ready, nready, e->params.gemm_mode == 0, &parts_needed,
-                              w->shared ? e->next_rs_begin : nullptr, prio ? &task_lane : nullptr, tiles, hbm_part_bytes));
+        TRY(build_gemm2_units(w, tasks, ntasks, succ, nsucc, ready, nready, e->params.gemm_mode == 0,
+                              w->shared ? e->next_rs_begin : nullptr, task_lane, tiles, hbm_part_bytes, plan));
     }
+    if (prio) TRY(build_lane_ring(w, plan));
+    TRY(dev_alloc_copy(w, &w->d_ready, plan.entries.data(), plan.entries.size()));
+    w->nready_entries = (int32_t)plan.entries.size();
     const int maxw = e->nworkers > e->nworkers_gemm ? e->nworkers : e->nworkers_gemm;
     uint32_t cap = 1024;
-    while (cap < (uint32_t)ntasks + extra_parts + parts_needed + (uint32_t)maxw + 2u) cap <<= 1;   // every slot is used at most once per run
-    WinDev& d = w->d;
-    d.tasks = w->d_tasks; d.succ = w->d_succ; d.tiles = w->d_tiles;
+    while (cap < plan.ring_slots + (uint32_t)maxw + 2u) cap <<= 1;   // every slot is used at most once per run
+    pb2_task_t* d_tasks = nullptr;
+    TRY(dev_alloc_copy(w, &d_tasks, dtasks.data(), (size_t)ntasks));
+    d.tasks = d_tasks;
+    TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
+    TRY(dev_alloc_copy(w, &d.tiles, (const pb2_tile_t*)nullptr, (size_t)ntiles));
     TRY(dev_alloc_copy(w, &d.dep, (const int32_t*)nullptr, (size_t)ntasks));
     TRY(dev_alloc_copy(w, &d.ring, (const int32_t*)nullptr, (size_t)cap));
     TRY(dev_alloc_copy(w, &d.ctl, (const Ctl*)nullptr, 1));
@@ -871,50 +908,14 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     TRY(dev_alloc_copy(w, &d.seen_version, (const uint32_t*)nullptr, (size_t)ntasks * PB2_MAX_FLOWS));
     TRY(dev_alloc_copy(w, &d.result, (const unsigned long long*)nullptr, (size_t)ntasks));
     TRY(dev_alloc_copy(w, &d.worker, (const int32_t*)nullptr, (size_t)ntasks));
-    d.parts_left = nullptr; d.rs_begin = nullptr; d.rs_rank = nullptr; d.rs_target = nullptr; d.peers = nullptr; d.shared = w->shared ? 1 : 0;
-    d.ps_begin = nullptr; d.ps = nullptr;
-    d.slice_claim = nullptr; d.slice_done = nullptr; d.part_bytes = e->params.part_bytes;
-    d.nparts = nullptr; d.remote_units = 0;
-    d.group = nullptr; d.group_mem = nullptr;
-    d.nlanes = nlanes;          // d.lanes / d.lane: build_lane_ring
-    if (grouped) {
-        uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
-        TRY(dev_alloc_copy(w, &d_group, group.data(), group.size()));
-        TRY(dev_alloc_copy(w, &d_gmem, gmem.data(), gmem.size()));
-        d.group = d_group; d.group_mem = d_gmem;
-    }
-    if (kind == 0 && extra_parts) {
-        uint16_t* d_np = nullptr;
-        TRY(dev_alloc_copy(w, &d_np, nparts.data(), (size_t)ntasks));
-        d.nparts = d_np;
-        TRY(dev_alloc_copy(w, &d.parts_left, (const int32_t*)nullptr, (size_t)ntasks));
-    }
-    if (kind == 0) {
-        // Stage-in is cut finer than tasks are: a tile that has to come from the host or a peer GPU is pulled in slices
-        // of stage_slice_bytes by EVERY worker that needs it (claim bit per slice), so the readers of a tile share the
-        // transfer instead of one moving it while the others wait.
-        int32_t slice = e->stage_slice_bytes > 0 ? e->stage_slice_bytes : 0;
-        if (e->params.part_bytes > 0 && (slice == 0 || e->params.part_bytes < slice)) slice = e->params.part_bytes;
-        bool sliced = false;
-        for (int32_t i = 0; i < ntiles && !sliced; ++i)
-            sliced = slice > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)slice;
-        if (sliced || extra_parts) {
-            d.part_bytes = slice > 0 ? slice : e->params.part_bytes;
-            TRY(dev_alloc_copy(w, &d.slice_claim, (const uint32_t*)nullptr, (size_t)ntiles * PB2_SLICE_WORDS));
-            TRY(dev_alloc_copy(w, &d.slice_done, (const uint32_t*)nullptr, (size_t)ntiles * (PB2_SLICE_WORDS + 1)));
-        }
-    }
-    if (kind == 1) {
-        // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every worker
-        // that needs them (the parts of one unit, the units that share an operand) instead of by one worker alone
-        d.part_bytes = 64 * 1024;
+    if (plan.claims) {
         TRY(dev_alloc_copy(w, &d.slice_claim, (const uint32_t*)nullptr, (size_t)ntiles * PB2_SLICE_WORDS));
         TRY(dev_alloc_copy(w, &d.slice_done, (const uint32_t*)nullptr, (size_t)ntiles * (PB2_SLICE_WORDS + 1)));
     }
 #undef TRY
+    d.part_bytes = plan.slice_bytes; d.shared = w->shared ? 1 : 0; d.nlanes = nlanes;
     d.cap_mask = cap - 1; d.ntasks = ntasks; d.ntiles = ntiles; d.stage_mode = e->params.stage_mode;
     d.timeout_ns = (unsigned long long)e->params.timeout_ms * 1000000ull;
-    if (kind == 1) { w->g.w = d; w->g.tmaps = w->d_tmaps; w->g.fresh_tmaps = 1; }
     PB2_CUDA(e, cudaEventCreate(&w->ev0));
     PB2_CUDA(e, cudaEventCreate(&w->ev1));
     PB2_CUDA(e, cudaEventCreate(&w->ev2));
@@ -951,15 +952,11 @@ int pb2_window_arm(pb2_window_t* w) {
     PB2_CUDA(e, cudaEventRecord(w->ev0, e->stream));
     {
         const int threads = 256;
-        size_t n = (size_t)w->ntasks > (size_t)w->d.cap_mask + 1 ? (size_t)w->ntasks : (size_t)w->d.cap_mask + 1;
+        size_t n = (size_t)w->ntasks > (size_t)w->g.w.cap_mask + 1 ? (size_t)w->ntasks : (size_t)w->g.w.cap_mask + 1;
         int blocks = (int)((n + threads - 1) / threads);
         if (blocks > e->prop.multiProcessorCount * 8) blocks = e->prop.multiProcessorCount * 8;
         if (blocks < 1) blocks = 1;
-        pb2_window_reset_kernel<<<blocks, threads, 0, e->stream>>>(w->d, w->d_tiles_init, w->d_ready, w->nready_entries);
-        PB2_CUDA(e, cudaGetLastError());
-    }
-    if (w->ntasks > 0 && w->kind == 1) {
-        pb2_window2_reset_kernel<<<64, 256, 0, e->stream>>>(w->g, w->d_ready_entries, w->nentries);
+        pb2_window_reset_kernel<<<blocks, threads, 0, e->stream>>>(w->g, w->d_tiles_init, w->d_ready, w->nready_entries);
         PB2_CUDA(e, cudaGetLastError());
     }
     PB2_CUDA(e, cudaEventRecord(w->ev1, e->stream));
@@ -972,13 +969,13 @@ int pb2_window_start(pb2_window_t* w) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
         if (w->kind == 0) {
-            if (w->d.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(w->d, e->nworkers, e->params.threads, e->stream));
+            if (w->g.w.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(w->g.w, e->nworkers, e->params.threads, e->stream));
             else {
-                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(w->d);
+                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(w->g.w);
                 PB2_CUDA(e, cudaGetLastError());
             }
         } else {
-            int rc = w->d.lanes ? pb2_gemm2_prio_launch(w->g, e->nworkers_gemm, e->stream)
+            int rc = w->g.w.lanes ? pb2_gemm2_prio_launch(w->g, e->nworkers_gemm, e->stream)
                                 : pb2_gemm2_launch<false>(w->g, e->nworkers_gemm, e->stream);
             if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
             w->g.fresh_tmaps = 0;
@@ -1001,18 +998,18 @@ int pb2_window_export(pb2_window_t* w, pb2_window_handle_t* h) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     memset(h, 0, sizeof *h);
     cudaIpcMemHandle_t ih;
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->kind == 1 ? w->g.udep : w->d.dep));  memcpy(h->dep, &ih, 64);   // GEMM windows: unit words
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.ring)); memcpy(h->ring, &ih, 64);
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.ctl));  memcpy(h->ctl, &ih, 64);
-    if (w->d.tiles && w->ntiles > 0) { PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->d.tiles)); memcpy(h->tiles, &ih, 64); h->ntiles = w->ntiles; }
-    h->cap_mask = w->d.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->kind == 1 ? 1 : 0;
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->kind == 1 ? w->g.udep : w->g.w.dep));  memcpy(h->dep, &ih, 64);   // GEMM windows: unit words
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.ring)); memcpy(h->ring, &ih, 64);
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.ctl));  memcpy(h->ctl, &ih, 64);
+    if (w->g.w.tiles && w->ntiles > 0) { PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.tiles)); memcpy(h->tiles, &ih, 64); h->ntiles = w->ntiles; }
+    h->cap_mask = w->g.w.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->kind == 1 ? 1 : 0;
     return PB2_SUCCESS;
 }
 
 int pb2_window_set_push(pb2_window_t* w, const int32_t* ps_begin, const pb2_push_t* push, int32_t npush) {
     if (!w || !ps_begin || npush < 0 || (npush && !push)) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
-    if (w->kind == 1 || !w->d.peers) { e->last_error = "pushes need an HBM window whose remote edges are set (pb2_window_set_remote)"; return PB2_ERR_NOT_SUPPORTED; }
+    if (w->kind == 1 || !w->g.w.peers) { e->last_error = "pushes need an HBM window whose remote edges are set (pb2_window_set_remote)"; return PB2_ERR_NOT_SUPPORTED; }
     if (ps_begin[w->ntasks] != npush) return PB2_ERR_BAD_PARAM;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     std::vector<PushDev> pd((size_t)npush);
@@ -1030,7 +1027,7 @@ int pb2_window_set_push(pb2_window_t* w, const int32_t* ps_begin, const pb2_push
     if ((rc = dev_alloc_copy(w, &d_b, ps_begin, (size_t)w->ntasks + 1)) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_p, pd.data(), pd.size())) != PB2_SUCCESS) return rc;
     PB2_CUDA(e, cudaStreamSynchronize(e->up_stream));
-    w->d.ps_begin = npush ? d_b : nullptr; w->d.ps = d_p;
+    w->g.w.ps_begin = npush ? d_b : nullptr; w->g.w.ps = d_p;
     return PB2_SUCCESS;
 }
 
@@ -1077,8 +1074,7 @@ int pb2_window_set_remote(pb2_window_t* w, int32_t my_rank, int32_t nranks, cons
     if ((rc = dev_alloc_copy(w, &d_r, rs_rank, (size_t)nrs)) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_t, rs_target, (size_t)nrs)) != PB2_SUCCESS) return rc;
     PB2_CUDA(e, cudaStreamSynchronize(e->up_stream));
-    w->d.peers = d_pw; w->d.rs_begin = d_b; w->d.rs_rank = d_r; w->d.rs_target = d_t; w->d.remote_units = my_kind;
-    if (w->kind == 1) w->g.w = w->d;
+    w->g.w.peers = d_pw; w->g.w.rs_begin = d_b; w->g.w.rs_rank = d_r; w->g.w.rs_target = d_t; w->g.w.remote_units = my_kind;
     return PB2_SUCCESS;
 }
 
@@ -1089,7 +1085,7 @@ int pb2_window_wait(pb2_window_t* w, pb2_window_stats_t* stats) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaEventSynchronize(w->ev2));
     Ctl c;
-    PB2_CUDA(e, cudaMemcpy(&c, w->d.ctl, sizeof c, cudaMemcpyDeviceToHost));
+    PB2_CUDA(e, cudaMemcpy(&c, w->g.w.ctl, sizeof c, cudaMemcpyDeviceToHost));
     if (stats) {
         memset(stats, 0, sizeof *stats);
         stats->tasks_retired = c.retired.v;
@@ -1111,13 +1107,13 @@ int pb2_window_results(pb2_window_t* w, int32_t* retire_order, uint32_t* start_s
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     const size_t n = (size_t)w->ntasks;
-    if (retire_order && n) PB2_CUDA(e, cudaMemcpy(retire_order, w->d.retire_log, n * 4, cudaMemcpyDeviceToHost));
-    if (start_seq && n) PB2_CUDA(e, cudaMemcpy(start_seq, w->d.start_seq, n * 4, cudaMemcpyDeviceToHost));
-    if (end_seq && n) PB2_CUDA(e, cudaMemcpy(end_seq, w->d.end_seq, n * 4, cudaMemcpyDeviceToHost));
-    if (seen_version && n) PB2_CUDA(e, cudaMemcpy(seen_version, w->d.seen_version, n * 4 * PB2_MAX_FLOWS, cudaMemcpyDeviceToHost));
-    if (result && n) PB2_CUDA(e, cudaMemcpy(result, w->d.result, n * 8, cudaMemcpyDeviceToHost));
-    if (worker && n) PB2_CUDA(e, cudaMemcpy(worker, w->d.worker, n * 4, cudaMemcpyDeviceToHost));
-    if (tiles_out && w->ntiles) PB2_CUDA(e, cudaMemcpy(tiles_out, w->d_tiles, (size_t)w->ntiles * sizeof(pb2_tile_t), cudaMemcpyDeviceToHost));
+    if (retire_order && n) PB2_CUDA(e, cudaMemcpy(retire_order, w->g.w.retire_log, n * 4, cudaMemcpyDeviceToHost));
+    if (start_seq && n) PB2_CUDA(e, cudaMemcpy(start_seq, w->g.w.start_seq, n * 4, cudaMemcpyDeviceToHost));
+    if (end_seq && n) PB2_CUDA(e, cudaMemcpy(end_seq, w->g.w.end_seq, n * 4, cudaMemcpyDeviceToHost));
+    if (seen_version && n) PB2_CUDA(e, cudaMemcpy(seen_version, w->g.w.seen_version, n * 4 * PB2_MAX_FLOWS, cudaMemcpyDeviceToHost));
+    if (result && n) PB2_CUDA(e, cudaMemcpy(result, w->g.w.result, n * 8, cudaMemcpyDeviceToHost));
+    if (worker && n) PB2_CUDA(e, cudaMemcpy(worker, w->g.w.worker, n * 4, cudaMemcpyDeviceToHost));
+    if (tiles_out && w->ntiles) PB2_CUDA(e, cudaMemcpy(tiles_out, w->g.w.tiles, (size_t)w->ntiles * sizeof(pb2_tile_t), cudaMemcpyDeviceToHost));
     return PB2_SUCCESS;
 }
 

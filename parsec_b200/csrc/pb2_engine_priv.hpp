@@ -1,4 +1,4 @@
-// pb2_engine_priv.hpp -- host-side engine object and part rule shared by the translation units of libparsec_b200.so
+// pb2_engine_priv.hpp -- host-side engine object, part and slice rules shared by the translation units of libparsec_b200.so
 // (pb2_engine.cu: windows; pb2_stream.cu: the streaming ring + persistent kernel).
 #pragma once
 #include <cuda_runtime.h>
@@ -42,6 +42,12 @@ static inline int task_parts(const pb2_task_t& t, TileBytes tile_bytes, int32_t 
         if (t.tile[f] >= 0 && tile_bytes(t.tile[f]) > big) big = tile_bytes(t.tile[f]);
     const uint32_t np = (big + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes;
     return np < 1 ? 1 : (np > (uint32_t)cap ? cap : (int)np);
+}
+
+// The stage-in slice size of HBM windows and streams: the smaller of stage_slice_bytes and part_bytes among those that
+// are positive, so a tile is never staged in coarser slices than wide tasks are cut into; part_bytes when neither is.
+static inline int32_t stage_slice(int32_t stage_slice_bytes, int32_t part_bytes) {
+    return (stage_slice_bytes > 0 && (part_bytes <= 0 || stage_slice_bytes < part_bytes)) ? stage_slice_bytes : part_bytes;
 }
 
 #define PB2_CUDA(e, call)                                                                        \

@@ -516,8 +516,7 @@ int pb2_stream_create(pb2_engine_t* e, const pb2_stream_params_t* params, pb2_st
 #undef TRY
     w.cap_mask = s->ring_cap - 1; w.ntasks = (int32_t)s->slots; w.ntiles = p.max_tiles;
     w.stage_mode = e->params.stage_mode;
-    // device-side slicing of stage-in (see pb2_window_create): finer than the parts of wide tasks
-    w.part_bytes = (e->stage_slice_bytes > 0 && (p.part_bytes <= 0 || e->stage_slice_bytes < p.part_bytes)) ? e->stage_slice_bytes : p.part_bytes;
+    w.part_bytes = stage_slice(e->stage_slice_bytes, p.part_bytes);     // device-side slicing of stage-in
     w.timeout_ns = (unsigned long long)p.timeout_ms * 1000000ull;
     d.idle_ns = (unsigned long long)p.idle_us * 1000ull;
     STREAM_CUDA(s, cudaStreamCreateWithFlags(&s->kstream, cudaStreamNonBlocking));
