@@ -260,7 +260,11 @@ int  pb2_window_create(pb2_engine_t* engine, pb2_window_t** window, int kind,
                        const pb2_tile_t* tiles, int32_t ntiles,
                        const int32_t* ready, int32_t nready);
 int  pb2_window_destroy(pb2_window_t* window);
-/* (re)arm dependency words, ring, counters, tile states; then launch; both are stream-ordered */
+/* (re)arm the window's per-run state (dependency words, ring, counters, tile states, cleared outputs); then launch; both
+ * are stream-ordered.  A non-shared HBM window keeps two copies of that state and alternates between them: each launch
+ * queues the reset of the other copy, for the next launch, on a stream of its own beside the run, so from a window's
+ * third launch on the arm launches nothing (its reset_ms reads about 0).  Waits, stats and results are those of the
+ * last launch. */
 int  pb2_window_launch(pb2_window_t* window);
 /* block until the window retired all its tasks (or the watchdog tripped); fills stats */
 int  pb2_window_wait(pb2_window_t* window, pb2_window_stats_t* stats);
@@ -295,7 +299,10 @@ int  pb2_window_export(pb2_window_t* window, pb2_window_handle_t* handle);
 int  pb2_window_set_remote(pb2_window_t* window, int32_t my_rank, int32_t nranks, const pb2_window_handle_t* peers,
                            const int32_t* rs_begin, const int32_t* rs_rank, const uint32_t* rs_target, int32_t nrs);
 /* two-phase launch for windows that are released into by peers: every rank arms, all ranks synchronise, every
- * rank starts.  pb2_window_launch == arm + start. */
+ * rank starts.  pb2_window_launch == arm + start.  arm picks the copy of the per-run state the next start runs on (the
+ * other one than the last start's, in a non-shared HBM window) and runs the reset kernel on it unless the last start
+ * queued that reset already (then the engine stream waits for it); shared windows and GEMM windows have one copy,
+ * which every arm resets. */
 int  pb2_window_arm(pb2_window_t* window);
 int  pb2_window_start(pb2_window_t* window);
 

@@ -36,48 +36,14 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // reset: (re)arm one window.  dep words, ring, counters, tile table; the units of a GEMM window.
 // ---------------------------------------------------------------------------------------------
-// queue_policy 1: every lane starts with its initial entries, which the ring image `ready` holds at the start of the
-// lane's segment (empty slots kEmpty).
-__device__ __forceinline__ void reset_lanes(Lanes* lanes, size_t gid) {
-    if (lanes && gid < PB2_PRIO_LANES) {
-        lanes->head[gid].v = lanes->begin[gid];
-        lanes->tail[gid].v = (unsigned long long)lanes->begin[gid] + lanes->ninit[gid];
-        lanes->avail[gid].v = lanes->ninit[gid];
-    }
-}
-
-// `ready` is the window's image of its first nready ring slots.  A GEMM window never has more units than tasks.
+// The per-run state of g.w (rearm_run) and, in a GEMM window, its units' words.  A GEMM window never has more units
+// than tasks.
 __global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
-    const WinDev& w = g.w;
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
     for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
-    for (size_t i = gid; i < (size_t)w.ntasks; i += gsz) {
-        const pb2_task_t& t = w.tasks[i];
-        // counter mode counts down from the goal (parsec.c:1625-1633); mask mode ORs up from 0 (:1693-1703)
-        w.dep[i] = (t.flags & PB2_TASK_DEPS_MASK) ? 0 : t.dep_goal;
-        if (w.parts_left) w.parts_left[i] = task_nparts(w, (int32_t)i);
-        w.start_seq[i] = 0; w.end_seq[i] = 0; w.result[i] = 0; w.worker[i] = -1; w.retire_log[i] = -1;
-        for (int f = 0; f < PB2_MAX_FLOWS; ++f) w.seen_version[i * PB2_MAX_FLOWS + f] = 0;
-    }
-    for (size_t i = gid; i <= (size_t)w.cap_mask; i += gsz)
-        w.ring[i] = (i < (size_t)nready) ? ready[i] : kEmpty;
-    for (size_t i = gid; i < (size_t)w.ntiles; i += gsz) {
-        w.tiles[i] = tiles_init[i];
-        if (w.slice_claim) {
-            for (int k = 0; k < PB2_SLICE_WORDS; ++k) w.slice_claim[i * PB2_SLICE_WORDS + k] = 0;
-            for (int k = 0; k <= PB2_SLICE_WORDS; ++k) w.slice_done[i * (PB2_SLICE_WORDS + 1) + k] = 0;
-        }
-    }
-    reset_lanes(w.lanes, gid);
-    if (gid == 0) {
-        w.ctl->head.v = 0; w.ctl->tail.v = (unsigned long long)nready; w.ctl->evt.v = 0;
-        w.ctl->retired.v = 0; w.ctl->done.v = (w.ntasks == 0) ? kDoneOK : 0;
-        w.ctl->progress_ns.v = globaltimer_ns();
-        w.ctl->bytes_h2d.v = 0; w.ctl->bytes_d2d.v = 0; w.ctl->bytes_d2h.v = 0;
-        w.ctl->stage_ins.v = 0; w.ctl->body_errors.v = 0;
-    }
+    rearm_run(g.w, tiles_init, ready, nready, gid, gsz);
 }
 
 // The same bodies as a stand-alone kernel on a caller's stream: what a BODY [type=CUDA] enqueues when it runs under a
@@ -138,6 +104,17 @@ struct pb2_window_s {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
     bool launched = false;
     bool shared = false;
+    // A non-shared HBM window with tasks keeps two copies of its per-run state (rearm_run's arrays): g.w's and, from
+    // its second arm on, run1's.  Consecutive runs alternate between them, and while a run runs, the reset kernel
+    // arms the other copy for the next one on the engine's arm stream (ev_arm: its end).  cur: the copy of the last
+    // arm; armed[c]: copy c is armed, or will be by work already queued, and no run has used it since; beside[c]:
+    // that work is the reset on the arm stream.
+    WinDev run1{};
+    int cur = 0;
+    int arms = 0;
+    bool armed[2] = {false, false};
+    bool beside[2] = {false, false};
+    cudaEvent_t ev_arm = nullptr;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
     std::vector<void*> allocs;
     std::vector<void*> peer_ptrs;
@@ -565,6 +542,55 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
     return PB2_SUCCESS;
 }
 
+// The descriptor of run-state copy c of window w: g.w with copy c's per-run arrays.
+static WinDev run_desc(const pb2_window_t* w, int c) {
+    WinDev d = w->g.w;
+    if (c == 1) {
+        const WinDev& r = w->run1;
+        d.tiles = r.tiles; d.dep = r.dep; d.ring = r.ring; d.ctl = r.ctl; d.retire_log = r.retire_log;
+        d.start_seq = r.start_seq; d.end_seq = r.end_seq; d.seen_version = r.seen_version; d.result = r.result;
+        d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
+        d.lanes = r.lanes;
+    }
+    return d;
+}
+
+// An array of n T on the engine stream (stream-ordered) where copy 0 has one (src), else none.
+template <class T>
+static cudaError_t alloc_like(pb2_window_t* w, T** dst, const T* src, size_t n) {
+    *dst = nullptr;
+    if (!src) return cudaSuccess;
+    void* p = nullptr;
+    const cudaError_t err = cudaMallocAsync(&p, (n ? n : 1) * sizeof(T), w->e->stream);
+    if (err == cudaSuccess) { w->allocs.push_back(p); *dst = reinterpret_cast<T*>(p); }
+    return err;
+}
+
+// Copy 1 of a window's per-run arrays, shaped as g.w's.  The lanes' segment bounds are constant: copied from copy 0.
+static int alloc_run1(pb2_window_t* w) {
+    pb2_engine_t* e = w->e;
+    const WinDev& d = w->g.w;
+    WinDev& r = w->run1;
+    const size_t nt = (size_t)w->ntasks, nl = (size_t)w->ntiles;
+    auto like = [&](auto** dst, auto* src, size_t n) { return alloc_like(w, dst, src, n); };
+    PB2_CUDA(e, like(&r.tiles, d.tiles, nl));
+    PB2_CUDA(e, like(&r.dep, d.dep, nt));
+    PB2_CUDA(e, like(&r.ring, d.ring, (size_t)d.cap_mask + 1));
+    PB2_CUDA(e, like(&r.ctl, d.ctl, 1));
+    PB2_CUDA(e, like(&r.retire_log, d.retire_log, nt));
+    PB2_CUDA(e, like(&r.start_seq, d.start_seq, nt));
+    PB2_CUDA(e, like(&r.end_seq, d.end_seq, nt));
+    PB2_CUDA(e, like(&r.seen_version, d.seen_version, nt * PB2_MAX_FLOWS));
+    PB2_CUDA(e, like(&r.result, d.result, nt));
+    PB2_CUDA(e, like(&r.worker, d.worker, nt));
+    PB2_CUDA(e, like(&r.parts_left, d.parts_left, nt));
+    PB2_CUDA(e, like(&r.slice_claim, d.slice_claim, nl * PB2_SLICE_WORDS));
+    PB2_CUDA(e, like(&r.slice_done, d.slice_done, nl * (PB2_SLICE_WORDS + 1)));
+    PB2_CUDA(e, like(&r.lanes, d.lanes, 1));
+    if (d.lanes) PB2_CUDA(e, cudaMemcpyAsync(r.lanes, d.lanes, sizeof(Lanes), cudaMemcpyDeviceToDevice, e->stream));
+    return PB2_SUCCESS;
+}
+
 extern "C" {
 
 int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_params_t* params) {
@@ -602,6 +628,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->up_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->dma_stream, cudaStreamNonBlocking));
+    PB2_CUDA(e, cudaStreamCreateWithFlags(&e->arm_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaEventCreateWithFlags(&e->dma_ev, cudaEventDisableTiming));
     e->stream = e->own_stream;
     {   // keep freed window scratch cached in the default mempool instead of returning it to the driver
@@ -630,6 +657,7 @@ int pb2_engine_destroy(pb2_engine_t* e) {
     if (e->own_stream) cudaStreamDestroy(e->own_stream);
     if (e->up_stream) cudaStreamDestroy(e->up_stream);
     if (e->dma_stream) cudaStreamDestroy(e->dma_stream);
+    if (e->arm_stream) cudaStreamDestroy(e->arm_stream);
     if (e->dma_ev) cudaEventDestroy(e->dma_ev);
     delete e;
     return PB2_SUCCESS;
@@ -919,6 +947,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     PB2_CUDA(e, cudaEventCreate(&w->ev0));
     PB2_CUDA(e, cudaEventCreate(&w->ev1));
     PB2_CUDA(e, cudaEventCreate(&w->ev2));
+    PB2_CUDA(e, cudaEventCreateWithFlags(&w->ev_arm, cudaEventDisableTiming));
     // every descriptor array is on the device when this returns (the host vectors above are temporaries); the
     // upload stream is not ordered behind the engine stream, so creating the next window does not wait for the
     // window that is running
@@ -931,12 +960,29 @@ int pb2_window_destroy(pb2_window_t* w) {
     if (!w) return PB2_ERR_BAD_PARAM;
     cudaSetDevice(w->e->cuda_device);
     if (w->launched) cudaEventSynchronize(w->ev2);        // this window only: a later one may be running
+    if (w->beside[0] || w->beside[1]) cudaEventSynchronize(w->ev_arm);     // a reset of the next run's copy
     for (void* p : w->peer_ptrs) cudaIpcCloseMemHandle(p);
     for (void* p : w->allocs) { if (w->shared) cudaFree(p); else cudaFreeAsync(p, w->e->stream); }
     if (w->ev0) cudaEventDestroy(w->ev0);
     if (w->ev1) cudaEventDestroy(w->ev1);
     if (w->ev2) cudaEventDestroy(w->ev2);
+    if (w->ev_arm) cudaEventDestroy(w->ev_arm);
     delete w;
+    return PB2_SUCCESS;
+}
+
+// The reset kernel over run-state copy c of window w on `stream`, at most per_sm 256-thread CTAs per SM.
+static int reset_copy(pb2_window_t* w, int c, cudaStream_t stream, int per_sm) {
+    pb2_engine_t* e = w->e;
+    const int threads = 256;
+    size_t n = (size_t)w->ntasks > (size_t)w->g.w.cap_mask + 1 ? (size_t)w->ntasks : (size_t)w->g.w.cap_mask + 1;
+    int blocks = (int)((n + threads - 1) / threads);
+    if (blocks > e->prop.multiProcessorCount * per_sm) blocks = e->prop.multiProcessorCount * per_sm;
+    if (blocks < 1) blocks = 1;
+    Win2Dev g = w->g;
+    g.w = run_desc(w, c);
+    pb2_window_reset_kernel<<<blocks, threads, 0, stream>>>(g, w->d_tiles_init, w->d_ready, w->nready_entries);
+    PB2_CUDA(e, cudaGetLastError());
     return PB2_SUCCESS;
 }
 
@@ -944,22 +990,28 @@ int pb2_window_arm(pb2_window_t* w) {
     if (!w) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    // shared windows keep one copy (peers hold IPC pointers to it), GEMM windows too (DESIGN.md §5)
+    const bool two = w->kind == 0 && !w->shared && w->ntasks > 0;
+    const int c = two && w->arms > 0 ? w->cur ^ 1 : 0;
+    if (c == 1 && !w->run1.ctl) {
+        const int rc = alloc_run1(w);
+        if (rc != PB2_SUCCESS) return rc;
+    }
     if (e->dma_pending) {                       // prefetches queued for this window land before its first worker starts
         PB2_CUDA(e, cudaEventRecord(e->dma_ev, e->dma_stream));
         PB2_CUDA(e, cudaStreamWaitEvent(e->stream, e->dma_ev, 0));
         e->dma_pending = false;
     }
     PB2_CUDA(e, cudaEventRecord(w->ev0, e->stream));
-    {
-        const int threads = 256;
-        size_t n = (size_t)w->ntasks > (size_t)w->g.w.cap_mask + 1 ? (size_t)w->ntasks : (size_t)w->g.w.cap_mask + 1;
-        int blocks = (int)((n + threads - 1) / threads);
-        if (blocks > e->prop.multiProcessorCount * 8) blocks = e->prop.multiProcessorCount * 8;
-        if (blocks < 1) blocks = 1;
-        pb2_window_reset_kernel<<<blocks, threads, 0, e->stream>>>(w->g, w->d_tiles_init, w->d_ready, w->nready_entries);
-        PB2_CUDA(e, cudaGetLastError());
+    if (!w->armed[c]) {
+        const int rc = reset_copy(w, c, e->stream, 8);
+        if (rc != PB2_SUCCESS) return rc;
+    } else if (w->beside[c]) {
+        // armed beside the last run; a wait here is part of this arm's time (after ev0)
+        PB2_CUDA(e, cudaStreamWaitEvent(e->stream, w->ev_arm, 0));
     }
     PB2_CUDA(e, cudaEventRecord(w->ev1, e->stream));
+    w->cur = c; w->armed[c] = true; w->beside[c] = false; w->arms++;
     return PB2_SUCCESS;
 }
 
@@ -969,9 +1021,10 @@ int pb2_window_start(pb2_window_t* w) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
         if (w->kind == 0) {
-            if (w->g.w.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(w->g.w, e->nworkers, e->params.threads, e->stream));
+            const WinDev d = run_desc(w, w->cur);
+            if (d.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(d, e->nworkers, e->params.threads, e->stream));
             else {
-                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(w->g.w);
+                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(d);
                 PB2_CUDA(e, cudaGetLastError());
             }
         } else {
@@ -983,6 +1036,17 @@ int pb2_window_start(pb2_window_t* w) {
     }
     PB2_CUDA(e, cudaEventRecord(w->ev2, e->stream));
     w->launched = true;
+    w->armed[w->cur] = false;
+    const int o = w->cur ^ 1;
+    if (w->kind == 0 && w->ntasks > 0 && w->run1.ctl && !w->armed[o]) {
+        // The other copy, for the next run, beside this one: after the run that used it last (ev1 of this arm follows
+        // it on the engine stream), on one CTA per SM, which fits next to the run's workers (DESIGN.md §5, §6).
+        PB2_CUDA(e, cudaStreamWaitEvent(e->arm_stream, w->ev1, 0));
+        const int rc = reset_copy(w, o, e->arm_stream, 1);
+        if (rc != PB2_SUCCESS) return rc;
+        PB2_CUDA(e, cudaEventRecord(w->ev_arm, e->arm_stream));
+        w->armed[o] = true; w->beside[o] = true;
+    }
     return PB2_SUCCESS;
 }
 
@@ -1085,7 +1149,7 @@ int pb2_window_wait(pb2_window_t* w, pb2_window_stats_t* stats) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaEventSynchronize(w->ev2));
     Ctl c;
-    PB2_CUDA(e, cudaMemcpy(&c, w->g.w.ctl, sizeof c, cudaMemcpyDeviceToHost));
+    PB2_CUDA(e, cudaMemcpy(&c, run_desc(w, w->cur).ctl, sizeof c, cudaMemcpyDeviceToHost));
     if (stats) {
         memset(stats, 0, sizeof *stats);
         stats->tasks_retired = c.retired.v;
@@ -1107,13 +1171,14 @@ int pb2_window_results(pb2_window_t* w, int32_t* retire_order, uint32_t* start_s
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     const size_t n = (size_t)w->ntasks;
-    if (retire_order && n) PB2_CUDA(e, cudaMemcpy(retire_order, w->g.w.retire_log, n * 4, cudaMemcpyDeviceToHost));
-    if (start_seq && n) PB2_CUDA(e, cudaMemcpy(start_seq, w->g.w.start_seq, n * 4, cudaMemcpyDeviceToHost));
-    if (end_seq && n) PB2_CUDA(e, cudaMemcpy(end_seq, w->g.w.end_seq, n * 4, cudaMemcpyDeviceToHost));
-    if (seen_version && n) PB2_CUDA(e, cudaMemcpy(seen_version, w->g.w.seen_version, n * 4 * PB2_MAX_FLOWS, cudaMemcpyDeviceToHost));
-    if (result && n) PB2_CUDA(e, cudaMemcpy(result, w->g.w.result, n * 8, cudaMemcpyDeviceToHost));
-    if (worker && n) PB2_CUDA(e, cudaMemcpy(worker, w->g.w.worker, n * 4, cudaMemcpyDeviceToHost));
-    if (tiles_out && w->ntiles) PB2_CUDA(e, cudaMemcpy(tiles_out, w->g.w.tiles, (size_t)w->ntiles * sizeof(pb2_tile_t), cudaMemcpyDeviceToHost));
+    const WinDev d = run_desc(w, w->cur);     // the copy of the last run
+    if (retire_order && n) PB2_CUDA(e, cudaMemcpy(retire_order, d.retire_log, n * 4, cudaMemcpyDeviceToHost));
+    if (start_seq && n) PB2_CUDA(e, cudaMemcpy(start_seq, d.start_seq, n * 4, cudaMemcpyDeviceToHost));
+    if (end_seq && n) PB2_CUDA(e, cudaMemcpy(end_seq, d.end_seq, n * 4, cudaMemcpyDeviceToHost));
+    if (seen_version && n) PB2_CUDA(e, cudaMemcpy(seen_version, d.seen_version, n * 4 * PB2_MAX_FLOWS, cudaMemcpyDeviceToHost));
+    if (result && n) PB2_CUDA(e, cudaMemcpy(result, d.result, n * 8, cudaMemcpyDeviceToHost));
+    if (worker && n) PB2_CUDA(e, cudaMemcpy(worker, d.worker, n * 4, cudaMemcpyDeviceToHost));
+    if (tiles_out && w->ntiles) PB2_CUDA(e, cudaMemcpy(tiles_out, d.tiles, (size_t)w->ntiles * sizeof(pb2_tile_t), cudaMemcpyDeviceToHost));
     return PB2_SUCCESS;
 }
 

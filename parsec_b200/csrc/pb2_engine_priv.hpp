@@ -17,6 +17,7 @@ struct pb2_engine_s {
     cudaStream_t own_stream = nullptr;   // created by the engine
     cudaStream_t up_stream = nullptr;    // descriptor uploads of the NEXT window: not ordered behind the running one
     cudaStream_t dma_stream = nullptr;   // pb2_engine_prefetch_h2d
+    cudaStream_t arm_stream = nullptr;   // re-arms the other copy of an HBM window's per-run state beside its run
     cudaEvent_t dma_ev = nullptr;
     bool dma_pending = false;
     int nworkers = 0;

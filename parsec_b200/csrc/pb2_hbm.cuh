@@ -32,15 +32,19 @@ constexpr int kHbmWorkersPerSm = 8;
 #ifndef PB2_HBM_THREADS
 #define PB2_HBM_THREADS 64
 #endif
-// A read group in flight on one worker: its members (the leader first), their CHECK constants, this part's results.
+// A read group in flight on one worker: its members (the leader first), their CHECK constants and out-edges, this
+// part's results.  The retire path takes what it needs of a member from here, not from its descriptor.
 struct GroupSmem {
     int32_t n;                              // members; 0: the popped task runs alone
     int32_t fused;                          // the popped task is a producer that runs with this group as one unit
     int32_t tile;                           // the tile the members read
     int32_t mem[PB2_GROUP_MAX];
     uint32_t k[PB2_GROUP_MAX];
+    int32_t succ_begin[PB2_GROUP_MAX];
+    int32_t succ_count[PB2_GROUP_MAX];
     unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
 };
+
 
 // All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
 // bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
@@ -115,12 +119,13 @@ pb2_engine_hbm_kernel(WinDev w) {
     __shared__ TaskSmem s;
     __shared__ BulkSmem bulk;
     __shared__ GroupSmem g;
-    if (threadIdx.x == 0) bulk_init(bulk);
+    __shared__ unsigned long long t_start;   // the watchdog's earliest reference (pop_idle)
+    if (threadIdx.x == 0) { bulk_init(bulk); t_start = globaltimer_ns(); }
     __syncthreads();
 
     for (;;) {
         if (threadIdx.x == 0) {
-            const int32_t e = pop_entry<PRIO>(w);
+            const int32_t e = pop_entry<PRIO>(w, &t_start);
             if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
             s.entry = e;
         }
@@ -141,6 +146,8 @@ pb2_engine_hbm_kernel(WinDev w) {
                 const pb2_task_t& mt = w.tasks[m];
                 g.mem[threadIdx.x] = m;
                 g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
+                g.succ_begin[threadIdx.x] = __ldg(&mt.succ_begin);
+                g.succ_count[threadIdx.x] = __ldg(&mt.succ_count);
                 if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
             }
             if (threadIdx.x == 0) {
@@ -185,7 +192,7 @@ pb2_engine_hbm_kernel(WinDev w) {
             if (threadIdx.x == 0) {
                 const pb2_task_t& t = s.task;
                 const int gn = g.n;
-                for (int i = 0; i < gn; ++i) store_result(w, w.tasks[g.mem[i]], g.mem[i], part, nparts, g.res[i]);
+                for (int i = 0; i < gn; ++i) store_check_result(w, g.mem[i], nparts, g.res[i]);   // members are CHECK bodies
                 if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
                 // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
                 int last = 1;
@@ -195,8 +202,7 @@ pb2_engine_hbm_kernel(WinDev w) {
                     // the producer, then its members as if they had run right after it: they saw the version it
                     // wrote; its end, their starts, their ends are consecutive events (end before start on every
                     // edge); they retire right after it, in member order
-                    epilog_written_flows(w, t);
-                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.tiles[g.tile].version);
+                    const uint32_t v = epilog_written_flows(w, t, g.tile);
                     const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)(1 + 2 * gn));
                     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)(1 + gn));
                     w.end_seq[id] = ev;
@@ -238,8 +244,8 @@ pb2_engine_hbm_kernel(WinDev w) {
         if (threadIdx.x < 32) {
             if (s.last) {
                 // a fused producer's own successors first (its edge to the group is not among them), then the members'
-                if (!g.n || g.fused) { release_successors_warp<PRIO>(w, s.task); release_remote_warp(w, id); }
-                for (int i = 0; i < g.n; ++i) release_successors_warp<PRIO>(w, w.tasks[g.mem[i]]);
+                if (!g.n || g.fused) { release_successors_warp<PRIO>(w, s.task.succ_begin, s.task.succ_count); release_remote_warp(w, id); }
+                for (int i = 0; i < g.n; ++i) release_successors_warp<PRIO>(w, g.succ_begin[i], g.succ_count[i]);
             }
             if (threadIdx.x == 0 && s.window_done) {
                 __threadfence();

@@ -96,6 +96,7 @@ struct alignas(32) PushDev { void* dst; int32_t* dst_state; uint32_t bytes; int3
 // the machine, not 1 ms of one CTA).  Parts per task (1..512) live in WinDev::nparts; ring entries of HBM windows
 // are (part << 22) | task, so such a window holds at most 2^22 tasks when it has wide tasks.
 #define PB2_MAX_PARTS 512
+#define PB2_SLICE_WORDS (PB2_MAX_PARTS / 32)   // claim words per tile of sliced stage-in (stage_in_slices)
 #define PB2_ENT_MAKE(task, part) ((int32_t)(((uint32_t)(part) << 22) | (uint32_t)(task)))
 #define PB2_ENT_TASK(e)          ((int32_t)((uint32_t)(e) & 0x3FFFFFu))
 #define PB2_ENT_PART(e)          ((int)((uint32_t)(e) >> 22))
@@ -151,12 +152,15 @@ __device__ __forceinline__ void push_entries_warp(int32_t* ring, uint32_t cap_ma
 // ---------------------------------------------------------------------------------------------
 
 // One thread, while it finds nothing to pop: true when the window is finished (or aborted, or the watchdog trips),
-// otherwise back off.
-__device__ __forceinline__ bool pop_idle(const WinDev& w, uint32_t& spins) {
+// otherwise back off.  since (null: none): the globaltimer at which the calling CTA started; the watchdog counts from
+// the later of it and the last retirement, because an HBM window's next run is armed during the run before it
+// (pb2_window_start), which can be long before the host starts it.
+__device__ __forceinline__ bool pop_idle(const WinDev& w, uint32_t& spins, const unsigned long long* since) {
     if (ld_relaxed_gpu(reinterpret_cast<const int32_t*>(&w.ctl->done.v)) != 0) return true;
     if ((++spins & 1023u) == 0) {
         // watchdog: a DAG whose dependency counts are wrong would spin forever
-        const unsigned long long last = *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v);
+        unsigned long long last = *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v);
+        if (since && *since > last) last = *since;
         // signed: %globaltimer read on another SM can be slightly behind the value a retiring SM just stored
         if ((long long)(globaltimer_ns() - last) > (long long)w.timeout_ns) {
             st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneTimeout);
@@ -169,7 +173,7 @@ __device__ __forceinline__ bool pop_idle(const WinDev& w, uint32_t& spins) {
 
 // One thread: take the next pop ticket and wait for its slot.  Returns a task id, or kEmpty when the
 // window is finished (or aborted).  Ticket order == push order, i.e. a strict FIFO ready queue.
-__device__ __forceinline__ int32_t pop_task(const WinDev& w) {
+__device__ __forceinline__ int32_t pop_task(const WinDev& w, const unsigned long long* since) {
     const uint32_t ticket = (uint32_t)atomicAdd(&w.ctl->head.v, 1ull);
     int32_t* slot = &w.ring[ticket & w.cap_mask];
     uint32_t spins = 0;
@@ -179,7 +183,7 @@ __device__ __forceinline__ int32_t pop_task(const WinDev& w) {
 #else
     while ((id = (w.shared ? ld_acquire_sys(slot) : ld_acquire_gpu(slot))) == kEmpty) {
 #endif
-        if (pop_idle(w, spins)) return kEmpty;
+        if (pop_idle(w, spins, since)) return kEmpty;
     }
     return id;
 }
@@ -191,7 +195,7 @@ __device__ __forceinline__ int32_t pop_task(const WinDev& w) {
 // below the tail claims the same slots, but a thousand workers polling one lane make it a retry round trip per claim:
 // 7x the FIFO time of the resident Ex05 window.)  Shared windows never get here: their peers push into one remote
 // ring (pb2_window_create refuses the combination).
-__device__ __forceinline__ int32_t pop_prio(const WinDev& w) {
+__device__ __forceinline__ int32_t pop_prio(const WinDev& w, const unsigned long long* since) {
     uint32_t spins = 0;
     for (;;) {
         for (int l = 0; l < w.nlanes; ++l) {
@@ -205,12 +209,14 @@ __device__ __forceinline__ int32_t pop_prio(const WinDev& w) {
             }
             atomicAdd(avail, 1ull);
         }
-        if (pop_idle(w, spins)) return kEmpty;
+        if (pop_idle(w, spins, since)) return kEmpty;
     }
 }
 
 template <bool PRIO>
-__device__ __forceinline__ int32_t pop_entry(const WinDev& w) { return PRIO ? pop_prio(w) : pop_task(w); }
+__device__ __forceinline__ int32_t pop_entry(const WinDev& w, const unsigned long long* since = nullptr) {
+    return PRIO ? pop_prio(w, since) : pop_task(w, since);
+}
 
 // Whole warp, queue_policy 1: lanes with np > 0 push np entries into priority lane `ln`.  One tail reservation per
 // lane in use (the lanes of the warp that push into the same one are aggregated); returns this lane's first slot.
@@ -235,17 +241,17 @@ static __device__ __noinline__ uint32_t reserve_lane_slots(Lanes* lanes, int ln,
     return (uint32_t)base + (uint32_t)pre;
 }
 
-// Whole warp: release the out-edges of task t (parsec_release_dep_fct semantics), push the newly
-// ready successors.  Must be called after a __threadfence() that follows the body's stores.
+// Whole warp: release the out-edges succ[succ_begin .. + succ_count) of a task (parsec_release_dep_fct semantics), push
+// the newly ready successors.  Must be called after a __threadfence() that follows the body's stores.
 template <bool PRIO>
-__device__ __forceinline__ void release_successors_warp(const WinDev& w, const pb2_task_t& t) {
+__device__ __forceinline__ void release_successors_warp(const WinDev& w, int32_t succ_begin, int32_t succ_count) {
     const int lane = threadIdx.x & 31;
-    for (int e0 = 0; e0 < t.succ_count; e0 += 32) {
+    for (int e0 = 0; e0 < succ_count; e0 += 32) {
         const int e = e0 + lane;
         bool ready = false;
         int32_t sid = -1;
-        if (e < t.succ_count) {
-            const uint32_t s = w.succ[t.succ_begin + e];
+        if (e < succ_count) {
+            const uint32_t s = w.succ[succ_begin + e];
             sid = PB2_SUCC_TASK(s);
             const pb2_task_t& st = w.tasks[sid];
             if (st.flags & PB2_TASK_DEPS_MASK) {
@@ -345,6 +351,47 @@ __device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// (re)arm the per-run state of a window
+// ---------------------------------------------------------------------------------------------
+// Thread gid of gsz: its grid-stride share of what a run starts from -- dependency words, ring, Ctl, tile table, part
+// counts, stage-in claims, priority lanes and the cleared per-task outputs.  `ready` is the window's image of its first
+// nready ring slots.  pb2_window_reset_kernel runs it over its grid.
+__device__ __forceinline__ void rearm_run(const WinDev& w, const pb2_tile_t* tiles_init, const int32_t* ready, int32_t nready,
+                                          size_t gid, size_t gsz) {
+    for (size_t i = gid; i < (size_t)w.ntasks; i += gsz) {
+        const pb2_task_t& t = w.tasks[i];
+        // counter mode counts down from the goal (parsec.c:1625-1633); mask mode ORs up from 0 (:1693-1703)
+        w.dep[i] = (t.flags & PB2_TASK_DEPS_MASK) ? 0 : t.dep_goal;
+        if (w.parts_left) w.parts_left[i] = task_nparts(w, (int32_t)i);
+        w.start_seq[i] = 0; w.end_seq[i] = 0; w.result[i] = 0; w.worker[i] = -1; w.retire_log[i] = -1;
+        for (int f = 0; f < PB2_MAX_FLOWS; ++f) w.seen_version[i * PB2_MAX_FLOWS + f] = 0;
+    }
+    for (size_t i = gid; i <= (size_t)w.cap_mask; i += gsz)
+        w.ring[i] = (i < (size_t)nready) ? ready[i] : kEmpty;
+    for (size_t i = gid; i < (size_t)w.ntiles; i += gsz) {
+        w.tiles[i] = tiles_init[i];
+        if (w.slice_claim) {
+            for (int k = 0; k < PB2_SLICE_WORDS; ++k) w.slice_claim[i * PB2_SLICE_WORDS + k] = 0;
+            for (int k = 0; k <= PB2_SLICE_WORDS; ++k) w.slice_done[i * (PB2_SLICE_WORDS + 1) + k] = 0;
+        }
+    }
+    // queue_policy 1: every lane starts with its initial entries, which `ready` holds at the start of the lane's
+    // segment (empty slots kEmpty)
+    if (w.lanes && gid < PB2_PRIO_LANES) {
+        w.lanes->head[gid].v = w.lanes->begin[gid];
+        w.lanes->tail[gid].v = (unsigned long long)w.lanes->begin[gid] + w.lanes->ninit[gid];
+        w.lanes->avail[gid].v = w.lanes->ninit[gid];
+    }
+    if (gid == 0) {
+        w.ctl->head.v = 0; w.ctl->tail.v = (unsigned long long)nready; w.ctl->evt.v = 0;
+        w.ctl->retired.v = 0; w.ctl->done.v = (w.ntasks == 0) ? kDoneOK : 0;
+        w.ctl->progress_ns.v = globaltimer_ns();
+        w.ctl->bytes_h2d.v = 0; w.ctl->bytes_d2d.v = 0; w.ctl->bytes_d2h.v = 0;
+        w.ctl->stage_ins.v = 0; w.ctl->body_errors.v = 0;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
 // stage-in / stage-out of one flow by the whole CTA
 // ---------------------------------------------------------------------------------------------
 // What the out-of-line stage-in helpers need from the window, passed BY VALUE in registers: a reference to the
@@ -393,7 +440,6 @@ static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* 
 
 
 // Number of stage-in slices of a tile: the same rule pb2_window_create uses for the parts of a wide task.
-#define PB2_SLICE_WORDS (PB2_MAX_PARTS / 32)
 __device__ __forceinline__ int tile_slices_of(int32_t part_bytes, const uint32_t* slice_claim, uint32_t bytes) {
     if (part_bytes <= 0 || !slice_claim) return 1;
     const uint32_t n = (bytes + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes;

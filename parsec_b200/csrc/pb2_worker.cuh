@@ -110,24 +110,33 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
 }
 
 // Thread 0 of the part that finished last: version / coherency epilog of the written flows
-// (version = candidate->version + 1 for WRITE flows, device_gpu.c:2148-2152).
-__device__ __forceinline__ void epilog_written_flows(const WinDev& w, const pb2_task_t& t) {
+// (version = candidate->version + 1 for WRITE flows, device_gpu.c:2148-2152).  Returns the version it gave tile x
+// (0: t does not write x).
+__device__ __forceinline__ uint32_t epilog_written_flows(const WinDev& w, const pb2_task_t& t, int32_t x = -1) {
+    uint32_t vx = 0;
     for (int f = 0; f < (int)t.nb_flows; ++f) {
         if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_ACCESS_WRITE)) continue;
         pb2_tile_t* tile = &w.tiles[t.tile[f]];
-        *reinterpret_cast<volatile uint32_t*>(&tile->version) = *reinterpret_cast<volatile uint32_t*>(&tile->version) + 1;
+        const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&tile->version) + 1;
+        *reinterpret_cast<volatile uint32_t*>(&tile->version) = v;
+        if (t.tile[f] == x) vx = v;
         if (!(t.access[f] & PB2_FLOW_ACCESS_READ)) st_relaxed_gpu(&tile->state, PB2_TILE_VALID);
     }
+    return vx;
 }
 
-// Thread 0: store the body result of this part (CHECK bodies add their mismatch counts over the parts).
+// Thread 0: store a CHECK body's result of this part (the mismatch counts of the parts add up).
+__device__ __forceinline__ void store_check_result(const WinDev& w, int32_t id, int nparts, unsigned long long r) {
+    if (nparts == 1) w.result[id] = r; else if (r) atomicAdd(&w.result[id], r);
+    if (r >> 32) atomicAdd(&w.ctl->body_errors.v, r >> 32);
+}
+
+// Thread 0: store the body result of this part.
 __device__ __forceinline__ void store_result(const WinDev& w, const pb2_task_t& t, int32_t id, int part, int nparts,
                                              unsigned long long r) {
     if (r == ~0ull) st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneBadBody);
-    if (t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) {
-        if (nparts == 1) w.result[id] = r; else if (r) atomicAdd(&w.result[id], r);
-        if (r >> 32) atomicAdd(&w.ctl->body_errors.v, r >> 32);
-    } else if (part == 0) w.result[id] = r;
+    if (t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) store_check_result(w, id, nparts, r);
+    else if (part == 0) w.result[id] = r;
 }
 
 }  // namespace pb2

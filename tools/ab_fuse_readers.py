@@ -5,12 +5,12 @@
 2. tools/l2_probe (compiled into a temporary directory): the L2 read rate and the DRAM rates of this GPU;
 3. a FILL-only window (the K producers of the Ex05 window, no readers): the write floor of the fused window;
 4. the resident Ex05 window (dags.ex05_broadcast(K, 14, 262144), tiles VALID) with fusion off and on;
-5. --ab LIB: the fused window on library LIB (another build of libparsec_b200.so, e.g. the parent
+5. --ab LIB [LIB ...]: the fused window on each library LIB (other builds of libparsec_b200.so, e.g. the parent
    commit's) and on this tree's library, alternated: --rounds child processes per build, each with PB2_LIB_PATH set,
-   --warmup and --runs runs each.
+   --warmup and --runs runs each; besides the sum, the medians of reset_ms and kernel_ms of each build.
 Each row: median / min / max / spread of reset_ms + kernel_ms.
 
-    python tools/ab_fuse_readers.py [--runs 30] [--ab /path/to/parent/libparsec_b200.so]
+    python tools/ab_fuse_readers.py [--runs 30] [--ab /path/to/parent/libparsec_b200.so ...]
 """
 import argparse
 import json
@@ -45,10 +45,12 @@ class Window:
         tiles["bytes"] = TB
         tiles["state"] = L.TILE_VALID
         self.w = self.e.window(0, tasks, succ, tiles, dag.ready)
+        self.split = []                    # (reset_ms, kernel_ms) of every run
 
     def run(self):
         st = self.w.run()
         assert st["body_errors"] == 0 and st["tasks_retired"] == self.ntasks
+        self.split.append((st["reset_ms"], st["kernel_ms"]))
         return st["reset_ms"] + st["kernel_ms"]
 
     def close(self):
@@ -59,6 +61,7 @@ class Window:
 def runs_of(x, warmup, runs):
     for _ in range(warmup):
         x.run()
+    x.split.clear()
     ms = [x.run() for _ in range(runs)]
     x.close()
     return ms
@@ -69,20 +72,27 @@ def measure(x, warmup, runs):
 
 
 def ab_libraries(args):
-    """The fused window on two library builds, one child process at a time, alternated."""
-    libs = {"lib_a": os.path.abspath(args.ab), "lib_b": L.LIB_PATH}
-    ms = {k: [] for k in libs}
+    """The fused window on the --ab library builds (lib_a, lib_a2, ...) and this tree's (lib_b), one child process at a
+    time, alternated."""
+    libs = {("lib_a%d" % i if i else "lib_a"): os.path.abspath(p) for i, p in enumerate(args.ab)}
+    libs["lib_b"] = L.LIB_PATH
+    got = {k: {"child_ms": [], "reset_ms": [], "kernel_ms": []} for k in libs}
     medians = {k: [] for k in libs}
     for _ in range(args.rounds):
         for k, lib in libs.items():
             out = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--K", str(args.K),
                                   "--runs", str(args.runs), "--warmup", str(args.warmup)],
                                  env=dict(os.environ, PB2_LIB_PATH=lib), capture_output=True, text=True, check=True).stdout
-            got = json.loads([l for l in out.splitlines() if l.startswith("{")][-1])["child_ms"]
-            ms[k] += got
-            medians[k].append(summary(got)["median_ms"])
-    res = {k: dict(summary(v), lib=libs[k], round_medians_ms=medians[k]) for k, v in ms.items()}
-    res["b_over_a_median"] = res["lib_b"]["median_ms"] / res["lib_a"]["median_ms"]
+            child = json.loads([l for l in out.splitlines() if l.startswith("{")][-1])
+            for key in got[k]:
+                got[k][key] += child[key]
+            medians[k].append(summary(child["child_ms"])["median_ms"])
+    res = {k: dict(summary(v["child_ms"]), lib=libs[k], round_medians_ms=medians[k],
+                   reset_median_ms=float(np.median(v["reset_ms"])), kernel_median_ms=float(np.median(v["kernel_ms"])))
+           for k, v in got.items()}
+    for k in libs:
+        if k != "lib_b":
+            res["b_over_%s_median" % k[4:]] = res["lib_b"]["median_ms"] / res[k]["median_ms"]
     return res
 
 
@@ -91,12 +101,14 @@ def main():
     ap.add_argument("--K", type=int, default=4096)
     ap.add_argument("--runs", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
-    ap.add_argument("--ab", metavar="LIB", help="alternate the fused window on library LIB (lib_a) and on this tree's (lib_b)")
+    ap.add_argument("--ab", metavar="LIB", nargs="+", help="alternate the fused window on libraries LIB (lib_a, lib_a1, ...) and on this tree's (lib_b)")
     ap.add_argument("--rounds", type=int, default=4, help="--ab: child processes per library")
     ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.child:
-        print(json.dumps({"child_ms": runs_of(Window(args.K, 0), args.warmup, args.runs)}), flush=True)
+        x = Window(args.K, 0)
+        ms = runs_of(x, args.warmup, args.runs)
+        print(json.dumps({"child_ms": ms, "reset_ms": [r for r, _ in x.split], "kernel_ms": [k for _, k in x.split]}), flush=True)
         return
     print(json.dumps({"card": card()}), flush=True)
     print(json.dumps({"l2_probe": l2_probe()}), flush=True)
