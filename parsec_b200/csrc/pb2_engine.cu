@@ -94,26 +94,45 @@ using namespace pb2;
 
 #include "pb2_engine_priv.hpp"
 
+// One copy of a window's per-run state: exactly the arrays that rearm_run and pb2_window_reset_kernel write.  alloc_run
+// allocates them and run_desc puts them into a launch descriptor; no other host code names them.
+struct RunState {
+    pb2_tile_t* tiles; int32_t* dep; int32_t* ring; Ctl* ctl; int32_t* retire_log;
+    uint32_t* start_seq; uint32_t* end_seq; uint32_t* seen_version; unsigned long long* result; int32_t* worker;
+    int32_t* parts_left;                  // RunShape::parts
+    uint32_t* slice_claim; uint32_t* slice_done;    // RunShape::claims
+    Lanes* lanes;                         // RunShape::lanes
+    int32_t* udep; int32_t* unit_parts_left;        // GEMM windows: the units' dependency words and part counts
+};
+
+// What every copy of a window's per-run state is sized from besides ntasks and ntiles, recorded by pb2_window_create.
+struct RunShape {
+    uint32_t ring = 0;                    // ring slots, a power of two
+    int32_t nunits = 0;                   // GEMM windows: units
+    bool parts = false;                   // per-task part counts (an HBM window with wide tasks)
+    bool claims = false;                  // stage-in is sliced: claim arrays per tile
+    bool lanes = false;                   // queue_policy 1: priority lanes, which start as lane_image
+    Lanes lane_image{};
+};
+
 struct pb2_window_s {
     pb2_engine_t* e = nullptr;
     int kind = 0;
     int32_t ntasks = 0, ntiles = 0, nready_entries = 0;
-    Win2Dev g{};                        // g.w: the window's device descriptor; the rest: kind 1's units and tensor maps
+    Win2Dev g{};                        // the descriptor without per-run arrays (run_desc adds a copy's)
+    RunShape shape;
     pb2_tile_t* d_tiles_init = nullptr;
     int32_t* d_ready = nullptr;         // image of the first nready_entries ring slots
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
     bool launched = false;
     bool shared = false;
-    // A non-shared HBM window with tasks keeps two copies of its per-run state (rearm_run's arrays): g.w's and, from
-    // its second arm on, run1's.  Consecutive runs alternate between them, and while a run runs, the reset kernel
-    // arms the other copy for the next one on the engine's arm stream (ev_arm: its end).  cur: the copy of the last
-    // arm; armed[c]: copy c is armed, or will be by work already queued, and no run has used it since; beside[c]:
-    // that work is the reset on the arm stream.
-    WinDev run1{};
-    int cur = 0;
-    int arms = 0;
-    bool armed[2] = {false, false};
-    bool beside[2] = {false, false};
+    // The per-run state by copy.  pb2_window_create fixes ncopies: 2 for a non-shared HBM window with tasks, else 1
+    // (DESIGN.md §5).  Copy 0 is allocated at create, copy 1 at the second arm.  Consecutive runs alternate between
+    // the copies, and while a run runs, the reset kernel arms the other copy for the next one on the engine's arm
+    // stream (ev_arm: its end).  cur: the copy of the last arm; armed: the copy is armed, or will be by work already
+    // queued, and no run has used it since; beside: that work is the reset on the arm stream.
+    struct Copy { RunState run{}; bool armed = false; bool beside = false; } copy[2];
+    int ncopies = 1, cur = 0, arms = 0;
     cudaEvent_t ev_arm = nullptr;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
     std::vector<void*> allocs;
@@ -131,21 +150,29 @@ struct WindowPlan {
     std::vector<uint32_t> owner_pushes;   // queue_policy 1: per owner, the entries it can ever push
     uint32_t ring_slots = 0;              // ring slots the window needs besides the workers' slack
     int32_t slice_bytes = 0;              // stage-in slice size (WinDev::part_bytes)
-    bool claims = false;                  // stage-in is sliced: allocate the claim arrays
+    RunShape run;                         // the per-run state's needs (its ring size is set by pb2_window_create)
 };
 
+// n T (at least one) for window w on `stream`, freed by pb2_window_destroy.
 template <class T>
-static int dev_alloc_copy(pb2_window_t* w, T** dptr, const T* host, size_t n) {
+static int dev_alloc(pb2_window_t* w, T** dptr, size_t n, cudaStream_t stream) {
     pb2_engine_t* e = w->e;
     void* p = nullptr;
     // stream-ordered pool allocation: after the first window of a size class this costs microseconds, whereas
     // cudaMalloc/cudaFree next to a slab that fills the device cost hundreds of microseconds each and synchronise the device
     if (w->shared) { PB2_CUDA(e, cudaMalloc(&p, (n ? n : 1) * sizeof(T))); }     // IPC needs cudaMalloc memory
-    else PB2_CUDA(e, cudaMallocAsync(&p, (n ? n : 1) * sizeof(T), e->up_stream));
+    else PB2_CUDA(e, cudaMallocAsync(&p, (n ? n : 1) * sizeof(T), stream));
     w->allocs.push_back(p);
-    if (host && n) PB2_CUDA(e, cudaMemcpyAsync(p, host, n * sizeof(T), cudaMemcpyHostToDevice, e->up_stream));
     *dptr = reinterpret_cast<T*>(p);
     return PB2_SUCCESS;
+}
+
+// The same on the upload stream, with host's n T uploaded into them.
+template <class T>
+static int dev_alloc_copy(pb2_window_t* w, T** dptr, const T* host, size_t n) {
+    const int rc = dev_alloc(w, dptr, n, w->e->up_stream);
+    if (rc == PB2_SUCCESS && host && n) PB2_CUDA(w->e, cudaMemcpyAsync(*dptr, host, n * sizeof(T), cudaMemcpyHostToDevice, w->e->up_stream));
+    return rc;
 }
 
 static int validate_window(pb2_engine_t* e, int kind, const pb2_task_t* tasks, int32_t ntasks,
@@ -252,10 +279,11 @@ static std::vector<uint8_t> task_priority_lanes(const pb2_task_t* tasks, int32_t
 
 // Cut the ring into one segment per lane, as long as the entries the lane's owners can ever push (owner o, in lane
 // p.owner_lane[o], pushes at most p.owner_pushes[o] entries).  p.entries becomes the image of the whole ring that the
-// reset kernel writes: each entry at the start of its owner's lane's segment, in the same order within a lane.
+// reset kernel writes: each entry at the start of its owner's lane's segment, in the same order within a lane; the
+// lanes start as p.run.lane_image.  Uploads the owners' lanes.
 static int build_lane_ring(pb2_window_t* w, WindowPlan& p) {
-    Lanes h;
-    memset(&h, 0, sizeof h);
+    Lanes& h = p.run.lane_image;
+    p.run.lanes = true;
     uint32_t size[PB2_PRIO_LANES] = {0};
     for (size_t o = 0; o < p.owner_lane.size(); ++o) size[p.owner_lane[o]] += p.owner_pushes[o];
     uint32_t b = 0;
@@ -266,13 +294,10 @@ static int build_lane_ring(pb2_window_t* w, WindowPlan& p) {
         ring[h.begin[l] + h.ninit[l]++] = p.entries[i];
     }
     p.entries.swap(ring);
-    int rc;
-    Lanes* d_lanes = nullptr;
     uint8_t* d_lane = nullptr;
-    if ((rc = dev_alloc_copy(w, &d_lanes, &h, 1)) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &d_lane, p.owner_lane.data(), p.owner_lane.size())) != PB2_SUCCESS) return rc;
-    w->g.w.lanes = d_lanes; w->g.w.lane = d_lane;
-    return PB2_SUCCESS;
+    const int rc = dev_alloc_copy(w, &d_lane, p.owner_lane.data(), p.owner_lane.size());
+    w->g.w.lane = d_lane;
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -378,7 +403,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every worker
     // that needs them (the parts of one unit, the units that share an operand) instead of by one worker alone
     plan.slice_bytes = 64 * 1024;
-    plan.claims = true;
+    plan.run.claims = true;
+    plan.run.nunits = (int32_t)units.size();
     w->task_entry.resize((size_t)ntasks);
     for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
     int rc;
@@ -387,10 +413,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     if ((rc = dev_alloc_copy(w, &d_units, units.data(), units.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_segs, segs.data(), segs.size())) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_usucc, usucc.data(), usucc.size())) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &w->g.udep, (const int32_t*)nullptr, units.size())) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &w->g.parts_left, (const int32_t*)nullptr, units.size())) != PB2_SUCCESS) return rc;
     w->g.w.succ = d_succ;
-    w->g.units = d_units; w->g.segs = d_segs; w->g.usucc = d_usucc; w->g.nunits = (int32_t)units.size();
+    w->g.units = d_units; w->g.segs = d_segs; w->g.usucc = d_usucc; w->g.nunits = plan.run.nunits;
     return PB2_SUCCESS;
 }
 
@@ -514,9 +538,9 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
     // by EVERY worker that needs it (claim bit per slice), so the readers of a tile share the transfer instead of one
     // moving it while the others wait.
     plan.slice_bytes = stage_slice(e->stage_slice_bytes, e->params.part_bytes);
-    plan.claims = extra_parts > 0;
-    for (int32_t i = 0; i < ntiles && !plan.claims; ++i)
-        plan.claims = plan.slice_bytes > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)plan.slice_bytes;
+    plan.run.parts = plan.run.claims = extra_parts > 0;
+    for (int32_t i = 0; i < ntiles && !plan.run.claims; ++i)
+        plan.run.claims = plan.slice_bytes > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)plan.slice_bytes;
     // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
     std::vector<uint32_t> gsucc, group;
     std::vector<int32_t> gmem;
@@ -536,59 +560,49 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
     if (extra_parts) {
         uint16_t* d_np = nullptr;
         if ((rc = dev_alloc_copy(w, &d_np, nparts.data(), nparts.size())) != PB2_SUCCESS) return rc;
-        if ((rc = dev_alloc_copy(w, &d.parts_left, (const int32_t*)nullptr, (size_t)ntasks)) != PB2_SUCCESS) return rc;
         d.nparts = d_np;
     }
     return PB2_SUCCESS;
 }
 
-// The descriptor of run-state copy c of window w: g.w with copy c's per-run arrays.
-static WinDev run_desc(const pb2_window_t* w, int c) {
-    WinDev d = w->g.w;
-    if (c == 1) {
-        const WinDev& r = w->run1;
-        d.tiles = r.tiles; d.dep = r.dep; d.ring = r.ring; d.ctl = r.ctl; d.retire_log = r.retire_log;
-        d.start_seq = r.start_seq; d.end_seq = r.end_seq; d.seen_version = r.seen_version; d.result = r.result;
-        d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
-        d.lanes = r.lanes;
-    }
-    return d;
-}
-
-// An array of n T on the engine stream (stream-ordered) where copy 0 has one (src), else none.
-template <class T>
-static cudaError_t alloc_like(pb2_window_t* w, T** dst, const T* src, size_t n) {
-    *dst = nullptr;
-    if (!src) return cudaSuccess;
-    void* p = nullptr;
-    const cudaError_t err = cudaMallocAsync(&p, (n ? n : 1) * sizeof(T), w->e->stream);
-    if (err == cudaSuccess) { w->allocs.push_back(p); *dst = reinterpret_cast<T*>(p); }
-    return err;
-}
-
-// Copy 1 of a window's per-run arrays, shaped as g.w's.  The lanes' segment bounds are constant: copied from copy 0.
-static int alloc_run1(pb2_window_t* w) {
+// Copy c of window w's per-run state, sized from w->shape.  pb2_window_create allocates copy 0 on the upload stream,
+// and the second pb2_window_arm copy 1, stream-ordered on the engine stream.  The lanes' segment bounds never change:
+// both copies hold lane_image's.
+static int alloc_run(pb2_window_t* w, int c) {
     pb2_engine_t* e = w->e;
-    const WinDev& d = w->g.w;
-    WinDev& r = w->run1;
+    const RunShape& s = w->shape;
+    const cudaStream_t stream = c == 0 ? e->up_stream : e->stream;
     const size_t nt = (size_t)w->ntasks, nl = (size_t)w->ntiles;
-    auto like = [&](auto** dst, auto* src, size_t n) { return alloc_like(w, dst, src, n); };
-    PB2_CUDA(e, like(&r.tiles, d.tiles, nl));
-    PB2_CUDA(e, like(&r.dep, d.dep, nt));
-    PB2_CUDA(e, like(&r.ring, d.ring, (size_t)d.cap_mask + 1));
-    PB2_CUDA(e, like(&r.ctl, d.ctl, 1));
-    PB2_CUDA(e, like(&r.retire_log, d.retire_log, nt));
-    PB2_CUDA(e, like(&r.start_seq, d.start_seq, nt));
-    PB2_CUDA(e, like(&r.end_seq, d.end_seq, nt));
-    PB2_CUDA(e, like(&r.seen_version, d.seen_version, nt * PB2_MAX_FLOWS));
-    PB2_CUDA(e, like(&r.result, d.result, nt));
-    PB2_CUDA(e, like(&r.worker, d.worker, nt));
-    PB2_CUDA(e, like(&r.parts_left, d.parts_left, nt));
-    PB2_CUDA(e, like(&r.slice_claim, d.slice_claim, nl * PB2_SLICE_WORDS));
-    PB2_CUDA(e, like(&r.slice_done, d.slice_done, nl * (PB2_SLICE_WORDS + 1)));
-    PB2_CUDA(e, like(&r.lanes, d.lanes, 1));
-    if (d.lanes) PB2_CUDA(e, cudaMemcpyAsync(r.lanes, d.lanes, sizeof(Lanes), cudaMemcpyDeviceToDevice, e->stream));
+    RunState r{};
+    int rc = PB2_SUCCESS;
+    auto alloc = [&](auto** p, size_t n) { if (rc == PB2_SUCCESS) rc = dev_alloc(w, p, n, stream); };
+    alloc(&r.tiles, nl); alloc(&r.dep, nt); alloc(&r.ring, s.ring); alloc(&r.ctl, 1); alloc(&r.retire_log, nt);
+    alloc(&r.start_seq, nt); alloc(&r.end_seq, nt); alloc(&r.seen_version, nt * PB2_MAX_FLOWS);
+    alloc(&r.result, nt); alloc(&r.worker, nt);
+    if (s.parts) alloc(&r.parts_left, nt);
+    if (s.claims) { alloc(&r.slice_claim, nl * PB2_SLICE_WORDS); alloc(&r.slice_done, nl * (PB2_SLICE_WORDS + 1)); }
+    if (s.lanes) alloc(&r.lanes, 1);
+    // every GEMM window has the unit words, even without units: pb2_window_export hands out udep
+    if (w->kind == 1) { alloc(&r.udep, (size_t)s.nunits); alloc(&r.unit_parts_left, (size_t)s.nunits); }
+    if (rc != PB2_SUCCESS) return rc;
+    // copy 1 takes copy 0's lanes device to device: a copy from pageable host memory may wait for the engine stream
+    if (s.lanes) PB2_CUDA(e, c == 0 ? cudaMemcpyAsync(r.lanes, &s.lane_image, sizeof(Lanes), cudaMemcpyHostToDevice, stream)
+                                    : cudaMemcpyAsync(r.lanes, w->copy[0].run.lanes, sizeof(Lanes), cudaMemcpyDeviceToDevice, stream));
+    w->copy[c].run = r;
     return PB2_SUCCESS;
+}
+
+// The launch descriptor of copy c of window w: the constant descriptor g with copy c's per-run arrays.
+static Win2Dev run_desc(const pb2_window_t* w, int c) {
+    const RunState& r = w->copy[c].run;
+    Win2Dev g = w->g;
+    WinDev& d = g.w;
+    d.tiles = r.tiles; d.dep = r.dep; d.ring = r.ring; d.ctl = r.ctl; d.retire_log = r.retire_log;
+    d.start_seq = r.start_seq; d.end_seq = r.end_seq; d.seen_version = r.seen_version; d.result = r.result;
+    d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
+    d.lanes = r.lanes;
+    g.udep = r.udep; g.parts_left = r.unit_parts_left;
+    return g;
 }
 
 extern "C" {
@@ -926,20 +940,11 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     TRY(dev_alloc_copy(w, &d_tasks, dtasks.data(), (size_t)ntasks));
     d.tasks = d_tasks;
     TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
-    TRY(dev_alloc_copy(w, &d.tiles, (const pb2_tile_t*)nullptr, (size_t)ntiles));
-    TRY(dev_alloc_copy(w, &d.dep, (const int32_t*)nullptr, (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &d.ring, (const int32_t*)nullptr, (size_t)cap));
-    TRY(dev_alloc_copy(w, &d.ctl, (const Ctl*)nullptr, 1));
-    TRY(dev_alloc_copy(w, &d.retire_log, (const int32_t*)nullptr, (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &d.start_seq, (const uint32_t*)nullptr, (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &d.end_seq, (const uint32_t*)nullptr, (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &d.seen_version, (const uint32_t*)nullptr, (size_t)ntasks * PB2_MAX_FLOWS));
-    TRY(dev_alloc_copy(w, &d.result, (const unsigned long long*)nullptr, (size_t)ntasks));
-    TRY(dev_alloc_copy(w, &d.worker, (const int32_t*)nullptr, (size_t)ntasks));
-    if (plan.claims) {
-        TRY(dev_alloc_copy(w, &d.slice_claim, (const uint32_t*)nullptr, (size_t)ntiles * PB2_SLICE_WORDS));
-        TRY(dev_alloc_copy(w, &d.slice_done, (const uint32_t*)nullptr, (size_t)ntiles * (PB2_SLICE_WORDS + 1)));
-    }
+    plan.run.ring = cap;
+    w->shape = plan.run;
+    // shared windows keep one copy (peers hold IPC pointers to it), GEMM windows too (DESIGN.md §5)
+    w->ncopies = kind == 0 && !w->shared && ntasks > 0 ? 2 : 1;
+    TRY(alloc_run(w, 0));
 #undef TRY
     d.part_bytes = plan.slice_bytes; d.shared = w->shared ? 1 : 0; d.nlanes = nlanes;
     d.cap_mask = cap - 1; d.ntasks = ntasks; d.ntiles = ntiles; d.stage_mode = e->params.stage_mode;
@@ -960,7 +965,7 @@ int pb2_window_destroy(pb2_window_t* w) {
     if (!w) return PB2_ERR_BAD_PARAM;
     cudaSetDevice(w->e->cuda_device);
     if (w->launched) cudaEventSynchronize(w->ev2);        // this window only: a later one may be running
-    if (w->beside[0] || w->beside[1]) cudaEventSynchronize(w->ev_arm);     // a reset of the next run's copy
+    if (w->copy[0].beside || w->copy[1].beside) cudaEventSynchronize(w->ev_arm);     // a reset of the next run's copy
     for (void* p : w->peer_ptrs) cudaIpcCloseMemHandle(p);
     for (void* p : w->allocs) { if (w->shared) cudaFree(p); else cudaFreeAsync(p, w->e->stream); }
     if (w->ev0) cudaEventDestroy(w->ev0);
@@ -975,13 +980,9 @@ int pb2_window_destroy(pb2_window_t* w) {
 static int reset_copy(pb2_window_t* w, int c, cudaStream_t stream, int per_sm) {
     pb2_engine_t* e = w->e;
     const int threads = 256;
-    size_t n = (size_t)w->ntasks > (size_t)w->g.w.cap_mask + 1 ? (size_t)w->ntasks : (size_t)w->g.w.cap_mask + 1;
-    int blocks = (int)((n + threads - 1) / threads);
-    if (blocks > e->prop.multiProcessorCount * per_sm) blocks = e->prop.multiProcessorCount * per_sm;
-    if (blocks < 1) blocks = 1;
-    Win2Dev g = w->g;
-    g.w = run_desc(w, c);
-    pb2_window_reset_kernel<<<blocks, threads, 0, stream>>>(g, w->d_tiles_init, w->d_ready, w->nready_entries);
+    const size_t n = std::max((size_t)w->ntasks, (size_t)w->shape.ring);     // the ring has at least 1024 slots
+    const int blocks = (int)std::min((n + threads - 1) / threads, (size_t)e->prop.multiProcessorCount * per_sm);
+    pb2_window_reset_kernel<<<blocks, threads, 0, stream>>>(run_desc(w, c), w->d_tiles_init, w->d_ready, w->nready_entries);
     PB2_CUDA(e, cudaGetLastError());
     return PB2_SUCCESS;
 }
@@ -990,11 +991,9 @@ int pb2_window_arm(pb2_window_t* w) {
     if (!w) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
-    // shared windows keep one copy (peers hold IPC pointers to it), GEMM windows too (DESIGN.md §5)
-    const bool two = w->kind == 0 && !w->shared && w->ntasks > 0;
-    const int c = two && w->arms > 0 ? w->cur ^ 1 : 0;
-    if (c == 1 && !w->run1.ctl) {
-        const int rc = alloc_run1(w);
+    const int c = w->ncopies == 2 && w->arms > 0 ? w->cur ^ 1 : 0;
+    if (!w->copy[c].run.ctl) {
+        const int rc = alloc_run(w, c);
         if (rc != PB2_SUCCESS) return rc;
     }
     if (e->dma_pending) {                       // prefetches queued for this window land before its first worker starts
@@ -1003,15 +1002,15 @@ int pb2_window_arm(pb2_window_t* w) {
         e->dma_pending = false;
     }
     PB2_CUDA(e, cudaEventRecord(w->ev0, e->stream));
-    if (!w->armed[c]) {
+    if (!w->copy[c].armed) {
         const int rc = reset_copy(w, c, e->stream, 8);
         if (rc != PB2_SUCCESS) return rc;
-    } else if (w->beside[c]) {
+    } else if (w->copy[c].beside) {
         // armed beside the last run; a wait here is part of this arm's time (after ev0)
         PB2_CUDA(e, cudaStreamWaitEvent(e->stream, w->ev_arm, 0));
     }
     PB2_CUDA(e, cudaEventRecord(w->ev1, e->stream));
-    w->cur = c; w->armed[c] = true; w->beside[c] = false; w->arms++;
+    w->cur = c; w->copy[c].armed = true; w->copy[c].beside = false; w->arms++;
     return PB2_SUCCESS;
 }
 
@@ -1020,32 +1019,30 @@ int pb2_window_start(pb2_window_t* w) {
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
+        const Win2Dev g = run_desc(w, w->cur);
         if (w->kind == 0) {
-            const WinDev d = run_desc(w, w->cur);
-            if (d.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(d, e->nworkers, e->params.threads, e->stream));
-            else {
-                pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(d);
-                PB2_CUDA(e, cudaGetLastError());
-            }
+            if (w->shape.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(g.w, e->nworkers, e->params.threads, e->stream));
+            else pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(g.w);
+            PB2_CUDA(e, cudaGetLastError());
         } else {
-            int rc = w->g.w.lanes ? pb2_gemm2_prio_launch(w->g, e->nworkers_gemm, e->stream)
-                                : pb2_gemm2_launch<false>(w->g, e->nworkers_gemm, e->stream);
+            int rc = w->shape.lanes ? pb2_gemm2_prio_launch(g, e->nworkers_gemm, e->stream)
+                                    : pb2_gemm2_launch<false>(g, e->nworkers_gemm, e->stream);
             if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
             w->g.fresh_tmaps = 0;
         }
     }
     PB2_CUDA(e, cudaEventRecord(w->ev2, e->stream));
     w->launched = true;
-    w->armed[w->cur] = false;
+    w->copy[w->cur].armed = false;
     const int o = w->cur ^ 1;
-    if (w->kind == 0 && w->ntasks > 0 && w->run1.ctl && !w->armed[o]) {
+    if (w->ncopies == 2 && w->copy[o].run.ctl && !w->copy[o].armed) {
         // The other copy, for the next run, beside this one: after the run that used it last (ev1 of this arm follows
         // it on the engine stream), on one CTA per SM, which fits next to the run's workers (DESIGN.md §5, §6).
         PB2_CUDA(e, cudaStreamWaitEvent(e->arm_stream, w->ev1, 0));
         const int rc = reset_copy(w, o, e->arm_stream, 1);
         if (rc != PB2_SUCCESS) return rc;
         PB2_CUDA(e, cudaEventRecord(w->ev_arm, e->arm_stream));
-        w->armed[o] = true; w->beside[o] = true;
+        w->copy[o].armed = true; w->copy[o].beside = true;
     }
     return PB2_SUCCESS;
 }
@@ -1061,12 +1058,13 @@ int pb2_window_export(pb2_window_t* w, pb2_window_handle_t* h) {
     if (!w->shared) { e->last_error = "window was not created with shared windows enabled"; return PB2_ERR_NOT_SUPPORTED; }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     memset(h, 0, sizeof *h);
+    const Win2Dev g = run_desc(w, 0);           // a shared window's only copy
     cudaIpcMemHandle_t ih;
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->kind == 1 ? w->g.udep : w->g.w.dep));  memcpy(h->dep, &ih, 64);   // GEMM windows: unit words
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.ring)); memcpy(h->ring, &ih, 64);
-    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.ctl));  memcpy(h->ctl, &ih, 64);
-    if (w->g.w.tiles && w->ntiles > 0) { PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->g.w.tiles)); memcpy(h->tiles, &ih, 64); h->ntiles = w->ntiles; }
-    h->cap_mask = w->g.w.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->kind == 1 ? 1 : 0;
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, w->kind == 1 ? g.udep : g.w.dep));  memcpy(h->dep, &ih, 64);   // GEMM windows: unit words
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, g.w.ring)); memcpy(h->ring, &ih, 64);
+    PB2_CUDA(e, cudaIpcGetMemHandle(&ih, g.w.ctl));  memcpy(h->ctl, &ih, 64);
+    if (g.w.tiles && w->ntiles > 0) { PB2_CUDA(e, cudaIpcGetMemHandle(&ih, g.w.tiles)); memcpy(h->tiles, &ih, 64); h->ntiles = w->ntiles; }
+    h->cap_mask = g.w.cap_mask; h->ntasks = w->ntasks; h->entry_kind = w->kind == 1 ? 1 : 0;
     return PB2_SUCCESS;
 }
 
@@ -1149,7 +1147,7 @@ int pb2_window_wait(pb2_window_t* w, pb2_window_stats_t* stats) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaEventSynchronize(w->ev2));
     Ctl c;
-    PB2_CUDA(e, cudaMemcpy(&c, run_desc(w, w->cur).ctl, sizeof c, cudaMemcpyDeviceToHost));
+    PB2_CUDA(e, cudaMemcpy(&c, run_desc(w, w->cur).w.ctl, sizeof c, cudaMemcpyDeviceToHost));
     if (stats) {
         memset(stats, 0, sizeof *stats);
         stats->tasks_retired = c.retired.v;
@@ -1171,7 +1169,7 @@ int pb2_window_results(pb2_window_t* w, int32_t* retire_order, uint32_t* start_s
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     const size_t n = (size_t)w->ntasks;
-    const WinDev d = run_desc(w, w->cur);     // the copy of the last run
+    const WinDev d = run_desc(w, w->cur).w;   // the copy of the last run
     if (retire_order && n) PB2_CUDA(e, cudaMemcpy(retire_order, d.retire_log, n * 4, cudaMemcpyDeviceToHost));
     if (start_seq && n) PB2_CUDA(e, cudaMemcpy(start_seq, d.start_seq, n * 4, cudaMemcpyDeviceToHost));
     if (end_seq && n) PB2_CUDA(e, cudaMemcpy(end_seq, d.end_seq, n * 4, cudaMemcpyDeviceToHost));

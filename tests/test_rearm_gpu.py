@@ -1,7 +1,9 @@
-"""One HBM window launched many times.  Consecutive runs of a non-shared HBM window alternate between two copies of its
-per-run state, and the CTAs of each run arm the other copy for the next run, so from the third launch on no reset
-kernel runs.  Every run must compute exactly what a fresh window's first run computes, and what the sequential oracle
-computes: retire log, start / end events, seen versions, results, tile table and statistics."""
+"""One window launched many times.  Consecutive runs of a non-shared HBM window alternate between two copies of its
+per-run state, and while a run runs the reset kernel arms the other copy for the next run on a stream of its own, so
+from the third launch on no reset kernel runs in front of a run.  A GEMM window keeps one copy, unit words included,
+and re-arms it in front of every run.  Every run must compute exactly what a fresh window's first run computes, and
+what the sequential oracle computes: retire log, start / end events, seen versions, results, tile table and
+statistics."""
 import numpy as np
 import pytest
 
@@ -39,6 +41,43 @@ def wide_group_dag(tb=1 << 20):
     return dags.Dag(t, np.arange(1, 9, dtype=np.uint32), np.array([0], np.int32), ntiles=1, tile_bytes=tb, name="wide")
 
 
+def gemm_chains_dag():
+    """A GEMM window over tiles of 256 x 256 bf16: two k-chains C0 = A0 B0 + A1 B1 and C1 = A0 B1 + A1 B0 (units of two
+    parts), CHECKs of C0 and C1, and INCR, COPY, SCALE and CHECKs of two integer tiles X and Y around them.  A holds
+    1.0 and B 1 / 256, so every GEMM adds exactly 1.0 to each element of C.  DTD dependency words; tiles A0 A1 B0 B1 C0
+    C1 X Y."""
+    T = 256
+    A0, A1, B0, B1, C0, C1, X, Y = range(8)
+    R, W = L.ACCESS_READ, L.ACCESS_RW
+    gemm = lambda a, b, c: (L.BODY_GEMM_BF16, [(a, R), (b, R), (c, W)], (T, T, T))
+    rows = [(L.BODY_INCR_I32, [(X, W)], (1, 0, 0)), gemm(A0, B0, C0), gemm(A1, B1, C0), gemm(A0, B1, C1),
+            gemm(A1, B0, C1), (L.BODY_CHECK_I32, [(C0, R)], (0x40004000, 0, 0)),
+            (L.BODY_CHECK_I32, [(C1, R)], (0x40004000, 0, 0)), (L.BODY_COPY, [(X, R), (Y, W)], (0, 0, 0)),
+            (L.BODY_CHECK_I32, [(X, R)], (5, 0, 0)), (L.BODY_SCALE_I32, [(Y, W)], (3, 0, 0)),
+            (L.BODY_CHECK_I32, [(Y, R)], (15, 0, 0))]
+    n = len(rows)
+    t = np.zeros(n, L.TASK_DTYPE)
+    t["tile"][:] = -1
+    ft, fo = np.full((n, 4), -1, np.int32), np.zeros((n, 4), np.int32)
+    for i, (body, flows, ip) in enumerate(rows):
+        t["body"][i], t["nb_flows"][i], t["iparam"][i] = body, len(flows), ip
+        for f, (tile, acc) in enumerate(flows):
+            t["tile"][i, f], t["access"][i, f] = tile, acc
+            ft[i, f], fo[i, f] = tile, orc.DTD_INPUT if acc == R else orc.DTD_INOUT
+    t["priority"] = [2, 0, 0, 3, 3, 1, 1, 2, 0, 1, 0]
+    src, dst, flow, dep = orc.dtd_build(t["nb_flows"].astype(np.int32), ft, fo, 8)
+    begin, count, succ = dags._csr_from_edges(n, src, dst, flow)
+    t["succ_begin"], t["succ_count"], t["dep_goal"] = begin, count, dep
+    tb = T * T * 2
+    host = np.zeros((8, tb // 4), np.uint32)
+    host[[A0, A1]] = 0x3F803F80                                  # bf16 1.0
+    host[[B0, B1]] = 0x3B803B80                                  # bf16 1 / 256
+    host[[X, Y]] = 4
+    host[X:].reshape(-1)[::977] = 0
+    return dags.Dag(t, succ, np.nonzero(dep == 0)[0].astype(np.int32), ntiles=8, tile_bytes=tb, kind=1,
+                    name="gemm_chains", meta={"host": host.view(np.int32).reshape(-1)})
+
+
 TB = 256 * 1024
 # (id, engine keywords, dag, tiles staged in from host memory every run)
 CASES = [
@@ -49,10 +88,14 @@ CASES = [
     ("ex05_counter_words", {}, lambda: counter_mode(dags.ex05_broadcast(64, 14, TB)), True),
     ("wide_check_parts", {"part_bytes": 64 * 1024}, wide_group_dag, True),
     ("chain_one_worker", {"max_workers": 1}, lambda: dags.ex02_chain(40), False),
+    ("gemm_chains_wide_parts", {"part_bytes": 32 * 1024}, gemm_chains_dag, True),
+    ("gemm_chains_wide_parts_queue_policy_1", {"part_bytes": 32 * 1024, "queue_policy": 1}, gemm_chains_dag, True),
 ]
 
 
 def host_data(dag):
+    if "host" in dag.meta:
+        return dag.meta["host"].copy()
     host = np.full(dag.ntiles * dag.tile_bytes // 4, 4, np.int32)
     host[::977] = 0
     return host
@@ -109,12 +152,12 @@ def test_every_run_matches_a_fresh_window(name, engine_kw, make_dag, staged, wai
     ref = oracle(dag, host, staged)
     with Engine(0, **engine_kw) as e:
         tiles, slab = tile_table(e, dag, host, staged)
-        fresh = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
+        fresh = e.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
         first = (fresh.run(), fresh.results())
         fresh.close()
         exact = engine_kw.get("max_workers") == 1
         assert_run_matches(dag, *first, first, ref, exact)
-        w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
+        w = e.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
         if wait_between:
             for _ in range(RUNS):
                 st = w.run()
