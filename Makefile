@@ -5,7 +5,8 @@ EXTRA     ?=
 NVCCFLAGS := $(EXTRA) -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 CSRC      := parsec_b200/csrc
 LIB       := parsec_b200/libparsec_b200.so
-CU_SRCS   := $(CSRC)/pb2_engine.cu $(CSRC)/pb2_engine_prio.cu $(CSRC)/pb2_stream.cu
+CU_SRCS   := $(CSRC)/pb2_engine.cu $(CSRC)/pb2_engine_prio.cu $(CSRC)/pb2_engine_trace.cu $(CSRC)/pb2_engine_prio_trace.cu \
+             $(CSRC)/pb2_stream.cu
 CPP_SRCS  := $(wildcard $(CSRC)/*.cpp)
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(wildcard $(CSRC)/*.hpp) $(wildcard include/*.h)
 

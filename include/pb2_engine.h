@@ -246,6 +246,9 @@ int  pb2_engine_set_shared_windows(pb2_engine_t* engine, int on, const int32_t* 
 /* part size for the windows created from now on (a serial chain of large tiles wants small parts: a 64-thread
  * worker keeps only 4 KiB in flight; wide DAGs want one part per tile) */
 int  pb2_engine_set_part_bytes(pb2_engine_t* engine, int32_t part_bytes);
+/* on != 0: the windows created from now on record when and on which SM each task ran (pb2_window_trace), through
+ * traced builds of the window kernels; off (the default) they run the untraced kernels */
+int  pb2_engine_set_window_trace(pb2_engine_t* engine, int on);
 /* granularity of cooperative stage-in (default 64 KiB, <= 0: whole tiles): a tile that has to be staged in is cut into
  * slices of this size and every worker that needs the tile pulls the slices nobody has claimed yet */
 int  pb2_engine_set_stage_slice_bytes(pb2_engine_t* engine, int32_t bytes);
@@ -277,6 +280,18 @@ int  pb2_window_results(pb2_window_t* window,
                         uint64_t* result,        /* [ntasks] body result (CHECK: mismatches<<40 | sum)   */
                         int32_t*  worker,        /* [ntasks] CTA that ran the task                       */
                         pb2_tile_t* tiles_out);  /* [ntiles] final tile table (state, version)           */
+/* Per-task device time stamps of the last launch of a window created with trace on (pb2_engine_set_window_trace),
+ * valid after wait; any pointer may be NULL.  Times are %globaltimer nanoseconds of this GPU's clock.  A task gets the
+ * interval of its scheduling entity: from the earliest pop of any of its parts to the retirement of the last part; the
+ * members of a read group, of a fused producer unit or of a GEMM unit share one interval and SM.  A task that never
+ * ran (a failed run) reads 0.  PB2_ERR_NOT_SUPPORTED for a window created without trace. */
+int  pb2_window_trace(pb2_window_t* window,
+                      uint64_t* t_start_ns,      /* [ntasks] earliest pop of a part of the task's entity  */
+                      uint64_t* t_end_ns,        /* [ntasks] its retirement                               */
+                      uint32_t* smid,            /* [ntasks] SM of the retiring part                      */
+                      int32_t*  unit);           /* [ntasks] the task that leads the entity (host side):
+                                                  * read-group leader, fused producer, GEMM unit's first
+                                                  * task, or the task itself                              */
 
 /* --- windows that release dependencies of tasks living in OTHER GPUs' windows (remote_dep edges, remote_dep.h:42-58,
  * without the host: the activation is a device atomic on the peer's dependency word plus a ring write over NVLink).

@@ -221,6 +221,11 @@ int  pb2_taskpool_set_device_types(pb2_taskpool_t* tp, int types);
 /* completion trace, one entry per task in the order the host ran __parsec_complete_execution:
  * out_task[i] = task id (insertion / enumeration order), out_device[i] = device_index that ran it */
 int  pb2_taskpool_completion_trace(pb2_taskpool_t* tp, int32_t* out_task, int32_t* out_device, int32_t cap);
+/* device time stamps, indexed by task id (arrays sized nb_tasks, may be NULL): with the MCA parameter
+ * device_engine_trace set, a task that ran in a GPU window gets that window's interval for it (%globaltimer ns of
+ * ITS device's clock: devices are not on one time axis) and the SM; every other task (CPU incarnations, user submit
+ * bodies, dry runs) gets 0, 0 and 0.  device[i] = device_index that ran task i (-1: not run) */
+int  pb2_taskpool_device_trace(pb2_taskpool_t* tp, uint64_t* t_start_ns, uint64_t* t_end_ns, int32_t* device, uint32_t* smid);
 /* per task: locals[0..1], class id, flow versions seen (4), body result; arrays sized nb_tasks (may be NULL) */
 int  pb2_taskpool_task_info(pb2_taskpool_t* tp, int32_t* class_id, int32_t* locals2, uint32_t* seen_version4,
                             uint64_t* result);

@@ -113,10 +113,10 @@ ENGINE_SYMBOLS = [
     "pb2_engine_create", "pb2_engine_destroy", "pb2_engine_info", "pb2_engine_last_error",
     "pb2_engine_malloc", "pb2_engine_free", "pb2_engine_host_register", "pb2_engine_host_unregister",
     "pb2_engine_memcpy_h2d", "pb2_engine_prefetch_h2d", "pb2_engine_memcpy_d2h", "pb2_engine_synchronize", "pb2_engine_set_stream", "pb2_engine_get_stream", "pb2_engine_copy_batch", "pb2_engine_ipc_export", "pb2_engine_ipc_open",
-    "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
+    "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_window_trace", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
     "pb2_window_arm", "pb2_window_start",
     "pb2_window_create", "pb2_window_destroy", "pb2_window_launch", "pb2_window_wait",
-    "pb2_window_results",
+    "pb2_window_results", "pb2_window_trace",
     "pb2_partition_create", "pb2_partition_sizes", "pb2_partition_get", "pb2_partition_destroy", "pb2_partition_error",
     "pb2_partition_set_push", "pb2_partition_push_count", "pb2_partition_get_push", "pb2_window_set_push",
 ]
@@ -157,6 +157,8 @@ def load():
     lib.pb2_engine_set_shared_windows.argtypes = [vp, C.c_int, vp]
     lib.pb2_window_task_entries.argtypes = [vp, vp]
     lib.pb2_engine_set_part_bytes.argtypes = [vp, i32]
+    lib.pb2_engine_set_window_trace.argtypes = [vp, C.c_int]
+    lib.pb2_window_trace.argtypes = [vp, vp, vp, vp, vp]
     lib.pb2_engine_set_stage_slice_bytes.argtypes = [vp, i32]
     lib.pb2_window_export.argtypes = [vp, vp]
     lib.pb2_window_set_remote.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32]

@@ -36,13 +36,15 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // reset: (re)arm one window.  dep words, ring, counters, tile table; the units of a GEMM window.
 // ---------------------------------------------------------------------------------------------
-// The per-run state of g.w (rearm_run) and, in a GEMM window, its units' words.  A GEMM window never has more units
-// than tasks.
+// The per-run state of g.w (rearm_run), in a GEMM window its units' words, in a traced window its time stamps.  A GEMM
+// window never has more units than tasks.
 __global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
     for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
+    if (g.trace.t_start)
+        for (size_t i = gid; i < (size_t)g.w.ntasks; i += gsz) { g.trace.t_start[i] = ~0ull; g.trace.t_end[i] = 0; g.trace.smid[i] = 0; }
     rearm_run(g.w, tiles_init, ready, nready, gid, gsz);
 }
 
@@ -103,6 +105,7 @@ struct RunState {
     uint32_t* slice_claim; uint32_t* slice_done;    // RunShape::claims
     Lanes* lanes;                         // RunShape::lanes
     int32_t* udep; int32_t* unit_parts_left;        // GEMM windows: the units' dependency words and part counts
+    unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid;     // RunShape::trace (TraceDev)
 };
 
 // What every copy of a window's per-run state is sized from besides ntasks and ntiles, recorded by pb2_window_create.
@@ -112,6 +115,7 @@ struct RunShape {
     bool parts = false;                   // per-task part counts (an HBM window with wide tasks)
     bool claims = false;                  // stage-in is sliced: claim arrays per tile
     bool lanes = false;                   // queue_policy 1: priority lanes, which start as lane_image
+    bool trace = false;                   // per-task device time stamps (pb2_engine_set_window_trace)
     Lanes lane_image{};
 };
 
@@ -135,6 +139,7 @@ struct pb2_window_s {
     int ncopies = 1, cur = 0, arms = 0;
     cudaEvent_t ev_arm = nullptr;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
+    std::vector<int32_t> task_unit;           // traced windows, per task: the task that leads its scheduling entity
     std::vector<void*> allocs;
     std::vector<void*> peer_ptrs;
     std::vector<pb2_tile_t*> peer_tiles;     // per rank: its tile table as mapped here (nullptr: none / self)
@@ -407,6 +412,8 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     plan.run.nunits = (int32_t)units.size();
     w->task_entry.resize((size_t)ntasks);
     for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
+    if (!w->task_unit.empty())
+        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = segs[(size_t)units[(size_t)unit_of[t]].seg_begin].task;
     int rc;
     uint32_t* d_succ = nullptr; GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
     if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
@@ -555,6 +562,15 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
         if ((rc = dev_alloc_copy(w, &d_group, group.data(), group.size())) != PB2_SUCCESS) return rc;
         if ((rc = dev_alloc_copy(w, &d_gmem, gmem.data(), gmem.size())) != PB2_SUCCESS) return rc;
         d.group = d_group; d.group_mem = d_gmem;
+        // a read group is led by its leader, unless a producer runs with it: then by the producer
+        if (!w->task_unit.empty())
+            for (int pass = 0; pass < 2; ++pass)
+                for (int32_t t = 0; t < ntasks; ++t) {
+                    const uint32_t gd = group[(size_t)t];
+                    if ((gd & 15u) == 0 || ((gd & PB2_GROUP_FUSED) != 0) != (pass == 1)) continue;
+                    const uint32_t b = (gd & ~PB2_GROUP_FUSED) >> 4;
+                    for (uint32_t i = 0; i < (gd & 15u); ++i) w->task_unit[(size_t)gmem[b + i]] = t;
+                }
     } else if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
     d.succ = d_succ;
     if (extra_parts) {
@@ -584,6 +600,7 @@ static int alloc_run(pb2_window_t* w, int c) {
     if (s.lanes) alloc(&r.lanes, 1);
     // every GEMM window has the unit words, even without units: pb2_window_export hands out udep
     if (w->kind == 1) { alloc(&r.udep, (size_t)s.nunits); alloc(&r.unit_parts_left, (size_t)s.nunits); }
+    if (s.trace) { alloc(&r.t_start, nt); alloc(&r.t_end, nt); alloc(&r.smid, nt); }
     if (rc != PB2_SUCCESS) return rc;
     // copy 1 takes copy 0's lanes device to device: a copy from pageable host memory may wait for the engine stream
     if (s.lanes) PB2_CUDA(e, c == 0 ? cudaMemcpyAsync(r.lanes, &s.lane_image, sizeof(Lanes), cudaMemcpyHostToDevice, stream)
@@ -602,6 +619,7 @@ static Win2Dev run_desc(const pb2_window_t* w, int c) {
     d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
     d.lanes = r.lanes;
     g.udep = r.udep; g.parts_left = r.unit_parts_left;
+    g.trace = TraceDev{r.t_start, r.t_end, r.smid};
     return g;
 }
 
@@ -653,7 +671,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
         }
     }
     int occ = 0;
-    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb2_engine_hbm_kernel<false>, p.threads, 0));
+    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb2_engine_hbm_kernel<false, false>, p.threads, 0));
     int per_sm = occ < p.workers_per_sm ? occ : p.workers_per_sm;
     if (per_sm < 1) per_sm = 1;
     e->nworkers = e->prop.multiProcessorCount * per_sm;
@@ -860,6 +878,11 @@ int pb2_engine_set_part_bytes(pb2_engine_t* e, int32_t part_bytes) {
     e->params.part_bytes = part_bytes == 0 ? kDefaultPartBytes : part_bytes;
     return PB2_SUCCESS;
 }
+int pb2_engine_set_window_trace(pb2_engine_t* e, int on) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    e->window_trace = on != 0;
+    return PB2_SUCCESS;
+}
 int pb2_engine_set_shared_windows(pb2_engine_t* e, int on, const int32_t* next_rs_begin) {
     if (!e) return PB2_ERR_BAD_PARAM;
     e->shared_windows = on != 0; e->next_rs_begin = on ? next_rs_begin : nullptr;
@@ -919,7 +942,12 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     int32_t nlanes = 0;
     std::vector<uint8_t> task_lane;
     if (prio) task_lane = task_priority_lanes(tasks, ntasks, &nlanes);
+    if (e->window_trace) {                      // every task leads itself until a plan groups it
+        w->task_unit.resize((size_t)ntasks);
+        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = t;
+    }
     WindowPlan plan;
+    plan.run.trace = e->window_trace;
     if (kind == 0) TRY(plan_hbm_window(w, dtasks, succ, nsucc, tiles, ntiles, ready, nready, task_lane, plan));
     else {
         // HBM bodies of a GEMM window are cut into parts as HBM windows cut them.  Not in shared windows: their units
@@ -1020,13 +1048,18 @@ int pb2_window_start(pb2_window_t* w) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
         const Win2Dev g = run_desc(w, w->cur);
+        const bool lanes = w->shape.lanes, trace = w->shape.trace;
         if (w->kind == 0) {
-            if (w->shape.lanes) PB2_CUDA(e, pb2_hbm_prio_launch(g.w, e->nworkers, e->params.threads, e->stream));
-            else pb2_engine_hbm_kernel<false><<<e->nworkers, e->params.threads, 0, e->stream>>>(g.w);
+            const int nw = e->nworkers, th = e->params.threads;
+            if (trace) PB2_CUDA(e, lanes ? pb2_hbm_prio_trace_launch(g.w, g.trace, nw, th, e->stream)
+                                         : pb2_hbm_trace_launch(g.w, g.trace, nw, th, e->stream));
+            else if (lanes) PB2_CUDA(e, pb2_hbm_prio_launch(g.w, nw, th, e->stream));
+            else pb2_engine_hbm_kernel<false, false><<<nw, th, 0, e->stream>>>(g.w, TraceDev{});
             PB2_CUDA(e, cudaGetLastError());
         } else {
-            int rc = w->shape.lanes ? pb2_gemm2_prio_launch(g, e->nworkers_gemm, e->stream)
-                                    : pb2_gemm2_launch<false>(g, e->nworkers_gemm, e->stream);
+            const int nw = e->nworkers_gemm;
+            int rc = trace ? (lanes ? pb2_gemm2_prio_trace_launch(g, nw, e->stream) : pb2_gemm2_trace_launch(g, nw, e->stream))
+                           : (lanes ? pb2_gemm2_prio_launch(g, nw, e->stream) : pb2_gemm2_launch<false, false>(g, nw, e->stream));
             if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
             w->g.fresh_tmaps = 0;
         }
@@ -1177,6 +1210,23 @@ int pb2_window_results(pb2_window_t* w, int32_t* retire_order, uint32_t* start_s
     if (result && n) PB2_CUDA(e, cudaMemcpy(result, d.result, n * 8, cudaMemcpyDeviceToHost));
     if (worker && n) PB2_CUDA(e, cudaMemcpy(worker, d.worker, n * 4, cudaMemcpyDeviceToHost));
     if (tiles_out && w->ntiles) PB2_CUDA(e, cudaMemcpy(tiles_out, d.tiles, (size_t)w->ntiles * sizeof(pb2_tile_t), cudaMemcpyDeviceToHost));
+    return PB2_SUCCESS;
+}
+
+int pb2_window_trace(pb2_window_t* w, uint64_t* t_start_ns, uint64_t* t_end_ns, uint32_t* smid, int32_t* unit) {
+    if (!w) return PB2_ERR_BAD_PARAM;
+    pb2_engine_t* e = w->e;
+    if (!w->shape.trace) { e->last_error = "window was created without trace (pb2_engine_set_window_trace)"; return PB2_ERR_NOT_SUPPORTED; }
+    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    const size_t n = (size_t)w->ntasks;
+    const TraceDev tr = run_desc(w, w->cur).trace;   // the copy of the last run
+    if (t_start_ns && n) {
+        PB2_CUDA(e, cudaMemcpy(t_start_ns, tr.t_start, n * 8, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < n; ++i) if (t_start_ns[i] == ~0ull) t_start_ns[i] = 0;     // never popped
+    }
+    if (t_end_ns && n) PB2_CUDA(e, cudaMemcpy(t_end_ns, tr.t_end, n * 8, cudaMemcpyDeviceToHost));
+    if (smid && n) PB2_CUDA(e, cudaMemcpy(smid, tr.smid, n * 4, cudaMemcpyDeviceToHost));
+    if (unit && n) memcpy(unit, w->task_unit.data(), n * sizeof(int32_t));
     return PB2_SUCCESS;
 }
 

@@ -8,12 +8,12 @@
 namespace pb2 {
 
 cudaError_t pb2_hbm_prio_launch(const WinDev& w, int nworkers, int threads, cudaStream_t stream) {
-    pb2_engine_hbm_kernel<true><<<nworkers, threads, 0, stream>>>(w);
+    pb2_engine_hbm_kernel<true, false><<<nworkers, threads, 0, stream>>>(w, TraceDev{});
     return cudaGetLastError();
 }
 
 int pb2_gemm2_prio_launch(const Win2Dev& g, int nworkers, cudaStream_t stream) {
-    return pb2_gemm2_launch<true>(g, nworkers, stream);
+    return pb2_gemm2_launch<true, false>(g, nworkers, stream);
 }
 
 }  // namespace pb2

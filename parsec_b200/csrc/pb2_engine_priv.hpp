@@ -26,6 +26,7 @@ struct pb2_engine_s {
     std::string last_error;
     std::mutex mu;
     bool shared_windows = false;
+    bool window_trace = false;           // windows created from now on record per-task device time stamps
     const int32_t* next_rs_begin = nullptr;   // remote out-degree CSR of the next shared window (not owned)
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
 };

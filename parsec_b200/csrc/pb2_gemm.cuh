@@ -220,6 +220,7 @@ struct Win2Dev {
     const CUtensorMap* tmaps;       // one per tile (w.ntiles)
     int32_t nunits;
     int32_t fresh_tmaps;            // first launch since tmaps were written: every producer acquires all of them first
+    TraceDev trace;                 // per-task time stamps of a traced window (null otherwise); the HBM kernel takes them beside w
 };
 
 namespace gemm {
@@ -240,23 +241,33 @@ struct Shared {
     uint64_t empty[kStages];
 };
 
-// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges
-template <bool PRIO>
+// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges.  TRACE: every
+// member gets the unit's interval (TraceDev), which starts at the earliest pop of a part of it (its first task's t_start).
+template <bool PRIO, bool TRACE>
 __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u, int unit_id) {
     const WinDev& w = g.w;
     const int lane = threadIdx.x & 31;
     const int L = u.seg_count;
-    unsigned long long ebase = 0, rbase = 0;
+    unsigned long long ebase = 0, rbase = 0, now = 0;
     if (lane == 0) {
         ebase = atomicAdd(&w.ctl->evt.v, (unsigned long long)(2 * L));
         rbase = atomicAdd(&w.ctl->retired.v, (unsigned long long)L);
-        *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+        now = globaltimer_ns();
+        *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
     }
     ebase = __shfl_sync(0xffffffffu, ebase, 0);
     rbase = __shfl_sync(0xffffffffu, rbase, 0);
+    unsigned long long t0 = 0;
+    uint32_t sm = 0;
+    if (TRACE) {
+        now = __shfl_sync(0xffffffffu, now, 0);
+        t0 = trace_start_of(g.trace, g.segs[u.seg_begin].task);
+        sm = smid();
+    }
     const uint32_t cver = (u.flags & 1) ? *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) : 0u;
     for (int i = lane; i < L; i += 32) {
         const GSeg s = g.segs[u.seg_begin + i];
+        if (TRACE) trace_task(g.trace, s.task, t0, now, sm);
         w.start_seq[s.task] = (uint32_t)(ebase + 2 * i);
         w.end_seq[s.task] = (uint32_t)(ebase + 2 * i + 1);
         w.retire_log[rbase + i] = s.task;
@@ -311,8 +322,9 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
 
 }  // namespace gemm
 
-// PRIO: queue_policy 1 (priority lanes of units, pop_prio)
-template <bool PRIO>
+// PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: record the device time stamps of every task in
+// g.trace (TraceDev); the untraced instantiations never touch it.
+template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(gemm::kThreads, 1)
 pb2_engine_gemm2_kernel(Win2Dev g) {
     using namespace gemm;
@@ -344,8 +356,10 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             if (e == kEmpty) { j.stop = 1; }
             else {
                 __threadfence();
+                const unsigned long long t_pop = TRACE ? globaltimer_ns() : 0ull;
                 j.unit = PB2_SUCC_TASK((uint32_t)e); j.part = PB2_SUCC_FLOW((uint32_t)e);
                 const GUnit u = g.units[j.unit];
+                if (TRACE) trace_pop(g.trace, g.segs[u.seg_begin].task, t_pop);     // the unit's first task leads it
                 j.is_gemm = u.flags & 1; j.pushout = (u.flags >> 1) & 1;
                 j.seg_begin = u.seg_begin; j.seg_count = u.seg_count; j.tileC = u.tileC; j.nparts = u.nparts;
                 j.M = u.M; j.N = u.N; j.K = u.K;
@@ -482,25 +496,28 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             int last = 0;
             if (lane == 0) { __threadfence(); last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
             last = __shfl_sync(0xffffffffu, last, 0);
-            if (last) { __threadfence(); retire_unit_warp<PRIO>(g, g.units[job.unit], job.unit); }
+            if (last) { __threadfence(); retire_unit_warp<PRIO, TRACE>(g, g.units[job.unit], job.unit); }
         }
         __syncthreads();             // sh.job is rewritten by the next pop
     }
 }
 
-template <bool PRIO>
+template <bool PRIO, bool TRACE>
 static inline int pb2_gemm2_launch(const Win2Dev& g, int nworkers, cudaStream_t stream) {
     static bool attr_set = false;       // one per instantiation
     if (!attr_set) {
-        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel<PRIO>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
+        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel<PRIO, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
         attr_set = true;
     }
     if (nworkers < 1) return PB2_ERR_BAD_PARAM;
-    pb2_engine_gemm2_kernel<PRIO><<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
+    pb2_engine_gemm2_kernel<PRIO, TRACE><<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
     return cudaGetLastError() == cudaSuccess ? PB2_SUCCESS : PB2_ERR_DEVICE;
 }
 
 // pb2_engine_prio.cu: launch the queue_policy 1 instantiation
 int pb2_gemm2_prio_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
+// pb2_engine_trace.cu, pb2_engine_prio_trace.cu: launch the traced FIFO / queue_policy 1 instantiations
+int pb2_gemm2_trace_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
+int pb2_gemm2_prio_trace_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
 
 }  // namespace pb2

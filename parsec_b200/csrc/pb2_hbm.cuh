@@ -1,8 +1,9 @@
 // pb2_hbm.cuh -- the persistent engine kernel of HBM-body windows (pb2_engine_hbm_kernel) and what it runs besides
 // the shared worker code of pb2_worker.cuh: read groups and fused producer units.  Instantiated for the FIFO ready ring
-// in pb2_engine.cu and for priority lanes (queue_policy 1) in pb2_engine_prio.cu: each translation unit holds one
-// instantiation, because a second kernel calling the same __noinline__ helpers makes ptxas give them the standard call
-// ABI, which costs the kernel a stack frame and spills at its 80-register budget.
+// in pb2_engine.cu and for priority lanes (queue_policy 1) in pb2_engine_prio.cu, and traced (window trace) in
+// pb2_engine_trace.cu and pb2_engine_prio_trace.cu: each translation unit holds one instantiation, because a second
+// kernel calling the same __noinline__ helpers makes ptxas give them the standard call ABI, which costs the kernel a
+// stack frame and spills at its 80-register budget.
 #pragma once
 #include "pb2_sched.cuh"
 #include "pb2_worker.cuh"
@@ -112,10 +113,20 @@ static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, G
     return r;
 }
 
+// Thread 0 of the retiring part, TRACE: the tasks of the entity led by `lead` -- itself and the n members mem[] of its
+// read group (a plain group's leader is mem[0]) -- get the entity's interval (TraceDev).
+__device__ __forceinline__ void trace_entity(const TraceDev& tr, int32_t lead, const int32_t* mem, int n, unsigned long long t_end) {
+    const unsigned long long t0 = trace_start_of(tr, lead);
+    const uint32_t sm = smid();
+    trace_task(tr, lead, t0, t_end, sm);
+    for (int i = 0; i < n; ++i) trace_task(tr, mem[i], t0, t_end, sm);
+}
+
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
-template <bool PRIO>
+// TRACE: record the device time stamps of every task in tr (TraceDev); the untraced instantiations never touch tr.
+template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
-pb2_engine_hbm_kernel(WinDev w) {
+pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
     __shared__ TaskSmem s;
     __shared__ BulkSmem bulk;
     __shared__ GroupSmem g;
@@ -127,6 +138,8 @@ pb2_engine_hbm_kernel(WinDev w) {
         if (threadIdx.x == 0) {
             const int32_t e = pop_entry<PRIO>(w, &t_start);
             if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
+            // the popped task leads its entity (a group's leader, a fused producer)
+            if (TRACE && e != kEmpty) trace_pop(tr, w.nparts ? PB2_ENT_TASK(e) : e, globaltimer_ns());
             s.entry = e;
         }
         __syncthreads();
@@ -214,7 +227,9 @@ pb2_engine_hbm_kernel(WinDev w) {
                         w.end_seq[m] = ev + 1u + (uint32_t)(gn + i);
                         w.retire_log[seq + 1u + (uint32_t)i] = m;
                     }
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    const unsigned long long now = globaltimer_ns();
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
+                    if (TRACE) trace_entity(tr, id, g.mem, gn, now);
                     s.window_done = (int32_t)(seq + 1u + (uint32_t)gn) == w.ntasks ? 1 : 0;
                     __threadfence();
                 } else if (last && gn) {
@@ -222,7 +237,9 @@ pb2_engine_hbm_kernel(WinDev w) {
                     const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
                     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
                     for (int i = 0; i < gn; ++i) { w.end_seq[g.mem[i]] = ev + (uint32_t)i; w.retire_log[seq + (uint32_t)i] = g.mem[i]; }
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+                    const unsigned long long now = globaltimer_ns();
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
+                    if (TRACE) trace_entity(tr, id, g.mem, gn, now);
                     s.window_done = (int32_t)(seq + (uint32_t)gn) == w.ntasks ? 1 : 0;
                     __threadfence();
                 } else if (last) {
@@ -230,7 +247,9 @@ pb2_engine_hbm_kernel(WinDev w) {
                     w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
                     // the retire log is written before the out-edges are released, so that it is a linear
                     // extension of the DAG's partial order (a successor can only retire after us)
-                    s.window_done = retire_task(w, id) ? 1 : 0;
+                    unsigned long long now;
+                    s.window_done = retire_task(w, id, now) ? 1 : 0;
+                    if (TRACE) trace_entity(tr, id, nullptr, 0, now);
                     __threadfence();
                 }
             }
@@ -258,5 +277,8 @@ pb2_engine_hbm_kernel(WinDev w) {
 
 // pb2_engine_prio.cu: launch the queue_policy 1 instantiation
 cudaError_t pb2_hbm_prio_launch(const WinDev& w, int nworkers, int threads, cudaStream_t stream);
+// pb2_engine_trace.cu, pb2_engine_prio_trace.cu: launch the traced FIFO / queue_policy 1 instantiations
+cudaError_t pb2_hbm_trace_launch(const WinDev& w, const TraceDev& tr, int nworkers, int threads, cudaStream_t stream);
+cudaError_t pb2_hbm_prio_trace_launch(const WinDev& w, const TraceDev& tr, int nworkers, int threads, cudaStream_t stream);
 
 }  // namespace pb2

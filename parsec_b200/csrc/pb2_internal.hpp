@@ -122,6 +122,9 @@ struct pb2_htask_s {
     uint32_t seen_version[PB2_MAX_FLOWS] = {0, 0, 0, 0};
     uint64_t result = 0;
     int8_t ran_on = -1;
+    // device_engine_trace: the window's time stamps of the task (its device's clock) and the SM; 0 when it ran elsewhere
+    uint64_t dev_t_start = 0, dev_t_end = 0;
+    uint32_t dev_smid = 0;
 };
 
 struct pb2_gpu_task_s {             // parsec_gpu_task_t, device_gpu.h:117-143
@@ -184,6 +187,7 @@ struct pb2_device_module_s {
     int cuda_index = -1;
     int major = 0, minor = 0;
     bool dry_run = false;
+    bool trace = false;                      // device_engine_trace at init: windows are created traced
     pb2_engine_t* engine = nullptr;
     std::deque<void*> inflight;              // windows launched and not yet retired (oldest first), pb2_runtime.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up

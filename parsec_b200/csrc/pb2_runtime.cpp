@@ -255,6 +255,8 @@ int pb2_init(pb2_context_t** pctx, int nb_cores) {
     ctx->mca["device_engine_gemm_mode"] = 0;
     // 1: windows pop ready tasks by priority (JDF priority expressions, DTD insert priorities), FIFO among equals
     ctx->mca["device_engine_queue_policy"] = 0;
+    // 1: windows record when and on which SM each task ran (pb2_taskpool_device_trace), through the traced kernels
+    ctx->mca["device_engine_trace"] = 0;
     // a batch of at least _min_roots ready GPU tasks is cut into _pipeline windows of whole dependency closures:
     // while one window runs, the host builds the next one and replays the bookkeeping of the previous one
     // tiles a window has to read from pinned host memory: runs of at least this many contiguous bytes (host and
@@ -298,6 +300,7 @@ int pb2_device_cuda_module_init(pb2_context_t* ctx, int cuda_index, int dry_run,
     d->device_index = (uint8_t)ctx->devices.size();
     char nm[64]; snprintf(nm, sizeof nm, "cuda(%d)", cuda_index); d->name = nm;
     d->mem_block_size = (size_t)ctx->mca["device_cuda_memory_block_size"];
+    d->trace = ctx->mca["device_engine_trace"] != 0;
     size_t total = 0, freeb = 0;
     if (!d->dry_run) {
         pb2_engine_params_t p{};
@@ -308,6 +311,7 @@ int pb2_device_cuda_module_init(pb2_context_t* ctx, int cuda_index, int dry_run,
         p.queue_policy = (int32_t)ctx->mca["device_engine_queue_policy"];
         int rc = pb2_engine_create(&d->engine, cuda_index, &p);
         if (rc != PB2_SUCCESS) { delete d; return rc; }                 // no GPU => loud failure, no fallback
+        if (d->trace) pb2_engine_set_window_trace(d->engine, 1);
         pb2_engine_info_t info;
         pb2_engine_info(d->engine, &info);
         d->major = info.cc_major; d->minor = info.cc_minor;
@@ -748,6 +752,18 @@ int pb2_taskpool_completion_trace(pb2_taskpool_t* tp, int32_t* out_task, int32_t
     const int32_t n = (int32_t)tp->trace_task.size();
     for (int32_t i = 0; i < n && i < cap; ++i) { if (out_task) out_task[i] = tp->trace_task[i]; if (out_device) out_device[i] = tp->trace_device[i]; }
     return n;
+}
+
+int pb2_taskpool_device_trace(pb2_taskpool_t* tp, uint64_t* t_start_ns, uint64_t* t_end_ns, int32_t* device, uint32_t* smid) {
+    if (!tp) return PB2_ERR_BAD_PARAM;
+    for (size_t i = 0; i < tp->tasks.size(); ++i) {
+        const pb2_htask_s& t = tp->tasks[i];
+        if (t_start_ns) t_start_ns[i] = t.dev_t_start;
+        if (t_end_ns) t_end_ns[i] = t.dev_t_end;
+        if (device) device[i] = t.ran_on;
+        if (smid) smid[i] = t.dev_smid;
+    }
+    return PB2_SUCCESS;
 }
 
 int pb2_taskpool_task_info(pb2_taskpool_t* tp, int32_t* class_id, int32_t* locals2, uint32_t* seen_version4, uint64_t* result) {
@@ -1315,6 +1331,14 @@ static int retire_one(pb2_device_module_t* dev) {
         pb2_window_stats_t st{};
         int rc = pb2_window_wait(f->win, &st);
         if (rc == PB2_SUCCESS) rc = pb2_window_results(f->win, retire.data(), nullptr, nullptr, seen.data(), result.data(), nullptr, nullptr);
+        if (rc == PB2_SUCCESS && dev->trace) {
+            // window task i is the pool task w.order[i]
+            std::vector<uint64_t> t0((size_t)n), t1((size_t)n);
+            std::vector<uint32_t> sm((size_t)n);
+            rc = pb2_window_trace(f->win, t0.data(), t1.data(), sm.data(), nullptr);
+            if (rc == PB2_SUCCESS)
+                for (int32_t i = 0; i < n; ++i) { pb2_htask_t* t = w.order[(size_t)i]; t->dev_t_start = t0[(size_t)i]; t->dev_t_end = t1[(size_t)i]; t->dev_smid = sm[(size_t)i]; }
+        }
         if (rc != PB2_SUCCESS) ctx->last_error = std::string("window run: ") + pb2_engine_last_error(dev->engine);
         pb2_window_destroy(f->win);
         if (rc != PB2_SUCCESS) { window_release(dev, w); delete f; return rc; }

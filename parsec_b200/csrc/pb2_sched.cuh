@@ -342,12 +342,36 @@ static __device__ __noinline__ void push_written_tiles(const pb2_tile_t* tiles, 
     __syncthreads();
 }
 
-// One thread: append to the retire log; returns true when this was the last task of the window.
-__device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id) {
+// One thread: append to the retire log; returns true when this was the last task of the window.  `when` gets the time
+// stamp stored as the watchdog's progress.
+__device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id, unsigned long long& when) {
     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, 1ull);
     w.retire_log[seq] = id;
-    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+    when = globaltimer_ns();
+    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = when;
     return (int32_t)(seq + 1) == w.ntasks;
+}
+
+// ---------------------------------------------------------------------------------------------
+// device time stamps of a traced window (pb2_engine_set_window_trace)
+// ---------------------------------------------------------------------------------------------
+// Per task of the run: t_start, t_end (%globaltimer, ns) and the SM.  A scheduling entity -- a task alone, a read group,
+// a fused producer with its group, a GEMM unit -- starts at the earliest pop of any of its parts and ends at the time
+// stamp its retiring part stores as the watchdog's progress; every task of the entity gets that interval and the SM of
+// the retiring part.  Only the TRACE instantiations of the window kernels touch these arrays (null in an untraced
+// window); the reset kernel starts t_start at ~0, the identity of the atomicMin of the pops.
+struct TraceDev { unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid; };
+
+// One thread, right after it popped a part of the entity led by task `lead` at time t.
+__device__ __forceinline__ void trace_pop(const TraceDev& tr, int32_t lead, unsigned long long t) { atomicMin(&tr.t_start[lead], t); }
+
+// One thread of the retiring part: task `id` gets its entity's interval [t0, t_end] and the SM sm.
+__device__ __forceinline__ void trace_task(const TraceDev& tr, int32_t id, unsigned long long t0, unsigned long long t_end, uint32_t sm) {
+    tr.t_start[id] = t0; tr.t_end[id] = t_end; tr.smid[id] = sm;
+}
+// The start of the entity led by `lead`: every pop of its parts is ordered before its retirement (parts_left chain).
+__device__ __forceinline__ unsigned long long trace_start_of(const TraceDev& tr, int32_t lead) {
+    return *reinterpret_cast<volatile unsigned long long*>(&tr.t_start[lead]);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -22,6 +22,41 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def chrome_trace(t_start_ns, t_end_ns, smid, class_id=None, locals=None, class_names=None, unit=None, pid=0,
+                 process_name=None):
+    """Per-task device intervals (Window.trace, Context.device_trace) as a Chrome trace: {"traceEvents": [...]}, one
+    complete ("X") event per recorded task on the row of its SM, times in microseconds from the earliest start.
+    A task is named from class_id (through class_names when given) and locals; unit, when given, goes into each event's
+    args.  Tasks with t_end_ns == 0 were not recorded and get no event.  pid: the trace process (one per device: every
+    device has its own clock)."""
+    t0 = np.asarray(t_start_ns, np.uint64)
+    t1 = np.asarray(t_end_ns, np.uint64)
+    sm = np.asarray(smid, np.uint32)
+    rec = np.nonzero(t1 != 0)[0]
+    base = int(t0[rec].min()) if len(rec) else 0
+    events = []
+    if process_name is not None:
+        events.append({"ph": "M", "name": "process_name", "pid": pid, "tid": 0, "args": {"name": process_name}})
+    for s in sorted({int(x) for x in sm[rec]}):
+        events.append({"ph": "M", "name": "thread_name", "pid": pid, "tid": s, "args": {"name": "SM %d" % s}})
+        events.append({"ph": "M", "name": "thread_sort_index", "pid": pid, "tid": s, "args": {"sort_index": s}})
+    for i in rec:
+        i = int(i)
+        if class_id is None:
+            name = "task %d" % i
+        else:
+            c = int(class_id[i])
+            name = class_names.get(c, "class %d" % c) if class_names else "class %d" % c
+        if locals is not None:
+            name += "(%s)" % ", ".join(str(int(v)) for v in np.atleast_1d(locals[i]))
+        args = {"task": i}
+        if unit is not None:
+            args["unit"] = int(unit[i])
+        events.append({"ph": "X", "name": name, "pid": pid, "tid": int(sm[i]),
+                       "ts": (int(t0[i]) - base) / 1000.0, "dur": (int(t1[i]) - int(t0[i])) / 1000.0, "args": args})
+    return {"traceEvents": events, "displayTimeUnit": "ns"}
+
+
 class Engine:
     """One engine per GPU (the reference's parsec_device_cuda_module_t, device_cuda.h:43-48).
 
@@ -31,7 +66,7 @@ class Engine:
 
     def __init__(self, cuda_device=0, workers_per_sm=0, threads=0, max_workers=0, stage_mode=0,
                  queue_policy=0, timeout_ms=0, gemm_mode=0, part_bytes=0, read_groups=0,
-                 fuse_readers=0):
+                 fuse_readers=0, window_trace=False):
         self._lib = L.load()
         self._h = C.c_void_p()
         p = L.EngineParams(workers_per_sm, threads, max_workers, stage_mode, queue_policy, timeout_ms, gemm_mode, part_bytes,
@@ -41,6 +76,8 @@ class Engine:
             self._h = C.c_void_p()
             raise L.Pb2Error(rc, "pb2_engine_create")
         self._allocs = []
+        if window_trace:
+            self.set_window_trace(True)
 
     def info(self):
         i = L.EngineInfo()
@@ -91,6 +128,10 @@ class Engine:
 
     def set_part_bytes(self, part_bytes):
         _check(self._lib.pb2_engine_set_part_bytes(self._h, part_bytes), "set_part_bytes", self)
+
+    def set_window_trace(self, on=True):
+        """Windows created from now on record per-task device time stamps (Window.trace)."""
+        _check(self._lib.pb2_engine_set_window_trace(self._h, 1 if on else 0), "set_window_trace", self)
 
     def ipc_export(self, dev_ptr):
         h = (C.c_ubyte * 64)()
@@ -206,6 +247,16 @@ class Window:
                                             _ptr(out["end_seq"]), _ptr(out["seen_version"]),
                                             _ptr(out["result"]), _ptr(out["worker"]), _ptr(out["tiles"])),
                "pb2_window_results", self.engine)
+        return out
+
+    def trace(self):
+        """Device time stamps of the last launch (a window created with trace on; pb2_window_trace): per task the
+        interval of its scheduling entity in %globaltimer ns, the SM that retired it and the task leading the entity."""
+        n = self.ntasks
+        out = {"t_start_ns": np.empty(n, np.uint64), "t_end_ns": np.empty(n, np.uint64),
+               "smid": np.empty(n, np.uint32), "unit": np.empty(n, np.int32)}
+        _check(self._lib.pb2_window_trace(self._h, _ptr(out["t_start_ns"]), _ptr(out["t_end_ns"]), _ptr(out["smid"]),
+                                          _ptr(out["unit"])), "pb2_window_trace", self.engine)
         return out
 
     def close(self):

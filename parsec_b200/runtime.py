@@ -39,7 +39,7 @@ PARSEC_SYMBOLS = [
     "pb2_dc_data_of", "pb2_dc_data_key", "pb2_dc_position", "pb2_dc_info", "pb2_dc_register_memory",
     "pb2_dc_distribute_on_devices", "pb2_dc_host_write_all", "pb2_context_add_taskpool", "pb2_context_start", "pb2_context_wait",
     "pb2_taskpool_wait", "pb2_taskpool_free", "pb2_taskpool_nb_tasks", "pb2_taskpool_set_device_types",
-    "pb2_taskpool_completion_trace", "pb2_taskpool_task_info", "pb2_taskpool_export_window", "pb2_dtd_taskpool_new",
+    "pb2_taskpool_completion_trace", "pb2_taskpool_device_trace", "pb2_taskpool_task_info", "pb2_taskpool_export_window", "pb2_dtd_taskpool_new",
     "pb2_dtd_tile_of", "pb2_dtd_tile_new", "pb2_dtd_tile_data", "pb2_dtd_create_task_class",
     "pb2_dtd_task_class_add_chore", "pb2_dtd_insert_task_with_task_class", "pb2_dtd_data_flush_all",
     "pb2_dtd_task_class_add_submit", "pb2_gpu_task_flow_ptr", "pb2_gpu_task_flow_bytes", "pb2_gpu_task_iparam",
@@ -89,6 +89,7 @@ def lib():
         "pb2_context_wait": (C.c_int, [vp]), "pb2_taskpool_wait": (C.c_int, [vp]), "pb2_taskpool_free": (C.c_int, [vp]),
         "pb2_taskpool_nb_tasks": (C.c_int, [vp]), "pb2_taskpool_set_device_types": (C.c_int, [vp, C.c_int]),
         "pb2_taskpool_completion_trace": (C.c_int, [vp, vp, vp, i32]),
+        "pb2_taskpool_device_trace": (C.c_int, [vp, vp, vp, vp, vp]),
         "pb2_taskpool_task_info": (C.c_int, [vp, vp, vp, vp, vp]),
         "pb2_taskpool_export_window": (C.c_int, [vp, vp, vp, P(i32), vp, P(i32), vp, P(i32), vp, P(i32), vp]),
         "pb2_dtd_taskpool_new": (vp, [vp]), "pb2_dtd_tile_of": (vp, [vp, vp, C.c_uint64]),
@@ -186,6 +187,15 @@ class Context:
         t, d = np.full(n, -1, np.int32), np.full(n, -1, np.int32)
         k = self.l.pb2_taskpool_completion_trace(tp, _p(t), _p(d), n)
         return t[:k], d[:k]
+
+    def device_trace(self, tp):
+        """Per task id: the device time stamps of its window run (MCA parameter device_engine_trace; 0 for tasks that
+        ran elsewhere), the device index that ran it and the SM.  Each device has its own clock."""
+        n = self.l.pb2_taskpool_nb_tasks(tp)
+        t0, t1 = np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+        dev, sm = np.zeros(n, np.int32), np.zeros(n, np.uint32)
+        _chk(self.l.pb2_taskpool_device_trace(tp, _p(t0), _p(t1), _p(dev), _p(sm)), "device_trace")
+        return dict(t_start_ns=t0, t_end_ns=t1, device=dev, smid=sm)
 
     def task_info(self, tp):
         n = self.l.pb2_taskpool_nb_tasks(tp)
