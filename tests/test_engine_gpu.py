@@ -5,30 +5,9 @@ import pytest
 from parsec_b200 import _lib as L
 from oracle import orc_dags as dags
 from parsec_b200.engine import Engine
+from window_harness import Layout, placed, run_engine
 
 pytestmark = pytest.mark.gpu
-
-
-def make_tiles(engine, dag, host, valid=False):
-    """One HBM slot per tile + the device-visible alias of its host home (memory_register)."""
-    nt, tb = dag.ntiles, dag.tile_bytes
-    slot = (tb + 511) // 512 * 512
-    slab = engine.malloc(max(nt * slot, 16))
-    alias = engine.host_register(host) if host is not None else 0
-    tiles = np.zeros(nt, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + np.arange(nt, dtype=np.uint64) * np.uint64(slot)
-    tiles["src_ptr"] = (alias + np.arange(nt, dtype=np.uint64) * np.uint64(tb)) if host is not None else 0
-    tiles["bytes"] = tb
-    tiles["state"] = L.TILE_VALID if valid else L.TILE_INVALID
-    return tiles, slab, slot
-
-
-def run(engine, dag, tiles):
-    w = engine.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
-    st = w.run()
-    res = w.results()
-    w.close()
-    return st, res
 
 
 @pytest.mark.parametrize("K,NB,tile_bytes", [(8, 6, 4), (64, 14, 256 * 256 * 4), (33, 4, 1000), (1, 0, 16)])
@@ -36,8 +15,8 @@ def test_ex05_broadcast(engine, K, NB, tile_bytes):
     """Ex05_Broadcast.jdf:33-39,53-57: every TaskRecv(k,n) observes k; each tile staged in exactly once."""
     dag = dags.ex05_broadcast(K, NB, tile_bytes)
     host = np.full(K * tile_bytes // 4, -7, np.int32)
-    tiles, slab, slot = make_tiles(engine, dag, host)
-    st, res = run(engine, dag, tiles)
+    layout = Layout.packed(dag, host)
+    st, res, dev, _, _, _ = run_engine(engine, dag, layout)
     assert st["tasks_retired"] == dag.ntasks
     assert st["body_errors"] == 0
     assert st["bytes_h2d"] == K * tile_bytes            # required_in == transferred: zero re-staging
@@ -51,40 +30,30 @@ def test_ex05_broadcast(engine, K, NB, tile_bytes):
     assert np.all(res["seen_version"][:K, 0] == 0)
     assert np.all(res["seen_version"][K:, 0] == 1)
     assert np.all(res["tiles"]["version"] == 1) and np.all(res["tiles"]["state"] == L.TILE_VALID)
-    got = np.empty(tile_bytes // 4, np.int32)
     for k in (0, K - 1):
-        engine.d2h(got, slab + k * slot)
-        assert np.all(got == k)
-    engine.host_unregister(host)
-    engine.free(slab)
+        assert np.all(layout.tile_bytes(dev, k).view(np.int32) == k)
 
 
 @pytest.mark.parametrize("NB", [0, 1, 10, 999])
 def test_ex02_chain(engine, NB):
     """Ex02_Chain.jdf:44-50: task k observes value k; final value NB (BASELINE config 1 known answer)."""
     dag = dags.ex02_chain(NB)
-    tiles, slab, slot = make_tiles(engine, dag, None)
-    st, res = run(engine, dag, tiles)
+    layout = Layout.packed(dag)
+    st, res, dev, _, _, _ = run_engine(engine, dag, layout)
     assert st["tasks_retired"] == NB + 1 and st["bytes_h2d"] == 0
     assert all(v == 0 for v in dags.check_execution(dag, res).values())
     assert np.array_equal(res["retire_order"], np.arange(NB + 1))      # strictly serial chain
     assert np.array_equal(res["seen_version"][:, 0], np.arange(NB + 1))
-    got = np.empty(1, np.int32)
-    engine.d2h(got, slab)
-    assert got[0] == NB
-    engine.free(slab)
+    assert layout.tile_bytes(dev, 0).view(np.int32)[0] == NB
 
 
 def test_single_worker_is_fifo_deterministic():
     """With one worker the ring is a strict FIFO: execution order is exactly breadth-first."""
     with Engine(0, max_workers=1) as e:
         dag = dags.ex05_broadcast(16, 6, 64)
-        host = np.zeros(16 * 16, np.int32)
-        tiles, slab, slot = make_tiles(e, dag, host)
-        st, res = run(e, dag, tiles)
+        res = run_engine(e, dag, Layout.packed(dag, np.zeros(16 * 16, np.int32))).res
         assert np.array_equal(res["retire_order"], np.arange(dag.ntasks))
         assert np.all(res["worker"] == 0)
-        e.host_unregister(host)
 
 
 def test_rtt_chain_pushout(engine):
@@ -93,20 +62,17 @@ def test_rtt_chain_pushout(engine):
     dag = dags.rtt_chain(NT, FRAGS, tb)
     host = np.arange(FRAGS * tb // 4, dtype=np.float32)
     expect = host + NT
-    tiles, slab, slot = make_tiles(engine, dag, host)
-    st, res = run(engine, dag, tiles)
+    st, res, _, got, _, _ = run_engine(engine, dag, Layout.packed(dag, host))
     assert all(v == 0 for v in dags.check_execution(dag, res).values())
     assert st["bytes_h2d"] == FRAGS * tb and st["bytes_d2h"] == FRAGS * tb
-    assert np.array_equal(host, expect)                                   # pushout landed in host memory
+    assert np.array_equal(got.view(np.float32), expect)                   # pushout landed in host memory
     assert np.all(res["tiles"]["version"] == NT)
-    engine.host_unregister(host)
-    engine.free(slab)
 
 
 def test_ep_schedmicro_shape(engine):
     """ep.jdf (schedmicro): NT x DEPTH empty CTL-chained tasks all retire, order respected."""
     dag = dags.ep(512, 8)
-    st, res = run(engine, dag, np.zeros(0, L.TILE_DTYPE))
+    st, res, _, _, _, _ = run_engine(engine, dag, Layout.packed(dag))
     assert st["tasks_retired"] == 1 + 512 * 8
     assert all(v == 0 for v in dags.check_execution(dag, res).values())
 
@@ -116,14 +82,14 @@ def test_malformed_dag_trips_watchdog():
     with Engine(0, timeout_ms=200) as e:
         dag = dags.ex02_chain(4)
         dag.tasks["dep_goal"][2] = 0x3          # waits for a flow bit nobody sets
-        tiles, slab, slot = make_tiles(e, dag, None)
-        w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
-        w.launch()
-        with pytest.raises(L.Pb2Error) as ei:
-            w.wait()
-        assert ei.value.rc == L.PB2_ERR_DEVICE
-        assert w.stats["tasks_retired"] == 2
-        w.close()
+        with placed(e, Layout.packed(dag)) as p:
+            w = e.window(0, dag.tasks, dag.succ, p.tiles, dag.ready)
+            w.launch()
+            with pytest.raises(L.Pb2Error) as ei:
+                w.wait()
+            assert ei.value.rc == L.PB2_ERR_DEVICE
+            assert w.stats["tasks_retired"] == 2
+            w.close()
 
 
 @pytest.mark.parametrize("tile_bytes,part_bytes", [(1 << 20, 64 * 1024), ((1 << 20) + 4, 100 * 1000), (4 << 20, 0), (40, 16)])
@@ -244,15 +210,13 @@ def test_big_tile_chain_uses_the_whole_gpu():
     host = np.zeros(tb // 4, np.float32)
     times = {}
     for pb in (-1, 0):
-        with Engine(0, part_bytes=pb) as e:
-            tiles, slab, slot = make_tiles(e, dag, host)
-            w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
-            w.run(); host[:] = 0
+        with Engine(0, part_bytes=pb) as e, placed(e, Layout.packed(dag, host)) as p:
+            w = e.window(0, dag.tasks, dag.succ, p.tiles, dag.ready)
+            w.run(); p.host[:] = 0
             st = w.run(); res = w.results(); w.close()
             assert all(v == 0 for v in dags.check_execution(dag, res).values())
-            assert np.all(host == NT)
+            assert np.all(p.host.view(np.float32) == NT)
             times[pb] = st["kernel_ms"]
-            e.host_unregister(host)
     assert times[0] < times[-1] / 4, times
 
 

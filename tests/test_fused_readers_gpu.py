@@ -5,114 +5,12 @@ import numpy as np
 import pytest
 
 from parsec_b200 import _lib as L
-from oracle import orc
 from oracle import orc_dags as dags
 from parsec_b200.engine import Engine
+from window_harness import (KS, Layout, assert_like_oracle, assert_same_run, check_pair, engines, fused,  # noqa: F401
+                            not_fused, readers_dag, run_engine, run_oracle)
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def engines():
-    on, off = Engine(0), Engine(0, fuse_readers=-1)
-    yield on, off
-    on.close()
-    off.close()
-
-
-def sizes_of(dag, sizes):
-    return np.full(dag.ntiles, dag.tile_bytes, np.int64) if sizes is None else np.asarray(sizes, np.int64)
-
-
-def run_on(e, dag, host, valid, sizes=None, pushout_home=False):
-    """One run of dag on engine e, tile i of sizes[i] bytes (default dag.tile_bytes) in a fresh slab: resident copies of
-    its bytes in host, or staged in from there.  Returns (stats, results, device bytes, host bytes after the run)."""
-    sz = sizes_of(dag, sizes)
-    offs = np.concatenate([[0], np.cumsum(sz)[:-1]]).astype(np.uint64)
-    slots = (sz + 511) // 512 * 512
-    soffs = np.concatenate([[0], np.cumsum(slots)[:-1]]).astype(np.uint64)
-    host = host.copy()
-    slab = e.malloc(max(int(slots.sum()), 16))
-    alias = e.host_register(host)
-    tiles = np.zeros(dag.ntiles, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + soffs
-    tiles["src_ptr"] = alias + offs
-    tiles["bytes"] = sz
-    tiles["state"] = L.TILE_VALID if valid else L.TILE_INVALID
-    hb = host.view(np.uint8)
-    if valid:
-        for i in range(dag.ntiles):
-            e.h2d(int(tiles["dev_ptr"][i]), hb[int(offs[i]):int(offs[i]) + int(sz[i])])
-    w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
-    st = w.run()
-    res = w.results()
-    w.close()
-    data = np.empty(int(sz.sum()), np.uint8)
-    for i in range(dag.ntiles):
-        e.d2h(data[int(offs[i]):int(offs[i]) + int(sz[i])], int(tiles["dev_ptr"][i]))
-    e.host_unregister(host)
-    e.free(slab)
-    return st, res, data, host
-
-
-def oracle(dag, host, sizes=None):
-    """The sequential oracle's run of dag (FIFO ready order), every tile staged in from host."""
-    sz = sizes_of(dag, sizes)
-    spec = np.zeros(dag.ntiles, orc.TILE_DTYPE)
-    spec["bytes"] = sz
-    spec["src_ptr"] = np.concatenate([[0], np.cumsum(sz)[:-1]]).astype(np.uint64)
-    spec["state"] = orc.TILE_INVALID
-    h = host.copy()
-    ref = orc.run_window(dag.tasks, dag.succ, spec, dag.ready, h)
-    assert ref["rc"] == 0
-    ref["data"] = np.concatenate([ref["device"][i][:int(sz[i])] for i in range(dag.ntiles)]) if dag.ntiles else np.zeros(0, np.uint8)
-    ref["host"] = h
-    return ref
-
-
-def assert_same(a, b):
-    (st_a, res_a, data_a, host_a), (st_b, res_b, data_b, host_b) = a, b
-    assert np.array_equal(res_a["result"], res_b["result"])
-    assert np.array_equal(res_a["seen_version"], res_b["seen_version"])
-    assert np.array_equal(res_a["tiles"]["version"], res_b["tiles"]["version"])
-    assert np.array_equal(res_a["tiles"]["state"], res_b["tiles"]["state"])
-    assert np.array_equal(data_a, data_b)
-    assert np.array_equal(host_a, host_b)
-    for k in ("tasks_retired", "bytes_h2d", "stage_ins", "body_errors"):
-        assert st_a[k] == st_b[k], k
-
-
-def assert_oracle(run, ref, dag):
-    st, res, data, _ = run
-    assert np.array_equal(res["result"], ref["result"])
-    assert np.array_equal(res["seen_version"], ref["seen_version"])
-    assert np.array_equal(data, ref["data"])
-    assert st["body_errors"] == ref["stats"]["body_errors"]
-    assert st["tasks_retired"] == dag.ntasks
-    assert all(v == 0 for v in dags.check_execution(dag, res).values())
-
-
-def fused(res, p, members):
-    """The members ran in p's unit: on p's worker, started right after p ended, in member order."""
-    ss, es = res["start_seq"].astype(np.int64), res["end_seq"].astype(np.int64)
-    return all(res["worker"][m] == res["worker"][p] and ss[m] == es[p] + 1 + i for i, m in enumerate(members))
-
-
-def not_fused(res, p, members):
-    """The group ran as a task of its own.  (A group popped from the ring by p's own worker right after p, with no other
-    event in between, would look fused; with every worker polling the ring that does not happen.)"""
-    return not fused(res, p, members)
-
-
-def check_both(engines, dag, host, valid=False, sizes=None):
-    on, off = engines
-    a = run_on(on, dag, host, valid, sizes)
-    b = run_on(off, dag, host, valid, sizes)
-    assert_same(a, b)
-    ref = oracle(dag, host, sizes)
-    assert_oracle(a, ref, dag)
-    assert_oracle(b, ref, dag)
-    return a[1], b[1]
 
 
 @pytest.mark.parametrize("valid", [False, True], ids=["staged", "resident"])
@@ -120,39 +18,12 @@ def check_both(engines, dag, host, valid=False, sizes=None):
 def test_ex05_fused_on_off_identical(engines, K, NB, tile_bytes, valid):
     dag = dags.ex05_broadcast(K, NB, tile_bytes)
     F = dag.meta["F"]
-    host = np.full(K * tile_bytes // 4, -7, np.int32)
-    on, off = check_both(engines, dag, host, valid)
+    on, off = check_pair(engines, dag, Layout.packed(dag, np.full(K * tile_bytes // 4, -7, np.int32), valid))
     assert np.array_equal(on["result"][K:], np.repeat(np.arange(K, dtype=np.uint64), F))   # 0 mismatches, first element k
     if F >= 2:
         units = [(k, list(range(K + k * F, K + (k + 1) * F))) for k in range(K)]
         assert all(fused(on, k, m) for k, m in units)
         assert not all(fused(off, k, m) for k, m in units)
-
-
-def readers_dag(producer_body, producer_k, reader_ks, tile_bytes, access=L.ACCESS_WRITE):
-    """Task 0 writes tile 0 (FILL k / IOTA), tasks 1.. read it with CHECK constants reader_ks (ints: CHECK_I32, floats:
-    CHECK_F32 with those bits)."""
-    n = 1 + len(reader_ks)
-    t = np.zeros(n, L.TASK_DTYPE)
-    t["tile"][:] = -1
-    t["nb_flows"] = 1
-    t["tile"][:, 0] = 0
-    t["body"][0], t["iparam"][0, 0], t["access"][0, 0] = producer_body, producer_k, access
-    for i, k in enumerate(reader_ks, start=1):
-        t["access"][i, 0] = L.ACCESS_READ
-        t["dep_goal"][i] = 1
-        if isinstance(k, float):
-            t["body"][i], t["fparam"][i] = L.BODY_CHECK_F32, np.float32(k)
-        else:
-            t["body"][i], t["iparam"][i, 0] = L.BODY_CHECK_I32, k
-    t["succ_begin"][0], t["succ_count"][0] = 0, n - 1
-    t["succ_begin"][1:] = n - 1
-    succ = np.arange(1, n, dtype=np.uint32)
-    return dags.Dag(t, succ, np.array([0], np.int32), ntiles=1, tile_bytes=tile_bytes, name="readers")
-
-
-f5 = float(np.array([5], np.int32).view(np.float32)[0])     # a CHECK_F32 constant whose bits are the integer 5
-KS = [5, 5, 6, f5, 0, 7, 1, 5]
 
 
 @pytest.mark.parametrize("producer", ["fill5", "iota"])
@@ -163,9 +34,9 @@ def test_mismatches_inside_a_fused_group(producer, tile_bytes, part_bytes):
     multiple of 16 bytes, not a multiple of the chunk, or split into 16 parts."""
     body, k = (L.BODY_FILL_I32, 5) if producer == "fill5" else (L.BODY_IOTA_I32, 0)
     dag = readers_dag(body, k, KS, tile_bytes)
-    host = np.zeros(tile_bytes // 4, np.int32)
+    layout = Layout.packed(dag, np.zeros(tile_bytes // 4, np.int32))
     with Engine(0, part_bytes=part_bytes) as on, Engine(0, part_bytes=part_bytes, fuse_readers=-1) as off:
-        a, b = check_both((on, off), dag, host)
+        a, b = check_pair((on, off), dag, layout)
     assert a["result"][1:].any() and (a["result"][1:] >> np.uint64(32)).any()
     assert fused(a, 0, list(range(1, 9)))
     assert not_fused(b, 0, list(range(1, 9)))
@@ -178,16 +49,16 @@ def test_chunk_sizes(engines, monkeypatch, chunk):
     with Engine(0) as e:
         for body, k, tb in ((L.BODY_IOTA_I32, 0, 4096 + 12), (L.BODY_FILL_I32, 5, 40000)):
             dag = readers_dag(body, k, KS, tb)
-            host = np.zeros(tb // 4, np.int32)
-            a = run_on(e, dag, host, False)
-            assert_same(a, run_on(engines[1], dag, host, False))
-            assert_oracle(a, oracle(dag, host), dag)
-            assert fused(a[1], 0, list(range(1, 9)))
+            layout = Layout.packed(dag, np.zeros(tb // 4, np.int32))
+            a = run_engine(e, dag, layout)
+            assert_same_run(a, run_engine(engines[1], dag, layout))
+            assert_like_oracle(a, run_oracle(dag, layout), dag)
+            assert fused(a.res, 0, list(range(1, 9)))
         dag = dags.ex05_broadcast(16, 14, 4096 + 16)
-        host = np.full(16 * (4096 + 16) // 4, -7, np.int32)
-        a = run_on(e, dag, host, True)
-        assert_same(a, run_on(engines[1], dag, host, True))
-        assert_oracle(a, oracle(dag, host), dag)
+        layout = Layout.packed(dag, np.full(16 * (4096 + 16) // 4, -7, np.int32), True)
+        a = run_engine(e, dag, layout)
+        assert_same_run(a, run_engine(engines[1], dag, layout))
+        assert_like_oracle(a, run_oracle(dag, layout), dag)
 
 
 def around_dag(mask):
@@ -222,8 +93,7 @@ def around_dag(mask):
 @pytest.mark.parametrize("mask", [False, True], ids=["counter", "mask"])
 def test_other_successors_and_a_second_group(engines, mask):
     dag = around_dag(mask)
-    host = np.arange(3 * 256, dtype=np.int32)
-    on, off = check_both(engines, dag, host)
+    on, off = check_pair(engines, dag, Layout.packed(dag, np.arange(3 * 256, dtype=np.int32)))
     assert fused(on, 0, [2, 3])
     assert not_fused(on, 0, [5, 6]) and on["worker"][5] == on["worker"][6]
     assert not_fused(off, 0, [2, 3])
@@ -245,7 +115,7 @@ def test_two_flow_producer(engines):
     dag = copy_dag(tb)
     host = np.concatenate([np.full(tb // 4, 5, np.int32), np.zeros(tb // 4, np.int32)])
     host[17] = 6
-    on, off = check_both(engines, dag, host)
+    on, off = check_pair(engines, dag, Layout.packed(dag, host))
     assert fused(on, 0, list(range(1, 9)))
 
 
@@ -256,34 +126,31 @@ def test_not_fused_when_the_read_tile_is_not_the_widest(engines):
     t["body"][0], t["iparam"][0, 0] = L.BODY_FILL_I32, 5
     t["tile"][0, 0], t["tile"][0, 1] = 1, 0
     t["access"][0, 0], t["access"][0, 1] = L.ACCESS_WRITE, L.ACCESS_READ
-    sizes = [8192, 4096]
-    host = np.zeros((8192 + 4096) // 4, np.int32)
-    on, _ = check_both(engines, dag, host, sizes=sizes)
+    on, _ = check_pair(engines, dag, Layout.packed(dag, np.zeros((8192 + 4096) // 4, np.int32), sizes=[8192, 4096]))
     assert not_fused(on, 0, list(range(1, 9)))
 
 
 def test_not_fused_with_pushout(engines):
     dag = readers_dag(L.BODY_FILL_I32, 5, KS, 4096, access=L.ACCESS_WRITE | L.FLOW_PUSHOUT)
-    host = np.zeros(1024, np.int32)
-    on, _ = check_both(engines, dag, host)
+    on, _ = check_pair(engines, dag, Layout.packed(dag, np.zeros(1024, np.int32)))
     assert not_fused(on, 0, list(range(1, 9)))
 
 
 def test_not_fused_without_read_groups():
     dag = readers_dag(L.BODY_FILL_I32, 5, KS, 4096)
-    host = np.zeros(1024, np.int32)
+    layout = Layout.packed(dag, np.zeros(1024, np.int32))
     with Engine(0, read_groups=-1) as e:
-        st, res, data, _ = run_on(e, dag, host, False)
-    assert_oracle((st, res, data, None), oracle(dag, host), dag)
-    assert not_fused(res, 0, list(range(1, 9)))
+        run = run_engine(e, dag, layout)
+    assert_like_oracle(run, run_oracle(dag, layout), dag)
+    assert not_fused(run.res, 0, list(range(1, 9)))
 
 
 def test_single_worker_keeps_fifo_order():
     """With one worker nothing is fused: two producers retire before their readers, as the oracle's FIFO has it."""
     dag = dags.ex05_broadcast(8, 6, 4096)
-    host = np.full(8 * 1024, -7, np.int32)
-    ref = oracle(dag, host)
+    layout = Layout.packed(dag, np.full(8 * 1024, -7, np.int32))
+    ref = run_oracle(dag, layout)
     with Engine(0, max_workers=1) as e:
-        run = run_on(e, dag, host, False)
-    assert_oracle(run, ref, dag)
-    assert np.array_equal(run[1]["retire_order"], ref["retire_order"])
+        run = run_engine(e, dag, layout)
+    assert_like_oracle(run, ref, dag)
+    assert np.array_equal(run.res["retire_order"], ref.res["retire_order"])

@@ -11,7 +11,7 @@ import pytest
 from parsec_b200 import _lib as L
 from oracle import orc_dags as dags
 from parsec_b200.engine import Engine
-from test_fused_readers_gpu import check_both, fused, not_fused, readers_dag
+from window_harness import Layout, check_pair, fused, not_fused, readers_dag
 
 pytestmark = pytest.mark.gpu
 
@@ -21,10 +21,8 @@ MEMBERS = list(range(1, 9))
 
 @pytest.fixture(scope="module")
 def engines():
-    on, off = Engine(0, part_bytes=PART), Engine(0, part_bytes=PART, fuse_readers=-1)
-    yield on, off
-    on.close()
-    off.close()
+    with Engine(0, part_bytes=PART) as on, Engine(0, part_bytes=PART, fuse_readers=-1) as off:
+        yield on, off
 
 
 def u32(x):
@@ -119,7 +117,7 @@ def unit_dag(body, tb, case):
 @pytest.mark.parametrize("body,case", CASES, ids=["%s-%s" % c for c in CASES])
 def test_checked_bodies(engines, body, case, tile_bytes, valid):
     dag, host = unit_dag(body, tile_bytes, case)
-    on, off = check_both(engines, dag, host, valid)
+    on, off = check_pair(engines, dag, Layout.packed(dag, host, valid))
     assert fused(on, 0, MEMBERS)
     assert not_fused(off, 0, MEMBERS)
     mism = on["result"][1:] >> np.uint64(32)

@@ -8,7 +8,7 @@ import pytest
 
 from parsec_b200 import _lib as L
 from oracle import orc_dags as dags
-from test_fused_readers_gpu import KS, check_both, engines, fused, not_fused, readers_dag  # noqa: F401
+from window_harness import KS, Layout, check_pair, engines, fused, not_fused, readers_dag  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -31,7 +31,7 @@ def test_read_modify_write_producer(engines, producer, tile_bytes, valid):
         dag = readers_dag(L.BODY_ADD_IOTA_I32, 0, KS, tile_bytes, access=L.ACCESS_RW)
         host[:] = 5 - np.arange(tile_bytes // 4, dtype=np.int32)     # element i becomes 5, the members' constant
         host[1000] = 0
-    on, off = check_both(engines, dag, host, valid)
+    on, off = check_pair(engines, dag, Layout.packed(dag, host, valid))
     assert (on["result"][1:] >> np.uint64(32)).all()                 # every member counts a mismatch
     assert fused(on, 0, list(range(1, 9)))
     assert not_fused(off, 0, list(range(1, 9)))
@@ -54,7 +54,7 @@ def test_axpy_producer_writes_flow_1(engines):
     y = np.full(tb // 4, 2.0, np.float32)
     y[4099] = 3.0
     host = np.concatenate([x, y]).view(np.int32)
-    on, _ = check_both(engines, dag, host)
+    on, _ = check_pair(engines, dag, Layout.packed(dag, host))
     assert (on["result"][1:] >> np.uint64(32)).all()
     assert fused(on, 0, list(range(1, 9)))
 
@@ -66,7 +66,7 @@ def test_memset_producer_ragged_tail(engines, tile_bytes):
     k = 0x05050505
     dag = readers_dag(L.BODY_MEMSET_U8, 5, [k, k, 5, 0, k, 7, 1, k], tile_bytes)
     host = np.full((tile_bytes + 3) // 4, -1, np.int32)
-    on, _ = check_both(engines, dag, host)
+    on, _ = check_pair(engines, dag, Layout.packed(dag, host))
     assert fused(on, 0, list(range(1, 9)))
 
 
@@ -76,7 +76,7 @@ def test_add_at_producer_is_not_fused(engines):
     dag = readers_dag(L.BODY_ADD_AT_I32, 123, KS, tb, access=L.ACCESS_RW)
     dag.tasks["iparam"][0, 1] = 4
     host = np.full(tb // 4, 1, np.int32)
-    on, off = check_both(engines, dag, host)
+    on, off = check_pair(engines, dag, Layout.packed(dag, host))
     members = list(range(1, 9))
     assert not_fused(on, 0, members)
     assert all(on["worker"][m] == on["worker"][1] for m in members)

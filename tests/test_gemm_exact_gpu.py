@@ -12,6 +12,7 @@ gaps between slots hold bf16 NaN, so a read past an operand shows up in C; C pad
 of another payload that must come back unchanged.  Besides the values, every run must match the oracle's bookkeeping:
 dependency order, seen versions, tile versions, retired tasks, bytes moved, and the host image after pushout byte for
 byte, padding included."""
+import dataclasses
 import functools
 
 import numpy as np
@@ -23,6 +24,7 @@ from parsec_b200 import _lib as L
 from parsec_b200.bf16 import bf16_bits_to_f32, f32_to_bf16_bits, round_to_bf16
 from parsec_b200.engine import Engine
 from parsec_b200.multigpu import cholesky_global
+from window_harness import Layout, assert_like_oracle, placed, run_engine, run_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -140,57 +142,11 @@ class Case:
             self.host[ho + n:ho + int(self.bytes[i])] = fill_u8(x["host_fill"], x["pad"])
             self.gap[o:o + int(self.bytes[i])] = False
         self.dag = dags.Dag(self.tasks, self.succ, self.ready, ntiles=nt, tile_bytes=0, kind=1)
-
-    def tile_array(self, dev_base, host_base):
-        t = np.zeros(len(self.bytes), L.TILE_DTYPE)
-        t["dev_ptr"] = np.uint64(dev_base) + self.doff.astype(np.uint64)
-        t["src_ptr"] = np.uint64(host_base) + self.hoff.astype(np.uint64)
-        t["bytes"] = self.bytes
-        t["state"] = np.where(self.valid, L.TILE_VALID, L.TILE_INVALID)
-        return t
+        self.layout = Layout(self.doff, self.hoff, self.bytes, self.valid, self.dev, self.host)
 
     def c_values(self, image, tile, M, N, host=False):
         o = int((self.hoff if host else self.doff)[tile])
         return bf16_bits_to_f32(image[o:o + M * N * 2].view(np.uint16)).reshape(M, N).astype(np.float64)
-
-
-def run_gpu(engine, case, launches=1, slab=None):
-    """Runs the window `launches` times on engine (in `slab` if given, else in a fresh one).  Returns one
-    (stats, results, slab image, host image) per launch."""
-    own = slab is None
-    if own:
-        slab = engine.malloc(len(case.dev))
-    engine.h2d(slab, case.dev)
-    host = case.host.copy()
-    alias = engine.host_register(host)
-    out = []
-    w = engine.window(1, case.tasks, case.succ, case.tile_array(slab, alias), case.ready)
-    try:
-        for _ in range(launches):
-            st = w.run()
-            res = w.results()
-            dev = np.empty_like(case.dev)
-            engine.d2h(dev, slab)
-            engine.synchronize()
-            out.append((st, res, dev, host.copy()))
-    finally:
-        w.close()
-        engine.host_unregister(host)
-        if own:
-            engine.free(slab)
-    return out
-
-
-def run_oracle(case, launches=1):
-    """The sequential oracle on copies of the images (its "device" is the slab image): one output per launch."""
-    dev, host = case.dev.copy(), case.host.copy()
-    tiles = case.tile_array(dev.ctypes.data, host.ctypes.data)
-    out = []
-    for _ in range(launches):
-        r = orc.run_window_raw(case.tasks, case.succ, tiles, case.ready)
-        assert r["rc"] == 0
-        out.append((r, dev.copy(), host.copy()))
-    return out
 
 
 def topo_order(case):
@@ -268,37 +224,20 @@ def evaluate(case, launches=1, limit=EXACT_MAX):
     return dev, host, result, nonzero / max(total, 1)
 
 
-def check_exact(case, ref_orc, ref_f64, min_nonzero):
-    """The data really is in the exact regime: the oracle equals the float64 evaluation, and enough GEMM products
-    are nonzero for the comparison to mean something."""
-    r, odev, ohost = ref_orc[-1]
+def check_exact(case, ref, ref_f64, min_nonzero):
+    """The data really is in the exact regime: the oracle's run `ref` equals the float64 evaluation, and enough GEMM
+    products are nonzero for the comparison to mean something."""
     fdev, fhost, fres, share = ref_f64
     assert share >= min_nonzero, f"only {share:.2f} of the GEMM products are nonzero"
-    assert np.array_equal(odev, fdev), "oracle differs from the float64 evaluation on the device image"
-    assert np.array_equal(ohost, fhost), "oracle differs from the float64 evaluation on the host image"
-    assert np.array_equal(r["result"], fres)
+    assert np.array_equal(ref.dev, fdev), "oracle differs from the float64 evaluation on the device image"
+    assert np.array_equal(ref.host, fhost), "oracle differs from the float64 evaluation on the host image"
+    assert np.array_equal(ref.res["result"], fres)
 
 
 def assert_matches(case, got, want):
-    """One GPU launch against the oracle's: bookkeeping, then the slab (gaps, padding and values) and the host image."""
-    st, res, dev, host = got
-    r, odev, ohost = want
-    assert all(v == 0 for v in dags.check_execution(case.dag, res).values()), dags.check_execution(case.dag, res)
-    assert np.array_equal(res["seen_version"], r["seen_version"])
-    assert np.array_equal(res["tiles"]["version"], r["tiles"]["version"])
-    assert np.array_equal(res["result"], r["result"])
-    for k in ("tasks_retired", "bytes_h2d", "bytes_d2h", "body_errors"):
-        assert st[k] == r["stats"][k], (k, st[k], r["stats"][k])
-    assert np.array_equal(dev[case.gap], case.dev[case.gap]), "a byte between slots changed on the device"
-    bad = np.nonzero(dev != odev)[0]
-    assert not len(bad), f"{len(bad)} slab bytes differ from the oracle, first at {bad[0]} (tile {tile_at(case, bad[0])})"
-    bad = np.nonzero(host != ohost)[0]
-    assert not len(bad), f"{len(bad)} host bytes differ from the oracle, first at {bad[0]}"
-
-
-def tile_at(case, byte):
-    i = int(np.searchsorted(case.doff, byte, side="right")) - 1
-    return (i, int(byte - case.doff[i]), int(case.bytes[i])) if i >= 0 else None
+    """One GPU run against the oracle's, and no byte between slots touched on the device."""
+    assert np.array_equal(got.dev[case.gap], case.dev[case.gap]), "a byte between slots changed on the device"
+    assert_like_oracle(got, want, case.dag)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -351,7 +290,7 @@ def sweep_exact(M, N, K):
 @functools.lru_cache(maxsize=None)
 def sweep_refs(M, N, K):
     case = sweep_exact(M, N, K)
-    return case, run_oracle(case), evaluate(case)
+    return case, run_oracle(case.dag, case.layout), evaluate(case)
 
 
 @pytest.mark.parametrize("mode", [0, 2, 1])
@@ -359,8 +298,7 @@ def sweep_refs(M, N, K):
 def test_shape_sweep_exact(engines, M, N, K, mode):
     case, ref_orc, ref_f64 = sweep_refs(M, N, K)
     check_exact(case, ref_orc, ref_f64, 0.3)
-    (got,) = run_gpu(engines(mode), case)
-    assert_matches(case, got, ref_orc[0])
+    assert_matches(case, run_engine(engines(mode), case.dag, case.layout), ref_orc)
 
 
 def bf16_ulp(x):
@@ -375,8 +313,7 @@ def test_shape_sweep_realistic(engines, M, N, K, mode):
     value per rounding (the chains round once in mode 0 and once per member in mode 2), plus L*K * 2^-22 * sum|a b| for
     the fp32 accumulation of the L*K products, in whatever order the tensor core adds them."""
     case = sweep_case(M, N, K, 3 * M + 5 * N + K, realistic_data)
-    (got,) = run_gpu(engines(mode), case)
-    st, res, dev, host = got
+    st, res, dev, host, _, _ = run_engine(engines(mode), case.dag, case.layout)
     assert all(v == 0 for v in dags.check_execution(case.dag, res).values())
     # the three C tiles: tasks 0, 1..3, 4..6
     for members, pushout in (([0], True), ([1, 2, 3], True), ([4, 5, 6], False)):
@@ -413,7 +350,7 @@ def rounding_case(M, N, K, seed):
 @functools.lru_cache(maxsize=None)
 def rounding_refs(M, N, K):
     case = rounding_case(M, N, K, M + N + K)
-    return case, run_oracle(case), evaluate(case, limit=2 ** 24 - 1)
+    return case, run_oracle(case.dag, case.layout), evaluate(case, limit=2 ** 24 - 1)
 
 
 @pytest.mark.parametrize("mode", [0, 2])
@@ -425,8 +362,7 @@ def test_rounding_of_exact_sums(engines, M, N, K, mode):
     check_exact(case, ref_orc, ref_f64, 0.5)
     c = [case.c_values(ref_f64[0], int(case.tasks["tile"][t, 2]), M, N) for t in range(2)]
     assert np.mean(np.abs(np.concatenate([x.ravel() for x in c])) > 256) > 0.5
-    (got,) = run_gpu(engines(mode), case)
-    assert_matches(case, got, ref_orc[0])
+    assert_matches(case, run_engine(engines(mode), case.dag, case.layout), ref_orc)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -464,16 +400,16 @@ def readback_case(copies=256, seed=5):
 @functools.lru_cache(maxsize=None)
 def readback_refs():
     case = readback_case()
-    return case, run_oracle(case), evaluate(case)
+    return case, run_oracle(case.dag, case.layout), evaluate(case)
 
 
 @pytest.mark.parametrize("mode", [0, 2])
 def test_readback_mixed_window(engines, mode):
     case, ref_orc, ref_f64 = readback_refs()
     check_exact(case, ref_orc, ref_f64, 0.3)
-    (got,) = run_gpu(engines(mode), case)
-    assert_matches(case, got, ref_orc[0])
-    res = got[1]
+    got = run_engine(engines(mode), case.dag, case.layout)
+    assert_matches(case, got, ref_orc)
+    res = got.res
     # a GEMM output or a COPY / FILL result read back as an operand by a task on another worker (another SM)
     # (the operand flows of a GEMM only read, so every edge into them comes from the tile's last writer)
     src, dst, flow = case.dag.edges()
@@ -502,7 +438,7 @@ def cholesky_case(NT, nb, seed):
 @functools.lru_cache(maxsize=None)
 def cholesky_refs(NT, nb):
     case = cholesky_case(NT, nb, 100 * NT + nb)
-    return case, run_oracle(case), evaluate(case)
+    return case, run_oracle(case.dag, case.layout), evaluate(case)
 
 
 @pytest.mark.parametrize("mode", [0, 2])
@@ -510,8 +446,7 @@ def cholesky_refs(NT, nb):
 def test_cholesky_exact(engines, NT, nb, mode):
     case, ref_orc, ref_f64 = cholesky_refs(NT, nb)
     check_exact(case, ref_orc, ref_f64, 0.02)
-    (got,) = run_gpu(engines(mode), case)
-    assert_matches(case, got, ref_orc[0])
+    assert_matches(case, run_engine(engines(mode), case.dag, case.layout), ref_orc)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -521,19 +456,30 @@ def test_relaunch_then_second_window(engines):
     engine = engines(0)
     first = sweep_exact(200, 520, 56)
     second = sweep_exact(7, 264, 72)
-    ref1 = run_oracle(first, 2)
-    ref2 = run_oracle(second, 1)
-    check_exact(first, ref1, evaluate(first, 2), 0.3)
+    ref1 = [run_oracle(first.dag, first.layout)]
+    ref1.append(run_oracle(first.dag, dataclasses.replace(first.layout, dev=ref1[0].dev, host=ref1[0].host)))
+    ref2 = run_oracle(second.dag, second.layout)
+    check_exact(first, ref1[-1], evaluate(first, 2), 0.3)
     check_exact(second, ref2, evaluate(second, 1), 0.3)
     slab = engine.malloc(max(len(first.dev), len(second.dev)))
     try:
-        runs = run_gpu(engine, first, launches=2, slab=slab)
+        with placed(engine, first.layout, slab=slab) as p:
+            w = engine.window(1, first.tasks, first.succ, p.tiles, first.ready)
+            try:
+                runs = [p.run(w.run(), w.results()) for _ in range(2)]
+            finally:
+                w.close()
         # the second launch stages C in again from the pushed-out host copy: the oracle run twice
-        assert not np.array_equal(runs[0][3], runs[1][3])
+        assert not np.array_equal(runs[0].host, runs[1].host)
         for got, want in zip(runs, ref1):
             assert_matches(first, got, want)
-        (got,) = run_gpu(engine, second, slab=slab)
-        assert_matches(second, got, ref2[0])
+        with placed(engine, second.layout, slab=slab) as p:
+            w = engine.window(1, second.tasks, second.succ, p.tiles, second.ready)
+            try:
+                got = p.run(w.run(), w.results())
+            finally:
+                w.close()
+        assert_matches(second, got, ref2)
     finally:
         engine.free(slab)
 
@@ -597,7 +543,7 @@ def test_window_refusals(engines, kind):
     try:
         engine.h2d(slab, case.dev)
         host = case.host.copy()
-        tiles = case.tile_array(slab, host.ctypes.data)
+        tiles = case.layout.table(slab, host.ctypes.data)
         if hook:
             hook(tiles)
         with pytest.raises(L.Pb2Error) as err:
@@ -611,5 +557,4 @@ def test_window_refusals(engines, kind):
     finally:
         engine.free(slab)
     good = refusal_base().finish()
-    (got,) = run_gpu(engine, good)
-    assert_matches(good, got, run_oracle(good)[0])
+    assert_matches(good, run_engine(engine, good.dag, good.layout), run_oracle(good.dag, good.layout))

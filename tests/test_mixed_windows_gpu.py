@@ -1,6 +1,8 @@
 """Windows that mix tile GEMMs with HBM bodies on the H100: the stand-alone runtime runs the mixed DTD pool in one
 launch, the GEMM kernel runs random mixed DAGs exactly as the sequential oracle does (DESIGN §6), and wide HBM bodies
 of a GEMM window are cut into byte-slice parts whose CHECK results add up exactly."""
+import dataclasses
+
 import numpy as np
 import pytest
 
@@ -12,6 +14,7 @@ from parsec_b200.bf16 import bf16_bits_to_f32, f32_to_bf16_bits
 from parsec_b200.engine import Engine
 from priority_order import LANES, priority_order, replay
 import mixed_pool as P
+from window_harness import Layout, assert_like_oracle, placed, run_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -195,20 +198,13 @@ class MixedDag:
             self.doff[i], self.hoff[i] = d, h
             d += (nb + 64 + 127) // 128 * 128
             h += nb
-        self.dev = np.full(d, 0xAB, np.uint8)
-        self.host = np.zeros(h, np.uint8)
+        dev = np.full(d, 0xAB, np.uint8)
+        host = np.zeros(h, np.uint8)
         for i, x in enumerate(self.init):
-            self.host[self.hoff[i]:self.hoff[i] + len(x)] = x
+            host[self.hoff[i]:self.hoff[i] + len(x)] = x
             if self.valid[i]:
-                self.dev[self.doff[i]:self.doff[i] + len(x)] = x
-
-    def tiles(self, dev_base, host_base, all_invalid=False):
-        t = np.zeros(len(self.kinds), L.TILE_DTYPE)
-        t["dev_ptr"] = np.uint64(dev_base) + self.doff.astype(np.uint64)
-        t["src_ptr"] = np.uint64(host_base) + self.hoff.astype(np.uint64)
-        t["bytes"] = self.bytes
-        t["state"] = L.TILE_INVALID if all_invalid else np.where(self.valid, L.TILE_VALID, L.TILE_INVALID)
-        return t
+                dev[self.doff[i]:self.doff[i] + len(x)] = x
+        self.layout = Layout(self.doff, self.hoff, self.bytes, self.valid, dev, host)
 
     def nparts(self, part_bytes):
         """Ring entries per task as build_gemm2_units cuts a GEMM window's HBM units (GEMM tasks: 0, not checked)."""
@@ -221,36 +217,18 @@ class MixedDag:
             out[i] = min(-(-widest // pb), 32) if pb > 0 and t["body"][i] != L.BODY_NOP else 1
         return out
 
-    def tile_bytes_of(self, image, offsets):
-        return [image[int(o):int(o) + int(b)] for o, b in zip(offsets, self.bytes)]
 
 
-def run_engine(eng, md, all_invalid=False):
-    slab = eng.malloc(len(md.dev))
-    eng.h2d(slab, md.dev)
-    host = md.host.copy()
-    alias = eng.host_register(host)
-    w = None
-    try:
-        w = eng.window(1, md.dag.tasks, md.dag.succ, md.tiles(slab, alias, all_invalid), md.dag.ready)
-        st = w.run()
-        res = w.results()
-        res["parts"] = (w.task_entries().view(np.uint32) >> np.uint32(27)).astype(np.int64) + 1
-        dev = eng.d2h(np.empty_like(md.dev), slab)
-        eng.synchronize()
-    finally:
-        if w is not None:
+def run_with_parts(eng, md, layout):
+    """A run of md's window over layout, with res["parts"]: the ring entries of every task."""
+    with placed(eng, layout) as p:
+        w = eng.window(1, md.dag.tasks, md.dag.succ, p.tiles, md.dag.ready)
+        try:
+            st, res = w.run(), w.results()
+            res["parts"] = (w.task_entries().view(np.uint32) >> np.uint32(27)).astype(np.int64) + 1
+        finally:
             w.close()
-        eng.host_unregister(host)
-        eng.free(slab)
-    return st, res, dev, host
-
-
-def run_oracle(md):
-    dev, host = md.dev.copy(), md.host.copy()
-    r = orc.run_window_raw(md.dag.tasks, md.dag.succ, md.tiles(dev.ctypes.data, host.ctypes.data), md.dag.ready)
-    assert r["rc"] == 0
-    return r, dev, host
+    return p.run(st, res, images=(p.dev, p.host))
 
 
 def assert_cut_into_parts(md, res, part_bytes):
@@ -262,29 +240,15 @@ def assert_cut_into_parts(md, res, part_bytes):
     assert np.count_nonzero(want > 1) > 10
 
 
-def assert_like_oracle(md, got, want):
-    st, res, dev, host = got
-    r, odev, ohost = want
-    assert all(v == 0 for v in dags.check_execution(md.dag, res).values()), dags.check_execution(md.dag, res)   # (1)-(3)
-    assert np.array_equal(res["seen_version"], r["seen_version"])                                                # (4)
-    assert np.array_equal(res["result"], r["result"])                                                            # (6)
-    assert np.array_equal(res["tiles"]["version"], r["tiles"]["version"])
-    for k in ("tasks_retired", "bytes_h2d", "bytes_d2h", "body_errors"):
-        assert st[k] == r["stats"][k], (k, st[k], r["stats"][k])
-    for i, (a, b) in enumerate(zip(md.tile_bytes_of(dev, md.doff), md.tile_bytes_of(odev, md.doff))):
-        assert np.array_equal(a, b), f"tile {i} ({md.kinds[i]}, {md.bytes[i]} bytes) differs from the oracle's"
-    assert np.array_equal(host, ohost), "host image differs from the oracle's"
-
-
 @pytest.mark.parametrize("seed", [21, 22, 23])
 @pytest.mark.parametrize("engine_kw", [dict(), dict(part_bytes=65536), dict(gemm_mode=2, part_bytes=16384)],
                          ids=["default", "parts64k", "per_task_units_parts16k"])
 def test_random_mixed_dag_all_workers(seed, engine_kw):
     md = MixedDag(seed)
     with Engine(0, timeout_ms=8000, **engine_kw) as e:
-        got = run_engine(e, md)
-    assert_like_oracle(md, got, run_oracle(md))
-    assert_cut_into_parts(md, got[1], engine_kw.get("part_bytes", 0))
+        got = run_with_parts(e, md, md.layout)
+    assert_like_oracle(got, run_oracle(md.dag, md.layout), md.dag)
+    assert_cut_into_parts(md, got.res, engine_kw.get("part_bytes", 0))
 
 
 @pytest.mark.parametrize("seed", [31, 32])
@@ -292,12 +256,12 @@ def test_random_mixed_dag_one_worker_retires_in_fifo_order(seed):
     """(5): with one worker and every task its own unit, the retire order is the oracle's FIFO order; the wide HBM
     bodies run as parts (a unit's parts are consecutive ring entries)."""
     md = MixedDag(seed, ntasks=120)
-    want = run_oracle(md)
+    want = run_oracle(md.dag, md.layout)
     with Engine(0, max_workers=1, gemm_mode=2, timeout_ms=8000) as e:
-        got = run_engine(e, md)
-    assert_like_oracle(md, got, want)
-    assert np.array_equal(got[1]["retire_order"], want[0]["retire_order"])
-    assert_cut_into_parts(md, got[1], 0)
+        got = run_with_parts(e, md, md.layout)
+    assert_like_oracle(got, want, md.dag)
+    assert np.array_equal(got.res["retire_order"], want.res["retire_order"])
+    assert_cut_into_parts(md, got.res, 0)
 
 
 def test_random_mixed_dag_one_worker_priority_lanes():
@@ -306,12 +270,11 @@ def test_random_mixed_dag_one_worker_priority_lanes():
     md = MixedDag(41, ntasks=120, nprio=40)
     assert len(np.unique(md.dag.tasks["priority"])) > LANES
     order = priority_order(md.dag, LANES)
-    spec = md.tiles(0, 0, all_invalid=True)
-    spec["src_ptr"] = md.hoff.astype(np.uint64)
-    ohost = md.host.copy()
-    ref = replay(md.dag, order, spec, ohost)
+    staged = dataclasses.replace(md.layout, valid=np.zeros(md.dag.ntiles, bool))
+    ohost = staged.host.copy()
+    ref = replay(md.dag, order, staged.offsets(), ohost)
     with Engine(0, max_workers=1, gemm_mode=2, queue_policy=1, part_bytes=65536, timeout_ms=8000) as e:
-        st, res, dev, host = run_engine(e, md, all_invalid=True)
+        st, res, dev, host, _, _ = run_with_parts(e, md, staged)
     assert st["tasks_retired"] == md.dag.ntasks
     assert_cut_into_parts(md, res, 65536)
     assert np.array_equal(res["retire_order"], order)
@@ -319,7 +282,8 @@ def test_random_mixed_dag_one_worker_priority_lanes():
     assert np.array_equal(res["seen_version"], ref["seen_version"])
     assert np.array_equal(res["result"], ref["result"])
     assert np.array_equal(res["tiles"]["version"], ref["tiles"]["version"])
-    for i, a in enumerate(md.tile_bytes_of(dev, md.doff)):
+    for i in range(md.dag.ntiles):
+        a = staged.tile_bytes(dev, i)
         assert np.array_equal(a, ref["device"][i][:len(a)]), i
     assert np.array_equal(host, ohost)
 

@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import orc, orc_dags as dags
+from oracle import orc_dags as dags
 from parsec_b200 import _lib as L
 from parsec_b200 import multigpu as M
 from parsec_b200 import runtime as R
@@ -13,6 +13,7 @@ from parsec_b200.bf16 import bf16_bits_to_f32, f32_to_bf16_bits
 from parsec_b200.engine import Engine
 from priority_order import LANES, priority_order, replay
 from test_priority import random_dag
+from window_harness import Layout, run_engine, run_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -25,47 +26,10 @@ def morton(x, y):
     return r
 
 
-def oracle_run(dag, host=None, lanes=LANES, state=L.TILE_INVALID):
-    """The oracle's execution of `dag`: in the priority order with `lanes` lanes (priority_order.py), or in its own FIFO
-    order with lanes=None."""
-    spec = np.zeros(dag.ntiles, orc.TILE_DTYPE)
-    spec["bytes"] = dag.tile_bytes
-    spec["src_ptr"] = np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-    spec["state"] = state
-    if host is None:
-        host = np.zeros(max(dag.ntiles * dag.tile_bytes, 1), np.uint8)
-    if lanes is None:
-        out = orc.run_window(dag.tasks, dag.succ, spec, dag.ready, host)
-    else:
-        out = replay(dag, priority_order(dag, lanes), spec, host)
-    assert out["rc"] == 0
-    return out
-
-
 def resident(dag):
     """The DAG with its tiles kept in HBM: no flow is pushed out to a home copy."""
     dag.tasks["access"] &= ~np.uint8(L.FLOW_PUSHOUT)
     return dag
-
-
-def run_resident(eng, dag, init):
-    """Run `dag` (no pushout flows) with its tiles in HBM, holding `init` (bytes, tile after tile); returns (stats,
-    results, final tile bytes)."""
-    tb, nt = dag.tile_bytes, dag.ntiles
-    assert not np.any(dag.tasks["access"] & L.FLOW_PUSHOUT)
-    slab = eng.malloc(nt * tb)
-    eng.h2d(slab, init)
-    tiles = np.zeros(nt, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + np.arange(nt, dtype=np.uint64) * np.uint64(tb)
-    tiles["bytes"] = tb
-    tiles["state"] = L.TILE_VALID
-    w = eng.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
-    st = w.run()
-    res = w.results()
-    w.close()
-    out = eng.d2h(np.empty(nt * tb, np.uint8), slab)
-    eng.free(slab)
-    return st, res, out
 
 
 def no_violations(dag, res):
@@ -78,18 +42,10 @@ def test_hbm_one_worker_retires_in_oracle_lane_order(seed, nprio, part_bytes):
     task into four parts that share their lane."""
     dag = random_dag(500, seed, nprio, tile_bytes=16384)
     host = np.random.default_rng(seed).integers(-100, 100, dag.ntiles * dag.tile_bytes // 4).astype(np.int32)
-    ref = oracle_run(dag, host.copy())
+    layout = Layout.contiguous(dag, host=host, valid=False)
+    ref = replay(dag, priority_order(dag, LANES), layout.offsets(), layout.host.copy())
     with Engine(0, max_workers=1, queue_policy=1, part_bytes=part_bytes) as e:
-        slab = e.malloc(dag.ntiles * dag.tile_bytes)
-        alias = e.host_register(host)
-        tiles = np.zeros(dag.ntiles, L.TILE_DTYPE)
-        tiles["dev_ptr"] = slab + np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-        tiles["src_ptr"] = alias + np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-        tiles["bytes"] = dag.tile_bytes
-        w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
-        st = w.run(); res = w.results(); w.close()
-        got = e.d2h(np.empty(dag.ntiles * dag.tile_bytes, np.uint8), slab)
-        e.host_unregister(host)
+        st, res, got, _, _, _ = run_engine(e, dag, layout)
     assert st["tasks_retired"] == dag.ntasks
     assert np.array_equal(res["retire_order"], ref["retire_order"])
     assert np.array_equal(res["result"], ref["result"])
@@ -107,12 +63,12 @@ def test_gemm_one_worker_retires_in_oracle_lane_order(NT):
     loc = dag.tasks["locals"][dag.ready]
     dag.ready = dag.ready[np.argsort([morton(int(i), int(j)) for i, j in loc], kind="stable")]
     rng = np.random.default_rng(NT)
-    init = f32_to_bf16_bits(rng.uniform(-0.5, 0.5, dag.ntiles * T * T).astype(np.float32)).view(np.uint8)
-    ref = oracle_run(dag, state=L.TILE_VALID)
+    layout = Layout.contiguous(dag, dev=f32_to_bf16_bits(rng.uniform(-0.5, 0.5, dag.ntiles * T * T).astype(np.float32)))
+    ref = replay(dag, priority_order(dag, LANES), layout.offsets(), np.zeros(dag.ntiles * dag.tile_bytes, np.uint8))
     outs = {}
     for pol in (0, 1):
         with Engine(0, max_workers=1, gemm_mode=2, queue_policy=pol) as e:
-            st, res, outs[pol] = run_resident(e, dag, init)
+            st, res, outs[pol], _, _, _ = run_engine(e, dag, layout)
         assert st["tasks_retired"] == dag.ntasks
         no_violations(dag, res)
     assert np.array_equal(res["retire_order"], ref["retire_order"])
@@ -122,11 +78,10 @@ def test_gemm_one_worker_retires_in_oracle_lane_order(NT):
 def test_equal_priorities_one_worker_retire_as_fifo():
     for dag in (random_dag(400, 14, 1), dags.ex05_broadcast(64, 14, 4096)):
         dag.tasks["priority"] = -3
-        init = np.zeros(dag.ntiles * dag.tile_bytes, np.uint8)
         orders = []
         for pol in (0, 1):
             with Engine(0, max_workers=1, queue_policy=pol) as e:
-                orders.append(run_resident(e, dag, init)[1]["retire_order"])
+                orders.append(run_engine(e, dag, Layout.contiguous(dag)).res["retire_order"])
         assert np.array_equal(orders[0], orders[1])
 
 
@@ -134,19 +89,10 @@ def test_ex05_all_workers_priority_policy():
     """K = 4096 tiles staged in from host memory: read groups and fused producer units run in their lanes."""
     K, NB, tb = 4096, 14, 16384
     dag = dags.ex05_broadcast(K, NB, tb)
-    host = np.full(K * tb // 4, -7, np.int32)
-    ref = oracle_run(dag, host.copy(), lanes=None)
+    layout = Layout.contiguous(dag, host=np.full(K * tb // 4, -7, np.int32), valid=False)
+    ref = run_oracle(dag, layout).res
     with Engine(0, queue_policy=1) as e:
-        slab = e.malloc(K * tb)
-        alias = e.host_register(host)
-        tiles = np.zeros(K, L.TILE_DTYPE)
-        tiles["dev_ptr"] = slab + np.arange(K, dtype=np.uint64) * np.uint64(tb)
-        tiles["src_ptr"] = alias + np.arange(K, dtype=np.uint64) * np.uint64(tb)
-        tiles["bytes"] = tb
-        w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
-        st = w.run(); res = w.results(); w.close()
-        e.host_unregister(host)
-        e.free(slab)
+        st, res, _, _, _, _ = run_engine(e, dag, layout)
     assert st["tasks_retired"] == dag.ntasks and st["body_errors"] == 0
     no_violations(dag, res)
     recv = res["result"][K:]
@@ -156,11 +102,13 @@ def test_ex05_all_workers_priority_policy():
 
 
 def _policies_agree(dag, init, **engine_kw):
-    ref = oracle_run(dag, state=L.TILE_VALID, lanes=None)
+    """Both policies leave the same tile bytes, and every task sees the tile versions it sees in the oracle's run."""
+    layout = Layout.contiguous(dag, dev=init)
+    ref = run_oracle(dag, layout).res
     outs = {}
     for pol in (0, 1):
         with Engine(0, queue_policy=pol, **engine_kw) as e:
-            st, res, outs[pol] = run_resident(e, dag, init)
+            st, res, outs[pol], _, _, _ = run_engine(e, dag, layout)
         assert st["tasks_retired"] == dag.ntasks
         no_violations(dag, res)
         assert np.array_equal(res["seen_version"], ref["seen_version"])

@@ -11,11 +11,11 @@ from parsec_b200 import _lib as L
 from oracle import orc
 from oracle import orc_dags as dags
 from parsec_b200.engine import Engine
+from window_harness import Layout, assert_like_oracle, assert_same_run, placed, run_oracle
 
 pytestmark = pytest.mark.gpu
 
 RUNS = 6
-STATS = ("tasks_retired", "bytes_h2d", "bytes_d2d", "bytes_d2h", "stage_ins", "body_errors")
 
 
 def counter_mode(dag):
@@ -93,80 +93,39 @@ CASES = [
 ]
 
 
-def host_data(dag):
-    if "host" in dag.meta:
-        return dag.meta["host"].copy()
-    host = np.full(dag.ntiles * dag.tile_bytes // 4, 4, np.int32)
-    host[::977] = 0
-    return host
-
-
-def tile_table(e, dag, host, staged):
-    tb = dag.tile_bytes
-    slot = (tb + 511) // 512 * 512
-    slab = e.malloc(max(dag.ntiles * slot, 16))
-    tiles = np.zeros(dag.ntiles, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(slot)
-    tiles["src_ptr"] = e.host_register(host) + np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(tb)
-    tiles["bytes"] = tb
-    tiles["state"] = L.TILE_INVALID if staged else L.TILE_VALID
-    if not staged:
-        for i in range(dag.ntiles):
-            e.h2d(int(tiles["dev_ptr"][i]), host.view(np.uint8)[i * tb:(i + 1) * tb])
-    return tiles, slab
-
-
-def oracle(dag, host, staged):
-    spec = np.zeros(dag.ntiles, orc.TILE_DTYPE)
-    spec["bytes"] = dag.tile_bytes
-    spec["src_ptr"] = np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-    spec["state"] = orc.TILE_INVALID if staged else orc.TILE_VALID
-    ref = orc.run_window(dag.tasks, dag.succ, spec, dag.ready, host.copy())
-    assert ref["rc"] == 0
-    return ref
-
-
-def assert_run_matches(dag, st, res, first, ref, exact_order):
-    st0, res0 = first
-    for k in STATS:
-        assert st[k] == st0[k], k
-    assert st["tasks_retired"] == dag.ntasks
-    assert st["bytes_h2d"] == ref["stats"]["bytes_h2d"] and st["body_errors"] == ref["stats"]["body_errors"]
-    assert np.array_equal(res["result"], res0["result"]) and np.array_equal(res["result"], ref["result"])
-    assert np.array_equal(res["seen_version"], res0["seen_version"]) and np.array_equal(res["seen_version"], ref["seen_version"])
-    assert res["tiles"].tobytes() == res0["tiles"].tobytes()
-    assert np.array_equal(res["tiles"]["version"], ref["tiles"]["version"])
-    assert np.array_equal(res["tiles"]["state"], ref["tiles"]["state"])
-    assert all(v == 0 for v in dags.check_execution(dag, res).values())
-    if exact_order:
-        for key in ("retire_order", "start_seq", "end_seq", "worker"):
-            assert np.array_equal(res[key], res0[key]), key
-        assert np.array_equal(res["retire_order"], ref["retire_order"])
-
-
 @pytest.mark.parametrize("wait_between", [True, False], ids=["wait_each", "queued"])
 @pytest.mark.parametrize("name,engine_kw,make_dag,staged", CASES, ids=[c[0] for c in CASES])
 def test_every_run_matches_a_fresh_window(name, engine_kw, make_dag, staged, wait_between):
     dag = make_dag()
-    host = host_data(dag)
-    ref = oracle(dag, host, staged)
-    with Engine(0, **engine_kw) as e:
-        tiles, slab = tile_table(e, dag, host, staged)
-        fresh = e.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
-        first = (fresh.run(), fresh.results())
-        fresh.close()
-        exact = engine_kw.get("max_workers") == 1
-        assert_run_matches(dag, *first, first, ref, exact)
-        w = e.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
-        if wait_between:
-            for _ in range(RUNS):
-                st = w.run()
-                assert_run_matches(dag, st, w.results(), first, ref, exact)
-        else:
-            # launches queued back to back: each run starts from the copy the run before it armed
-            for _ in range(RUNS):
-                w.launch()
-            assert_run_matches(dag, w.wait(), w.results(), first, ref, exact)
-        w.close()
-        e.host_unregister(host)
-        e.free(slab)
+    if "host" in dag.meta:
+        host = dag.meta["host"]
+    else:
+        host = np.full(dag.ntiles * dag.tile_bytes // 4, 4, np.int32)
+        host[::977] = 0
+    layout = Layout.packed(dag, host, valid=not staged)
+    with Engine(0, **engine_kw) as e, placed(e, layout) as p:
+        fresh = e.window(dag.kind, dag.tasks, dag.succ, p.tiles, dag.ready)
+        try:
+            runs = [p.run(fresh.run(), fresh.results())]
+        finally:
+            fresh.close()
+        w = e.window(dag.kind, dag.tasks, dag.succ, p.tiles, dag.ready)
+        try:
+            if wait_between:
+                for _ in range(RUNS):
+                    runs.append(p.run(w.run(), w.results()))
+            else:
+                # launches queued back to back: each run starts from the copy the run before it armed
+                for _ in range(RUNS):
+                    w.launch()
+                runs.append(p.run(w.wait(), w.results()))
+        finally:
+            w.close()
+    ref = run_oracle(dag, layout)
+    for run in runs:
+        assert_same_run(run, runs[0])
+        assert_like_oracle(run, ref, dag)
+        if engine_kw.get("max_workers") == 1:
+            for key in ("retire_order", "start_seq", "end_seq", "worker"):
+                assert np.array_equal(run.res[key], runs[0].res[key]), key
+            assert np.array_equal(run.res["retire_order"], ref.res["retire_order"])

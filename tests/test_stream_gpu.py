@@ -3,34 +3,12 @@ window tests use, driven (a) with device-side release of look-ahead edges and (b
 import numpy as np
 import pytest
 
-from oracle import orc, orc_dags as dags
+from oracle import orc_dags as dags
 from parsec_b200 import _lib as L
 from parsec_b200.stream import Stream, run_dag
+from window_harness import Layout, placed, run_oracle
 
 pytestmark = pytest.mark.gpu
-
-
-def _setup(engine, dag, host, valid):
-    nt, tb = dag.ntiles, dag.tile_bytes
-    slot = (tb + 511) // 512 * 512
-    slab = engine.malloc(max(nt * slot, 16))
-    alias = engine.host_register(host)
-    tiles = np.zeros(nt, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + np.arange(nt, dtype=np.uint64) * np.uint64(slot)
-    tiles["src_ptr"] = alias + np.arange(nt, dtype=np.uint64) * np.uint64(tb)
-    tiles["bytes"] = tb
-    tiles["state"] = L.TILE_VALID if valid else L.TILE_INVALID
-    return tiles, slab, slot
-
-
-def _oracle(dag, host0):
-    spec = np.zeros(dag.ntiles, orc.TILE_DTYPE)
-    spec["bytes"] = dag.tile_bytes
-    spec["src_ptr"] = np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-    h = host0.copy()
-    ref = orc.run_window(dag.tasks, dag.succ, spec, dag.ready, h)
-    assert ref["rc"] == 0
-    return ref, h
 
 
 @pytest.mark.parametrize("mode", ["lookahead", "host"])
@@ -47,10 +25,10 @@ def test_stream_matches_oracle(engine, mode, name, maker):
     host = (np.arange(words, dtype=np.int64) % 1000).astype(np.int32) if name.startswith("rtt") else np.full(words, -7, np.int32)
     if name.startswith("rtt"):
         host = host.view(np.float32).copy(); host[:] = 1.0; host = host.view(np.int32)
-    ref, href = _oracle(dag, host)
-    tiles, slab, slot = _setup(engine, dag, host, valid=False)
-    with Stream(engine, cmd_slots=4096, max_tiles=max(dag.ntiles, 1), idle_us=500) as s:
-        out = run_dag(s, dag, tiles, mode=mode)
+    layout = Layout.packed(dag, host)
+    ref = run_oracle(dag, layout)
+    with placed(engine, layout) as p, Stream(engine, cmd_slots=4096, max_tiles=max(dag.ntiles, 1), idle_us=500) as s:
+        out = run_dag(s, dag, p.tiles, mode=mode)
         s.quiesce()
         st = s.stats()
     n = len(dag.tasks)
@@ -61,39 +39,32 @@ def test_stream_matches_oracle(engine, mode, name, maker):
         t = dag.tasks[u]
         for e in dag.succ[t["succ_begin"]:t["succ_begin"] + t["succ_count"]]:
             assert pos[u] < pos[int(e) & 0x07FFFFFF], "retire order is not a linear extension of the DAG"
-    assert np.array_equal(out["result"], ref["result"]), "body results differ from the oracle"
-    assert np.array_equal(out["seen_version"], ref["seen_version"]), "flow versions differ from the oracle"
-    assert st["body_errors"] == ref["stats"]["body_errors"]
-    assert st["bytes_h2d"] == ref["stats"]["bytes_h2d"]
-    assert st["bytes_d2h"] == ref["stats"]["bytes_d2h"]
-    assert np.array_equal(host, href), "pushed-out tiles differ from the oracle"
-    got = np.empty(dag.tile_bytes // 4, np.int32)
+    assert np.array_equal(out["result"], ref.res["result"]), "body results differ from the oracle"
+    assert np.array_equal(out["seen_version"], ref.res["seen_version"]), "flow versions differ from the oracle"
+    for k in ("body_errors", "bytes_h2d", "bytes_d2h"):
+        assert st[k] == ref.stats[k], k
+    assert np.array_equal(p.host, ref.host), "pushed-out tiles differ from the oracle"
     for i in (0, dag.ntiles - 1):
         if dag.tile_bytes >= 4:
-            engine.d2h(got, slab + i * slot)
-            assert np.array_equal(got.view(np.uint8), ref["device"][i][:got.nbytes]), "final tile bytes differ"
+            nb = dag.tile_bytes // 4 * 4
+            assert np.array_equal(layout.tile_bytes(p.dev, i)[:nb], layout.tile_bytes(ref.dev, i)[:nb]), "final tile bytes differ"
     if mode == "lookahead" and any(t["succ_count"] for t in dag.tasks):
         assert st["released_on_device"] + st["edges_late"] > 0
-    engine.host_unregister(host)
-    engine.free(slab)
 
 
 def test_stream_parks_and_restarts(engine):
     """The persistent kernel exits when idle and is relaunched by the next submission; tickets survive the gap."""
     import time
     dag = dags.ex02_chain(20)
-    host = np.zeros(1, np.int32)
-    tiles, slab, slot = _setup(engine, dag, host, valid=True)
-    with Stream(engine, cmd_slots=1024, max_tiles=1, idle_us=200) as s:
+    layout = Layout.packed(dag, np.zeros(1, np.int32), valid=True)
+    with placed(engine, layout) as p, Stream(engine, cmd_slots=1024, max_tiles=1, idle_us=200) as s:
         for rnd in range(3):
-            out = run_dag(s, dag, tiles, mode="lookahead")
+            out = run_dag(s, dag, p.tiles, mode="lookahead")
             assert out["retire_order"].tolist() == list(range(21))
             time.sleep(0.05)                     # >> idle_us: the kernel parks
         st = s.stats()
         assert st["kernel_launches"] >= 3
         assert st["retired"] == 63
-    engine.host_unregister(host)
-    engine.free(slab)
 
 
 def test_stream_unknown_body_is_reported(engine):

@@ -14,6 +14,7 @@ from oracle import orc_dags as dags
 from parsec_b200 import _lib as L
 from parsec_b200 import runtime as R
 from parsec_b200.engine import Engine
+from window_harness import Layout, assert_same_run, placed, run_engine
 from test_priority import random_dag
 from test_rearm_gpu import gemm_chains_dag
 
@@ -73,37 +74,6 @@ def groups_dag(seed, n_rmw=300, ngroups=24, tile_bytes=64 * 1024):
     return dags.Dag(t, succ, ready, ntiles=6 + ngroups, tile_bytes=tile_bytes, name="groups")
 
 
-def host_of(dag, seed=0):
-    if "host" in dag.meta:
-        return dag.meta["host"].copy()
-    return np.random.default_rng(seed).integers(-100, 100, dag.ntiles * dag.tile_bytes // 4).astype(np.int32)
-
-
-def run_once(e, dag, host, trace, runs=1):
-    """`runs` launches of one window over tiles resident in HBM (a copy of host); returns stats, results, the trace of
-    each launch (trace on) and the final tile bytes."""
-    tb, nt = dag.tile_bytes, dag.ntiles
-    slab = e.malloc(nt * tb)
-    e.h2d(slab, host)
-    tiles = np.zeros(nt, L.TILE_DTYPE)
-    tiles["dev_ptr"] = slab + np.arange(nt, dtype=np.uint64) * np.uint64(tb)
-    tiles["bytes"] = tb
-    tiles["state"] = L.TILE_VALID
-    e.set_window_trace(trace)
-    w = e.window(dag.kind, dag.tasks, dag.succ, tiles, dag.ready)
-    e.set_window_trace(False)
-    traces = []
-    for _ in range(runs):
-        st = w.run()
-        if trace:
-            traces.append(w.trace())
-    res = w.results()
-    w.close()
-    data = e.d2h(np.empty(nt * tb, np.uint8), slab)
-    e.free(slab)
-    return st, res, traces, data
-
-
 def check_trace(dag, tr, sm_count, what):
     t0, t1, sm, unit = (tr[k].astype(np.int64) for k in ("t_start_ns", "t_end_ns", "smid", "unit"))
     assert np.all(t0 > 0) and np.all(t0 <= t1), what
@@ -122,28 +92,25 @@ def check_trace(dag, tr, sm_count, what):
     return unit
 
 
-def assert_identical(dag, plain, traced):
-    (st_a, res_a, _, data_a), (st_b, res_b, _, data_b) = plain, traced
-    for k in ("result", "seen_version"):
-        assert np.array_equal(res_a[k], res_b[k]), k
-    assert res_a["tiles"].tobytes() == res_b["tiles"].tobytes()
-    assert np.array_equal(data_a, data_b)
-    for k in ("tasks_retired", "body_errors", "bytes_h2d", "stage_ins"):
-        assert st_a[k] == st_b[k], k
-    assert st_b["tasks_retired"] == dag.ntasks
-    assert all(v == 0 for v in dags.check_execution(dag, res_b).values())     # end_seq[u] < start_seq[v] on every edge
+def run_twice(e, dag, host):
+    """The window over tiles resident in HBM (holding host), untraced and traced: both compute the same thing, in an
+    order that respects every edge.  Returns the traced run."""
+    plain = run_engine(e, dag, Layout.contiguous(dag, dev=host))
+    traced = run_engine(e, dag, Layout.contiguous(dag, dev=host), trace=True)
+    assert_same_run(plain, traced)
+    assert traced.stats["tasks_retired"] == dag.ntasks
+    assert all(v == 0 for v in dags.check_execution(dag, traced.res).values())     # end_seq[u] < start_seq[v] on every edge
+    return traced
 
 
 @pytest.mark.parametrize("seed,part_bytes,queue_policy", [(1, 0, 0), (2, 16 * 1024, 0), (3, 0, 1), (4, 16 * 1024, 1)])
 def test_random_hbm_dags_with_groups(seed, part_bytes, queue_policy):
     dag = groups_dag(seed)
-    host = host_of(dag, seed)
+    host = np.random.default_rng(seed).integers(-100, 100, dag.ntiles * dag.tile_bytes // 4).astype(np.int32)
     with Engine(0, part_bytes=part_bytes, queue_policy=queue_policy) as e:
-        plain = run_once(e, dag, host, False)
-        traced = run_once(e, dag, host, True)
+        traced = run_twice(e, dag, host)
         sm_count = e.info()["sm_count"]
-    assert_identical(dag, plain, traced)
-    unit = check_trace(dag, traced[2][0], sm_count, "groups seed %d part_bytes %d policy %d" % (seed, part_bytes, queue_policy))
+    unit = check_trace(dag, traced.traces[0], sm_count, "groups seed %d part_bytes %d policy %d" % (seed, part_bytes, queue_policy))
     # every producer runs fused with its readers and leads them
     fills = np.flatnonzero(dag.tasks["body"] == L.BODY_FILL_I32)
     readers = np.flatnonzero(dag.tasks["body"] == L.BODY_CHECK_I32)
@@ -156,12 +123,10 @@ def test_ex05_window(fuse_readers):
     dag = dags.ex05_broadcast(256, 14, 256 * 1024)
     host = np.full(dag.ntiles * dag.tile_bytes // 4, -1, np.int32)
     with Engine(0, fuse_readers=fuse_readers) as e:
-        plain = run_once(e, dag, host, False)
-        traced = run_once(e, dag, host, True)
+        traced = run_twice(e, dag, host)
         sm_count = e.info()["sm_count"]
-    assert_identical(dag, plain, traced)
     K, F = 256, dag.meta["F"]
-    unit = check_trace(dag, traced[2][0], sm_count, "ex05 fuse_readers %d" % fuse_readers)
+    unit = check_trace(dag, traced.traces[0], sm_count, "ex05 fuse_readers %d" % fuse_readers)
     lead = np.repeat(np.arange(K), F) if fuse_readers == 0 else K + np.repeat(np.arange(K) * F, F)
     assert np.array_equal(unit[K:], lead)
 
@@ -175,13 +140,10 @@ def test_gemm_window(make, gemm_mode, queue_policy):
         rng = np.random.default_rng(5)
         bits = (rng.integers(-64, 64, dag.ntiles * dag.tile_bytes // 2) * 0x10 + 0x3C00).astype(np.uint16)   # small bf16
         dag.meta["host"] = bits.view(np.int32)
-    host = host_of(dag)
     with Engine(0, gemm_mode=gemm_mode, queue_policy=queue_policy, part_bytes=32 * 1024) as e:
-        plain = run_once(e, dag, host, False)
-        traced = run_once(e, dag, host, True)
+        traced = run_twice(e, dag, dag.meta["host"])
         sm_count = e.info()["sm_count"]
-    assert_identical(dag, plain, traced)
-    unit = check_trace(dag, traced[2][0], sm_count, "gemm mode %d policy %d" % (gemm_mode, queue_policy))
+    unit = check_trace(dag, traced.traces[0], sm_count, "gemm mode %d policy %d" % (gemm_mode, queue_policy))
     gemm = dag.tasks["body"] == L.BODY_GEMM_BF16
     fused = int(np.sum(unit[gemm] != np.flatnonzero(gemm)))
     if gemm_mode == 2:
@@ -192,9 +154,9 @@ def test_gemm_window(make, gemm_mode, queue_policy):
 
 def test_rearmed_window_reads_the_copy_each_launch_used():
     dag = groups_dag(9)
-    host = host_of(dag, 9)
+    host = np.random.default_rng(9).integers(-100, 100, dag.ntiles * dag.tile_bytes // 4).astype(np.int32)
     with Engine(0) as e:
-        _, _, traces, _ = run_once(e, dag, host, True, runs=3)
+        traces = run_engine(e, dag, Layout.contiguous(dag, dev=host), launches=3, trace=True).traces
         sm_count = e.info()["sm_count"]
     prev_end = 0
     for i, tr in enumerate(traces):
@@ -205,12 +167,8 @@ def test_rearmed_window_reads_the_copy_each_launch_used():
 
 def test_untraced_window_refuses_trace():
     dag = dags.ex05_broadcast(4, 2, 4096)
-    with Engine(0) as e:
-        slab = e.malloc(dag.ntiles * dag.tile_bytes)
-        tiles = np.zeros(dag.ntiles, L.TILE_DTYPE)
-        tiles["dev_ptr"] = slab + np.arange(dag.ntiles, dtype=np.uint64) * np.uint64(dag.tile_bytes)
-        tiles["bytes"], tiles["state"] = dag.tile_bytes, L.TILE_VALID
-        w = e.window(0, dag.tasks, dag.succ, tiles, dag.ready)
+    with Engine(0) as e, placed(e, Layout.contiguous(dag)) as p:
+        w = e.window(0, dag.tasks, dag.succ, p.tiles, dag.ready)
         w.run()
         with pytest.raises(L.Pb2Error) as exc:
             w.trace()
