@@ -292,6 +292,29 @@ int  pb2_window_trace(pb2_window_t* window,
                       int32_t*  unit);           /* [ntasks] the task that leads the entity (host side):
                                                   * read-group leader, fused producer, GEMM unit's first
                                                   * task, or the task itself                              */
+/* One part of a scheduling entity as a worker ran it (a window created with trace on): the entity's parts are its ring
+ * entries -- the byte slices of a wide task, of a read group or of a fused producer unit, the sub-tile sets of a GEMM
+ * unit.  The four stamps are %globaltimer nanoseconds taken by one thread on one SM, so they are ordered:
+ *   t_pop   the pop of the entry (the value the entity's t_start is the minimum of)
+ *   t_in    stage-in done (the tiles the part found INVALID are in HBM); t_pop..t_in is "movein"
+ *   t_exec  body done (a read group's members, a fused unit's check, a GEMM unit's TMA operand stream and MMAs)
+ *   t_out   pushout done (= t_exec when the part pushes nothing out); t_exec..t_out is "moveout"
+ * in_bytes: bytes this worker staged in itself (from the host or a peer); out_bytes: bytes it pushed out. */
+#define PB2_PART_WAITED_INPUT 1u    /* the part found an input tile not VALID                                    */
+#define PB2_PART_RETIRED      2u    /* the part retired its entity (the SM of pb2_window_trace)                  */
+typedef struct pb2_part_trace_s {
+    uint64_t t_pop_ns, t_in_ns, t_exec_ns, t_out_ns;   /* %globaltimer of this GPU                                  */
+    uint64_t in_bytes, out_bytes;
+    int32_t  task;                                     /* the task leading the entity: pb2_window_trace's unit[]    */
+    uint16_t part, nparts;
+    uint32_t smid;
+    uint32_t flags;                                    /* PB2_PART_WAITED_INPUT | PB2_PART_RETIRED                   */
+} pb2_part_trace_t;                                    /* 64 bytes */
+/* The part records of the last launch of a window created with trace on, valid after wait: one per ring entry, ordered
+ * by leading task id, then by part.  *n gets the number of records; at most cap of them are written to out (out may be
+ * NULL).  A part that never ran (a failed run) has zero stamps.  PB2_ERR_NOT_SUPPORTED for a window created without
+ * trace. */
+int  pb2_window_part_trace(pb2_window_t* window, pb2_part_trace_t* out, int32_t cap, int32_t* n);
 
 /* --- windows that release dependencies of tasks living in OTHER GPUs' windows (remote_dep edges, remote_dep.h:42-58,
  * without the host: the activation is a device atomic on the peer's dependency word plus a ring write over NVLink).

@@ -226,6 +226,11 @@ int  pb2_taskpool_completion_trace(pb2_taskpool_t* tp, int32_t* out_task, int32_
  * ITS device's clock: devices are not on one time axis) and the SM; every other task (CPU incarnations, user submit
  * bodies, dry runs) gets 0, 0 and 0.  device[i] = device_index that ran task i (-1: not run) */
 int  pb2_taskpool_device_trace(pb2_taskpool_t* tp, uint64_t* t_start_ns, uint64_t* t_end_ns, int32_t* device, uint32_t* smid);
+/* device part records (pb2_window_part_trace), with the MCA parameter device_engine_trace: every part of every entity
+ * the pool's tasks led in a GPU window, window by window as the windows retired; task is the pool task id of the
+ * leading task, device[i] the device_index that ran record i (its clock).  *n gets the number of records; at most cap
+ * are written (out and device may be NULL). */
+int  pb2_taskpool_device_part_trace(pb2_taskpool_t* tp, pb2_part_trace_t* out, int32_t* device, int32_t cap, int32_t* n);
 /* per task: locals[0..1], class id, flow versions seen (4), body result; arrays sized nb_tasks (may be NULL) */
 int  pb2_taskpool_task_info(pb2_taskpool_t* tp, int32_t* class_id, int32_t* locals2, uint32_t* seen_version4,
                             uint64_t* result);

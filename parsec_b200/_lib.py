@@ -60,6 +60,15 @@ TILE_DTYPE = np.dtype([
 ], align=False)
 assert TILE_DTYPE.itemsize == 32
 
+# numpy mirror of the 64-byte pb2_part_trace_t (pb2_window_part_trace)
+PART_WAITED_INPUT, PART_RETIRED = 1, 2
+PART_TRACE_DTYPE = np.dtype([
+    ("t_pop_ns", "<u8"), ("t_in_ns", "<u8"), ("t_exec_ns", "<u8"), ("t_out_ns", "<u8"),
+    ("in_bytes", "<u8"), ("out_bytes", "<u8"), ("task", "<i4"), ("part", "<u2"), ("nparts", "<u2"),
+    ("smid", "<u4"), ("flags", "<u4"),
+], align=False)
+assert PART_TRACE_DTYPE.itemsize == 64
+
 
 def succ_make(task, flow=0):
     return (np.uint32(flow) << np.uint32(27)) | np.uint32(task)
@@ -116,7 +125,7 @@ ENGINE_SYMBOLS = [
     "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_window_trace", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
     "pb2_window_arm", "pb2_window_start",
     "pb2_window_create", "pb2_window_destroy", "pb2_window_launch", "pb2_window_wait",
-    "pb2_window_results", "pb2_window_trace",
+    "pb2_window_results", "pb2_window_trace", "pb2_window_part_trace",
     "pb2_partition_create", "pb2_partition_sizes", "pb2_partition_get", "pb2_partition_destroy", "pb2_partition_error",
     "pb2_partition_set_push", "pb2_partition_push_count", "pb2_partition_get_push", "pb2_window_set_push",
 ]
@@ -159,6 +168,7 @@ def load():
     lib.pb2_engine_set_part_bytes.argtypes = [vp, i32]
     lib.pb2_engine_set_window_trace.argtypes = [vp, C.c_int]
     lib.pb2_window_trace.argtypes = [vp, vp, vp, vp, vp]
+    lib.pb2_window_part_trace.argtypes = [vp, vp, i32, P(i32)]
     lib.pb2_engine_set_stage_slice_bytes.argtypes = [vp, i32]
     lib.pb2_window_export.argtypes = [vp, vp]
     lib.pb2_window_set_remote.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32]

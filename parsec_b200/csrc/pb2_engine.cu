@@ -36,8 +36,8 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // reset: (re)arm one window.  dep words, ring, counters, tile table; the units of a GEMM window.
 // ---------------------------------------------------------------------------------------------
-// The per-run state of g.w (rearm_run), in a GEMM window its units' words, in a traced window its time stamps.  A GEMM
-// window never has more units than tasks.
+// The per-run state of g.w (rearm_run), in a GEMM window its units' words, in a traced window its time stamps and part
+// records.  A GEMM window never has more units than tasks.
 __global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -45,6 +45,8 @@ __global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
     for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
     if (g.trace.t_start)
         for (size_t i = gid; i < (size_t)g.w.ntasks; i += gsz) { g.trace.t_start[i] = ~0ull; g.trace.t_end[i] = 0; g.trace.smid[i] = 0; }
+    if (g.trace.parts)
+        for (size_t i = gid; i < (size_t)g.trace.nparts * 8; i += gsz) reinterpret_cast<unsigned long long*>(g.trace.parts)[i] = 0;
     rearm_run(g.w, tiles_init, ready, nready, gid, gsz);
 }
 
@@ -106,6 +108,7 @@ struct RunState {
     Lanes* lanes;                         // RunShape::lanes
     int32_t* udep; int32_t* unit_parts_left;        // GEMM windows: the units' dependency words and part counts
     unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid;     // RunShape::trace (TraceDev)
+    pb2_part_trace_t* parts;              // RunShape::trace: part_records of them
 };
 
 // What every copy of a window's per-run state is sized from besides ntasks and ntiles, recorded by pb2_window_create.
@@ -116,6 +119,7 @@ struct RunShape {
     bool claims = false;                  // stage-in is sliced: claim arrays per tile
     bool lanes = false;                   // queue_policy 1: priority lanes, which start as lane_image
     bool trace = false;                   // per-task device time stamps (pb2_engine_set_window_trace)
+    int32_t part_records = 0;             // trace: one part record per ring entry of a run
     Lanes lane_image{};
 };
 
@@ -140,6 +144,8 @@ struct pb2_window_s {
     cudaEvent_t ev_arm = nullptr;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
     std::vector<int32_t> task_unit;           // traced windows, per task: the task that leads its scheduling entity
+    struct PartEntity { int32_t lead, base, nparts; };
+    std::vector<PartEntity> part_entities;   // traced windows: the ring-entry owners by leading task, their records
     std::vector<void*> allocs;
     std::vector<void*> peer_ptrs;
     std::vector<pb2_tile_t*> peer_tiles;     // per rank: its tile table as mapped here (nullptr: none / self)
@@ -305,6 +311,29 @@ static int build_lane_ring(pb2_window_t* w, WindowPlan& p) {
     return rc;
 }
 
+// Traced windows: where the part records of each ring-entry owner o (a task of an HBM window, a unit of a GEMM window)
+// start.  Owner o leads the entity of task lead[o] and runs nparts[o] parts (0: o owns no entries, as the members of a
+// read group).  Its records are part_base[o] .. + nparts[o], in owner order; pb2_window_part_trace returns them by
+// leading task.
+static int plan_part_records(pb2_window_t* w, const std::vector<int32_t>& lead, const std::vector<int32_t>& nparts, WindowPlan& plan) {
+    std::vector<int32_t> base(nparts.size());
+    int32_t n = 0;
+    w->part_entities.clear();
+    for (size_t o = 0; o < nparts.size(); ++o) {
+        base[o] = n;
+        if (nparts[o] > 0) w->part_entities.push_back({lead[o], n, nparts[o]});
+        n += nparts[o];
+    }
+    std::stable_sort(w->part_entities.begin(), w->part_entities.end(),
+                     [](const pb2_window_s::PartEntity& a, const pb2_window_s::PartEntity& b) { return a.lead < b.lead; });
+    int32_t* d_base = nullptr;
+    const int rc = dev_alloc_copy(w, &d_base, base.data(), base.size());
+    if (rc != PB2_SUCCESS) return rc;
+    w->g.trace.part_base = d_base; w->g.trace.nparts = n;
+    plan.run.part_records = n;
+    return PB2_SUCCESS;
+}
+
 // ---------------------------------------------------------------------------------------------
 // GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
 // ---------------------------------------------------------------------------------------------
@@ -412,9 +441,13 @@ static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
     plan.run.nunits = (int32_t)units.size();
     w->task_entry.resize((size_t)ntasks);
     for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
-    if (!w->task_unit.empty())
-        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = segs[(size_t)units[(size_t)unit_of[t]].seg_begin].task;
     int rc;
+    if (!w->task_unit.empty()) {
+        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = segs[(size_t)units[(size_t)unit_of[t]].seg_begin].task;
+        std::vector<int32_t> lead(units.size()), np(units.size());
+        for (size_t u = 0; u < units.size(); ++u) { lead[u] = segs[(size_t)units[u].seg_begin].task; np[u] = units[u].nparts; }
+        if ((rc = plan_part_records(w, lead, np, plan)) != PB2_SUCCESS) return rc;
+    }
     uint32_t* d_succ = nullptr; GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
     if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
     if ((rc = dev_alloc_copy(w, &d_units, units.data(), units.size())) != PB2_SUCCESS) return rc;
@@ -573,6 +606,11 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
                 }
     } else if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
     d.succ = d_succ;
+    if (!w->task_unit.empty()) {                // a task owns ring entries unless a group member is led by another task
+        std::vector<int32_t> lead((size_t)ntasks), np((size_t)ntasks);
+        for (int32_t t = 0; t < ntasks; ++t) { lead[(size_t)t] = t; np[(size_t)t] = w->task_unit[(size_t)t] == t ? nparts[(size_t)t] : 0; }
+        if ((rc = plan_part_records(w, lead, np, plan)) != PB2_SUCCESS) return rc;
+    }
     if (extra_parts) {
         uint16_t* d_np = nullptr;
         if ((rc = dev_alloc_copy(w, &d_np, nparts.data(), nparts.size())) != PB2_SUCCESS) return rc;
@@ -600,7 +638,7 @@ static int alloc_run(pb2_window_t* w, int c) {
     if (s.lanes) alloc(&r.lanes, 1);
     // every GEMM window has the unit words, even without units: pb2_window_export hands out udep
     if (w->kind == 1) { alloc(&r.udep, (size_t)s.nunits); alloc(&r.unit_parts_left, (size_t)s.nunits); }
-    if (s.trace) { alloc(&r.t_start, nt); alloc(&r.t_end, nt); alloc(&r.smid, nt); }
+    if (s.trace) { alloc(&r.t_start, nt); alloc(&r.t_end, nt); alloc(&r.smid, nt); alloc(&r.parts, (size_t)s.part_records); }
     if (rc != PB2_SUCCESS) return rc;
     // copy 1 takes copy 0's lanes device to device: a copy from pageable host memory may wait for the engine stream
     if (s.lanes) PB2_CUDA(e, c == 0 ? cudaMemcpyAsync(r.lanes, &s.lane_image, sizeof(Lanes), cudaMemcpyHostToDevice, stream)
@@ -619,7 +657,7 @@ static Win2Dev run_desc(const pb2_window_t* w, int c) {
     d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
     d.lanes = r.lanes;
     g.udep = r.udep; g.parts_left = r.unit_parts_left;
-    g.trace = TraceDev{r.t_start, r.t_end, r.smid};
+    g.trace.t_start = r.t_start; g.trace.t_end = r.t_end; g.trace.smid = r.smid; g.trace.parts = r.parts;
     return g;
 }
 
@@ -1227,6 +1265,25 @@ int pb2_window_trace(pb2_window_t* w, uint64_t* t_start_ns, uint64_t* t_end_ns, 
     if (t_end_ns && n) PB2_CUDA(e, cudaMemcpy(t_end_ns, tr.t_end, n * 8, cudaMemcpyDeviceToHost));
     if (smid && n) PB2_CUDA(e, cudaMemcpy(smid, tr.smid, n * 4, cudaMemcpyDeviceToHost));
     if (unit && n) memcpy(unit, w->task_unit.data(), n * sizeof(int32_t));
+    return PB2_SUCCESS;
+}
+
+int pb2_window_part_trace(pb2_window_t* w, pb2_part_trace_t* out, int32_t cap, int32_t* n) {
+    if (!w || !n || cap < 0) return PB2_ERR_BAD_PARAM;
+    pb2_engine_t* e = w->e;
+    if (!w->shape.trace) { e->last_error = "window was created without trace (pb2_engine_set_window_trace)"; return PB2_ERR_NOT_SUPPORTED; }
+    const int32_t total = w->shape.part_records;
+    *n = total;
+    if (!out || cap == 0 || total == 0) return PB2_SUCCESS;
+    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    std::vector<pb2_part_trace_t> rec((size_t)total);
+    PB2_CUDA(e, cudaMemcpy(rec.data(), run_desc(w, w->cur).trace.parts, (size_t)total * sizeof(pb2_part_trace_t), cudaMemcpyDeviceToHost));
+    int32_t k = 0;
+    for (const pb2_window_s::PartEntity& pe : w->part_entities)
+        for (int32_t p = 0; p < pe.nparts && k < cap; ++p, ++k) {
+            out[k] = rec[(size_t)(pe.base + p)];
+            out[k].task = pe.lead; out[k].part = (uint16_t)p; out[k].nparts = (uint16_t)pe.nparts;
+        }
     return PB2_SUCCESS;
 }
 

@@ -323,7 +323,7 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
 }  // namespace gemm
 
 // PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: record the device time stamps of every task in
-// g.trace (TraceDev); the untraced instantiations never touch it.
+// g.trace (TraceDev) and a record of every part (PartSmem, then trace_part); the untraced instantiations never touch it.
 template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(gemm::kThreads, 1)
 pb2_engine_gemm2_kernel(Win2Dev g) {
@@ -332,6 +332,8 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     __shared__ Shared sh;
+    PartSmem* rec = nullptr;
+    if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
@@ -359,7 +361,10 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 const unsigned long long t_pop = TRACE ? globaltimer_ns() : 0ull;
                 j.unit = PB2_SUCC_TASK((uint32_t)e); j.part = PB2_SUCC_FLOW((uint32_t)e);
                 const GUnit u = g.units[j.unit];
-                if (TRACE) trace_pop(g.trace, g.segs[u.seg_begin].task, t_pop);     // the unit's first task leads it
+                if (TRACE) {
+                    trace_pop(g.trace, g.segs[u.seg_begin].task, t_pop);     // the unit's first task leads it
+                    *rec = PartSmem{t_pop, 0, 0, 0, 0, 0, 0};
+                }
                 j.is_gemm = u.flags & 1; j.pushout = (u.flags >> 1) & 1;
                 j.seg_begin = u.seg_begin; j.seg_count = u.seg_count; j.tileC = u.tileC; j.nparts = u.nparts;
                 j.M = u.M; j.N = u.N; j.K = u.K;
@@ -381,12 +386,18 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 __syncthreads();
                 if (sh.ts.need) {
                     const int ns = tile_slices(w, tile->bytes);
-                    if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.ts.decide);
+                    if (TRACE) {
+                        if (threadIdx.x == 0) rec->flags |= PB2_PART_WAITED_INPUT;
+                        if (ns == 1) stage_in_flow_counted(stage_ctx(w), tile, acc, &sh.ts.decide, nullptr, &rec->in_bytes);
+                        else stage_in_slices_counted(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide, nullptr, &rec->in_bytes);
+                    }
+                    else if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.ts.decide);
                     else stage_in_slices(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide);     // take what nobody has claimed, wait for the rest
                     fence_proxy_async();
                 }
                 __syncthreads();
             }
+            if (TRACE && sh.job.is_gemm && threadIdx.x == 0) rec->t_in = globaltimer_ns();
         }
         const Job& job = sh.job;       // read from shared memory, not held in registers across the wgmma loop
 
@@ -450,17 +461,19 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.ts.task)[threadIdx.x] =
                 __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
             __syncthreads();
-            const unsigned long long r = run_task_part<false>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
+            const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
                 const unsigned long long body_r = run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
                 fence_proxy_async();
                 return body_r;
-            });
+            }, rec);
             // CHECK parts add their mismatch counts; the first element comes from part 0
             if (threadIdx.x == 0) store_result(w, sh.ts.task, id, job.part, job.nparts, r);
         }
         __threadfence();
         __syncthreads();             // every store of the part is done and visible
+        // a GEMM unit's exec ends here: its TMA operand stream cannot be told apart from its MMAs
+        if (TRACE && job.is_gemm && threadIdx.x == 0) rec->t_exec = globaltimer_ns();
 
         // ---------------- part complete: pushout of its sub-tiles' C rows, then unit retirement by the last part
         if (job.is_gemm && job.pushout) {
@@ -473,6 +486,7 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                     cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + (size_t)m0 * row_bytes,
                                     reinterpret_cast<const uint8_t*>(tile->dev_ptr) + (size_t)m0 * row_bytes, (size_t)rows * row_bytes);
                     if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)rows * row_bytes);
+                    if (TRACE && threadIdx.x == 0) rec->out_bytes += (unsigned long long)rows * row_bytes;
                 } else {
                     // a column block of a tile wider than one sub-tile: row segments
                     for (int r = 0; r < rows; ++r) {
@@ -480,6 +494,7 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                         cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + o, reinterpret_cast<const uint8_t*>(tile->dev_ptr) + o, (size_t)Nj * 2);
                     }
                     if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)rows * (unsigned long long)Nj * 2ull);
+                    if (TRACE && threadIdx.x == 0) rec->out_bytes += (unsigned long long)rows * (unsigned long long)Nj * 2ull;
                 }
             }
             // a pushout writes the whole tile back, as every other body's does: the part that runs the last sub-tile also
@@ -489,12 +504,15 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + c_bytes,
                                 reinterpret_cast<const uint8_t*>(tile->dev_ptr) + c_bytes, tile->bytes - c_bytes);
                 if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)(tile->bytes - c_bytes));
+                if (TRACE && threadIdx.x == 0) rec->out_bytes += (unsigned long long)(tile->bytes - c_bytes);
             }
             __syncthreads();
         }
         if (warp == 0) {
             int last = 0;
+            if (TRACE && lane == 0 && job.is_gemm) rec->t_out = globaltimer_ns();
             if (lane == 0) { __threadfence(); last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
+            if (TRACE && lane == 0) trace_part(g.trace, job.unit, job.part, *rec, last);
             last = __shfl_sync(0xffffffffu, last, 0);
             if (last) { __threadfence(); retire_unit_warp<PRIO, TRACE>(g, g.units[job.unit], job.unit); }
         }

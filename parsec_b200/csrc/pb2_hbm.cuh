@@ -123,7 +123,8 @@ __device__ __forceinline__ void trace_entity(const TraceDev& tr, int32_t lead, c
 }
 
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
-// TRACE: record the device time stamps of every task in tr (TraceDev); the untraced instantiations never touch tr.
+// TRACE: record the device time stamps of every task in tr (TraceDev) and a record of every part (PartSmem, then
+// trace_part); the untraced instantiations never touch tr.
 template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
 pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
@@ -131,6 +132,8 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
     __shared__ BulkSmem bulk;
     __shared__ GroupSmem g;
     __shared__ unsigned long long t_start;   // the watchdog's earliest reference (pop_idle)
+    PartSmem* rec = nullptr;
+    if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
     if (threadIdx.x == 0) { bulk_init(bulk); t_start = globaltimer_ns(); }
     __syncthreads();
 
@@ -139,7 +142,11 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
             const int32_t e = pop_entry<PRIO>(w, &t_start);
             if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
             // the popped task leads its entity (a group's leader, a fused producer)
-            if (TRACE && e != kEmpty) trace_pop(tr, w.nparts ? PB2_ENT_TASK(e) : e, globaltimer_ns());
+            if (TRACE && e != kEmpty) {
+                const unsigned long long t_pop = globaltimer_ns();
+                trace_pop(tr, w.nparts ? PB2_ENT_TASK(e) : e, t_pop);
+                *rec = PartSmem{t_pop, 0, 0, 0, 0, 0, 0};
+            }
             s.entry = e;
         }
         __syncthreads();
@@ -183,9 +190,9 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         }
         __syncthreads();
         const int nparts = task_nparts(w, id);
-        const unsigned long long r = run_task_part<true>(w, s, &bulk, id, part, nparts, [&] {
+        const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
             return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
-        });
+        }, rec);
         if (g.n && !g.fused) {
             // the leader's part stored the version it saw; every member saw the same one
             if (threadIdx.x == 0) {
@@ -197,6 +204,8 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
             }
             __syncthreads();
             group_results(&s, &g);
+            // the members' results are part of the body; the readers push nothing out
+            if (TRACE && threadIdx.x == 0) rec->t_exec = rec->t_out = globaltimer_ns();
         }
 
         if (threadIdx.x < 32) {
@@ -270,6 +279,12 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
                 __threadfence();
                 st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
             }
+        }
+        if (TRACE && threadIdx.x == 0) {
+            // the part's record, off the retire path (its stamps were taken before it); owner and part from shared
+            // memory: nothing of the part has to stay in registers until here
+            const int32_t e = s.entry;
+            trace_part(tr, w.nparts ? PB2_ENT_TASK(e) : e, w.nparts ? PB2_ENT_PART(e) : 0, *rec, s.last != 0);
         }
         __syncthreads();
     }

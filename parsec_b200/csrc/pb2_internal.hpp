@@ -174,6 +174,9 @@ struct pb2_taskpool_s {
     int32_t nb_done = 0;
     bool added = false;
     std::vector<int32_t> trace_task, trace_device;
+    // device_engine_trace: the part records of the entities its tasks led (task = pool task id) and their device index
+    std::vector<pb2_part_trace_t> part_trace;
+    std::vector<int32_t> part_trace_device;
     std::map<std::pair<pb2_data_collection_t*, uint64_t>, pb2_dtd_tile_t*> tiles;
     std::vector<pb2_dtd_tile_t*> tile_list;
     uint32_t devices_index_mask = 0xffffffffu;

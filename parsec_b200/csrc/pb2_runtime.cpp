@@ -766,6 +766,17 @@ int pb2_taskpool_device_trace(pb2_taskpool_t* tp, uint64_t* t_start_ns, uint64_t
     return PB2_SUCCESS;
 }
 
+int pb2_taskpool_device_part_trace(pb2_taskpool_t* tp, pb2_part_trace_t* out, int32_t* device, int32_t cap, int32_t* n) {
+    if (!tp || !n || cap < 0) return PB2_ERR_BAD_PARAM;
+    const int32_t total = (int32_t)tp->part_trace.size();
+    *n = total;
+    for (int32_t i = 0; i < total && i < cap; ++i) {
+        if (out) out[i] = tp->part_trace[(size_t)i];
+        if (device) device[i] = tp->part_trace_device[(size_t)i];
+    }
+    return PB2_SUCCESS;
+}
+
 int pb2_taskpool_task_info(pb2_taskpool_t* tp, int32_t* class_id, int32_t* locals2, uint32_t* seen_version4, uint64_t* result) {
     if (!tp) return PB2_ERR_BAD_PARAM;
     for (size_t i = 0; i < tp->tasks.size(); ++i) {
@@ -1338,6 +1349,18 @@ static int retire_one(pb2_device_module_t* dev) {
             rc = pb2_window_trace(f->win, t0.data(), t1.data(), sm.data(), nullptr);
             if (rc == PB2_SUCCESS)
                 for (int32_t i = 0; i < n; ++i) { pb2_htask_t* t = w.order[(size_t)i]; t->dev_t_start = t0[(size_t)i]; t->dev_t_end = t1[(size_t)i]; t->dev_smid = sm[(size_t)i]; }
+            // the part records go to the pool of the task that led each entity, which they name by its pool task id
+            int32_t nrec = 0;
+            if (rc == PB2_SUCCESS) rc = pb2_window_part_trace(f->win, nullptr, 0, &nrec);
+            std::vector<pb2_part_trace_t> rec((size_t)nrec);
+            if (rc == PB2_SUCCESS && nrec) rc = pb2_window_part_trace(f->win, rec.data(), nrec, &nrec);
+            if (rc == PB2_SUCCESS)
+                for (pb2_part_trace_t r : rec) {
+                    pb2_htask_t* t = w.order[(size_t)r.task];
+                    r.task = t->id;
+                    t->tp->part_trace.push_back(r);
+                    t->tp->part_trace_device.push_back(dev->device_index);
+                }
         }
         if (rc != PB2_SUCCESS) ctx->last_error = std::string("window run: ") + pb2_engine_last_error(dev->engine);
         pb2_window_destroy(f->win);

@@ -360,7 +360,29 @@ __device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id, unsigne
 // stamp its retiring part stores as the watchdog's progress; every task of the entity gets that interval and the SM of
 // the retiring part.  Only the TRACE instantiations of the window kernels touch these arrays (null in an untraced
 // window); the reset kernel starts t_start at ~0, the identity of the atomicMin of the pops.
-struct TraceDev { unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid; };
+// Per ring entry of the run, the part record (pb2_part_trace_t) of the worker that ran it, at part_base[owner] + part;
+// the owner is the popped task of an HBM window, the unit of a GEMM window.  The host fills task, part and nparts.
+struct TraceDev {
+    unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid;
+    pb2_part_trace_t* parts;          // nparts records, cleared by the reset kernel
+    const int32_t* part_base;         // per ring-entry owner: its first record
+    int32_t nparts;
+};
+static_assert(sizeof(pb2_part_trace_t) == 64, "pb2_part_trace_t is a 64-byte public record");
+
+// A traced worker's record of the part it runs, in shared memory: nothing of it is held in registers across the body.
+// Thread 0 writes it.
+struct PartSmem { unsigned long long t_pop, t_in, t_exec, t_out, in_bytes, out_bytes; uint32_t flags; };
+
+// Thread 0, after the part's pushout, once it knows whether the part retired its entity: the record of part `part` of
+// ring-entry owner `owner`.  A part that pushed nothing out ends at t_exec (deciding that here, not where t_out is
+// stamped, keeps the HBM kernels' pushout path free of spills at their 80-register budget).
+__device__ __forceinline__ void trace_part(const TraceDev& tr, int32_t owner, int part, const PartSmem& r, bool retired) {
+    pb2_part_trace_t* p = &tr.parts[tr.part_base[owner] + part];
+    p->t_pop_ns = r.t_pop; p->t_in_ns = r.t_in; p->t_exec_ns = r.t_exec; p->t_out_ns = r.out_bytes ? r.t_out : r.t_exec;
+    p->in_bytes = r.in_bytes; p->out_bytes = r.out_bytes;
+    p->smid = smid(); p->flags = r.flags | (retired ? PB2_PART_RETIRED : 0u);
+}
 
 // One thread, right after it popped a part of the entity led by task `lead` at time t.
 __device__ __forceinline__ void trace_pop(const TraceDev& tr, int32_t lead, unsigned long long t) { atomicMin(&tr.t_start[lead], t); }
@@ -427,8 +449,14 @@ __device__ __forceinline__ StageCtx stage_ctx(const WinDev& w) {
     return StageCtx{w.tiles, w.ctl, w.slice_claim, w.slice_done, w.stage_mode == 0 ? 1 : 0, w.part_bytes};
 }
 
+// The stage-in helpers below are out of line.  Each has a COUNT form, called by the traced window kernels only, that
+// also adds the bytes the calling CTA moved to *moved (its PartSmem::in_bytes, thread 0): the untraced kernels keep the
+// helpers as they are.
+
 // Thread 0 decides (s_decide[0]): 1 = this CTA moves the tile, 0 = already valid (possibly after waiting)
-static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk = nullptr) {
+template <bool COUNT>
+__device__ __forceinline__ void stage_in_flow_impl(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk,
+                                                   unsigned long long* moved) {
     if (threadIdx.x == 0) {
         int decide = 0;
         if ((access & PB2_FLOW_ACCESS_READ) && tile->src_kind == PB2_SRC_PUSH) {
@@ -457,9 +485,17 @@ static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* 
             atomicAdd(tile->src_kind == PB2_SRC_PEER ? &w.ctl->bytes_d2d.v : &w.ctl->bytes_h2d.v,
                       (unsigned long long)tile->bytes);
             atomicAdd(&w.ctl->stage_ins.v, 1ull);
+            if (COUNT) *moved += tile->bytes;
         }
     }
     __syncthreads();
+}
+static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk = nullptr) {
+    stage_in_flow_impl<false>(w, tile, access, s_decide, bulk, nullptr);
+}
+static __device__ __noinline__ void stage_in_flow_counted(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk,
+                                                          unsigned long long* moved) {
+    stage_in_flow_impl<true>(w, tile, access, s_decide, bulk, moved);
 }
 
 
@@ -475,7 +511,9 @@ __device__ __forceinline__ int tile_slices(const WinDev& w, uint32_t bytes) { re
 // bit), so the parts of a wide task -- and the parts of other readers of the same version -- pull the tile in
 // parallel instead of one CTA moving 4 MiB alone; a CTA that finds a slice claimed by someone else only waits
 // for it.  The worker whose slice completes the tile publishes PB2_TILE_VALID.
-static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide, BulkSmem* bulk = nullptr) {
+template <bool COUNT>
+__device__ __forceinline__ void stage_in_slices_impl(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
+                                                     BulkSmem* bulk, unsigned long long* moved) {
     pb2_tile_t* tile = &w.tiles[tile_id];
     if (tile->src_kind == PB2_SRC_PUSH) {       // written by its producer (see stage_in_flow)
         if (threadIdx.x == 0) while (ld_acquire_sys(&tile->state) != PB2_TILE_VALID) __nanosleep(64);
@@ -499,6 +537,7 @@ static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t ti
                 __threadfence();
                 atomicOr(&done[sl >> 5], bit);
                 atomicAdd(tile->src_kind == PB2_SRC_PEER ? &w.ctl->bytes_d2d.v : &w.ctl->bytes_h2d.v, (unsigned long long)len);
+                if (COUNT) *moved += len;
                 if ((int)atomicAdd(&done[PB2_SLICE_WORDS], 1u) + 1 == nslices) {
                     __threadfence();
                     st_release_gpu(&tile->state, PB2_TILE_VALID);
@@ -516,6 +555,13 @@ static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t ti
         __threadfence();
     }
     __syncthreads();
+}
+static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide, BulkSmem* bulk = nullptr) {
+    stage_in_slices_impl<false>(w, tile_id, nslices, s0, s1, s_decide, bulk, nullptr);
+}
+static __device__ __noinline__ void stage_in_slices_counted(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
+                                                            BulkSmem* bulk, unsigned long long* moved) {
+    stage_in_slices_impl<true>(w, tile_id, nslices, s0, s1, s_decide, bulk, moved);
 }
 
 }  // namespace pb2

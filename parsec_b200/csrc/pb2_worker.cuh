@@ -30,9 +30,10 @@ struct alignas(16) TaskSmem {
 // All threads (uniform): stage in every flow whose bit is set in s.need.  One CTA-wide call per task at most.
 // BULK: the calling kernel has a TMA bulk ring (without one the copies take the SIMT loops).  Each instantiation has
 // one caller kernel per translation unit: a second caller kernel makes ptxas give this helper the standard call ABI,
-// which costs the HBM kernels a stack frame and spills at their 80-register budget (see pb2_hbm.cuh).
-template <bool BULK>
-static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, TaskSmem* sp, BulkSmem* bulk) {
+// which costs the HBM kernels a stack frame and spills at their 80-register budget (see pb2_hbm.cuh).  COUNT (traced
+// kernels, stage_in_needed_flows_counted): add the bytes this CTA moved to *moved.
+template <bool BULK, bool COUNT>
+__device__ __forceinline__ void stage_in_needed_flows_impl(const StageCtx c, TaskSmem* sp, BulkSmem* bulk, unsigned long long* moved) {
     TaskSmem& s = *sp;
     const int need = s.need;
 #pragma unroll 1
@@ -41,21 +42,34 @@ static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, Task
         const int32_t tid = s.task.tile[f];
         const uint32_t bytes = s.tbytes[f];
         const int ns = tile_slices_of(c.part_bytes, c.slice_claim, bytes);
-        if (ns == 1) stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr);
-        else {
+        if (ns == 1) {
+            if (COUNT) stage_in_flow_counted(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr, moved);
+            else stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr);
+        } else {
             int s0, s1;
             slices_over(bytes, ns, s.off[f], s.args.bytes[f], s0, s1);     // the slices under this part's bytes
-            stage_in_slices(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr);
+            if (COUNT) stage_in_slices_counted(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr, moved);
+            else stage_in_slices(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr);
         }
     }
+}
+template <bool BULK>
+static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, TaskSmem* sp, BulkSmem* bulk) {
+    stage_in_needed_flows_impl<BULK, false>(c, sp, bulk, nullptr);
+}
+template <bool BULK>
+static __device__ __noinline__ void stage_in_needed_flows_counted(const StageCtx c, TaskSmem* sp, BulkSmem* bulk, unsigned long long* moved) {
+    stage_in_needed_flows_impl<BULK, true>(c, sp, bulk, moved);
 }
 
 // All threads.  On entry s.task holds the descriptor (published by a barrier).  exec() runs the body over s.args (all
 // threads) and returns its result in thread 0.  Returns the body result (thread 0).  BULK as for
-// stage_in_needed_flows; without it `bulk` is not used.
-template <bool BULK, class Exec>
+// stage_in_needed_flows; without it `bulk` is not used.  TRACE (traced window kernels): thread 0 stamps the end of the
+// stage-in, of the body and of the pushout into *rec, and counts the bytes this CTA moved in and pushed out there.
+template <bool BULK, bool TRACE = false, class Exec>
 __device__ __forceinline__ unsigned long long
-run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts, Exec exec) {
+run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts, Exec exec,
+              PartSmem* rec = nullptr) {
     const pb2_task_t& t = s.task;
     // ---- push: one thread per flow works out its slice and whether the tile has to be staged in -----------------
     if (threadIdx.x < 32) {
@@ -89,11 +103,15 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     __syncthreads();
     // the cold path, out of line and called once: everything it needs is in shared memory, nothing of the caller's
     // has to survive the call in registers
-    if (s.need) stage_in_needed_flows<BULK>(stage_ctx(w), &s, bulk);
+    if (TRACE) {
+        if (s.need) stage_in_needed_flows_counted<BULK>(stage_ctx(w), &s, bulk, &rec->in_bytes);
+        if (threadIdx.x == 0) { if (s.need) rec->flags |= PB2_PART_WAITED_INPUT; rec->t_in = globaltimer_ns(); }
+    } else if (s.need) stage_in_needed_flows<BULK>(stage_ctx(w), &s, bulk);
 
     // ---- exec: the body (parsec_device_kernel_exec -> submit) ----
     const unsigned long long r = exec();
     __syncthreads();
+    if (TRACE && threadIdx.x == 0) rec->t_exec = globaltimer_ns();
 
     // ---- pop: pushout of written flows to their home copy (parsec_device_kernel_pop stage_out) ----
 #pragma unroll
@@ -103,9 +121,11 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
             cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + s.off[f], s.args.flow[f], s.args.bytes[f],
                             BULK ? bulk : nullptr);
             if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)s.args.bytes[f]);
+            if (TRACE && threadIdx.x == 0) rec->out_bytes += s.args.bytes[f];
         }
     }
     __syncthreads();
+    if (TRACE && threadIdx.x == 0) rec->t_out = globaltimer_ns();     // trace_part reports t_exec if nothing went out
     return r;
 }
 

@@ -57,6 +57,40 @@ def chrome_trace(t_start_ns, t_end_ns, smid, class_id=None, locals=None, class_n
     return {"traceEvents": events, "displayTimeUnit": "ns"}
 
 
+def chrome_trace_parts(records, class_id=None, class_names=None, pid=0, process_name=None):
+    """Part records (Window.part_trace, Context.device_part_trace; PART_TRACE_DTYPE) as a Chrome trace: one row per SM,
+    and per part up to three complete ("X") events -- "movein" from its pop to the end of its stage-in, the body (named
+    from class_id[task] through class_names when given, else "exec") and "moveout" for its pushout.  Phases of zero
+    length get no event, nor do records that were never stamped.  Times in microseconds from the earliest pop; args:
+    task, part, nparts and, for movein and moveout, the bytes moved.  pid: the trace process (one per device)."""
+    rec = np.asarray(records)
+    rec = rec[rec["t_pop_ns"] != 0]
+    base = int(rec["t_pop_ns"].min()) if len(rec) else 0
+    events = []
+    if process_name is not None:
+        events.append({"ph": "M", "name": "process_name", "pid": pid, "tid": 0, "args": {"name": process_name}})
+    for s in sorted({int(x) for x in rec["smid"]}):
+        events.append({"ph": "M", "name": "thread_name", "pid": pid, "tid": s, "args": {"name": "SM %d" % s}})
+        events.append({"ph": "M", "name": "thread_sort_index", "pid": pid, "tid": s, "args": {"sort_index": s}})
+    for r in rec:
+        task = int(r["task"])
+        if class_id is None:
+            body = "exec"
+        else:
+            c = int(class_id[task])
+            body = class_names.get(c, "class %d" % c) if class_names else "class %d" % c
+        args = {"task": task, "part": int(r["part"]), "nparts": int(r["nparts"])}
+        t = [int(r["t_pop_ns"]), int(r["t_in_ns"]), int(r["t_exec_ns"]), int(r["t_out_ns"])]
+        for (name, t0, t1, nbytes) in (("movein", t[0], t[1], int(r["in_bytes"])), (body, t[1], t[2], None),
+                                       ("moveout", t[2], t[3], int(r["out_bytes"]))):
+            if t1 <= t0:
+                continue
+            a = dict(args) if nbytes is None else dict(args, bytes=nbytes)
+            events.append({"ph": "X", "name": name, "pid": pid, "tid": int(r["smid"]),
+                           "ts": (t0 - base) / 1000.0, "dur": (t1 - t0) / 1000.0, "args": a})
+    return {"traceEvents": events, "displayTimeUnit": "ns"}
+
+
 class Engine:
     """One engine per GPU (the reference's parsec_device_cuda_module_t, device_cuda.h:43-48).
 
@@ -257,6 +291,16 @@ class Window:
                "smid": np.empty(n, np.uint32), "unit": np.empty(n, np.int32)}
         _check(self._lib.pb2_window_trace(self._h, _ptr(out["t_start_ns"]), _ptr(out["t_end_ns"]), _ptr(out["smid"]),
                                           _ptr(out["unit"])), "pb2_window_trace", self.engine)
+        return out
+
+    def part_trace(self):
+        """Part records of the last launch (a window created with trace on; pb2_window_part_trace): one PART_TRACE_DTYPE
+        record per ring entry, by leading task, then part."""
+        n = C.c_int32(0)
+        _check(self._lib.pb2_window_part_trace(self._h, None, 0, C.byref(n)), "pb2_window_part_trace", self.engine)
+        out = np.zeros(n.value, L.PART_TRACE_DTYPE)
+        _check(self._lib.pb2_window_part_trace(self._h, _ptr(out), n.value, C.byref(n)), "pb2_window_part_trace",
+               self.engine)
         return out
 
     def close(self):

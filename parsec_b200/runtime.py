@@ -39,7 +39,7 @@ PARSEC_SYMBOLS = [
     "pb2_dc_data_of", "pb2_dc_data_key", "pb2_dc_position", "pb2_dc_info", "pb2_dc_register_memory",
     "pb2_dc_distribute_on_devices", "pb2_dc_host_write_all", "pb2_context_add_taskpool", "pb2_context_start", "pb2_context_wait",
     "pb2_taskpool_wait", "pb2_taskpool_free", "pb2_taskpool_nb_tasks", "pb2_taskpool_set_device_types",
-    "pb2_taskpool_completion_trace", "pb2_taskpool_device_trace", "pb2_taskpool_task_info", "pb2_taskpool_export_window", "pb2_dtd_taskpool_new",
+    "pb2_taskpool_completion_trace", "pb2_taskpool_device_trace", "pb2_taskpool_device_part_trace", "pb2_taskpool_task_info", "pb2_taskpool_export_window", "pb2_dtd_taskpool_new",
     "pb2_dtd_tile_of", "pb2_dtd_tile_new", "pb2_dtd_tile_data", "pb2_dtd_create_task_class",
     "pb2_dtd_task_class_add_chore", "pb2_dtd_insert_task_with_task_class", "pb2_dtd_data_flush_all",
     "pb2_dtd_task_class_add_submit", "pb2_gpu_task_flow_ptr", "pb2_gpu_task_flow_bytes", "pb2_gpu_task_iparam",
@@ -90,6 +90,7 @@ def lib():
         "pb2_taskpool_nb_tasks": (C.c_int, [vp]), "pb2_taskpool_set_device_types": (C.c_int, [vp, C.c_int]),
         "pb2_taskpool_completion_trace": (C.c_int, [vp, vp, vp, i32]),
         "pb2_taskpool_device_trace": (C.c_int, [vp, vp, vp, vp, vp]),
+        "pb2_taskpool_device_part_trace": (C.c_int, [vp, vp, vp, i32, P(i32)]),
         "pb2_taskpool_task_info": (C.c_int, [vp, vp, vp, vp, vp]),
         "pb2_taskpool_export_window": (C.c_int, [vp, vp, vp, P(i32), vp, P(i32), vp, P(i32), vp, P(i32), vp]),
         "pb2_dtd_taskpool_new": (vp, [vp]), "pb2_dtd_tile_of": (vp, [vp, vp, C.c_uint64]),
@@ -196,6 +197,15 @@ class Context:
         dev, sm = np.zeros(n, np.int32), np.zeros(n, np.uint32)
         _chk(self.l.pb2_taskpool_device_trace(tp, _p(t0), _p(t1), _p(dev), _p(sm)), "device_trace")
         return dict(t_start_ns=t0, t_end_ns=t1, device=dev, smid=sm)
+
+    def device_part_trace(self, tp):
+        """The part records (PART_TRACE_DTYPE) of the entities the pool's tasks led in GPU windows (MCA parameter
+        device_engine_trace), window by window; task is the pool task id.  Returns (records, device index per record)."""
+        n = C.c_int32(0)
+        _chk(self.l.pb2_taskpool_device_part_trace(tp, None, None, 0, C.byref(n)), "device_part_trace")
+        rec, dev = np.zeros(n.value, L.PART_TRACE_DTYPE), np.zeros(n.value, np.int32)
+        _chk(self.l.pb2_taskpool_device_part_trace(tp, _p(rec), _p(dev), n.value, C.byref(n)), "device_part_trace")
+        return rec, dev
 
     def task_info(self, tp):
         n = self.l.pb2_taskpool_nb_tasks(tp)
