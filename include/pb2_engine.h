@@ -282,13 +282,15 @@ int  pb2_window_results(pb2_window_t* window,
                         pb2_tile_t* tiles_out);  /* [ntiles] final tile table (state, version)           */
 /* Per-task device time stamps of the last launch of a window created with trace on (pb2_engine_set_window_trace),
  * valid after wait; any pointer may be NULL.  Times are %globaltimer nanoseconds of this GPU's clock.  A task gets the
- * interval of its scheduling entity: from the earliest pop of any of its parts to the retirement of the last part; the
- * members of a read group, of a fused producer unit or of a GEMM unit share one interval and SM.  A task that never
- * ran (a failed run) reads 0.  PB2_ERR_NOT_SUPPORTED for a window created without trace. */
+ * interval of its scheduling entity, derived from the entity's part records (pb2_window_part_trace): from the earliest
+ * t_pop of its parts to the latest t_out, so the retirement bookkeeping after the last part's pushout (the epilog, a
+ * few atomics, a fused unit's member stores) is not part of it.  The members of a read group, of a fused producer unit
+ * or of a GEMM unit share one interval and SM.  A task whose entity was never popped reads 0; one whose entity did not
+ * retire (a failed run) reads 0 as t_end and SM.  PB2_ERR_NOT_SUPPORTED for a window created without trace. */
 int  pb2_window_trace(pb2_window_t* window,
                       uint64_t* t_start_ns,      /* [ntasks] earliest pop of a part of the task's entity  */
-                      uint64_t* t_end_ns,        /* [ntasks] its retirement                               */
-                      uint32_t* smid,            /* [ntasks] SM of the retiring part                      */
+                      uint64_t* t_end_ns,        /* [ntasks] latest pushout end of one of its parts       */
+                      uint32_t* smid,            /* [ntasks] SM of the part that retired it               */
                       int32_t*  unit);           /* [ntasks] the task that leads the entity (host side):
                                                   * read-group leader, fused producer, GEMM unit's first
                                                   * task, or the task itself                              */

@@ -36,15 +36,13 @@ namespace pb2 {
 // ---------------------------------------------------------------------------------------------
 // reset: (re)arm one window.  dep words, ring, counters, tile table; the units of a GEMM window.
 // ---------------------------------------------------------------------------------------------
-// The per-run state of g.w (rearm_run), in a GEMM window its units' words, in a traced window its time stamps and part
-// records.  A GEMM window never has more units than tasks.
+// The per-run state of g.w (rearm_run), in a GEMM window its units' words, in a traced window its part records (a zero
+// t_pop marks a part that was not popped).  A GEMM window never has more units than tasks.
 __global__ void pb2_window_reset_kernel(Win2Dev g, const pb2_tile_t* tiles_init,
                                         const int32_t* ready, int32_t nready) {
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t gsz = (size_t)gridDim.x * blockDim.x;
     for (size_t i = gid; i < (size_t)g.nunits; i += gsz) { g.udep[i] = g.units[i].dep_goal; g.parts_left[i] = g.units[i].nparts; }
-    if (g.trace.t_start)
-        for (size_t i = gid; i < (size_t)g.w.ntasks; i += gsz) { g.trace.t_start[i] = ~0ull; g.trace.t_end[i] = 0; g.trace.smid[i] = 0; }
     if (g.trace.parts)
         for (size_t i = gid; i < (size_t)g.trace.nparts * 8; i += gsz) reinterpret_cast<unsigned long long*>(g.trace.parts)[i] = 0;
     rearm_run(g.w, tiles_init, ready, nready, gid, gsz);
@@ -107,8 +105,7 @@ struct RunState {
     uint32_t* slice_claim; uint32_t* slice_done;    // RunShape::claims
     Lanes* lanes;                         // RunShape::lanes
     int32_t* udep; int32_t* unit_parts_left;        // GEMM windows: the units' dependency words and part counts
-    unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid;     // RunShape::trace (TraceDev)
-    pb2_part_trace_t* parts;              // RunShape::trace: part_records of them
+    pb2_part_trace_t* parts;              // RunShape::trace: part_records of them (TraceDev)
 };
 
 // What every copy of a window's per-run state is sized from besides ntasks and ntiles, recorded by pb2_window_create.
@@ -118,7 +115,7 @@ struct RunShape {
     bool parts = false;                   // per-task part counts (an HBM window with wide tasks)
     bool claims = false;                  // stage-in is sliced: claim arrays per tile
     bool lanes = false;                   // queue_policy 1: priority lanes, which start as lane_image
-    bool trace = false;                   // per-task device time stamps (pb2_engine_set_window_trace)
+    bool trace = false;                   // part records (pb2_engine_set_window_trace)
     int32_t part_records = 0;             // trace: one part record per ring entry of a run
     Lanes lane_image{};
 };
@@ -638,7 +635,7 @@ static int alloc_run(pb2_window_t* w, int c) {
     if (s.lanes) alloc(&r.lanes, 1);
     // every GEMM window has the unit words, even without units: pb2_window_export hands out udep
     if (w->kind == 1) { alloc(&r.udep, (size_t)s.nunits); alloc(&r.unit_parts_left, (size_t)s.nunits); }
-    if (s.trace) { alloc(&r.t_start, nt); alloc(&r.t_end, nt); alloc(&r.smid, nt); alloc(&r.parts, (size_t)s.part_records); }
+    if (s.trace) alloc(&r.parts, (size_t)s.part_records);
     if (rc != PB2_SUCCESS) return rc;
     // copy 1 takes copy 0's lanes device to device: a copy from pageable host memory may wait for the engine stream
     if (s.lanes) PB2_CUDA(e, c == 0 ? cudaMemcpyAsync(r.lanes, &s.lane_image, sizeof(Lanes), cudaMemcpyHostToDevice, stream)
@@ -657,8 +654,26 @@ static Win2Dev run_desc(const pb2_window_t* w, int c) {
     d.worker = r.worker; d.parts_left = r.parts_left; d.slice_claim = r.slice_claim; d.slice_done = r.slice_done;
     d.lanes = r.lanes;
     g.udep = r.udep; g.parts_left = r.unit_parts_left;
-    g.trace.t_start = r.t_start; g.trace.t_end = r.t_end; g.trace.smid = r.smid; g.trace.parts = r.parts;
+    g.trace.parts = r.parts;
     return g;
+}
+
+// The part records of the last launch of traced window w, ordered as part_entities (by leading task, then part), with
+// task, part and nparts filled in.
+static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out) {
+    pb2_engine_t* e = w->e;
+    std::vector<pb2_part_trace_t> rec((size_t)w->shape.part_records);
+    out.clear();
+    if (rec.empty()) return PB2_SUCCESS;
+    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    PB2_CUDA(e, cudaMemcpy(rec.data(), run_desc(w, w->cur).trace.parts, rec.size() * sizeof(pb2_part_trace_t), cudaMemcpyDeviceToHost));
+    out.reserve(rec.size());
+    for (const pb2_window_s::PartEntity& pe : w->part_entities)
+        for (int32_t p = 0; p < pe.nparts; ++p) {
+            out.push_back(rec[(size_t)(pe.base + p)]);
+            out.back().task = pe.lead; out.back().part = (uint16_t)p; out.back().nparts = (uint16_t)pe.nparts;
+        }
+    return PB2_SUCCESS;
 }
 
 extern "C" {
@@ -1255,16 +1270,27 @@ int pb2_window_trace(pb2_window_t* w, uint64_t* t_start_ns, uint64_t* t_end_ns, 
     if (!w) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
     if (!w->shape.trace) { e->last_error = "window was created without trace (pb2_engine_set_window_trace)"; return PB2_ERR_NOT_SUPPORTED; }
-    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     const size_t n = (size_t)w->ntasks;
-    const TraceDev tr = run_desc(w, w->cur).trace;   // the copy of the last run
-    if (t_start_ns && n) {
-        PB2_CUDA(e, cudaMemcpy(t_start_ns, tr.t_start, n * 8, cudaMemcpyDeviceToHost));
-        for (size_t i = 0; i < n; ++i) if (t_start_ns[i] == ~0ull) t_start_ns[i] = 0;     // never popped
-    }
-    if (t_end_ns && n) PB2_CUDA(e, cudaMemcpy(t_end_ns, tr.t_end, n * 8, cudaMemcpyDeviceToHost));
-    if (smid && n) PB2_CUDA(e, cudaMemcpy(smid, tr.smid, n * 4, cudaMemcpyDeviceToHost));
     if (unit && n) memcpy(unit, w->task_unit.data(), n * sizeof(int32_t));
+    if (!n || (!t_start_ns && !t_end_ns && !smid)) return PB2_SUCCESS;
+    std::vector<pb2_part_trace_t> rec;
+    const int rc = read_part_records(w, rec);
+    if (rc != PB2_SUCCESS) return rc;
+    // per leading task, from its entity's parts: the earliest pop, the latest pushout end, the SM of the retiring part
+    struct Span { uint64_t t0 = 0, t1 = 0; uint32_t sm = 0; bool retired = false; };
+    std::vector<Span> of(n);
+    for (const pb2_part_trace_t& r : rec) {
+        Span& sp = of[(size_t)r.task];
+        if (r.t_pop_ns && (!sp.t0 || r.t_pop_ns < sp.t0)) sp.t0 = r.t_pop_ns;     // 0: not popped
+        sp.t1 = std::max(sp.t1, r.t_out_ns);
+        if (r.flags & PB2_PART_RETIRED) { sp.sm = r.smid; sp.retired = true; }
+    }
+    for (size_t t = 0; t < n; ++t) {
+        const Span& sp = of[(size_t)w->task_unit[t]];
+        if (t_start_ns) t_start_ns[t] = sp.t0;
+        if (t_end_ns) t_end_ns[t] = sp.retired ? sp.t1 : 0;
+        if (smid) smid[t] = sp.sm;
+    }
     return PB2_SUCCESS;
 }
 
@@ -1272,18 +1298,12 @@ int pb2_window_part_trace(pb2_window_t* w, pb2_part_trace_t* out, int32_t cap, i
     if (!w || !n || cap < 0) return PB2_ERR_BAD_PARAM;
     pb2_engine_t* e = w->e;
     if (!w->shape.trace) { e->last_error = "window was created without trace (pb2_engine_set_window_trace)"; return PB2_ERR_NOT_SUPPORTED; }
-    const int32_t total = w->shape.part_records;
-    *n = total;
-    if (!out || cap == 0 || total == 0) return PB2_SUCCESS;
-    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
-    std::vector<pb2_part_trace_t> rec((size_t)total);
-    PB2_CUDA(e, cudaMemcpy(rec.data(), run_desc(w, w->cur).trace.parts, (size_t)total * sizeof(pb2_part_trace_t), cudaMemcpyDeviceToHost));
-    int32_t k = 0;
-    for (const pb2_window_s::PartEntity& pe : w->part_entities)
-        for (int32_t p = 0; p < pe.nparts && k < cap; ++p, ++k) {
-            out[k] = rec[(size_t)(pe.base + p)];
-            out[k].task = pe.lead; out[k].part = (uint16_t)p; out[k].nparts = (uint16_t)pe.nparts;
-        }
+    *n = w->shape.part_records;
+    if (!out || cap == 0 || *n == 0) return PB2_SUCCESS;
+    std::vector<pb2_part_trace_t> rec;
+    const int rc = read_part_records(w, rec);
+    if (rc != PB2_SUCCESS) return rc;
+    memcpy(out, rec.data(), (size_t)std::min(cap, *n) * sizeof(pb2_part_trace_t));
     return PB2_SUCCESS;
 }
 

@@ -220,7 +220,7 @@ struct Win2Dev {
     const CUtensorMap* tmaps;       // one per tile (w.ntiles)
     int32_t nunits;
     int32_t fresh_tmaps;            // first launch since tmaps were written: every producer acquires all of them first
-    TraceDev trace;                 // per-task time stamps of a traced window (null otherwise); the HBM kernel takes them beside w
+    TraceDev trace;                 // part records of a traced window (null otherwise); the HBM kernel takes them beside w
 };
 
 namespace gemm {
@@ -241,33 +241,23 @@ struct Shared {
     uint64_t empty[kStages];
 };
 
-// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges.  TRACE: every
-// member gets the unit's interval (TraceDev), which starts at the earliest pop of a part of it (its first task's t_start).
-template <bool PRIO, bool TRACE>
-__device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u, int unit_id) {
+// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges.
+template <bool PRIO>
+__device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u) {
     const WinDev& w = g.w;
     const int lane = threadIdx.x & 31;
     const int L = u.seg_count;
-    unsigned long long ebase = 0, rbase = 0, now = 0;
+    unsigned long long ebase = 0, rbase = 0;
     if (lane == 0) {
         ebase = atomicAdd(&w.ctl->evt.v, (unsigned long long)(2 * L));
         rbase = atomicAdd(&w.ctl->retired.v, (unsigned long long)L);
-        now = globaltimer_ns();
-        *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
+        *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
     }
     ebase = __shfl_sync(0xffffffffu, ebase, 0);
     rbase = __shfl_sync(0xffffffffu, rbase, 0);
-    unsigned long long t0 = 0;
-    uint32_t sm = 0;
-    if (TRACE) {
-        now = __shfl_sync(0xffffffffu, now, 0);
-        t0 = trace_start_of(g.trace, g.segs[u.seg_begin].task);
-        sm = smid();
-    }
     const uint32_t cver = (u.flags & 1) ? *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) : 0u;
     for (int i = lane; i < L; i += 32) {
         const GSeg s = g.segs[u.seg_begin + i];
-        if (TRACE) trace_task(g.trace, s.task, t0, now, sm);
         w.start_seq[s.task] = (uint32_t)(ebase + 2 * i);
         w.end_seq[s.task] = (uint32_t)(ebase + 2 * i + 1);
         w.retire_log[rbase + i] = s.task;
@@ -317,13 +307,12 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
         __threadfence();
         st_release_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneOK);
     }
-    (void)unit_id;
 }
 
 }  // namespace gemm
 
-// PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: record the device time stamps of every task in
-// g.trace (TraceDev) and a record of every part (PartSmem, then trace_part); the untraced instantiations never touch it.
+// PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: write a record of every part into g.trace (PartSmem,
+// then trace_part); the untraced instantiations never touch it.
 template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(gemm::kThreads, 1)
 pb2_engine_gemm2_kernel(Win2Dev g) {
@@ -358,13 +347,9 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             if (e == kEmpty) { j.stop = 1; }
             else {
                 __threadfence();
-                const unsigned long long t_pop = TRACE ? globaltimer_ns() : 0ull;
+                if (TRACE) *rec = PartSmem{globaltimer_ns(), 0, 0, 0, 0, 0, 0};
                 j.unit = PB2_SUCC_TASK((uint32_t)e); j.part = PB2_SUCC_FLOW((uint32_t)e);
                 const GUnit u = g.units[j.unit];
-                if (TRACE) {
-                    trace_pop(g.trace, g.segs[u.seg_begin].task, t_pop);     // the unit's first task leads it
-                    *rec = PartSmem{t_pop, 0, 0, 0, 0, 0, 0};
-                }
                 j.is_gemm = u.flags & 1; j.pushout = (u.flags >> 1) & 1;
                 j.seg_begin = u.seg_begin; j.seg_count = u.seg_count; j.tileC = u.tileC; j.nparts = u.nparts;
                 j.M = u.M; j.N = u.N; j.K = u.K;
@@ -386,13 +371,10 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 __syncthreads();
                 if (sh.ts.need) {
                     const int ns = tile_slices(w, tile->bytes);
-                    if (TRACE) {
-                        if (threadIdx.x == 0) rec->flags |= PB2_PART_WAITED_INPUT;
-                        if (ns == 1) stage_in_flow_counted(stage_ctx(w), tile, acc, &sh.ts.decide, nullptr, &rec->in_bytes);
-                        else stage_in_slices_counted(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide, nullptr, &rec->in_bytes);
-                    }
-                    else if (ns == 1) stage_in_flow(stage_ctx(w), tile, acc, &sh.ts.decide);
-                    else stage_in_slices(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide);     // take what nobody has claimed, wait for the rest
+                    if (TRACE && threadIdx.x == 0) rec->flags |= PB2_PART_WAITED_INPUT;
+                    unsigned long long* moved = TRACE ? &rec->in_bytes : nullptr;
+                    if (ns == 1) stage_in_flow<TRACE>(stage_ctx(w), tile, acc, &sh.ts.decide, nullptr, moved);
+                    else stage_in_slices<TRACE>(stage_ctx(w), tile_id, ns, 0, ns, &sh.ts.decide, nullptr, moved);     // take what nobody has claimed, wait for the rest
                     fence_proxy_async();
                 }
                 __syncthreads();
@@ -514,7 +496,7 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             if (lane == 0) { __threadfence(); last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
             if (TRACE && lane == 0) trace_part(g.trace, job.unit, job.part, *rec, last);
             last = __shfl_sync(0xffffffffu, last, 0);
-            if (last) { __threadfence(); retire_unit_warp<PRIO, TRACE>(g, g.units[job.unit], job.unit); }
+            if (last) { __threadfence(); retire_unit_warp<PRIO>(g, g.units[job.unit]); }
         }
         __syncthreads();             // sh.job is rewritten by the next pop
     }

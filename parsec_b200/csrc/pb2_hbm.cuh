@@ -113,18 +113,8 @@ static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, G
     return r;
 }
 
-// Thread 0 of the retiring part, TRACE: the tasks of the entity led by `lead` -- itself and the n members mem[] of its
-// read group (a plain group's leader is mem[0]) -- get the entity's interval (TraceDev).
-__device__ __forceinline__ void trace_entity(const TraceDev& tr, int32_t lead, const int32_t* mem, int n, unsigned long long t_end) {
-    const unsigned long long t0 = trace_start_of(tr, lead);
-    const uint32_t sm = smid();
-    trace_task(tr, lead, t0, t_end, sm);
-    for (int i = 0; i < n; ++i) trace_task(tr, mem[i], t0, t_end, sm);
-}
-
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
-// TRACE: record the device time stamps of every task in tr (TraceDev) and a record of every part (PartSmem, then
-// trace_part); the untraced instantiations never touch tr.
+// TRACE: write a record of every part into tr (PartSmem, then trace_part); the untraced instantiations never touch tr.
 template <bool PRIO, bool TRACE>
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
 pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
@@ -141,12 +131,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         if (threadIdx.x == 0) {
             const int32_t e = pop_entry<PRIO>(w, &t_start);
             if (e != kEmpty) __threadfence();   // acquire side: order the tile reads below after the slot read
-            // the popped task leads its entity (a group's leader, a fused producer)
-            if (TRACE && e != kEmpty) {
-                const unsigned long long t_pop = globaltimer_ns();
-                trace_pop(tr, w.nparts ? PB2_ENT_TASK(e) : e, t_pop);
-                *rec = PartSmem{t_pop, 0, 0, 0, 0, 0, 0};
-            }
+            if (TRACE && e != kEmpty) *rec = PartSmem{globaltimer_ns(), 0, 0, 0, 0, 0, 0};
             s.entry = e;
         }
         __syncthreads();
@@ -236,9 +221,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
                         w.end_seq[m] = ev + 1u + (uint32_t)(gn + i);
                         w.retire_log[seq + 1u + (uint32_t)i] = m;
                     }
-                    const unsigned long long now = globaltimer_ns();
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
-                    if (TRACE) trace_entity(tr, id, g.mem, gn, now);
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
                     s.window_done = (int32_t)(seq + 1u + (uint32_t)gn) == w.ntasks ? 1 : 0;
                     __threadfence();
                 } else if (last && gn) {
@@ -246,9 +229,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
                     const uint32_t ev = (uint32_t)atomicAdd(&w.ctl->evt.v, (unsigned long long)gn);
                     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, (unsigned long long)gn);
                     for (int i = 0; i < gn; ++i) { w.end_seq[g.mem[i]] = ev + (uint32_t)i; w.retire_log[seq + (uint32_t)i] = g.mem[i]; }
-                    const unsigned long long now = globaltimer_ns();
-                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = now;
-                    if (TRACE) trace_entity(tr, id, g.mem, gn, now);
+                    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
                     s.window_done = (int32_t)(seq + (uint32_t)gn) == w.ntasks ? 1 : 0;
                     __threadfence();
                 } else if (last) {
@@ -256,9 +237,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
                     w.end_seq[id] = (uint32_t)atomicAdd(&w.ctl->evt.v, 1ull);
                     // the retire log is written before the out-edges are released, so that it is a linear
                     // extension of the DAG's partial order (a successor can only retire after us)
-                    unsigned long long now;
-                    s.window_done = retire_task(w, id, now) ? 1 : 0;
-                    if (TRACE) trace_entity(tr, id, nullptr, 0, now);
+                    s.window_done = retire_task(w, id) ? 1 : 0;
                     __threadfence();
                 }
             }

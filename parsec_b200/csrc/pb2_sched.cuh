@@ -342,28 +342,23 @@ static __device__ __noinline__ void push_written_tiles(const pb2_tile_t* tiles, 
     __syncthreads();
 }
 
-// One thread: append to the retire log; returns true when this was the last task of the window.  `when` gets the time
-// stamp stored as the watchdog's progress.
-__device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id, unsigned long long& when) {
+// One thread: append to the retire log and store the watchdog's progress; returns true when this was the last task of
+// the window.
+__device__ __forceinline__ bool retire_task(const WinDev& w, int32_t id) {
     const uint32_t seq = (uint32_t)atomicAdd(&w.ctl->retired.v, 1ull);
     w.retire_log[seq] = id;
-    when = globaltimer_ns();
-    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = when;
+    *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
     return (int32_t)(seq + 1) == w.ntasks;
 }
 
 // ---------------------------------------------------------------------------------------------
 // device time stamps of a traced window (pb2_engine_set_window_trace)
 // ---------------------------------------------------------------------------------------------
-// Per task of the run: t_start, t_end (%globaltimer, ns) and the SM.  A scheduling entity -- a task alone, a read group,
-// a fused producer with its group, a GEMM unit -- starts at the earliest pop of any of its parts and ends at the time
-// stamp its retiring part stores as the watchdog's progress; every task of the entity gets that interval and the SM of
-// the retiring part.  Only the TRACE instantiations of the window kernels touch these arrays (null in an untraced
-// window); the reset kernel starts t_start at ~0, the identity of the atomicMin of the pops.
 // Per ring entry of the run, the part record (pb2_part_trace_t) of the worker that ran it, at part_base[owner] + part;
-// the owner is the popped task of an HBM window, the unit of a GEMM window.  The host fills task, part and nparts.
+// the owner is the popped task of an HBM window, the unit of a GEMM window.  The host fills task, part and nparts, and
+// derives each entity's interval and SM from its parts' records (pb2_window_trace).  Only the TRACE instantiations of
+// the window kernels touch the records (null in an untraced window).
 struct TraceDev {
-    unsigned long long* t_start; unsigned long long* t_end; uint32_t* smid;
     pb2_part_trace_t* parts;          // nparts records, cleared by the reset kernel
     const int32_t* part_base;         // per ring-entry owner: its first record
     int32_t nparts;
@@ -382,18 +377,6 @@ __device__ __forceinline__ void trace_part(const TraceDev& tr, int32_t owner, in
     p->t_pop_ns = r.t_pop; p->t_in_ns = r.t_in; p->t_exec_ns = r.t_exec; p->t_out_ns = r.out_bytes ? r.t_out : r.t_exec;
     p->in_bytes = r.in_bytes; p->out_bytes = r.out_bytes;
     p->smid = smid(); p->flags = r.flags | (retired ? PB2_PART_RETIRED : 0u);
-}
-
-// One thread, right after it popped a part of the entity led by task `lead` at time t.
-__device__ __forceinline__ void trace_pop(const TraceDev& tr, int32_t lead, unsigned long long t) { atomicMin(&tr.t_start[lead], t); }
-
-// One thread of the retiring part: task `id` gets its entity's interval [t0, t_end] and the SM sm.
-__device__ __forceinline__ void trace_task(const TraceDev& tr, int32_t id, unsigned long long t0, unsigned long long t_end, uint32_t sm) {
-    tr.t_start[id] = t0; tr.t_end[id] = t_end; tr.smid[id] = sm;
-}
-// The start of the entity led by `lead`: every pop of its parts is ordered before its retirement (parts_left chain).
-__device__ __forceinline__ unsigned long long trace_start_of(const TraceDev& tr, int32_t lead) {
-    return *reinterpret_cast<volatile unsigned long long*>(&tr.t_start[lead]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -449,14 +432,13 @@ __device__ __forceinline__ StageCtx stage_ctx(const WinDev& w) {
     return StageCtx{w.tiles, w.ctl, w.slice_claim, w.slice_done, w.stage_mode == 0 ? 1 : 0, w.part_bytes};
 }
 
-// The stage-in helpers below are out of line.  Each has a COUNT form, called by the traced window kernels only, that
-// also adds the bytes the calling CTA moved to *moved (its PartSmem::in_bytes, thread 0): the untraced kernels keep the
-// helpers as they are.
+// The stage-in helpers below are out of line.  COUNT (the traced window kernels): thread 0 also adds the bytes the
+// calling CTA moved to *moved (its PartSmem::in_bytes); without it `moved` is not used.
 
 // Thread 0 decides (s_decide[0]): 1 = this CTA moves the tile, 0 = already valid (possibly after waiting)
 template <bool COUNT>
-__device__ __forceinline__ void stage_in_flow_impl(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk,
-                                                   unsigned long long* moved) {
+static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk,
+                                                  unsigned long long* moved) {
     if (threadIdx.x == 0) {
         int decide = 0;
         if ((access & PB2_FLOW_ACCESS_READ) && tile->src_kind == PB2_SRC_PUSH) {
@@ -490,14 +472,6 @@ __device__ __forceinline__ void stage_in_flow_impl(const StageCtx w, pb2_tile_t*
     }
     __syncthreads();
 }
-static __device__ __noinline__ void stage_in_flow(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk = nullptr) {
-    stage_in_flow_impl<false>(w, tile, access, s_decide, bulk, nullptr);
-}
-static __device__ __noinline__ void stage_in_flow_counted(const StageCtx w, pb2_tile_t* tile, uint8_t access, int* s_decide, BulkSmem* bulk,
-                                                          unsigned long long* moved) {
-    stage_in_flow_impl<true>(w, tile, access, s_decide, bulk, moved);
-}
-
 
 // Number of stage-in slices of a tile: the same rule pb2_window_create uses for the parts of a wide task.
 __device__ __forceinline__ int tile_slices_of(int32_t part_bytes, const uint32_t* slice_claim, uint32_t bytes) {
@@ -512,8 +486,8 @@ __device__ __forceinline__ int tile_slices(const WinDev& w, uint32_t bytes) { re
 // parallel instead of one CTA moving 4 MiB alone; a CTA that finds a slice claimed by someone else only waits
 // for it.  The worker whose slice completes the tile publishes PB2_TILE_VALID.
 template <bool COUNT>
-__device__ __forceinline__ void stage_in_slices_impl(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
-                                                     BulkSmem* bulk, unsigned long long* moved) {
+static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
+                                                    BulkSmem* bulk, unsigned long long* moved) {
     pb2_tile_t* tile = &w.tiles[tile_id];
     if (tile->src_kind == PB2_SRC_PUSH) {       // written by its producer (see stage_in_flow)
         if (threadIdx.x == 0) while (ld_acquire_sys(&tile->state) != PB2_TILE_VALID) __nanosleep(64);
@@ -555,13 +529,6 @@ __device__ __forceinline__ void stage_in_slices_impl(const StageCtx w, int32_t t
         __threadfence();
     }
     __syncthreads();
-}
-static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide, BulkSmem* bulk = nullptr) {
-    stage_in_slices_impl<false>(w, tile_id, nslices, s0, s1, s_decide, bulk, nullptr);
-}
-static __device__ __noinline__ void stage_in_slices_counted(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
-                                                            BulkSmem* bulk, unsigned long long* moved) {
-    stage_in_slices_impl<true>(w, tile_id, nslices, s0, s1, s_decide, bulk, moved);
 }
 
 }  // namespace pb2

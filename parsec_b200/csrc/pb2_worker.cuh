@@ -31,9 +31,9 @@ struct alignas(16) TaskSmem {
 // BULK: the calling kernel has a TMA bulk ring (without one the copies take the SIMT loops).  Each instantiation has
 // one caller kernel per translation unit: a second caller kernel makes ptxas give this helper the standard call ABI,
 // which costs the HBM kernels a stack frame and spills at their 80-register budget (see pb2_hbm.cuh).  COUNT (traced
-// kernels, stage_in_needed_flows_counted): add the bytes this CTA moved to *moved.
+// kernels): add the bytes this CTA moved to *moved.
 template <bool BULK, bool COUNT>
-__device__ __forceinline__ void stage_in_needed_flows_impl(const StageCtx c, TaskSmem* sp, BulkSmem* bulk, unsigned long long* moved) {
+static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, TaskSmem* sp, BulkSmem* bulk, unsigned long long* moved) {
     TaskSmem& s = *sp;
     const int need = s.need;
 #pragma unroll 1
@@ -43,23 +43,13 @@ __device__ __forceinline__ void stage_in_needed_flows_impl(const StageCtx c, Tas
         const uint32_t bytes = s.tbytes[f];
         const int ns = tile_slices_of(c.part_bytes, c.slice_claim, bytes);
         if (ns == 1) {
-            if (COUNT) stage_in_flow_counted(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr, moved);
-            else stage_in_flow(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr);
+            stage_in_flow<COUNT>(c, &c.tiles[tid], s.task.access[f], &s.decide, BULK ? bulk : nullptr, moved);
         } else {
             int s0, s1;
             slices_over(bytes, ns, s.off[f], s.args.bytes[f], s0, s1);     // the slices under this part's bytes
-            if (COUNT) stage_in_slices_counted(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr, moved);
-            else stage_in_slices(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr);
+            stage_in_slices<COUNT>(c, tid, ns, s0, s1, &s.decide, BULK ? bulk : nullptr, moved);
         }
     }
-}
-template <bool BULK>
-static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, TaskSmem* sp, BulkSmem* bulk) {
-    stage_in_needed_flows_impl<BULK, false>(c, sp, bulk, nullptr);
-}
-template <bool BULK>
-static __device__ __noinline__ void stage_in_needed_flows_counted(const StageCtx c, TaskSmem* sp, BulkSmem* bulk, unsigned long long* moved) {
-    stage_in_needed_flows_impl<BULK, true>(c, sp, bulk, moved);
 }
 
 // All threads.  On entry s.task holds the descriptor (published by a barrier).  exec() runs the body over s.args (all
@@ -103,10 +93,8 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     __syncthreads();
     // the cold path, out of line and called once: everything it needs is in shared memory, nothing of the caller's
     // has to survive the call in registers
-    if (TRACE) {
-        if (s.need) stage_in_needed_flows_counted<BULK>(stage_ctx(w), &s, bulk, &rec->in_bytes);
-        if (threadIdx.x == 0) { if (s.need) rec->flags |= PB2_PART_WAITED_INPUT; rec->t_in = globaltimer_ns(); }
-    } else if (s.need) stage_in_needed_flows<BULK>(stage_ctx(w), &s, bulk);
+    if (s.need) stage_in_needed_flows<BULK, TRACE>(stage_ctx(w), &s, bulk, TRACE ? &rec->in_bytes : nullptr);
+    if (TRACE && threadIdx.x == 0) { if (s.need) rec->flags |= PB2_PART_WAITED_INPUT; rec->t_in = globaltimer_ns(); }
 
     // ---- exec: the body (parsec_device_kernel_exec -> submit) ----
     const unsigned long long r = exec();

@@ -7,11 +7,11 @@ The same tasks then run as two windows of one engine, one created with window tr
 (reset_ms + kernel_ms, the quantity bench.py sums) are printed side by side: the difference is the cost of tracing.
 
 From the last traced run it prints
-  - span: the first pop to the last retirement (device clock);
-  - tail: the last pop to the last retirement;
+  - span: the first pop to the last entity's end (device clock);
+  - tail: the last pop to the last entity's end;
   - per SM, the busy fraction of the span: the union of the intervals that SM retired.  A task's interval is its
     scheduling entity's (a fused producer with its read group here), from the earliest pop of any of its parts to the
-    retirement of the last one, so an entity cut into parts counts on the SM that retired it;
+    latest end of their pushouts, so an entity cut into parts counts on the SM that retired it;
 and writes the trace (one row per SM) to --out.  The card's name and power limit are read in the same run.
 
     python tools/trace_window.py --runs 30 --out trace_ex05.json
