@@ -9,18 +9,38 @@ CU_SRCS   := $(CSRC)/pb2_engine.cu $(CSRC)/pb2_engine_prio.cu $(CSRC)/pb2_engine
              $(CSRC)/pb2_stream.cu
 CPP_SRCS  := $(wildcard $(CSRC)/*.cpp)
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(wildcard $(CSRC)/*.hpp) $(wildcard include/*.h)
+# the HBM window kernel with application bodies: relocatable device code, linked at run time (pb2_engine_link_bodies)
+LINKED_CUBIN := build/pb2_engine_linked.cubin
+LINKED_OBJ   := build/pb2_linked_image.o
+# the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py), as a relocatable cubin and as PTX
+TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx
 
-all: $(LIB) oracle
+all: $(LIB) linked_bodies oracle
 
-$(LIB): $(CU_SRCS) $(CPP_SRCS) $(HDRS)
-	$(NVCC) $(NVCCFLAGS) -shared -o $@ $(CU_SRCS) $(CPP_SRCS) -Iinclude 2> build_ptxas.log || (cat build_ptxas.log; exit 1)
+$(LIB): $(CU_SRCS) $(CPP_SRCS) $(HDRS) $(LINKED_OBJ)
+	$(NVCC) $(NVCCFLAGS) -shared -o $@ $(CU_SRCS) $(CPP_SRCS) $(LINKED_OBJ) -Iinclude 2> build_ptxas.log || (cat build_ptxas.log; exit 1)
 	@grep -E "error|warning" build_ptxas.log | grep -v "ptxas info" || true
+
+$(LINKED_CUBIN): $(CSRC)/pb2_engine_linked.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_ptxas.log || (cat build/linked_ptxas.log; exit 1)
+
+$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN)
+	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -o $@ $<
+
+linked_bodies: $(TEST_BODIES)
+
+tests/cuda/linked_bodies.cubin: tests/cuda/linked_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -Iinclude -o $@ $<
+
+tests/cuda/linked_bodies.ptx: tests/cuda/linked_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
 
 oracle:
 	$(MAKE) -C oracle
 
 clean:
-	rm -f $(LIB) build_ptxas.log
+	rm -f $(LIB) build_ptxas.log $(LINKED_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log $(TEST_BODIES)
 	$(MAKE) -C oracle clean
 
-.PHONY: all oracle clean
+.PHONY: all linked_bodies oracle clean

@@ -70,6 +70,9 @@ enum pb2_body_e {
     PB2_BODY_GEMM_BF16  = 16, /* flow2 (C, M x N row-major bf16) += flow0 (A, M x K row-major) *
                                * flow1 (B, N x K row-major == K x N column-major), fp32 accumulate in registers
                                * iparam[0]=M, iparam[1]=N, iparam[2]=K (each tile edge)                     */
+    PB2_BODY_LINKED_0   = 20, /* .. PB2_BODY_LINKED_7: the application's device body, linked into the HBM window
+                               * kernel by pb2_engine_link_bodies (include/pb2_device_body.h); HBM windows only   */
+    PB2_BODY_LINKED_7   = 27,
     PB2_BODY_USER       = 31, /* host-side only: the chore is a user `submit` callback that enqueues its own CUDA work
                                * on a stream (device_gpu.h:49-51); such tasks never enter an engine window           */
     PB2_BODY_MAX        = 32
@@ -253,10 +256,29 @@ int  pb2_engine_set_window_trace(pb2_engine_t* engine, int on);
  * slices of this size and every worker that needs the tile pulls the slices nobody has claimed yet */
 int  pb2_engine_set_stage_slice_bytes(pb2_engine_t* engine, int32_t bytes);
 
+/* --- application device bodies (include/pb2_device_body.h) ---
+ * Link `image` -- PTX (PB2_IMAGE_PTX, text, compiled with -rdc=true) or a relocatable sm_90a cubin (PB2_IMAGE_CUBIN) that
+ * defines pb2_linked_body -- into the engine's relocatable build of the HBM window kernel, with the driver's JIT linker.
+ * Afterwards HBM windows (kind 0) whose tasks name PB2_BODY_LINKED_0 .. _7 run the linked kernel; every other window runs
+ * the built-in kernels as before.  Bit i of `sliceable` lets the engine cut the tasks of body PB2_BODY_LINKED_0 + i into
+ * byte-slice parts (pb2_engine_params_t::part_bytes); a clear bit runs them as one part over whole tiles.
+ * PB2_ERR_BAD_PARAM for a NULL or empty image, an unknown format, mask bits above bit 7, or a link error (the linker's
+ * log is in pb2_engine_last_error); PB2_ERR_EXISTS when the engine has linked an image already (once per engine). */
+#define PB2_IMAGE_PTX   1
+#define PB2_IMAGE_CUBIN 2
+int  pb2_engine_link_bodies(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable);
+/* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill
+ * and stack) bytes per thread, static shared memory per CTA, and the workers a linked window runs (the engine's HBM
+ * worker count, or fewer when the linked kernel's occupancy allows fewer).  Any pointer may be NULL.
+ * PB2_ERR_NOT_FOUND before pb2_engine_link_bodies. */
+int  pb2_engine_linked_info(pb2_engine_t* engine, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers);
+
 /* --- one window of the DAG ---
  * tasks[ntasks], succ[nsucc] (CSR via succ_begin/succ_count), tiles[ntiles] and the ids of
  * the tasks that are ready at submission (startup tasks, parsec.c:1724-1740).
- * 'kind' selects the kernel instantiation: 0 = HBM bodies, 1 = tensor-core GEMM bodies. */
+ * 'kind' selects the kernel instantiation: 0 = HBM bodies, 1 = tensor-core GEMM bodies.  An HBM window with a task of
+ * a linked body (PB2_BODY_LINKED_0 .. _7) runs the engine's linked kernel (pb2_engine_link_bodies); such a task in a
+ * GEMM window, in a shared window or on an engine without an image is refused (PB2_ERR_NOT_SUPPORTED). */
 int  pb2_window_create(pb2_engine_t* engine, pb2_window_t** window, int kind,
                        const pb2_task_t* tasks, int32_t ntasks,
                        const uint32_t* succ, int32_t nsucc,

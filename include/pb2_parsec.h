@@ -148,6 +148,12 @@ int  pb2_mca_device_registration_complete(pb2_context_t* ctx);
 int  pb2_nb_devices(pb2_context_t* ctx);
 pb2_device_module_t* pb2_mca_device_get(pb2_context_t* ctx, int device_index);
 int  pb2_device_get_stats(pb2_device_module_t* dev, pb2_device_stats_t* stats);
+/* Link the application's device bodies into the module's engine (pb2_engine_link_bodies: image, format, sliceable as
+ * there), before the module's first window.  Afterwards DTD chores may name PB2_BODY_LINKED_0 .. _7 once every GPU
+ * module of the context has linked an image, and the module's windows run those tasks in the linked HBM kernel; a window
+ * never holds both GEMM tasks and linked-body tasks.  A dry-run module checks the arguments and records the link.
+ * PB2_ERR_EXISTS for a second image, PB2_ERR_NOT_SUPPORTED after the module's first window. */
+int  pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes
  * required in / moved H2D and D2D (with the percentage of "required"), bytes required out / written back, evictions --
  * plus the engine's own columns (windows launched, successors released by the device).  Writes a NUL-terminated

@@ -39,6 +39,9 @@ ACCESS_NONE, ACCESS_READ, ACCESS_WRITE, ACCESS_RW, FLOW_PUSHOUT = 0x00, 0x04, 0x
 BODY_NOP, BODY_FILL_I32, BODY_CHECK_I32, BODY_INCR_I32, BODY_ADD_IOTA_I32 = 0, 1, 2, 3, 4
 BODY_SCALE_I32, BODY_IOTA_I32, BODY_COPY, BODY_FILL_F32, BODY_CHECK_F32 = 5, 6, 7, 8, 9
 BODY_INCR_F32, BODY_AXPY_F32, BODY_MEMSET_U8, BODY_ADD_AT_I32, BODY_GEMM_BF16 = 10, 11, 12, 13, 16
+# application device bodies linked into HBM windows (pb2_engine_link_bodies): BODY_LINKED_0 + i, i < 8
+BODY_LINKED_0, BODY_LINKED_7 = 20, 27
+IMAGE_PTX, IMAGE_CUBIN = 1, 2
 
 TASK_DEPS_MASK = 0x01
 TILE_INVALID, TILE_STAGING, TILE_VALID = 0, 1, 2
@@ -68,6 +71,13 @@ PART_TRACE_DTYPE = np.dtype([
     ("smid", "<u4"), ("flags", "<u4"),
 ], align=False)
 assert PART_TRACE_DTYPE.itemsize == 64
+
+# numpy mirror of pb2_body_args_t (include/pb2_device_body.h), what a linked body is handed: 72 bytes
+BODY_ARGS_DTYPE = np.dtype([
+    ("flow", "<u8", (4,)), ("bytes", "<u4", (4,)), ("elem0", "<u4"), ("part", "<u4"),
+    ("iparam", "<i4", (3,)), ("fparam", "<f4"),
+], align=True)
+assert BODY_ARGS_DTYPE.itemsize == 72
 
 
 def succ_make(task, flow=0):
@@ -128,6 +138,7 @@ ENGINE_SYMBOLS = [
     "pb2_window_results", "pb2_window_trace", "pb2_window_part_trace",
     "pb2_partition_create", "pb2_partition_sizes", "pb2_partition_get", "pb2_partition_destroy", "pb2_partition_error",
     "pb2_partition_set_push", "pb2_partition_push_count", "pb2_partition_get_push", "pb2_window_set_push",
+    "pb2_engine_link_bodies", "pb2_engine_linked_info",
 ]
 
 
@@ -170,6 +181,8 @@ def load():
     lib.pb2_window_trace.argtypes = [vp, vp, vp, vp, vp]
     lib.pb2_window_part_trace.argtypes = [vp, vp, i32, P(i32)]
     lib.pb2_engine_set_stage_slice_bytes.argtypes = [vp, i32]
+    lib.pb2_engine_link_bodies.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32]
+    lib.pb2_engine_linked_info.argtypes = [vp, P(i32), P(i32), P(i32), P(i32)]
     lib.pb2_window_export.argtypes = [vp, vp]
     lib.pb2_window_set_remote.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32]
     lib.pb2_partition_set_push.argtypes = [vp, C.c_int]

@@ -13,7 +13,9 @@
 //   contrib/build_with_parsec/write_check.cu:7-35,
 //   tests/runtime/cuda/get_best_device_check.jdf:82.
 #pragma once
+#include <stddef.h>
 #include "pb2_dev_utils.cuh"
+#include "../../include/pb2_device_body.h"
 
 namespace pb2 {
 
@@ -208,6 +210,13 @@ struct BodyArgs {
     int32_t  iparam[3];
     float    fparam;
 };
+// linked bodies (include/pb2_device_body.h) are handed TaskSmem::args as a pb2_body_args_t
+static_assert(sizeof(BodyArgs) == sizeof(pb2_body_args_t) && alignof(BodyArgs) == alignof(pb2_body_args_t) &&
+              offsetof(BodyArgs, bytes) == offsetof(pb2_body_args_t, bytes) &&
+              offsetof(BodyArgs, elem0) == offsetof(pb2_body_args_t, elem0) &&
+              offsetof(BodyArgs, part) == offsetof(pb2_body_args_t, part) &&
+              offsetof(BodyArgs, iparam) == offsetof(pb2_body_args_t, iparam) &&
+              offsetof(BodyArgs, fparam) == offsetof(pb2_body_args_t, fparam), "BodyArgs and pb2_body_args_t differ");
 
 // Returns the body result (only meaningful in thread 0): CHECK -> (mismatches << 32) | first element bits.
 // CHECKED: the checked form of a producer that runs with its read group as one unit (run_fused_part, pb2_hbm.cuh).  The

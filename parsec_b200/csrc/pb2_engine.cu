@@ -25,6 +25,7 @@
 #include <map>
 #include <algorithm>
 #include <functional>
+#include <type_traits>
 
 #include "../../include/pb2_engine.h"
 #include "pb2_sched.cuh"
@@ -131,6 +132,7 @@ struct pb2_window_s {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
     bool launched = false;
     bool shared = false;
+    bool linked = false;                // a task names a linked body: the window runs the engine's linked kernel
     // The per-run state by copy.  pb2_window_create fixes ncopies: 2 for a non-shared HBM window with tasks, else 1
     // (DESIGN.md §5).  Copy 0 is allocated at create, copy 1 at the second arm.  Consecutive runs alternate between
     // the copies, and while a run runs, the reset kernel arms the other copy for the next one on the engine's arm
@@ -201,6 +203,13 @@ static int validate_window(pb2_engine_t* e, int kind, const pb2_task_t* tasks, i
         if (t.body >= PB2_BODY_MAX || t.body == PB2_BODY_USER) { e->last_error = "unknown body id"; return PB2_ERR_BAD_PARAM; }
         if (kind == 0 && t.body == PB2_BODY_GEMM_BF16) {
             e->last_error = "GEMM body in an HBM-kind window (use kind 1)"; return PB2_ERR_BAD_PARAM; }
+        if (is_linked_body(t.body)) {
+            const char* why = kind != 0 ? "linked body in a GEMM window (linked bodies run in HBM windows only)"
+                            : e->shared_windows ? "linked body in a shared window (not supported)"
+                            : !e->linked_module ? "linked body id, but the engine has not linked an image (pb2_engine_link_bodies)"
+                            : nullptr;
+            if (why) { e->last_error = why; return PB2_ERR_NOT_SUPPORTED; }
+        }
     }
     for (int32_t i = 0; i < nsucc; ++i)
         if (PB2_SUCC_TASK(succ[i]) >= ntasks) { e->last_error = "successor id out of bounds"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
@@ -560,7 +569,10 @@ static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, con
     uint32_t extra_parts = 0;
     w->task_entry.resize((size_t)ntasks);
     for (int32_t i = 0; i < ntasks; ++i) {
-        const int np = task_parts(dtasks[(size_t)i], [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
+        // a linked body whose sliceable bit is clear runs over whole tiles (a stencil reads its neighbours' tiles)
+        const pb2_task_t& t = dtasks[(size_t)i];
+        const bool whole = is_linked_body(t.body) && !((e->linked_sliceable >> (t.body - PB2_BODY_LINKED_0)) & 1u);
+        const int np = whole ? 1 : task_parts(t, [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
         nparts[(size_t)i] = (uint16_t)np; extra_parts += (uint32_t)np - 1;
         w->task_entry[(size_t)i] = PB2_ENT_MAKE(i, np - 1);
     }
@@ -676,7 +688,141 @@ static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out
     return PB2_SUCCESS;
 }
 
+// ---------------------------------------------------------------------------------------------
+// linked bodies: the relocatable linked kernels (pb2_engine_linked.cu, embedded by pb2_linked_image.S) + the
+// application's image, linked by the driver's JIT linker
+// ---------------------------------------------------------------------------------------------
+extern "C" const unsigned char pb2_linked_engine_image[], pb2_linked_engine_image_end[];
+
+// pb2_engine_hbm_kernel<PRIO, TRACE, true> by (PRIO) + 2 * (TRACE)
+static const char* const kLinkedKernels[4] = {
+    "_ZN3pb221pb2_engine_hbm_kernelILb0ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
+    "_ZN3pb221pb2_engine_hbm_kernelILb1ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
+    "_ZN3pb221pb2_engine_hbm_kernelILb0ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
+    "_ZN3pb221pb2_engine_hbm_kernelILb1ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
+};
+
+// The driver calls the linking point needs, fetched through the runtime (as cuTensorMapEncodeTiled is): the library
+// gains no link dependency on libcuda.
+struct DriverLink {
+    decltype(&cuLinkCreate) link_create = nullptr;
+    decltype(&cuLinkAddData) link_add = nullptr;
+    decltype(&cuLinkComplete) link_complete = nullptr;
+    decltype(&cuLinkDestroy) link_destroy = nullptr;
+    decltype(&cuModuleLoadData) module_load = nullptr;
+    decltype(&cuModuleUnload) module_unload = nullptr;
+    decltype(&cuModuleGetFunction) get_function = nullptr;
+    decltype(&cuFuncGetAttribute) func_attr = nullptr;
+    decltype(&cuOccupancyMaxActiveBlocksPerMultiprocessor) occupancy = nullptr;
+    decltype(&cuLaunchKernel) launch = nullptr;
+    bool complete() const {
+        return link_create && link_add && link_complete && link_destroy && module_load && module_unload && get_function &&
+               func_attr && occupancy && launch;
+    }
+};
+
+static const DriverLink& driver_link() {
+    static const DriverLink d = [] {
+        DriverLink r;
+        auto get = [](const char* name, auto& fn) {
+            void* p = nullptr;
+            cudaDriverEntryPointQueryResult q;
+            if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+                fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(p);
+        };
+        get("cuLinkCreate", r.link_create); get("cuLinkAddData", r.link_add); get("cuLinkComplete", r.link_complete);
+        get("cuLinkDestroy", r.link_destroy); get("cuModuleLoadData", r.module_load); get("cuModuleUnload", r.module_unload);
+        get("cuModuleGetFunction", r.get_function); get("cuFuncGetAttribute", r.func_attr);
+        get("cuOccupancyMaxActiveBlocksPerMultiprocessor", r.occupancy); get("cuLaunchKernel", r.launch);
+        return r;
+    }();
+    return d;
+}
+
+// The linked kernel of a window's queue policy and trace on the engine stream, with the linked worker count.
+static int launch_linked(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool trace) {
+    const int i = (lanes ? 1 : 0) + (trace ? 2 : 0);
+    WinDev wd = g.w;
+    TraceDev tr = trace ? g.trace : TraceDev{};
+    void* args[] = {&wd, &tr};
+    const CUresult r = driver_link().launch(e->linked_fn[i], (unsigned)e->linked_nworkers[i], 1, 1, (unsigned)e->params.threads, 1, 1,
+                                            0, reinterpret_cast<CUstream>(e->stream), args, nullptr);
+    if (r != CUDA_SUCCESS) { e->last_error = "cuLaunchKernel of the linked HBM window kernel failed (CUresult " + std::to_string((int)r) + ")"; return PB2_ERR_DEVICE; }
+    return PB2_SUCCESS;
+}
+
 extern "C" {
+
+int pb2_engine_link_bodies(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    if (const char* why = link_args_error(image, bytes, format, sliceable)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
+    const DriverLink& d = driver_link();
+    if (!d.complete()) { e->last_error = "the driver's JIT linker entry points are not available"; return PB2_ERR_NOT_SUPPORTED; }
+    PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    PB2_CUDA(e, cudaFree(nullptr));             // the device's primary context is current: the module is loaded into it
+    std::vector<char> err(16384, 0), info(16384, 0);
+    CUjit_option opt[] = {CU_JIT_ERROR_LOG_BUFFER, CU_JIT_ERROR_LOG_BUFFER_SIZE_BYTES, CU_JIT_INFO_LOG_BUFFER,
+                          CU_JIT_INFO_LOG_BUFFER_SIZE_BYTES, CU_JIT_TARGET};
+    void* val[] = {err.data(), reinterpret_cast<void*>((uintptr_t)err.size()), info.data(), reinterpret_cast<void*>((uintptr_t)info.size()),
+                   reinterpret_cast<void*>((uintptr_t)CU_TARGET_COMPUTE_90A)};
+    std::string ptx;                             // the JIT wants PTX NUL-terminated
+    const void* data = image;
+    size_t size = bytes;
+    if (format == PB2_IMAGE_PTX) { ptx.assign(static_cast<const char*>(image), bytes); data = ptx.c_str(); size = ptx.size() + 1; }
+    CUlinkState st = nullptr;
+    CUmodule mod = nullptr;
+    CUresult r = d.link_create(5, opt, val, &st);
+    if (r == CUDA_SUCCESS)
+        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(pb2_linked_engine_image),
+                       (size_t)(pb2_linked_engine_image_end - pb2_linked_engine_image), "pb2_engine_linked.cubin", 0, nullptr, nullptr);
+    if (r == CUDA_SUCCESS)
+        r = d.link_add(st, format == PB2_IMAGE_PTX ? CU_JIT_INPUT_PTX : CU_JIT_INPUT_CUBIN, const_cast<void*>(data), size,
+                       "linked bodies", 0, nullptr, nullptr);
+    void* out = nullptr;
+    size_t out_bytes = 0;
+    if (r == CUDA_SUCCESS) r = d.link_complete(st, &out, &out_bytes);
+    if (r == CUDA_SUCCESS) r = d.module_load(&mod, out);      // out belongs to the link state: load before destroying it
+    if (st) d.link_destroy(st);
+    if (r != CUDA_SUCCESS) {
+        e->last_error = "linking the application's bodies failed (CUresult " + std::to_string((int)r) + "): " + err.data();
+        return PB2_ERR_BAD_PARAM;
+    }
+    CUfunction fn[4] = {};
+    int nw[4] = {};
+    for (int i = 0; i < 4 && r == CUDA_SUCCESS; ++i) {
+        int occ = 0;
+        r = d.get_function(&fn[i], mod, kLinkedKernels[i]);
+        if (r == CUDA_SUCCESS) r = d.occupancy(&occ, fn[i], e->params.threads, 0);
+        nw[i] = std::max(1, std::min(e->nworkers, e->prop.multiProcessorCount * occ));
+    }
+    const int mine = e->params.queue_policy == 1 ? 1 : 0;
+    int regs = 0, local = 0, smem = 0;
+    if (r == CUDA_SUCCESS) r = d.func_attr(&regs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn[mine]);
+    if (r == CUDA_SUCCESS) r = d.func_attr(&local, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn[mine]);
+    if (r == CUDA_SUCCESS) r = d.func_attr(&smem, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, fn[mine]);
+    if (r != CUDA_SUCCESS) {
+        d.module_unload(mod);
+        e->last_error = "the linked module has no usable HBM window kernel (CUresult " + std::to_string((int)r) + ")";
+        return PB2_ERR_DEVICE;
+    }
+    e->linked_module = mod;
+    for (int i = 0; i < 4; ++i) { e->linked_fn[i] = fn[i]; e->linked_nworkers[i] = nw[i]; }
+    e->linked_regs = regs; e->linked_local = local; e->linked_smem = smem;
+    e->linked_sliceable = sliceable;
+    return PB2_SUCCESS;
+}
+
+int pb2_engine_linked_info(pb2_engine_t* e, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    if (!e->linked_module) { e->last_error = "the engine has not linked an image (pb2_engine_link_bodies)"; return PB2_ERR_NOT_FOUND; }
+    if (regs) *regs = e->linked_regs;
+    if (local_bytes) *local_bytes = e->linked_local;
+    if (static_smem) *static_smem = e->linked_smem;
+    if (nworkers) *nworkers = e->linked_nworkers[e->params.queue_policy == 1 ? 1 : 0];
+    return PB2_SUCCESS;
+}
 
 int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_params_t* params) {
     if (!engine) return PB2_ERR_BAD_PARAM;
@@ -744,6 +890,7 @@ int pb2_engine_destroy(pb2_engine_t* e) {
     if (e->dma_stream) cudaStreamDestroy(e->dma_stream);
     if (e->arm_stream) cudaStreamDestroy(e->arm_stream);
     if (e->dma_ev) cudaEventDestroy(e->dma_ev);
+    if (e->linked_module) driver_link().module_unload(e->linked_module);
     delete e;
     return PB2_SUCCESS;
 }
@@ -991,7 +1138,7 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
 #define TRY(x) do { rc = (x); if (rc != PB2_SUCCESS) { pb2_window_destroy(w); return rc; } } while (0)
     WinDev& d = w->g.w;
     std::vector<pb2_task_t> dtasks(tasks, tasks + ntasks);
-    for (pb2_task_t& t : dtasks) t.flags &= 0x07;
+    for (pb2_task_t& t : dtasks) { t.flags &= 0x07; w->linked |= is_linked_body(t.body); }
     int32_t nlanes = 0;
     std::vector<uint8_t> task_lane;
     if (prio) task_lane = task_priority_lanes(tasks, ntasks, &nlanes);
@@ -1102,7 +1249,10 @@ int pb2_window_start(pb2_window_t* w) {
     if (w->ntasks > 0) {
         const Win2Dev g = run_desc(w, w->cur);
         const bool lanes = w->shape.lanes, trace = w->shape.trace;
-        if (w->kind == 0) {
+        if (w->kind == 0 && w->linked) {
+            const int rc = launch_linked(e, g, lanes, trace);
+            if (rc != PB2_SUCCESS) return rc;
+        } else if (w->kind == 0) {
             const int nw = e->nworkers, th = e->params.threads;
             if (trace) PB2_CUDA(e, lanes ? pb2_hbm_prio_trace_launch(g.w, g.trace, nw, th, e->stream)
                                          : pb2_hbm_trace_launch(g.w, g.trace, nw, th, e->stream));

@@ -1,6 +1,7 @@
 // pb2_engine_priv.hpp -- host-side engine object, part and slice rules shared by the translation units of libparsec_b200.so
 // (pb2_engine.cu: windows; pb2_stream.cu: the streaming ring + persistent kernel).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <map>
@@ -29,7 +30,25 @@ struct pb2_engine_s {
     bool window_trace = false;           // windows created from now on record per-task device time stamps
     const int32_t* next_rs_begin = nullptr;   // remote out-degree CSR of the next shared window (not owned)
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
+    // pb2_engine_link_bodies: the module of the linked HBM window kernels, each kernel and its worker count by
+    // (queue_policy 1) + 2 * (trace), what the linker made of the untraced one of this engine's policy, and which
+    // linked body ids may be cut into parts (bit i: PB2_BODY_LINKED_0 + i)
+    CUmodule linked_module = nullptr;
+    CUfunction linked_fn[4] = {};
+    int linked_nworkers[4] = {};
+    int32_t linked_regs = 0, linked_local = 0, linked_smem = 0;
+    uint32_t linked_sliceable = 0;
 };
+
+static inline bool is_linked_body(int body) { return body >= PB2_BODY_LINKED_0 && body <= PB2_BODY_LINKED_7; }
+
+// The argument check of pb2_engine_link_bodies and pb2_device_link_bodies: nullptr, or why the arguments are refused.
+static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable) {
+    if (!image || !bytes) return "linked body image is NULL or empty";
+    if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
+    if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";
+    return nullptr;
+}
 
 // part_bytes of engines and streams whose parameters leave it 0
 constexpr int32_t kDefaultPartBytes = 256 * 1024;

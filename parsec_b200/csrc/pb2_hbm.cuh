@@ -113,9 +113,14 @@ static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, G
     return r;
 }
 
+__device__ __forceinline__ bool linked_body_id(int body) { return body >= PB2_BODY_LINKED_0 && body <= PB2_BODY_LINKED_7; }
+
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
 // TRACE: write a record of every part into tr (PartSmem, then trace_part); the untraced instantiations never touch tr.
-template <bool PRIO, bool TRACE>
+// LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body (include/pb2_device_body.h); built
+// only in pb2_engine_linked.cu, as relocatable device code that pb2_engine_link_bodies links with the application's
+// image.  The other instantiations compile as if the flag did not exist.
+template <bool PRIO, bool TRACE, bool LINKED = false>
 __global__ void __launch_bounds__(PB2_HBM_THREADS, PB2_HBM_MINB)
 pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
     __shared__ TaskSmem s;
@@ -176,6 +181,10 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         __syncthreads();
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
+            if constexpr (LINKED) {
+                if (linked_body_id(s.task.body))
+                    return (unsigned long long)pb2_linked_body(s.task.body, reinterpret_cast<const pb2_body_args_t*>(&s.args), s.red);
+            }
             return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         }, rec);
         if (g.n && !g.fused) {

@@ -191,6 +191,7 @@ struct pb2_device_module_s {
     int major = 0, minor = 0;
     bool dry_run = false;
     bool trace = false;                      // device_engine_trace at init: windows are created traced
+    bool linked = false;                     // pb2_device_link_bodies: windows may run linked bodies
     pb2_engine_t* engine = nullptr;
     std::deque<void*> inflight;              // windows launched and not yet retired (oldest first), pb2_runtime.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up

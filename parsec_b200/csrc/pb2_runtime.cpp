@@ -11,6 +11,7 @@
 #include <stdio.h>
 
 #include "pb2_internal.hpp"
+#include "pb2_engine_priv.hpp"
 
 static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 static const bool g_timing = getenv("PB2_TIMING") != nullptr;
@@ -372,6 +373,20 @@ int pb2_nb_devices(pb2_context_t* ctx) { return ctx ? (int)ctx->devices.size() :
 pb2_device_module_t* pb2_mca_device_get(pb2_context_t* ctx, int idx) {
     return (ctx && idx >= 0 && idx < (int)ctx->devices.size()) ? ctx->devices[idx] : nullptr;
 }
+int pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable) {
+    if (!dev || !PB2_DEV_IS_GPU(dev->type)) return PB2_ERR_BAD_PARAM;
+    pb2_context_t* ctx = dev->ctx;
+    if (const char* why = link_args_error(image, bytes, format, sliceable)) { ctx->last_error = why; return PB2_ERR_BAD_PARAM; }
+    if (dev->linked) { ctx->last_error = "the module has linked an image already (one per module)"; return PB2_ERR_EXISTS; }
+    if (dev->st.windows_launched) { ctx->last_error = "linked bodies must be linked before the module's first window"; return PB2_ERR_NOT_SUPPORTED; }
+    if (!dev->dry_run) {
+        const int rc = pb2_engine_link_bodies(dev->engine, image, bytes, format, sliceable);
+        if (rc != PB2_SUCCESS) { ctx->last_error = pb2_engine_last_error(dev->engine); return rc; }
+    }
+    dev->linked = true;
+    return PB2_SUCCESS;
+}
+
 int pb2_device_get_stats(pb2_device_module_t* dev, pb2_device_stats_t* st) { if (!dev || !st) return PB2_ERR_BAD_PARAM; *st = dev->st; return PB2_SUCCESS; }
 static void best_unit(uint64_t bytes, double* v, const char** unit) {       // parsec_compute_best_unit: 1024-based
     static const char* units[] = {"B", "KB", "MB", "GB", "TB", "PB"};
@@ -935,12 +950,21 @@ static bool predicted_on_device(pb2_device_module_t* dev, pb2_htask_t* s) {
 // Build the dependency-closed window reachable from the pending tasks of one taskpool.  An engine window takes tile
 // GEMMs and HBM bodies together, so that a GEMM chain and the element-wise tasks around it are released on the device
 // instead of through the host; its kind is decided by the closure: 1 (the GEMM kernel, which also runs HBM bodies) when
-// it holds a GEMM task, else 0.  User submit tasks never mix with engine tasks.
+// it holds a GEMM task, else 0.  User submit tasks never mix with engine tasks, and tasks of linked bodies (which run in
+// the linked HBM kernel only) never mix with GEMM tasks: the first of the two kinds the closure takes in keeps the other
+// out of this window.
 static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu_task_t*>& taken, size_t max_roots) {
     if (dev->pending.empty()) return PB2_SUCCESS;
     w.tp = dev->pending.front()->ec->tp;
     const bool want_user = dev->pending.front()->ec->body == PB2_BODY_USER;      // the host-driven stream lane
-    auto fits = [&](const pb2_htask_t* t) { return (t->body == PB2_BODY_USER) == want_user; };
+    int engine_side = 0;                        // PB2_BODY_GEMM_BF16 or PB2_BODY_LINKED_0 once the window holds one
+    auto fits = [&](const pb2_htask_t* t) {
+        if ((t->body == PB2_BODY_USER) != want_user) return false;
+        const int side = t->body == PB2_BODY_GEMM_BF16 ? PB2_BODY_GEMM_BF16 : is_linked_body(t->body) ? PB2_BODY_LINKED_0 : 0;
+        if (side && engine_side && side != engine_side) return false;
+        if (side) engine_side = side;
+        return true;
+    };
     bool has_gemm = false;
     std::deque<pb2_htask_t*> queue;
     std::deque<pb2_gpu_task_t*> keep;

@@ -167,6 +167,20 @@ class Engine:
         """Windows created from now on record per-task device time stamps (Window.trace)."""
         _check(self._lib.pb2_engine_set_window_trace(self._h, 1 if on else 0), "set_window_trace", self)
 
+    def link_bodies(self, image, format, sliceable=0):
+        """Link the application's device bodies (include/pb2_device_body.h) into this engine's HBM window kernel, once:
+        image is PTX text (format L.IMAGE_PTX) or a relocatable sm_90a cubin (L.IMAGE_CUBIN), as bytes; bit i of
+        sliceable lets tasks of body L.BODY_LINKED_0 + i be cut into byte-slice parts."""
+        image = bytes(image)
+        _check(self._lib.pb2_engine_link_bodies(self._h, image, len(image), format, sliceable), "pb2_engine_link_bodies", self)
+
+    def linked_info(self):
+        """What the linker made of the linked kernel: registers and local bytes per thread, static shared memory per
+        CTA, and the workers a linked window runs."""
+        v = [C.c_int32() for _ in range(4)]
+        _check(self._lib.pb2_engine_linked_info(self._h, *[C.byref(x) for x in v]), "pb2_engine_linked_info", self)
+        return dict(zip(("regs", "local_bytes", "static_smem", "nworkers"), (x.value for x in v)))
+
     def ipc_export(self, dev_ptr):
         h = (C.c_ubyte * 64)()
         _check(self._lib.pb2_engine_ipc_export(self._h, C.c_void_p(dev_ptr), h), "ipc_export", self)
