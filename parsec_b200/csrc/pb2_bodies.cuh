@@ -223,7 +223,7 @@ static_assert(sizeof(BodyArgs) == sizeof(pb2_body_args_t) && alignof(BodyArgs) =
 // body writes its output flow (flow 1 for COPY and AXPY, else flow 0) as the unchecked form does, through ck: each
 // thread ORs (element ^ ck->k) of every whole 4-byte element it stores into ck->diff (a byte tail, MEMSET's or COPY's,
 // is stored but not checked, as cta_xor_scan does not check it).  Bodies without a checked form (NOP, CHECK, ADD_AT)
-// return ~0 there; form_read_groups fuses none of them.
+// return ~0 there; form_read_groups (pb2_window_plan.cpp) fuses none of them.
 template <bool CHECKED = false>
 __device__ __forceinline__ uint64_t run_hbm_body(int body, const BodyArgs& a, uint32_t* red_smem, Checked* ck = nullptr) {
     switch (body) {

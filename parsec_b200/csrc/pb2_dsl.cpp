@@ -214,7 +214,7 @@ int pb2_dtd_task_class_add_chore(pb2_taskpool_t* tp, pb2_task_class_t* tc, int d
     if (!tp || !tc) return PB2_ERR_BAD_PARAM;
     if (device_type & PB2_DEV_CUDA) {
         if (body < 0 || body >= PB2_BODY_MAX) return PB2_ERR_BAD_PARAM;
-        if (is_linked_body(body))
+        if (pb2::is_linked_body(body))
             for (auto* d : tp->ctx->devices)
                 if (PB2_DEV_IS_GPU(d->type) && !d->linked) {
                     tp->ctx->last_error = "linked body chore, but a GPU module has not linked an image (pb2_device_link_bodies)";

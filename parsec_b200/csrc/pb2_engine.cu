@@ -24,7 +24,6 @@
 #include <mutex>
 #include <map>
 #include <algorithm>
-#include <functional>
 #include <type_traits>
 
 #include "../../include/pb2_engine.h"
@@ -96,6 +95,7 @@ pb2_copy_batch_kernel(const CopyDesc* __restrict__ d, int32_t n) {
 using namespace pb2;
 
 #include "pb2_engine_priv.hpp"
+#include "pb2_window_plan.hpp"
 
 // One copy of a window's per-run state: exactly the arrays that rearm_run and pb2_window_reset_kernel write.  alloc_run
 // allocates them and run_desc puts them into a launch descriptor; no other host code names them.
@@ -107,18 +107,6 @@ struct RunState {
     Lanes* lanes;                         // RunShape::lanes
     int32_t* udep; int32_t* unit_parts_left;        // GEMM windows: the units' dependency words and part counts
     pb2_part_trace_t* parts;              // RunShape::trace: part_records of them (TraceDev)
-};
-
-// What every copy of a window's per-run state is sized from besides ntasks and ntiles, recorded by pb2_window_create.
-struct RunShape {
-    uint32_t ring = 0;                    // ring slots, a power of two
-    int32_t nunits = 0;                   // GEMM windows: units
-    bool parts = false;                   // per-task part counts (an HBM window with wide tasks)
-    bool claims = false;                  // stage-in is sliced: claim arrays per tile
-    bool lanes = false;                   // queue_policy 1: priority lanes, which start as lane_image
-    bool trace = false;                   // part records (pb2_engine_set_window_trace)
-    int32_t part_records = 0;             // trace: one part record per ring entry of a run
-    Lanes lane_image{};
 };
 
 struct pb2_window_s {
@@ -143,24 +131,11 @@ struct pb2_window_s {
     cudaEvent_t ev_arm = nullptr;
     std::vector<int32_t> task_entry;          // per task: its ring entry with (parts - 1) in the part field
     std::vector<int32_t> task_unit;           // traced windows, per task: the task that leads its scheduling entity
-    struct PartEntity { int32_t lead, base, nparts; };
     std::vector<PartEntity> part_entities;   // traced windows: the ring-entry owners by leading task, their records
     std::vector<void*> allocs;
     std::vector<void*> peer_ptrs;
     std::vector<pb2_tile_t*> peer_tiles;     // per rank: its tile table as mapped here (nullptr: none / self)
     std::vector<int32_t> peer_ntiles;
-};
-
-// What the plan of a window kind (plan_hbm_window, build_gemm2_units) hands to pb2_window_create.  An entry owner is a
-// task of an HBM window or a unit of a GEMM window.
-struct WindowPlan {
-    std::vector<int32_t> entries;         // the initial ready-ring entries, in FIFO order
-    std::vector<int32_t> entry_owner;     // the owner of each of them
-    std::vector<uint8_t> owner_lane;      // queue_policy 1: per owner, its lane
-    std::vector<uint32_t> owner_pushes;   // queue_policy 1: per owner, the entries it can ever push
-    uint32_t ring_slots = 0;              // ring slots the window needs besides the workers' slack
-    int32_t slice_bytes = 0;              // stage-in slice size (WinDev::part_bytes)
-    RunShape run;                         // the per-run state's needs (its ring size is set by pb2_window_create)
 };
 
 // n T (at least one) for window w on `stream`, freed by pb2_window_destroy.
@@ -185,40 +160,6 @@ static int dev_alloc_copy(pb2_window_t* w, T** dptr, const T* host, size_t n) {
     return rc;
 }
 
-static int validate_window(pb2_engine_t* e, int kind, const pb2_task_t* tasks, int32_t ntasks,
-                           const uint32_t* succ, int32_t nsucc, int32_t ntiles,
-                           const int32_t* ready, int32_t nready) {
-    if (ntasks < 0 || nsucc < 0 || ntiles < 0 || nready < 0) return PB2_ERR_BAD_PARAM;
-    if (kind != 0 && kind != 1) { e->last_error = "window kind must be 0 (HBM bodies) or 1 (GEMM bodies)"; return PB2_ERR_BAD_PARAM; }
-    if (ntasks >= (1 << 27)) return PB2_ERR_VALUE_OUT_OF_BOUNDS;
-    // ready-ring entries of the HBM kernel carry the task id in 22 bits (PB2_ENT_MAKE: part << 22 | task)
-    if (kind == 0 && ntasks >= (1 << 22)) { e->last_error = "an HBM window holds at most 4194303 tasks (22-bit task id in the ready ring)"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-    for (int32_t i = 0; i < ntasks; ++i) {
-        const pb2_task_t& t = tasks[i];
-        if (t.nb_flows > PB2_MAX_FLOWS) { e->last_error = "task with more than PB2_MAX_FLOWS flows"; return PB2_ERR_BAD_PARAM; }
-        if (t.succ_count < 0 || t.succ_begin < 0 || (int64_t)t.succ_begin + t.succ_count > nsucc) {
-            e->last_error = "successor range out of bounds"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-        for (int f = 0; f < t.nb_flows; ++f)
-            if (t.tile[f] >= ntiles) { e->last_error = "tile id out of bounds"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-        if (t.body >= PB2_BODY_MAX || t.body == PB2_BODY_USER) { e->last_error = "unknown body id"; return PB2_ERR_BAD_PARAM; }
-        if (kind == 0 && t.body == PB2_BODY_GEMM_BF16) {
-            e->last_error = "GEMM body in an HBM-kind window (use kind 1)"; return PB2_ERR_BAD_PARAM; }
-        if (is_linked_body(t.body)) {
-            const char* why = kind != 0 ? "linked body in a GEMM window (linked bodies run in HBM windows only)"
-                            : e->shared_windows ? "linked body in a shared window (not supported)"
-                            : !e->linked_module ? "linked body id, but the engine has not linked an image (pb2_engine_link_bodies)"
-                            : nullptr;
-            if (why) { e->last_error = why; return PB2_ERR_NOT_SUPPORTED; }
-        }
-    }
-    for (int32_t i = 0; i < nsucc; ++i)
-        if (PB2_SUCC_TASK(succ[i]) >= ntasks) { e->last_error = "successor id out of bounds"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-    for (int32_t i = 0; i < nready; ++i)
-        if (ready[i] < 0 || ready[i] >= ntasks) { e->last_error = "ready id out of bounds"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-    return PB2_SUCCESS;
-}
-
-
 // One tensor map per tile used as a GEMM operand: global tensor [rows][inner] bf16, row pitch inner*2 bytes,
 // box {64 (inner, 128 bytes), 128 rows}, 128-byte swizzle: exactly the K-major SWIZZLE_128B smem layout the
 // wgmma descriptors in pb2_gemm.cuh describe.  OOB rows/columns of ragged tiles are zero-filled by TMA.
@@ -226,9 +167,9 @@ typedef CUresult (*pb2_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuin
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                         CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks,
-                             const pb2_tile_t* tiles, int32_t ntiles) {
-    pb2_engine_t* e = w->e;
+// The tensor maps of a GEMM window, one per tile (zero for a tile that is no operand), from the operand shapes of its plan.
+static int encode_tensor_maps(pb2_engine_t* e, const WindowPlan& plan, const pb2_tile_t* tiles, int32_t ntiles,
+                              std::vector<CUtensorMap>& maps) {
     static pb2_encode_tiled_fn encode = nullptr;
     if (!encode) {
         void* fn = nullptr;
@@ -237,29 +178,13 @@ static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
         if (!fn || q != cudaDriverEntryPointSuccess) { e->last_error = "cuTensorMapEncodeTiled not available"; return PB2_ERR_NOT_SUPPORTED; }
         encode = reinterpret_cast<pb2_encode_tiled_fn>(fn);
     }
-    std::vector<int32_t> rows(ntiles, 0), inner(ntiles, 0);
-    for (int32_t i = 0; i < ntasks; ++i) {
-        const pb2_task_t& t = tasks[i];
-        if (t.body != PB2_BODY_GEMM_BF16) continue;
-        if (t.nb_flows < 3 || t.tile[0] < 0 || t.tile[1] < 0 || t.tile[2] < 0) { e->last_error = "GEMM task needs 3 data flows"; return PB2_ERR_BAD_PARAM; }
-        const int M = t.iparam[0], N = t.iparam[1], K = t.iparam[2];
-        if (M <= 0 || N <= 0 || K <= 0 || (K % 8) || (N % 8)) { e->last_error = "GEMM tile: need M,N,K > 0, K % 8 == 0, N % 8 == 0"; return PB2_ERR_NOT_SUPPORTED; }
-        const int32_t need[2][2] = {{M, K}, {N, K}};
-        for (int f = 0; f < 2; ++f) {
-            const int32_t id = t.tile[f];
-            if (rows[id] == 0) { rows[id] = need[f][0]; inner[id] = need[f][1]; }
-            else if (rows[id] != need[f][0] || inner[id] != need[f][1]) { e->last_error = "tile used with two different operand shapes"; return PB2_ERR_NOT_SUPPORTED; }
-            if ((uint64_t)need[f][0] * need[f][1] * 2 > tiles[id].bytes) { e->last_error = "GEMM operand larger than its tile"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-        }
-        if ((uint64_t)M * N * 2 > tiles[t.tile[2]].bytes) { e->last_error = "GEMM C larger than its tile"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
-    }
-    std::vector<CUtensorMap> maps(ntiles ? ntiles : 1);
+    maps.resize(ntiles ? ntiles : 1);
     memset(maps.data(), 0, maps.size() * sizeof(CUtensorMap));
     for (int32_t i = 0; i < ntiles; ++i) {
-        if (rows[i] == 0) continue;
-        if ((uintptr_t)tiles[i].dev_ptr & 15) { e->last_error = "GEMM tile not 16-byte aligned"; return PB2_ERR_BAD_PARAM; }
-        cuuint64_t gdim[2] = {(cuuint64_t)inner[i], (cuuint64_t)rows[i]};
-        cuuint64_t gstride[1] = {(cuuint64_t)inner[i] * 2};
+        const int32_t rows = plan.operand_rows[(size_t)i], inner = plan.operand_inner[(size_t)i];
+        if (rows == 0) continue;
+        cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)rows};
+        cuuint64_t gstride[1] = {(cuuint64_t)inner * 2};
         cuuint32_t box[2] = {64, 128};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = encode(&maps[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, tiles[i].dev_ptr, gdim, gstride, box, estr,
@@ -267,365 +192,48 @@ static int build_tensor_maps(pb2_window_t* w, const pb2_task_t* tasks, int32_t n
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { e->last_error = "cuTensorMapEncodeTiled failed"; return PB2_ERR_DEVICE; }
     }
-    CUtensorMap* d_tmaps = nullptr;
-    const int rc = dev_alloc_copy(w, &d_tmaps, maps.data(), maps.size());
-    w->g.tmaps = d_tmaps; w->g.fresh_tmaps = 1;
-    return rc;
-}
-
-
-// ---------------------------------------------------------------------------------------------
-// queue_policy 1: priority lanes
-// ---------------------------------------------------------------------------------------------
-// The lane of every task: the distinct priorities of the window's tasks ranked highest first, lane = rank r with at most
-// PB2_PRIO_LANES of them, floor(r * PB2_PRIO_LANES / ndistinct) otherwise.  tests/priority_order.py restates it.
-static std::vector<uint8_t> task_priority_lanes(const pb2_task_t* tasks, int32_t ntasks, int32_t* nlanes) {
-    std::vector<int32_t> v((size_t)ntasks);
-    for (int32_t i = 0; i < ntasks; ++i) v[(size_t)i] = tasks[i].priority;
-    std::sort(v.begin(), v.end(), std::greater<int32_t>());
-    v.erase(std::unique(v.begin(), v.end()), v.end());
-    const int64_t nd = (int64_t)v.size();
-    std::vector<uint8_t> lane((size_t)ntasks, 0);
-    for (int32_t i = 0; i < ntasks; ++i) {
-        const int64_t r = std::lower_bound(v.begin(), v.end(), tasks[i].priority, std::greater<int32_t>()) - v.begin();
-        lane[(size_t)i] = (uint8_t)(nd <= PB2_PRIO_LANES ? r : r * PB2_PRIO_LANES / nd);
-    }
-    *nlanes = nd == 0 ? 1 : (int32_t)std::min<int64_t>(nd, PB2_PRIO_LANES);
-    return lane;
-}
-
-// Cut the ring into one segment per lane, as long as the entries the lane's owners can ever push (owner o, in lane
-// p.owner_lane[o], pushes at most p.owner_pushes[o] entries).  p.entries becomes the image of the whole ring that the
-// reset kernel writes: each entry at the start of its owner's lane's segment, in the same order within a lane; the
-// lanes start as p.run.lane_image.  Uploads the owners' lanes.
-static int build_lane_ring(pb2_window_t* w, WindowPlan& p) {
-    Lanes& h = p.run.lane_image;
-    p.run.lanes = true;
-    uint32_t size[PB2_PRIO_LANES] = {0};
-    for (size_t o = 0; o < p.owner_lane.size(); ++o) size[p.owner_lane[o]] += p.owner_pushes[o];
-    uint32_t b = 0;
-    for (int l = 0; l < PB2_PRIO_LANES; ++l) { h.begin[l] = b; b += size[l]; }
-    std::vector<int32_t> ring(b, kEmpty);
-    for (size_t i = 0; i < p.entries.size(); ++i) {
-        const int l = p.owner_lane[(size_t)p.entry_owner[i]];
-        ring[h.begin[l] + h.ninit[l]++] = p.entries[i];
-    }
-    p.entries.swap(ring);
-    uint8_t* d_lane = nullptr;
-    const int rc = dev_alloc_copy(w, &d_lane, p.owner_lane.data(), p.owner_lane.size());
-    w->g.w.lane = d_lane;
-    return rc;
-}
-
-// Traced windows: where the part records of each ring-entry owner o (a task of an HBM window, a unit of a GEMM window)
-// start.  Owner o leads the entity of task lead[o] and runs nparts[o] parts (0: o owns no entries, as the members of a
-// read group).  Its records are part_base[o] .. + nparts[o], in owner order; pb2_window_part_trace returns them by
-// leading task.
-static int plan_part_records(pb2_window_t* w, const std::vector<int32_t>& lead, const std::vector<int32_t>& nparts, WindowPlan& plan) {
-    std::vector<int32_t> base(nparts.size());
-    int32_t n = 0;
-    w->part_entities.clear();
-    for (size_t o = 0; o < nparts.size(); ++o) {
-        base[o] = n;
-        if (nparts[o] > 0) w->part_entities.push_back({lead[o], n, nparts[o]});
-        n += nparts[o];
-    }
-    std::stable_sort(w->part_entities.begin(), w->part_entities.end(),
-                     [](const pb2_window_s::PartEntity& a, const pb2_window_s::PartEntity& b) { return a.lead < b.lead; });
-    int32_t* d_base = nullptr;
-    const int rc = dev_alloc_copy(w, &d_base, base.data(), base.size());
-    if (rc != PB2_SUCCESS) return rc;
-    w->g.trace.part_base = d_base; w->g.trace.nparts = n;
-    plan.run.part_records = n;
     return PB2_SUCCESS;
 }
 
-// ---------------------------------------------------------------------------------------------
-// GEMM windows: group tasks into units (fused k-chains), see pb2_gemm.cuh
-// ---------------------------------------------------------------------------------------------
-// The plan of a GEMM window: its units are the ring-entry owners.  task_lane (queue_policy 1, else empty): a unit's
-// lane is the lane of its first task, for all its parts.  A unit that runs an HBM body is cut into
-// task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.  Uploads the CSR and the unit arrays.
-static int build_gemm2_units(pb2_window_t* w, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ, int32_t nsucc,
-                             const int32_t* ready, int32_t nready, bool fuse, const int32_t* rs_begin,
-                             const std::vector<uint8_t>& task_lane, const pb2_tile_t* tiles, int32_t part_bytes,
-                             WindowPlan& plan) {
-    std::vector<int32_t> indeg((size_t)ntasks, 0), cpred((size_t)ntasks, -1), ccons((size_t)ntasks, 0), next((size_t)ntasks, -1);
-    auto is_gemm = [&](int32_t t) { return tasks[t].body == PB2_BODY_GEMM_BF16; };
-    for (int32_t u = 0; u < ntasks; ++u)
-        for (int32_t e = 0; e < tasks[u].succ_count; ++e) {
-            const uint32_t s = succ[tasks[u].succ_begin + e];
-            const int32_t t = PB2_SUCC_TASK(s);
-            indeg[t]++;
-            if (PB2_SUCC_FLOW(s) == 2 && is_gemm(u) && is_gemm(t) && tasks[u].tile[2] == tasks[t].tile[2]) { ccons[u]++; cpred[t] = u; }
-        }
-    // A window that peers release into: the tasks' dependency goals (counter mode, set by the partitioner) also
-    // count the in-edges that come from other GPUs; the local CSR does not show them.
-    if (w->shared)
-        for (int32_t t = 0; t < ntasks; ++t) {
-            const int32_t need = (tasks[t].flags & PB2_TASK_DEPS_MASK) ? __builtin_popcount((unsigned)tasks[t].dep_goal) : tasks[t].dep_goal;
-            if (need < indeg[t]) { w->e->last_error = "dependency goal smaller than the in-window in-degree"; return PB2_ERR_BAD_PARAM; }
-            indeg[t] = need;
-        }
-    if (fuse)
-        for (int32_t t = 0; t < ntasks; ++t) {
-            const int32_t u = cpred[t];
-            if (u < 0 || indeg[t] != 1 || ccons[u] != 1) continue;                 // the chain link must be t's only missing input
-            if (rs_begin && rs_begin[u + 1] > rs_begin[u]) continue;               // u's result is awaited on another GPU: retire it on its own
-            if (tasks[u].access[2] & PB2_FLOW_PUSHOUT) continue;                   // u's C has to reach the host: flush there
-            if (memcmp(tasks[u].iparam, tasks[t].iparam, sizeof tasks[u].iparam)) continue;
-            next[u] = t;
-        }
-    std::vector<uint8_t> has_pred((size_t)ntasks, 0);
-    for (int32_t u = 0; u < ntasks; ++u) if (next[u] >= 0) has_pred[next[u]] = 1;
-    std::vector<GUnit> units; std::vector<GSeg> segs; std::vector<int32_t> unit_of((size_t)ntasks, -1);
-    for (int32_t h = 0; h < ntasks; ++h) {
-        if (has_pred[h]) continue;
-        GUnit u{}; u.seg_begin = (int32_t)segs.size(); u.dep_goal = indeg[h];
-        const bool g = is_gemm(h);
-        u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
-        u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
-        // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body
-        u.nparts = g ? std::min(((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN), gemm::kMaxParts)
-                     : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
-        for (int32_t t = h; t >= 0; t = next[t]) {
-            unit_of[t] = (int32_t)units.size();
-            segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});
-            if (g && (tasks[t].access[2] & PB2_FLOW_PUSHOUT)) u.flags |= 2;
-        }
-        u.seg_count = (int32_t)segs.size() - u.seg_begin;
-        units.push_back(u);
-    }
-    std::vector<int32_t> usucc;
-    for (GUnit& u : units) {
-        u.succ_begin = (int32_t)usucc.size();
-        for (int32_t i = 0; i < u.seg_count; ++i) {
-            const int32_t t = segs[u.seg_begin + i].task;
-            for (int32_t e = 0; e < tasks[t].succ_count; ++e) {
-                const int32_t d = PB2_SUCC_TASK(succ[tasks[t].succ_begin + e]);
-                if (d == next[t] && PB2_SUCC_FLOW(succ[tasks[t].succ_begin + e]) == 2) continue;   // the fused link
-                usucc.push_back(unit_of[d]);
-            }
-        }
-        u.succ_count = (int32_t)usucc.size() - u.succ_begin;
-    }
-    uint32_t total_parts = 0;
-    for (const GUnit& u : units) total_parts += (uint32_t)u.nparts;
-    // Ready GEMM units enter the ring in Z-order of their (locals[0], locals[1]) = C(i,j) coordinates: the units
-    // that run concurrently then form a compact block of C tiles that shares A rows and B columns in L2 (a FIFO
-    // ring keeps whatever order the host gives it; the reference's priority hint mt*nt*kt - i*nt + j plays the
-    // same role for its sorted pending list, device_gpu.c:2169-2174).
-    std::vector<std::pair<uint64_t, int32_t>> order;
-    auto morton = [](uint32_t x, uint32_t y) {
-        uint64_t r = 0;
-        for (int b = 0; b < 16; ++b) r |= ((uint64_t)((x >> b) & 1) << (2 * b + 1)) | ((uint64_t)((y >> b) & 1) << (2 * b));
-        return r;
-    };
-    for (int32_t i = 0; i < nready; ++i) {
-        const int32_t uid = unit_of[ready[i]];
-        if (units[uid].dep_goal != 0) { w->e->last_error = "ready task has in-window predecessors"; return PB2_ERR_BAD_PARAM; }
-        const pb2_task_t& t = tasks[ready[i]];
-        const uint64_t key = (units[uid].flags & 1) ? morton((uint32_t)t.locals[0], (uint32_t)t.locals[1]) : 0;
-        order.emplace_back(key, uid);
-    }
-    std::stable_sort(order.begin(), order.end(), [](const std::pair<uint64_t, int32_t>& a, const std::pair<uint64_t, int32_t>& b) { return a.first < b.first; });
-    for (auto& o : order)
-        for (int32_t p = 0; p < units[o.second].nparts; ++p) {
-            plan.entries.push_back((int32_t)PB2_SUCC_MAKE(o.second, p));
-            plan.entry_owner.push_back(o.second);
-        }
-    if (!task_lane.empty())
-        for (const GUnit& u : units) {
-            plan.owner_lane.push_back(task_lane[(size_t)segs[(size_t)u.seg_begin].task]);
-            plan.owner_pushes.push_back((uint32_t)u.nparts);
-        }
-    plan.ring_slots = (uint32_t)ntasks + total_parts;
-    // operand tiles that have to be staged in (host or peer GPU) are pulled in 64 KiB slices by every worker
-    // that needs them (the parts of one unit, the units that share an operand) instead of by one worker alone
-    plan.slice_bytes = 64 * 1024;
-    plan.run.claims = true;
-    plan.run.nunits = (int32_t)units.size();
-    w->task_entry.resize((size_t)ntasks);
-    for (int32_t t = 0; t < ntasks; ++t) w->task_entry[(size_t)t] = (int32_t)PB2_SUCC_MAKE(unit_of[t], units[(size_t)unit_of[t]].nparts - 1);
-    int rc;
-    if (!w->task_unit.empty()) {
-        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = segs[(size_t)units[(size_t)unit_of[t]].seg_begin].task;
-        std::vector<int32_t> lead(units.size()), np(units.size());
-        for (size_t u = 0; u < units.size(); ++u) { lead[u] = segs[(size_t)units[u].seg_begin].task; np[u] = units[u].nparts; }
-        if ((rc = plan_part_records(w, lead, np, plan)) != PB2_SUCCESS) return rc;
-    }
-    uint32_t* d_succ = nullptr; GUnit* d_units = nullptr; GSeg* d_segs = nullptr; int32_t* d_usucc = nullptr;
-    if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &d_units, units.data(), units.size())) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &d_segs, segs.data(), segs.size())) != PB2_SUCCESS) return rc;
-    if ((rc = dev_alloc_copy(w, &d_usucc, usucc.data(), usucc.size())) != PB2_SUCCESS) return rc;
-    w->g.w.succ = d_succ;
-    w->g.units = d_units; w->g.segs = d_segs; w->g.usucc = d_usucc; w->g.nunits = plan.run.nunits;
-    return PB2_SUCCESS;
+// The engine's settings a window of `kind` is planned with.
+static PlanParams params_of(const pb2_engine_t* e, int kind) {
+    PlanParams p;
+    p.kind = kind; p.shared = e->shared_windows; p.trace = e->window_trace; p.linked_image = e->linked_module != nullptr;
+    p.queue_policy = e->params.queue_policy; p.gemm_mode = e->params.gemm_mode;
+    p.read_groups = e->params.read_groups; p.fuse_readers = e->params.fuse_readers;
+    p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
+    p.part_bytes = e->params.part_bytes; p.stage_slice_bytes = e->stage_slice_bytes;
+    p.linked_sliceable = e->linked_sliceable; p.next_rs_begin = e->next_rs_begin;
+    return p;
 }
 
-// ---------------------------------------------------------------------------------------------
-// read groups of HBM windows
-// ---------------------------------------------------------------------------------------------
-// A run of >= 2 consecutive out-edges of one task whose targets all
-//   - have that edge as their only input (in-degree 1, not ready at start; counter goal 1, or the edge's one mask bit),
-//   - run a CHECK body over exactly one data flow, flow 0, READ only, on the same tile,
-// becomes one edge to the run's first target (the leader) in the device CSR, and the leader's worker streams the tile
-// once for all the members (pb2_engine_hbm_kernel).  Without groups F readers of a tile each pull it through L2 into
-// their own SM, F passes where one carries the same bytes.  The members become ready together and would have entered
-// the FIFO ring back to back: with one worker the retire order is the ungrouped one.  Runs longer than PB2_GROUP_MAX
-// are split.  O(ntasks + nsucc); tasks keep their own out-edges.  Returns false when no group formed.
-//
-// With `fuse`, a task P also runs with the first group among its out-edges as one unit when P has a body, writes the
-// group's tile X without pushing it out, and X is P's widest tile (so P's parts cut X as the members' parts do): the
-// edge P -> leader leaves the device CSR and group[P] = PB2_GROUP_FUSED | the leader's group word.  The worker that
-// runs a part of P writes it to X and checks every value for the members in registers before it stores it
-// (run_fused_part); so P's body must have a checked form that writes X (fusable).  The
-// caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
-// every task that was queued when P retired, and a fused unit runs them right after P.
-static bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
-                             const pb2_tile_t* tiles, bool fuse,
-                             std::vector<uint32_t>& gsucc, std::vector<uint32_t>& group, std::vector<int32_t>& gmem) {
-    const size_t n = tasks.size();
-    std::vector<uint8_t> indeg(n, 0);                        // saturates at 2
-    for (size_t u = 0; u < n; ++u)
-        for (int32_t j = 0; j < tasks[u].succ_count; ++j) {
-            uint8_t& d = indeg[(size_t)PB2_SUCC_TASK(succ[tasks[u].succ_begin + j])];
-            if (d < 2) ++d;
-        }
-    for (int32_t i = 0; i < nready; ++i) indeg[(size_t)ready[i]] = 2;
-    auto reader = [&](uint32_t s) {
-        const pb2_task_t& t = tasks[(size_t)PB2_SUCC_TASK(s)];
-        if (indeg[(size_t)PB2_SUCC_TASK(s)] != 1) return false;
-        if (t.dep_goal != ((t.flags & PB2_TASK_DEPS_MASK) ? (int32_t)(1u << PB2_SUCC_FLOW(s)) : 1)) return false;
-        if (t.body != PB2_BODY_CHECK_I32 && t.body != PB2_BODY_CHECK_F32) return false;
-        if (t.nb_flows < 1 || t.tile[0] < 0 || (t.access[0] & (PB2_FLOW_ACCESS_RW | PB2_FLOW_PUSHOUT)) != PB2_FLOW_ACCESS_READ) return false;
-        for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
-        return true;
+// Every array of window w's plan on the device, with the window's initial tile table and, in a GEMM window, its tensor
+// maps: allocated and queued on the upload stream, and named in w's descriptor with the scalars the plan fixes.  An
+// array the device tests for null is uploaded only when the plan has it.
+static int upload_plan(pb2_window_t* w, const WindowPlan& plan, const pb2_tile_t* tiles, const std::vector<CUtensorMap>& tmaps) {
+    int rc = PB2_SUCCESS;
+    auto up = [&](const auto& v) {
+        typename std::decay_t<decltype(v)>::value_type* p = nullptr;
+        if (rc == PB2_SUCCESS) rc = dev_alloc_copy(w, &p, v.data(), v.size());
+        return p;
     };
-    // the bodies with a checked form (run_hbm_body<true>), whose output flow `out` writes X
-    auto fusable = [&](const pb2_task_t& p, int32_t x) {
-        int out = 0;
-        switch (p.body) {
-        case PB2_BODY_FILL_I32: case PB2_BODY_FILL_F32: case PB2_BODY_MEMSET_U8: case PB2_BODY_INCR_I32:
-        case PB2_BODY_SCALE_I32: case PB2_BODY_ADD_IOTA_I32: case PB2_BODY_IOTA_I32: case PB2_BODY_INCR_F32: break;
-        case PB2_BODY_COPY: case PB2_BODY_AXPY_F32: out = 1; break;
-        default: return false;
-        }
-        if (p.nb_flows <= out || p.tile[out] != x || !(p.access[out] & PB2_FLOW_ACCESS_WRITE)) return false;
-        // the checked COPY / AXPY writes every byte of the slice: the tile they read is as long as X
-        if (out == 1 && (p.tile[0] < 0 || tiles[p.tile[0]].bytes != tiles[x].bytes)) return false;
-        for (int f = 0; f < p.nb_flows; ++f) {
-            if (p.tile[f] < 0) continue;
-            if (tiles[p.tile[f]].bytes > tiles[x].bytes) return false;
-            if (p.tile[f] == x && (p.access[f] & PB2_FLOW_ACCESS_WRITE) && (p.access[f] & PB2_FLOW_PUSHOUT)) return false;
-        }
-        return true;
-    };
-    std::vector<int32_t> begin(n), count(n);
-    group.assign(n, 0u);
-    gsucc.clear(); gmem.clear();
-    for (size_t u = 0; u < n; ++u) {
-        const uint32_t* out = succ + tasks[u].succ_begin;
-        const int32_t c = tasks[u].succ_count;
-        begin[u] = (int32_t)gsucc.size();
-        bool first_group = true;
-        for (int32_t j = 0; j < c;) {
-            int32_t r = j + 1;
-            int32_t tile = -1;
-            if (reader(out[j])) {
-                tile = tasks[(size_t)PB2_SUCC_TASK(out[j])].tile[0];
-                while (r < c && r - j < PB2_GROUP_MAX && reader(out[r]) && tasks[(size_t)PB2_SUCC_TASK(out[r])].tile[0] == tile) ++r;
-            }
-            bool fused = false;
-            if (r - j >= 2) {
-                const uint32_t gw = ((uint32_t)gmem.size() << 4) | (uint32_t)(r - j);
-                group[(size_t)PB2_SUCC_TASK(out[j])] = gw;
-                for (int32_t q = j; q < r; ++q) gmem.push_back(PB2_SUCC_TASK(out[q]));
-                fused = fuse && first_group && fusable(tasks[u], tile);
-                if (fused) group[u] = PB2_GROUP_FUSED | gw;
-                first_group = false;
-            }
-            if (!fused) gsucc.push_back(out[j]);
-            j = r;
-        }
-        count[u] = (int32_t)gsucc.size() - begin[u];
-    }
-    if (gmem.empty()) return false;
-    for (size_t u = 0; u < n; ++u) { tasks[u].succ_begin = begin[u]; tasks[u].succ_count = count[u]; }
-    return true;
-}
-
-// The plan of an HBM window: its tasks are the ring-entry owners, each cut into task_parts(..., PB2_MAX_PARTS) parts.
-// task_lane: as for build_gemm2_units.  Forms the read groups (which rewrites the out-edges of dtasks) and uploads the
-// CSR, the group arrays and, with wide tasks, the part counts.
-static int plan_hbm_window(pb2_window_t* w, std::vector<pb2_task_t>& dtasks, const uint32_t* succ, int32_t nsucc,
-                           const pb2_tile_t* tiles, int32_t ntiles, const int32_t* ready, int32_t nready,
-                           const std::vector<uint8_t>& task_lane, WindowPlan& plan) {
-    pb2_engine_t* e = w->e;
     WinDev& d = w->g.w;
-    const int32_t ntasks = (int32_t)dtasks.size();
-    std::vector<uint16_t> nparts((size_t)ntasks);
-    uint32_t extra_parts = 0;
-    w->task_entry.resize((size_t)ntasks);
-    for (int32_t i = 0; i < ntasks; ++i) {
-        // a linked body whose sliceable bit is clear runs over whole tiles (a stencil reads its neighbours' tiles)
-        const pb2_task_t& t = dtasks[(size_t)i];
-        const bool whole = is_linked_body(t.body) && !((e->linked_sliceable >> (t.body - PB2_BODY_LINKED_0)) & 1u);
-        const int np = whole ? 1 : task_parts(t, [&](int32_t id) { return tiles[id].bytes; }, e->params.part_bytes, PB2_MAX_PARTS);
-        nparts[(size_t)i] = (uint16_t)np; extra_parts += (uint32_t)np - 1;
-        w->task_entry[(size_t)i] = PB2_ENT_MAKE(i, np - 1);
+    d.tasks = up(plan.tasks);
+    d.succ = up(plan.succ);
+    if (!plan.group_mem.empty()) { d.group = up(plan.group); d.group_mem = up(plan.group_mem); }
+    if (!plan.nparts.empty()) d.nparts = up(plan.nparts);
+    if (plan.run.lanes) d.lane = up(plan.lane);
+    if (!plan.part_base.empty()) w->g.trace.part_base = up(plan.part_base);
+    if (w->kind == 1) {
+        w->g.units = up(plan.units); w->g.segs = up(plan.segs); w->g.usucc = up(plan.usucc);
+        w->g.tmaps = up(tmaps); w->g.fresh_tmaps = 1;
     }
-    for (int32_t i = 0; i < nready; ++i)
-        for (int p = 0; p < (int)nparts[(size_t)ready[i]]; ++p) {
-            plan.entries.push_back(PB2_ENT_MAKE(ready[i], p));
-            plan.entry_owner.push_back(ready[i]);
-        }
-    if (!task_lane.empty()) { plan.owner_lane = task_lane; plan.owner_pushes.assign(nparts.begin(), nparts.end()); }
-    plan.ring_slots = (uint32_t)ntasks + extra_parts;
-    // Stage-in is cut finer than tasks are: a tile that has to come from the host or a peer GPU is pulled in slices
-    // by EVERY worker that needs it (claim bit per slice), so the readers of a tile share the transfer instead of one
-    // moving it while the others wait.
-    plan.slice_bytes = stage_slice(e->stage_slice_bytes, e->params.part_bytes);
-    plan.run.parts = plan.run.claims = extra_parts > 0;
-    for (int32_t i = 0; i < ntiles && !plan.run.claims; ++i)
-        plan.run.claims = plan.slice_bytes > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)plan.slice_bytes;
-    // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
-    std::vector<uint32_t> gsucc, group;
-    std::vector<int32_t> gmem;
-    const bool grouped = !w->shared && e->params.read_groups >= 0 &&
-                         form_read_groups(dtasks, succ, ready, nready, tiles, e->params.fuse_readers >= 0 && e->nworkers > 1,
-                                          gsucc, group, gmem);
-    int rc;
-    uint32_t* d_succ = nullptr;
-    if (grouped) {
-        uint32_t* d_group = nullptr; int32_t* d_gmem = nullptr;
-        if ((rc = dev_alloc_copy(w, &d_succ, gsucc.data(), gsucc.size())) != PB2_SUCCESS) return rc;
-        if ((rc = dev_alloc_copy(w, &d_group, group.data(), group.size())) != PB2_SUCCESS) return rc;
-        if ((rc = dev_alloc_copy(w, &d_gmem, gmem.data(), gmem.size())) != PB2_SUCCESS) return rc;
-        d.group = d_group; d.group_mem = d_gmem;
-        // a read group is led by its leader, unless a producer runs with it: then by the producer
-        if (!w->task_unit.empty())
-            for (int pass = 0; pass < 2; ++pass)
-                for (int32_t t = 0; t < ntasks; ++t) {
-                    const uint32_t gd = group[(size_t)t];
-                    if ((gd & 15u) == 0 || ((gd & PB2_GROUP_FUSED) != 0) != (pass == 1)) continue;
-                    const uint32_t b = (gd & ~PB2_GROUP_FUSED) >> 4;
-                    for (uint32_t i = 0; i < (gd & 15u); ++i) w->task_unit[(size_t)gmem[b + i]] = t;
-                }
-    } else if ((rc = dev_alloc_copy(w, &d_succ, succ, (size_t)nsucc)) != PB2_SUCCESS) return rc;
-    d.succ = d_succ;
-    if (!w->task_unit.empty()) {                // a task owns ring entries unless a group member is led by another task
-        std::vector<int32_t> lead((size_t)ntasks), np((size_t)ntasks);
-        for (int32_t t = 0; t < ntasks; ++t) { lead[(size_t)t] = t; np[(size_t)t] = w->task_unit[(size_t)t] == t ? nparts[(size_t)t] : 0; }
-        if ((rc = plan_part_records(w, lead, np, plan)) != PB2_SUCCESS) return rc;
-    }
-    if (extra_parts) {
-        uint16_t* d_np = nullptr;
-        if ((rc = dev_alloc_copy(w, &d_np, nparts.data(), nparts.size())) != PB2_SUCCESS) return rc;
-        d.nparts = d_np;
-    }
-    return PB2_SUCCESS;
+    w->d_ready = up(plan.ring_image);
+    if (rc == PB2_SUCCESS) rc = dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)w->ntiles);
+    w->nready_entries = (int32_t)plan.ring_image.size();
+    w->g.nunits = plan.run.nunits; w->g.trace.nparts = plan.run.part_records;
+    d.part_bytes = plan.slice_bytes; d.nlanes = plan.nlanes; d.cap_mask = plan.run.ring - 1;
+    return rc;
 }
 
 // Copy c of window w's per-run state, sized from w->shape.  pb2_window_create allocates copy 0 on the upload stream,
@@ -680,7 +288,7 @@ static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaMemcpy(rec.data(), run_desc(w, w->cur).trace.parts, rec.size() * sizeof(pb2_part_trace_t), cudaMemcpyDeviceToHost));
     out.reserve(rec.size());
-    for (const pb2_window_s::PartEntity& pe : w->part_entities)
+    for (const PartEntity& pe : w->part_entities)
         for (int32_t p = 0; p < pe.nparts; ++p) {
             out.push_back(rec[(size_t)(pe.base + p)]);
             out.back().task = pe.lead; out.back().part = (uint16_t)p; out.back().nparts = (uint16_t)pe.nparts;
@@ -1124,58 +732,31 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
     if (!e || !window) return PB2_ERR_BAD_PARAM;
     *window = nullptr;
     if ((ntasks && !tasks) || (nsucc && !succ) || (ntiles && !tiles) || (nready && !ready)) return PB2_ERR_BAD_PARAM;
-    int rc = validate_window(e, kind, tasks, ntasks, succ, nsucc, ntiles, ready, nready);
-    if (rc != PB2_SUCCESS) return rc;
-    const bool prio = e->params.queue_policy == 1;
-    if (prio && e->shared_windows) {
-        e->last_error = "queue_policy 1 (priority lanes) is not supported with shared windows: peers push into one FIFO ring";
-        return PB2_ERR_NOT_SUPPORTED;
+    WindowPlan plan;
+    const char* why = nullptr;
+    int rc = plan_window(params_of(e, kind), tasks, ntasks, succ, nsucc, tiles, ntiles, ready, nready, plan, &why);
+    if (rc != PB2_SUCCESS) {
+        if (why) e->last_error = why;
+        return rc;
     }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    std::vector<CUtensorMap> tmaps;
+    if (kind == 1 && (rc = encode_tensor_maps(e, plan, tiles, ntiles, tmaps)) != PB2_SUCCESS) return rc;
     pb2_window_t* w = new pb2_window_s();
     w->shared = e->shared_windows;
     w->e = e; w->kind = kind; w->ntasks = ntasks; w->ntiles = ntiles;
-#define TRY(x) do { rc = (x); if (rc != PB2_SUCCESS) { pb2_window_destroy(w); return rc; } } while (0)
-    WinDev& d = w->g.w;
-    std::vector<pb2_task_t> dtasks(tasks, tasks + ntasks);
-    for (pb2_task_t& t : dtasks) { t.flags &= 0x07; w->linked |= is_linked_body(t.body); }
-    int32_t nlanes = 0;
-    std::vector<uint8_t> task_lane;
-    if (prio) task_lane = task_priority_lanes(tasks, ntasks, &nlanes);
-    if (e->window_trace) {                      // every task leads itself until a plan groups it
-        w->task_unit.resize((size_t)ntasks);
-        for (int32_t t = 0; t < ntasks; ++t) w->task_unit[(size_t)t] = t;
-    }
-    WindowPlan plan;
-    plan.run.trace = e->window_trace;
-    if (kind == 0) TRY(plan_hbm_window(w, dtasks, succ, nsucc, tiles, ntiles, ready, nready, task_lane, plan));
-    else {
-        // HBM bodies of a GEMM window are cut into parts as HBM windows cut them.  Not in shared windows: their units
-        // are released by peers over NVLink, and the multi-GPU runs that check those releases cover single-part HBM
-        // units only, so shared windows keep one part per HBM unit.
-        const int32_t hbm_part_bytes = w->shared ? 0 : e->params.part_bytes;
-        TRY(build_tensor_maps(w, tasks, ntasks, tiles, ntiles));
-        TRY(build_gemm2_units(w, tasks, ntasks, succ, nsucc, ready, nready, e->params.gemm_mode == 0,
-                              w->shared ? e->next_rs_begin : nullptr, task_lane, tiles, hbm_part_bytes, plan));
-    }
-    if (prio) TRY(build_lane_ring(w, plan));
-    TRY(dev_alloc_copy(w, &w->d_ready, plan.entries.data(), plan.entries.size()));
-    w->nready_entries = (int32_t)plan.entries.size();
-    const int maxw = e->nworkers > e->nworkers_gemm ? e->nworkers : e->nworkers_gemm;
-    uint32_t cap = 1024;
-    while (cap < plan.ring_slots + (uint32_t)maxw + 2u) cap <<= 1;   // every slot is used at most once per run
-    pb2_task_t* d_tasks = nullptr;
-    TRY(dev_alloc_copy(w, &d_tasks, dtasks.data(), (size_t)ntasks));
-    d.tasks = d_tasks;
-    TRY(dev_alloc_copy(w, &w->d_tiles_init, tiles, (size_t)ntiles));
-    plan.run.ring = cap;
+    w->linked = plan.linked;
     w->shape = plan.run;
     // shared windows keep one copy (peers hold IPC pointers to it), GEMM windows too (DESIGN.md §5)
     w->ncopies = kind == 0 && !w->shared && ntasks > 0 ? 2 : 1;
-    TRY(alloc_run(w, 0));
-#undef TRY
-    d.part_bytes = plan.slice_bytes; d.shared = w->shared ? 1 : 0; d.nlanes = nlanes;
-    d.cap_mask = cap - 1; d.ntasks = ntasks; d.ntiles = ntiles; d.stage_mode = e->params.stage_mode;
+    rc = upload_plan(w, plan, tiles, tmaps);
+    if (rc == PB2_SUCCESS) rc = alloc_run(w, 0);
+    if (rc != PB2_SUCCESS) { pb2_window_destroy(w); return rc; }
+    w->task_entry.swap(plan.task_entry);
+    w->task_unit.swap(plan.task_unit);
+    w->part_entities.swap(plan.part_entities);
+    WinDev& d = w->g.w;
+    d.shared = w->shared ? 1 : 0; d.ntasks = ntasks; d.ntiles = ntiles; d.stage_mode = e->params.stage_mode;
     d.timeout_ns = (unsigned long long)e->params.timeout_ms * 1000000ull;
     PB2_CUDA(e, cudaEventCreate(&w->ev0));
     PB2_CUDA(e, cudaEventCreate(&w->ev1));

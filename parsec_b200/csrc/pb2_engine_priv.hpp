@@ -1,4 +1,4 @@
-// pb2_engine_priv.hpp -- host-side engine object, part and slice rules shared by the translation units of libparsec_b200.so
+// pb2_engine_priv.hpp -- host-side engine object shared by the translation units of libparsec_b200.so
 // (pb2_engine.cu: windows; pb2_stream.cu: the streaming ring + persistent kernel).
 #pragma once
 #include <cuda.h>
@@ -9,6 +9,7 @@
 #include <string>
 #include <utility>
 #include "../../include/pb2_engine.h"
+#include "pb2_window_layout.h"
 
 struct pb2_engine_s {
     int cuda_device = 0;
@@ -40,35 +41,12 @@ struct pb2_engine_s {
     uint32_t linked_sliceable = 0;
 };
 
-static inline bool is_linked_body(int body) { return body >= PB2_BODY_LINKED_0 && body <= PB2_BODY_LINKED_7; }
-
 // The argument check of pb2_engine_link_bodies and pb2_device_link_bodies: nullptr, or why the arguments are refused.
 static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable) {
     if (!image || !bytes) return "linked body image is NULL or empty";
     if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
     if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";
     return nullptr;
-}
-
-// part_bytes of engines and streams whose parameters leave it 0
-constexpr int32_t kDefaultPartBytes = 256 * 1024;
-
-// The parts a task runs as: min(ceil(widest tile / part_bytes), cap) byte slices; one for a NOP body or part_bytes <= 0.
-// tile_bytes(id) is the byte count of tile id.  The device cuts the slices of a tile by the same rule (tile_slices_of).
-template <class TileBytes>
-static inline int task_parts(const pb2_task_t& t, TileBytes tile_bytes, int32_t part_bytes, int cap) {
-    if (part_bytes <= 0 || t.body == PB2_BODY_NOP) return 1;
-    uint32_t big = 0;
-    for (int f = 0; f < t.nb_flows; ++f)
-        if (t.tile[f] >= 0 && tile_bytes(t.tile[f]) > big) big = tile_bytes(t.tile[f]);
-    const uint32_t np = (big + (uint32_t)part_bytes - 1) / (uint32_t)part_bytes;
-    return np < 1 ? 1 : (np > (uint32_t)cap ? cap : (int)np);
-}
-
-// The stage-in slice size of HBM windows and streams: the smaller of stage_slice_bytes and part_bytes among those that
-// are positive, so a tile is never staged in coarser slices than wide tasks are cut into; part_bytes when neither is.
-static inline int32_t stage_slice(int32_t stage_slice_bytes, int32_t part_bytes) {
-    return (stage_slice_bytes > 0 && (part_bytes <= 0 || stage_slice_bytes < part_bytes)) ? stage_slice_bytes : part_bytes;
 }
 
 #define PB2_CUDA(e, call)                                                                        \

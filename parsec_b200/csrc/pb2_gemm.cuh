@@ -6,7 +6,7 @@
 // (BASELINE config 3); tiles are K-contiguous for both operands: A row-major [M][K], B stored
 // [N][K] (== column-major K x N, what a "TN" cuBLAS call consumes), C row-major [M][N].
 //
-// The host groups GEMM tasks into UNITS (build_gemm2_units): a maximal chain of tasks that accumulate into the same C
+// The host groups GEMM tasks into UNITS (build_gemm2_units, pb2_window_plan.cpp): a maximal chain of tasks that accumulate into the same C
 // tile and whose only missing dependency is the previous link (the C(i,j) k-chain of dtd_test_simple_gemm.c:675-696,
 // the k-chains of a tile Cholesky); with gemm_mode 1 or 2 every task is a unit of its own.  A unit's C is cut into
 // sub-tiles of 128 rows x 256 columns, run by nparts = min(sub-tiles, kMaxParts) independent parts: part p runs
@@ -37,7 +37,7 @@ namespace pb2 {
 
 namespace gemm {
 
-constexpr int BM = 128, BN = 256, BK = 64, UK = 16;
+constexpr int BK = 64, UK = 16;     // BM, BN: pb2_window_layout.h
 constexpr int kStages = 4;
 constexpr int kAStageBytes = BM * BK * 2;          // 16 KiB
 constexpr int kBStageBytes = BN * BK * 2;          // 32 KiB
@@ -197,19 +197,6 @@ __device__ __forceinline__ void epilogue_add(const float (&acc)[128], uint8_t* C
 
 }  // namespace gemm
 
-struct GUnit {                  // 48 bytes, read-only
-    int32_t seg_begin, seg_count;   // members, in chain order
-    int32_t succ_begin, succ_count; // out-edges of all members (chain links removed): target unit ids
-    int32_t dep_goal;               // in-edges from other units
-    int32_t nparts;                 // ring entries: min(sub-tiles of C, kMaxParts) for GEMM units; for an HBM body
-                                    // min(ceil(widest tile / part_bytes), kMaxParts) byte slices (1 in shared windows)
-    int32_t tileC;                  // GEMM units: the C tile; -1 otherwise
-    int32_t M, N, K;
-    int32_t flags;                  // bit0 is_gemm, bit1 pushout C
-    int32_t pad;
-};
-struct GSeg { int32_t task, tileA, tileB, pad; };
-
 struct Win2Dev {
     WinDev w;                       // task-level arrays (descriptors, tiles, outputs, ctl, ring)
     const GUnit* units;
@@ -224,8 +211,6 @@ struct Win2Dev {
 };
 
 namespace gemm {
-
-constexpr int kMaxParts = 32;      // the part index travels in the 5-bit flow field of a ring entry
 
 struct Job {
     int32_t unit, part, stop, is_gemm;

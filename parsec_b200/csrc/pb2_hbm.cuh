@@ -18,7 +18,7 @@ namespace pb2 {
 // a window that streams tiles through L2 responds to (r02 sweep in DESIGN.md: 20 x 4 requests 0.76 ms, 20 x 6 0.62 ms,
 // 12 x 16 0.60 ms), while many small workers still overlap the serial pop / release sections of one task with the
 // streaming of the others.  The Ex05 window is no longer L2-bound: its eight readers of a tile run as one read group
-// (form_read_groups), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
+// (form_read_groups, pb2_window_plan.cpp), so each tile crosses L2 -> SM twice (FILL, one grouped CHECK) instead of nine times.  And the
 // producer runs with its group as one unit (run_fused_part) that checks every value in registers before it stores it:
 // the tile goes SM -> L2 -> DRAM once and never comes back to the SM (DESIGN.md §5, §8).
 // What one worker does with a task is in pb2_worker.cuh (shared with the streaming kernel of pb2_stream.cu and the
@@ -113,8 +113,6 @@ static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, G
     return r;
 }
 
-__device__ __forceinline__ bool linked_body_id(int body) { return body >= PB2_BODY_LINKED_0 && body <= PB2_BODY_LINKED_7; }
-
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
 // TRACE: write a record of every part into tr (PartSmem, then trace_part); the untraced instantiations never touch tr.
 // LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body (include/pb2_device_body.h); built
@@ -182,7 +180,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
             if constexpr (LINKED) {
-                if (linked_body_id(s.task.body))
+                if (is_linked_body(s.task.body))
                     return (unsigned long long)pb2_linked_body(s.task.body, reinterpret_cast<const pb2_body_args_t*>(&s.args), s.red);
             }
             return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);

@@ -960,7 +960,7 @@ static int build_window(pb2_device_module_t* dev, Window& w, std::vector<pb2_gpu
     int engine_side = 0;                        // PB2_BODY_GEMM_BF16 or PB2_BODY_LINKED_0 once the window holds one
     auto fits = [&](const pb2_htask_t* t) {
         if ((t->body == PB2_BODY_USER) != want_user) return false;
-        const int side = t->body == PB2_BODY_GEMM_BF16 ? PB2_BODY_GEMM_BF16 : is_linked_body(t->body) ? PB2_BODY_LINKED_0 : 0;
+        const int side = t->body == PB2_BODY_GEMM_BF16 ? PB2_BODY_GEMM_BF16 : pb2::is_linked_body(t->body) ? PB2_BODY_LINKED_0 : 0;
         if (side && engine_side && side != engine_side) return false;
         if (side) engine_side = side;
         return true;

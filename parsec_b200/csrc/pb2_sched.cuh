@@ -4,16 +4,14 @@
 #include "../../include/pb2_engine.h"
 #include "pb2_dev_utils.cuh"
 #include "pb2_bodies.cuh"
+#include "pb2_window_layout.h"
 
 namespace pb2 {
 
-constexpr int32_t kEmpty = -1;
 constexpr int32_t kDoneOK = 1;
 constexpr int32_t kDoneTimeout = 2;
 constexpr int32_t kDoneBadBody = 3;
 
-// Hot control words, one per 128-byte line so that atomics on them do not false-share.
-struct alignas(128) Line { unsigned long long v; unsigned long long pad[15]; };
 struct Ctl {
     Line head;       // pop tickets handed out
     Line tail;       // push tickets handed out
@@ -58,48 +56,20 @@ struct WinDev {
     int32_t           part_bytes;
     const uint16_t*   nparts;         // HBM windows with wide tasks: parts per task (null: every task is one part)
     int32_t           remote_units;   // remote targets are (parts-1) << 27 | unit of a fused-GEMM window, not << 22 | task
-    // read groups of HBM windows (form_read_groups in pb2_engine.cu; null: none): task id leads the members
+    // read groups of HBM windows (form_read_groups in pb2_window_plan.cpp; null: none): task id leads the members
     // group_mem[group[id] >> 4 .. + (group[id] & 15)), itself first; a count of 0 means the task runs alone.  The other
     // members are never released or popped on their own.  A producer fused with a group (PB2_GROUP_FUSED set in its
     // group word) names that group's members, the leader included, and its edge to the leader is gone from succ[].
     const uint32_t*   group;
     const int32_t*    group_mem;
-    // queue_policy 1 (null / 0 otherwise): the ready ring is cut into priority lanes, see Lanes below
+    // queue_policy 1 (null / 0 otherwise): the ready ring is cut into priority lanes, see Lanes (pb2_window_layout.h)
     int32_t           nlanes;         // lanes in use (1 .. PB2_PRIO_LANES)
     struct Lanes*     lanes;
     const uint8_t*    lane;           // lane of each ring-entry owner: a task (HBM windows) or a unit (GEMM windows)
 };
 
-// Priority policy (queue_policy 1): PB2_PRIO_LANES FIFO lanes, lane 0 popped first.  pb2_window_create ranks the
-// distinct priorities of the window's tasks, highest first; with at most PB2_PRIO_LANES of them a value's lane is its
-// rank r (the reference's order exactly: higher priority first, FIFO among equals), otherwise floor(r * LANES / n).
-// Each lane owns a contiguous segment of the ring as long as the entries its owners can ever push, so nothing wraps
-// and head / tail are absolute ring indices.  avail counts the entries pushed and not yet claimed: a popper takes one
-// from it before it takes a head ticket, so a ticket never runs past the entries that exist.
-#define PB2_PRIO_LANES 16
-struct Lanes {
-    Line head[PB2_PRIO_LANES];        // next slot to pop
-    Line tail[PB2_PRIO_LANES];        // next slot to push
-    Line avail[PB2_PRIO_LANES];       // entries reserved by pushers and not claimed yet (may dip below 0 briefly)
-    uint32_t begin[PB2_PRIO_LANES];   // first slot of each lane's segment
-    uint32_t ninit[PB2_PRIO_LANES];   // initial ready entries at the start of each segment
-};
-
-#define PB2_GROUP_MAX 8     // members per read group (at most 15: the count is 4 bits of group[])
-#define PB2_GROUP_FUSED 0x80000000u   // group[] of a producer that runs with its group as one unit
-
 struct PeerWin { int32_t* dep; int32_t* ring; Ctl* ctl; uint32_t cap_mask; int32_t pad; pb2_tile_t* tiles; };
 struct alignas(32) PushDev { void* dst; int32_t* dst_state; uint32_t bytes; int32_t src_tile; int32_t pad[2]; };
-
-// A task whose tiles are large is executed as several PARTS (byte slices of its tiles) by different workers: one
-// tile at HBM / NVLink speed needs the whole GPU (a 64-thread CTA keeps 4 KiB in flight; a 4 MiB tile is 1.3 us of
-// the machine, not 1 ms of one CTA).  Parts per task (1..512) live in WinDev::nparts; ring entries of HBM windows
-// are (part << 22) | task, so such a window holds at most 2^22 tasks when it has wide tasks.
-#define PB2_MAX_PARTS 512
-#define PB2_SLICE_WORDS (PB2_MAX_PARTS / 32)   // claim words per tile of sliced stage-in (stage_in_slices)
-#define PB2_ENT_MAKE(task, part) ((int32_t)(((uint32_t)(part) << 22) | (uint32_t)(task)))
-#define PB2_ENT_TASK(e)          ((int32_t)((uint32_t)(e) & 0x3FFFFFu))
-#define PB2_ENT_PART(e)          ((int)((uint32_t)(e) >> 22))
 
 __device__ __forceinline__ int task_nparts(const WinDev& w, int32_t id) { return w.nparts ? (int)w.nparts[id] : 1; }
 

@@ -5,7 +5,7 @@ device_gpu.c:2169-2174): the ready task with the highest priority first, FIFO am
 the priorities are first quantised the way the engine's windows do it (include/pb2_engine.h, queue_policy): the distinct
 priorities of the window ranked highest first, rank r -> lane r when there are at most `lanes` of them, else
 floor(r * lanes / ndistinct); then the lowest lane first, FIFO within a lane.  The engine's host code implements the
-same rule a second time (task_priority_lanes in pb2_engine.cu); this one is what the tests compare it against.
+same rule a second time (task_priority_lanes in pb2_window_plan.cpp); this one is what the tests compare it against.
 
 `replay` executes a given order with the sequential oracle (oracle/orc.py, one single-task window per task, tiles and
 their bytes carried from one to the next), so bodies, stage-in, versions and pushout follow the oracle's rules."""

@@ -207,7 +207,7 @@ class MixedDag:
         self.layout = Layout(self.doff, self.hoff, self.bytes, self.valid, dev, host)
 
     def nparts(self, part_bytes):
-        """Ring entries per task as build_gemm2_units cuts a GEMM window's HBM units (GEMM tasks: 0, not checked)."""
+        """Ring entries per task as build_gemm2_units (pb2_window_plan.cpp) cuts a GEMM window's HBM units (GEMM tasks: 0, not checked)."""
         t, out = self.dag.tasks, np.zeros(self.dag.ntasks, np.int64)
         pb = PART if part_bytes == 0 else part_bytes
         for i in range(len(t)):
@@ -292,7 +292,7 @@ def test_random_mixed_dag_one_worker_priority_lanes():
 # 3. wide CHECK parts add their mismatch counts exactly
 # ----------------------------------------------------------------------------------------------------------------------
 def part_cut(nbytes, part_bytes):
-    """(nparts, bytes per part) of a one-flow task, by the rule of build_gemm2_units / run_task_part."""
+    """(nparts, bytes per part) of a one-flow task, by the rule of build_gemm2_units (pb2_window_plan.cpp) / run_task_part."""
     np_ = min(-(-nbytes // part_bytes), 32) if part_bytes > 0 else 1
     return np_, ((nbytes // np_) + 15) & ~15
 

@@ -19,7 +19,7 @@ pytestmark = pytest.mark.gpu
 
 
 def morton(x, y):
-    """The Z-order key build_gemm2_units sorts the initial ready GEMM units by."""
+    """The Z-order key build_gemm2_units (pb2_window_plan.cpp) sorts the initial ready GEMM units by."""
     r = 0
     for b in range(16):
         r |= (((x >> b) & 1) << (2 * b + 1)) | (((y >> b) & 1) << (2 * b))
