@@ -16,7 +16,7 @@
  *
  * Plain C, plain pointers and sizes; no torch / C++ types cross this boundary.
  * The reference-shaped module API (parsec_device_module_t, parsec_gpu_task_t,
- * kernel_scheduler, ...) is layered on top of this file in pb2_device.h.
+ * kernel_scheduler, ...) is layered on top of this file in pb2_parsec.h.
  */
 #ifndef PB2_ENGINE_H
 #define PB2_ENGINE_H

@@ -1,8 +1,9 @@
-// pb2_internal.hpp -- private structures of the host side (pb2_runtime.cpp, pb2_dsl.cpp).
+// pb2_internal.hpp -- private structures of the host side (pb2_runtime.cpp, pb2_device_module.cpp, pb2_dsl.cpp).
 #pragma once
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
+#include <chrono>
 #include <deque>
 #include <functional>
 #include <map>
@@ -183,6 +184,8 @@ struct pb2_taskpool_s {
     std::function<void()> on_complete;       // PTG: final checks (e.g. CHECK task of pingpong)
 };
 
+struct pb2_device_window;                    // a window of the GPU device module, private to pb2_device_module.cpp
+
 struct pb2_device_module_s {
     pb2_context_t* ctx = nullptr;
     std::string name;
@@ -193,7 +196,7 @@ struct pb2_device_module_s {
     bool trace = false;                      // device_engine_trace at init: windows are created traced
     bool linked = false;                     // pb2_device_link_bodies: windows may run linked bodies
     pb2_engine_t* engine = nullptr;
-    std::deque<void*> inflight;              // windows launched and not yet retired (oldest first), pb2_runtime.cpp
+    std::deque<pb2_device_window*> inflight; // windows launched and not yet retired (oldest first), pb2_device_module.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up
     pb2_device_stats_t st{};
     uint32_t peer_access_mask = 0;
@@ -222,12 +225,21 @@ struct pb2_context_s {
     std::string last_error;
 };
 
-// ---- internal entry points shared by the two translation units
+// ---- internal entry points shared by the translation units
 pb2_htask_t* pb2i_new_task(pb2_taskpool_t* tp, pb2_task_class_t* tc);
 void pb2i_add_edge(pb2_taskpool_t* tp, int32_t src, int32_t dst, int dst_flow);
 void pb2i_schedule(pb2_context_t* ctx, pb2_htask_t* t);
 int  pb2i_complete_execution(pb2_context_t* ctx, pb2_htask_t* t, int device_index);
+int64_t pb2i_time_estimate(pb2_htask_t* t, pb2_device_module_t* d);
 void pb2i_lru_remove(pb2_device_module_t* dev, pb2_data_copy_t* c);
 void pb2i_lru_push_back(pb2_device_module_t* dev, int list, pb2_data_copy_t* c);
 pb2_data_copy_t* pb2i_host_copy(pb2_data_t* d);
 void* pb2i_device_visible_host_ptr(pb2_device_module_t* dev, pb2_data_t* data);
+// the GPU device module (pb2_device_module.cpp): one step of a module with pending or in-flight windows (launch what
+// is pending, retire the oldest window), and the end of every window still in flight, for pb2_fini
+int  pb2i_device_progress(pb2_device_module_t* dev);
+void pb2i_device_drain(pb2_device_module_t* dev);
+
+// PB2_TIMING=1: the runtime reports on stderr where the host time of a wait goes
+inline const bool pb2i_timing = getenv("PB2_TIMING") != nullptr;
+inline double pb2i_now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
