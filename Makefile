@@ -12,8 +12,10 @@ HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(wildcard $(CSRC
 # the HBM window kernel with application bodies: relocatable device code, linked at run time (pb2_engine_link_bodies)
 LINKED_CUBIN := build/pb2_engine_linked.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
-# the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py), as a relocatable cubin and as PTX
-TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx
+# the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py), as
+# relocatable cubins and as PTX
+TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
+                tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx
 
 all: $(LIB) linked_bodies oracle
 
@@ -34,6 +36,12 @@ tests/cuda/linked_bodies.cubin: tests/cuda/linked_bodies.cu include/pb2_device_b
 	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -Iinclude -o $@ $<
 
 tests/cuda/linked_bodies.ptx: tests/cuda/linked_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
+
+tests/cuda/checked_bodies.cubin: tests/cuda/checked_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -Iinclude -o $@ $<
+
+tests/cuda/checked_bodies.ptx: tests/cuda/checked_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
 
 oracle:

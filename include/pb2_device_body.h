@@ -23,6 +23,19 @@
  *     pb2_engine_linked_info reports.
  *   - Stores to the flows are made visible to successor tasks by the engine (barrier + fence after the body).
  *
+ * Checked bodies (pb2_engine_link_bodies_checked): `a` always points at the `args` member of a pb2_body_check_t, whose
+ * `check` and `k0` follow the 72 bytes of pb2_body_args_t; an image compiled against a header without them never reads
+ * them, and `check` is 1 only for a body id whose bit is set in the link's `checked` mask.  The engine then runs the
+ * task fused with the CHECK tasks that read its output tile (one read group), on the same worker, and calls the body in
+ * check mode.  A body in check mode
+ *   - writes its slice of the output flow (the one flow it writes) exactly as it does with check 0, and stores every
+ *     whole 4-byte element of that slice (bytes past the last whole element are stored but not checked);
+ *   - returns, from EVERY thread, a value whose low 32 bits are nonzero if and only if some element that thread stored
+ *     differs from k0, and whose high 32 bits are zero.
+ * Thread 0 returning ~0ull still aborts the window as a bad body.  A fused producer's own result is recorded as 0.  The
+ * engine decides the readers' results from one barrier over these values, and counts their mismatches exactly from the
+ * tile only when some thread reported one.  The body's stores carry whatever cache policy the body gives them.
+ *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */
 #ifndef PB2_DEVICE_BODY_H
@@ -38,6 +51,15 @@ typedef struct pb2_body_args_s {
     int          iparam[3];                    /* pb2_task_t::iparam                                               */
     float        fparam;                       /* pb2_task_t::fparam                                               */
 } pb2_body_args_t;                             /* 72 bytes on LP64 */
+
+/* The block `a` of pb2_linked_body points into (at args): a body declared checked reads check and k0 through
+ * ((const pb2_body_check_t*)a).  The layout of pb2_body_args_t is fixed by the images already compiled against it, so
+ * the two words follow it rather than grow it. */
+typedef struct pb2_body_check_s {
+    pb2_body_args_t args;
+    unsigned int    check;                     /* 1: check mode (only for ids in the link's `checked` mask), else 0 */
+    unsigned int    k0;                        /* check mode: the constant every stored element is compared with    */
+} pb2_body_check_t;                            /* 80 bytes on LP64 */
 
 #if defined(__CUDACC__)
 extern "C" __device__ unsigned long long pb2_linked_body(int body, const pb2_body_args_t* a, unsigned int* scratch);

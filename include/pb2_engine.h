@@ -267,6 +267,13 @@ int  pb2_engine_set_stage_slice_bytes(pb2_engine_t* engine, int32_t bytes);
 #define PB2_IMAGE_PTX   1
 #define PB2_IMAGE_CUBIN 2
 int  pb2_engine_link_bodies(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable);
+/* pb2_engine_link_bodies (which is this call with checked = 0), where bit i of `checked` declares that body
+ * PB2_BODY_LINKED_0 + i has a checked form (include/pb2_device_body.h).  Such a task that writes exactly one tile, does
+ * not push it out, has no wider tile, and releases a read group of that tile (CHECK readers) runs fused with the group
+ * as a built-in producer does (pb2_engine_params_t::fuse_readers): its readers never stream the tile from DRAM again.
+ * `checked` must be a subset of `sliceable`, without bits above bit 7: PB2_ERR_BAD_PARAM otherwise. */
+int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
+                                    uint32_t checked);
 /* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill
  * and stack) bytes per thread, static shared memory per CTA, and the workers a linked window runs (the engine's HBM
  * worker count, or fewer when the linked kernel's occupancy allows fewer).  Any pointer may be NULL.

@@ -154,6 +154,10 @@ int  pb2_device_get_stats(pb2_device_module_t* dev, pb2_device_stats_t* stats);
  * never holds both GEMM tasks and linked-body tasks.  A dry-run module checks the arguments and records the link.
  * PB2_ERR_EXISTS for a second image, PB2_ERR_NOT_SUPPORTED after the module's first window. */
 int  pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable);
+/* pb2_device_link_bodies with the `checked` mask of pb2_engine_link_bodies_checked (pb2_device_link_bodies is this call
+ * with checked = 0). */
+int  pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
+                                    uint32_t checked);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes
  * required in / moved H2D and D2D (with the percentage of "required"), bytes required out / written back, evictions --
  * plus the engine's own columns (windows launched, successors released by the device).  Writes a NUL-terminated

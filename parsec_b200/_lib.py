@@ -138,7 +138,7 @@ ENGINE_SYMBOLS = [
     "pb2_window_results", "pb2_window_trace", "pb2_window_part_trace",
     "pb2_partition_create", "pb2_partition_sizes", "pb2_partition_get", "pb2_partition_destroy", "pb2_partition_error",
     "pb2_partition_set_push", "pb2_partition_push_count", "pb2_partition_get_push", "pb2_window_set_push",
-    "pb2_engine_link_bodies", "pb2_engine_linked_info",
+    "pb2_engine_link_bodies", "pb2_engine_link_bodies_checked", "pb2_engine_linked_info",
 ]
 
 
@@ -182,6 +182,7 @@ def load():
     lib.pb2_window_part_trace.argtypes = [vp, vp, i32, P(i32)]
     lib.pb2_engine_set_stage_slice_bytes.argtypes = [vp, i32]
     lib.pb2_engine_link_bodies.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32]
+    lib.pb2_engine_link_bodies_checked.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32]
     lib.pb2_engine_linked_info.argtypes = [vp, P(i32), P(i32), P(i32), P(i32)]
     lib.pb2_window_export.argtypes = [vp, vp]
     lib.pb2_window_set_remote.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32]

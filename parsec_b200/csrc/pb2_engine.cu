@@ -203,7 +203,7 @@ static PlanParams params_of(const pb2_engine_t* e, int kind) {
     p.read_groups = e->params.read_groups; p.fuse_readers = e->params.fuse_readers;
     p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
     p.part_bytes = e->params.part_bytes; p.stage_slice_bytes = e->stage_slice_bytes;
-    p.linked_sliceable = e->linked_sliceable; p.next_rs_begin = e->next_rs_begin;
+    p.linked_sliceable = e->linked_sliceable; p.linked_checked = e->linked_checked; p.next_rs_begin = e->next_rs_begin;
     return p;
 }
 
@@ -362,8 +362,13 @@ static int launch_linked(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool tra
 extern "C" {
 
 int pb2_engine_link_bodies(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable) {
+    return pb2_engine_link_bodies_checked(e, image, bytes, format, sliceable, 0);
+}
+
+int pb2_engine_link_bodies_checked(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable,
+                                   uint32_t checked) {
     if (!e) return PB2_ERR_BAD_PARAM;
-    if (const char* why = link_args_error(image, bytes, format, sliceable)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
+    if (const char* why = link_args_error(image, bytes, format, sliceable, checked)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
     const DriverLink& d = driver_link();
@@ -418,7 +423,7 @@ int pb2_engine_link_bodies(pb2_engine_t* e, const void* image, size_t bytes, int
     e->linked_module = mod;
     for (int i = 0; i < 4; ++i) { e->linked_fn[i] = fn[i]; e->linked_nworkers[i] = nw[i]; }
     e->linked_regs = regs; e->linked_local = local; e->linked_smem = smem;
-    e->linked_sliceable = sliceable;
+    e->linked_sliceable = sliceable; e->linked_checked = checked;
     return PB2_SUCCESS;
 }
 

@@ -33,19 +33,23 @@ struct pb2_engine_s {
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
     // pb2_engine_link_bodies: the module of the linked HBM window kernels, each kernel and its worker count by
     // (queue_policy 1) + 2 * (trace), what the linker made of the untraced one of this engine's policy, and which
-    // linked body ids may be cut into parts (bit i: PB2_BODY_LINKED_0 + i)
+    // linked body ids may be cut into parts (bit i: PB2_BODY_LINKED_0 + i) and which have a checked form
     CUmodule linked_module = nullptr;
     CUfunction linked_fn[4] = {};
     int linked_nworkers[4] = {};
     int32_t linked_regs = 0, linked_local = 0, linked_smem = 0;
-    uint32_t linked_sliceable = 0;
+    uint32_t linked_sliceable = 0, linked_checked = 0;
 };
 
-// The argument check of pb2_engine_link_bodies and pb2_device_link_bodies: nullptr, or why the arguments are refused.
-static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable) {
+// The argument check of pb2_engine_link_bodies(_checked) and pb2_device_link_bodies(_checked): nullptr, or why the
+// arguments are refused.
+static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable, uint32_t checked) {
     if (!image || !bytes) return "linked body image is NULL or empty";
     if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
     if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";
+    if (checked >> 8) return "checked mask has bits above bit 7 (there are 8 linked body ids)";
+    // a fused producer's parts cut its tile as its readers' parts do
+    if (checked & ~sliceable) return "checked mask has a bit that is clear in the sliceable mask (a checked body must be sliceable)";
     return nullptr;
 }
 

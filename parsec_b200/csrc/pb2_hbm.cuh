@@ -72,6 +72,28 @@ static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
     __syncthreads();
 }
 
+// All threads, after the producer of a fused unit stored its slice of output flow fx and one barrier told them whether
+// any element it stored differed from the leader's constant k0: the members' results (run_fused_part).
+static __device__ __forceinline__ void fused_member_results(TaskSmem& s, GroupSmem& g, uint32_t k0, bool mismatch, int fx) {
+    const uint32_t len = s.args.bytes[fx];
+    const uint32_t* const out = static_cast<const uint32_t*>(s.args.flow[fx]);
+    // the slice's first element: k0 if nothing mismatched, else what thread 0 stored there
+    const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && len >= 4 ? (mismatch ? __ldcg(out) : k0) : 0u;
+    if (!mismatch) {
+        if (threadIdx.x == 0)
+            for (int m = 0; m < g.n; ++m) g.res[m] = g.k[m] == k0 ? first : ((unsigned long long)(len >> 2) << 32) | first;
+        return;
+    }
+    unsigned long long r0 = 0;
+#pragma unroll 1
+    for (int m = 0; m < g.n; ++m) {
+        const uint32_t k = g.k[m];
+        unsigned long long rm = r0;
+        if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne(out, len, k, s.red) << 32) | first;
+        if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = rm; }
+    }
+}
+
 // All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
 // producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
 // writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
@@ -93,24 +115,32 @@ static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, G
     const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, &ck);
     const bool mismatch = __syncthreads_or(ck.diff != 0u) != 0;
     const int fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
-    const uint32_t len = s.args.bytes[fx];
-    const uint32_t* const out = static_cast<const uint32_t*>(s.args.flow[fx]);
-    // the slice's first element: k0 if nothing mismatched, else what thread 0 stored there
-    const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && len >= 4 ? (mismatch ? __ldcg(out) : k0) : 0u;
-    if (!mismatch) {
-        if (threadIdx.x == 0)
-            for (int m = 0; m < g.n; ++m) g.res[m] = g.k[m] == k0 ? first : ((unsigned long long)(len >> 2) << 32) | first;
-        return r;
-    }
-    unsigned long long r0 = 0;
-#pragma unroll 1
-    for (int m = 0; m < g.n; ++m) {
-        const uint32_t k = g.k[m];
-        unsigned long long rm = r0;
-        if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne(out, len, k, s.red) << 32) | first;
-        if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = rm; }
-    }
+    fused_member_results(s, g, k0, mismatch, fx);
     return r;
+}
+
+// All threads, in place of a linked body (LINKED instantiations).  The body gets its slice in the 80-byte block *lp
+// (include/pb2_device_body.h), with check 0, unless the task is a checked linked producer fused with its read group:
+// then it runs in check mode against the leader's constant, its threads' return values stand for run_fused_part's
+// Checked::diff, and the members get their results as there.  Its output flow is the flow whose tile is the group's
+// (the one flow it writes, fusable() in form_read_groups).  Its stores carry the body's own cache policy: unlike the
+// built-in producers it writes without the evict-first hint.  A fused producer's own result is 0 (~0 still aborts).
+static __device__ __noinline__ unsigned long long run_linked_part(TaskSmem* sp, GroupSmem* gp, pb2_body_check_t* lp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const bool fused = g.fused != 0;
+    static_assert(sizeof(BodyArgs) % 4 == 0 && sizeof(BodyArgs) / 4 <= PB2_HBM_THREADS, "one word of BodyArgs per thread");
+    if (threadIdx.x < sizeof(BodyArgs) / 4)
+        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&s.args)[threadIdx.x];
+    if (threadIdx.x == 0) { lp->check = fused ? 1u : 0u; lp->k0 = fused ? g.k[0] : 0u; }
+    __syncthreads();
+    const unsigned long long r = pb2_linked_body(s.task.body, &lp->args, s.red);
+    if (!fused) return r;
+    const bool mismatch = __syncthreads_or((uint32_t)r != 0u) != 0;
+    int fx = 0;
+    while (fx + 1 < (int)s.task.nb_flows && !(s.task.tile[fx] == g.tile && (s.task.access[fx] & PB2_FLOW_ACCESS_WRITE))) ++fx;
+    fused_member_results(s, g, lp->k0, mismatch, fx);
+    return threadIdx.x == 0 && r == ~0ull ? ~0ull : 0ull;
 }
 
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
@@ -127,6 +157,8 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
     __shared__ unsigned long long t_start;   // the watchdog's earliest reference (pop_idle)
     PartSmem* rec = nullptr;
     if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
+    pb2_body_check_t* lk = nullptr;          // LINKED: what a linked body is handed (run_linked_part)
+    if constexpr (LINKED) { __shared__ pb2_body_check_t linked_args; lk = &linked_args; }
     if (threadIdx.x == 0) { bulk_init(bulk); t_start = globaltimer_ns(); }
     __syncthreads();
 
@@ -180,8 +212,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
             if constexpr (LINKED) {
-                if (is_linked_body(s.task.body))
-                    return (unsigned long long)pb2_linked_body(s.task.body, reinterpret_cast<const pb2_body_args_t*>(&s.args), s.red);
+                if (is_linked_body(s.task.body)) return run_linked_part(&s, &g, lk);
             }
             return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         }, rec);

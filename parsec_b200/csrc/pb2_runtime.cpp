@@ -370,13 +370,17 @@ pb2_device_module_t* pb2_mca_device_get(pb2_context_t* ctx, int idx) {
     return (ctx && idx >= 0 && idx < (int)ctx->devices.size()) ? ctx->devices[idx] : nullptr;
 }
 int pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable) {
+    return pb2_device_link_bodies_checked(dev, image, bytes, format, sliceable, 0);
+}
+int pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
+                                   uint32_t checked) {
     if (!dev || !PB2_DEV_IS_GPU(dev->type)) return PB2_ERR_BAD_PARAM;
     pb2_context_t* ctx = dev->ctx;
-    if (const char* why = link_args_error(image, bytes, format, sliceable)) { ctx->last_error = why; return PB2_ERR_BAD_PARAM; }
+    if (const char* why = link_args_error(image, bytes, format, sliceable, checked)) { ctx->last_error = why; return PB2_ERR_BAD_PARAM; }
     if (dev->linked) { ctx->last_error = "the module has linked an image already (one per module)"; return PB2_ERR_EXISTS; }
     if (dev->st.windows_launched) { ctx->last_error = "linked bodies must be linked before the module's first window"; return PB2_ERR_NOT_SUPPORTED; }
     if (!dev->dry_run) {
-        const int rc = pb2_engine_link_bodies(dev->engine, image, bytes, format, sliceable);
+        const int rc = pb2_engine_link_bodies_checked(dev->engine, image, bytes, format, sliceable, checked);
         if (rc != PB2_SUCCESS) { ctx->last_error = pb2_engine_last_error(dev->engine); return rc; }
     }
     dev->linked = true;

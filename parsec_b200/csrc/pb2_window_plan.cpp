@@ -271,11 +271,13 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
 // group's tile X without pushing it out, and X is P's widest tile (so P's parts cut X as the members' parts do): the
 // edge P -> leader leaves the device CSR and group[P] = PB2_GROUP_FUSED | the leader's group word.  The worker that
 // runs a part of P writes it to X and checks every value for the members in registers before it stores it
-// (run_fused_part); so P's body must have a checked form that writes X (fusable).  The
+// (run_fused_part); so P's body must have a checked form that writes X (fusable).  A linked body has one when its bit
+// is set in `linked_checked` (pb2_engine_link_bodies_checked); X must then be the only tile P writes, since the kernel
+// knows nothing else of what the body stores (run_linked_part).  The
 // caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
 // every task that was queued when P retired, and a fused unit runs them right after P.
 bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
-                      const pb2_tile_t* tiles, bool fuse,
+                      const pb2_tile_t* tiles, bool fuse, uint32_t linked_checked,
                       std::vector<uint32_t>& gsucc, std::vector<uint32_t>& group, std::vector<int32_t>& gmem) {
     const size_t n = tasks.size();
     std::vector<uint8_t> indeg(n, 0);                        // saturates at 2
@@ -296,6 +298,18 @@ bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, cons
     };
     // the bodies with a checked form (run_hbm_body<true>), whose output flow `out` writes X
     auto fusable = [&](const pb2_task_t& p, int32_t x) {
+        if (is_linked_body(p.body)) {
+            if (!((linked_checked >> (p.body - PB2_BODY_LINKED_0)) & 1u)) return false;
+            int writes = 0;
+            for (int f = 0; f < p.nb_flows; ++f) {
+                if (p.tile[f] < 0) continue;
+                if (tiles[p.tile[f]].bytes > tiles[x].bytes) return false;
+                if (!(p.access[f] & PB2_FLOW_ACCESS_WRITE)) continue;
+                if (p.tile[f] != x || (p.access[f] & PB2_FLOW_PUSHOUT)) return false;
+                ++writes;
+            }
+            return writes == 1;
+        }
         int out = 0;
         switch (p.body) {
         case PB2_BODY_FILL_I32: case PB2_BODY_FILL_F32: case PB2_BODY_MEMSET_U8: case PB2_BODY_INCR_I32:
@@ -385,7 +399,7 @@ void plan_hbm_window(const PlanParams& p, const uint32_t* succ, int32_t nsucc, c
     std::vector<int32_t> gmem;
     const bool grouped = !p.shared && p.read_groups >= 0 &&
                          form_read_groups(dtasks, succ, ready, nready, tiles, p.fuse_readers >= 0 && p.nworkers > 1,
-                                          gsucc, group, gmem);
+                                          p.linked_checked, gsucc, group, gmem);
     if (grouped) {
         plan.succ.swap(gsucc); plan.group.swap(group); plan.group_mem.swap(gmem);
         // a read group is led by its leader, unless a producer runs with it: then by the producer

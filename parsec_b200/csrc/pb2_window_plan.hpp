@@ -18,6 +18,7 @@ struct PlanParams {
     int nworkers = 1, nworkers_gemm = 1;
     int32_t part_bytes = 0, stage_slice_bytes = 0;
     uint32_t linked_sliceable = 0;        // bit i: PB2_BODY_LINKED_0 + i may be cut into parts
+    uint32_t linked_checked = 0;          // bit i: PB2_BODY_LINKED_0 + i has a checked form (a subset of linked_sliceable)
     const int32_t* next_rs_begin = nullptr;     // shared windows: remote out-degree CSR (not owned)
 };
 

@@ -167,12 +167,14 @@ class Engine:
         """Windows created from now on record per-task device time stamps (Window.trace)."""
         _check(self._lib.pb2_engine_set_window_trace(self._h, 1 if on else 0), "set_window_trace", self)
 
-    def link_bodies(self, image, format, sliceable=0):
+    def link_bodies(self, image, format, sliceable=0, checked=0):
         """Link the application's device bodies (include/pb2_device_body.h) into this engine's HBM window kernel, once:
         image is PTX text (format L.IMAGE_PTX) or a relocatable sm_90a cubin (L.IMAGE_CUBIN), as bytes; bit i of
-        sliceable lets tasks of body L.BODY_LINKED_0 + i be cut into byte-slice parts."""
+        sliceable lets tasks of body L.BODY_LINKED_0 + i be cut into byte-slice parts, and bit i of checked (a subset
+        of sliceable) declares that body's checked form, so that it runs fused with its read group."""
         image = bytes(image)
-        _check(self._lib.pb2_engine_link_bodies(self._h, image, len(image), format, sliceable), "pb2_engine_link_bodies", self)
+        _check(self._lib.pb2_engine_link_bodies_checked(self._h, image, len(image), format, sliceable, checked),
+               "pb2_engine_link_bodies_checked", self)
 
     def linked_info(self):
         """What the linker made of the linked kernel: registers and local bytes per thread, static shared memory per
