@@ -11,6 +11,8 @@ CPP_SRCS  := $(wildcard $(CSRC)/*.cpp)
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(wildcard $(CSRC)/*.hpp) $(wildcard include/*.h)
 # the HBM window kernel with application bodies: relocatable device code, linked at run time (pb2_engine_link_bodies)
 LINKED_CUBIN := build/pb2_engine_linked.cubin
+# the GEMM window kernel with application bodies, linked only when asked for (PB2_LINK_GEMM_WINDOWS)
+LINKED_GEMM_CUBIN := build/pb2_engine_linked_gemm.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
 # the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py), as
 # relocatable cubins and as PTX
@@ -27,8 +29,12 @@ $(LINKED_CUBIN): $(CSRC)/pb2_engine_linked.cu $(HDRS)
 	@mkdir -p build
 	$(NVCC) $(NVCCFLAGS) -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_ptxas.log || (cat build/linked_ptxas.log; exit 1)
 
-$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN)
-	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -o $@ $<
+$(LINKED_GEMM_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_ptxas.log || (cat build/linked_gemm_ptxas.log; exit 1)
+
+$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN)
+	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -DPB2_LINKED_GEMM_CUBIN='"$(abspath $(LINKED_GEMM_CUBIN))"' -o $@ $<
 
 linked_bodies: $(TEST_BODIES)
 
@@ -48,7 +54,8 @@ oracle:
 	$(MAKE) -C oracle
 
 clean:
-	rm -f $(LIB) build_ptxas.log $(LINKED_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log $(TEST_BODIES)
+	rm -f $(LIB) build_ptxas.log $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
+	      build/linked_gemm_ptxas.log $(TEST_BODIES)
 	$(MAKE) -C oracle clean
 
 .PHONY: all linked_bodies oracle clean

@@ -10,22 +10,25 @@
  *
  *     extern "C" __device__ unsigned long long pb2_linked_body(int body, const pb2_body_args_t* a, unsigned int* scratch);
  *
- * with the task's body id unchanged.  Contract:
- *   - All 64 threads of the worker CTA call it together (uniform control flow), so __syncthreads() is allowed.
+ * with the task's body id unchanged.  Linked with PB2_LINK_GEMM_WINDOWS (pb2_engine_link_bodies_ex), GEMM windows run
+ * it too.  Contract:
+ *   - All threads of the worker CTA call it together (uniform control flow), so __syncthreads() is allowed: 64 in HBM
+ *     windows, 384 in GEMM windows; use blockDim.x.
  *   - a: this part's slice of every flow (flow[f] / bytes[f]; NULL / 0 for a flow without a tile), the slice's first
  *     4-byte element inside the tile (elem0), the part index and the task's immediates.  A body whose bit is clear in
  *     the `sliceable` mask of the link call always runs as one part over whole tiles (part 0, elem0 0); a body whose bit
  *     is set may be cut into byte-slice parts like the built-in element-wise bodies, each part run by another worker.
- *   - scratch: 32 words of the worker's shared memory, free for the body's use.
+ *   - scratch: 32 words of the worker's shared memory, free for the body's use (32 in GEMM windows too).
  *   - The result is taken from thread 0.  A multi-part task keeps the result of part 0.
  *   - Returning ~0ull aborts the window as a bad body (pb2_window_wait: PB2_ERR_BAD_PARAM).
  *   - Static __shared__ variables are allowed; they count against the linked kernel's occupancy, which
- *     pb2_engine_linked_info reports.
+ *     pb2_engine_linked_info reports (pb2_engine_linked_gemm_info for GEMM windows, where they come on top of the
+ *     kernel's 193 KiB of dynamic shared memory).
  *   - Stores to the flows are made visible to successor tasks by the engine (barrier + fence after the body).
  *
  * Checked bodies (pb2_engine_link_bodies_checked): `a` always points at the `args` member of a pb2_body_check_t, whose
  * `check` and `k0` follow the 72 bytes of pb2_body_args_t; an image compiled against a header without them never reads
- * them, and `check` is 1 only for a body id whose bit is set in the link's `checked` mask.  The engine then runs the
+ * them, and `check` is 1 only for a body id whose bit is set in the link's `checked` mask, and never in a GEMM window.  The engine then runs the
  * task fused with the CHECK tasks that read its output tile (one read group), on the same worker, and calls the body in
  * check mode.  A body in check mode
  *   - writes its slice of the output flow (the one flow it writes) exactly as it does with check 0, and stores every

@@ -71,7 +71,8 @@ enum pb2_body_e {
                                * flow1 (B, N x K row-major == K x N column-major), fp32 accumulate in registers
                                * iparam[0]=M, iparam[1]=N, iparam[2]=K (each tile edge)                     */
     PB2_BODY_LINKED_0   = 20, /* .. PB2_BODY_LINKED_7: the application's device body, linked into the HBM window
-                               * kernel by pb2_engine_link_bodies (include/pb2_device_body.h); HBM windows only   */
+                               * kernel by pb2_engine_link_bodies (include/pb2_device_body.h); HBM windows, and
+                               * GEMM windows when linked with PB2_LINK_GEMM_WINDOWS                              */
     PB2_BODY_LINKED_7   = 27,
     PB2_BODY_USER       = 31, /* host-side only: the chore is a user `submit` callback that enqueues its own CUDA work
                                * on a stream (device_gpu.h:49-51); such tasks never enter an engine window           */
@@ -274,18 +275,35 @@ int  pb2_engine_link_bodies(pb2_engine_t* engine, const void* image, size_t byte
  * `checked` must be a subset of `sliceable`, without bits above bit 7: PB2_ERR_BAD_PARAM otherwise. */
 int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
                                     uint32_t checked);
+/* pb2_engine_link_bodies_checked (which is this call with flags = 0) with link flags:
+ *   PB2_LINK_GEMM_WINDOWS  also link the engine's relocatable build of the GEMM window kernel.  GEMM windows (kind 1)
+ *                          whose tasks name a linked body then run it beside their GEMM units, and GEMM windows without
+ *                          one keep the built-in kernel.  In a GEMM window a body runs on the 384 threads of the GEMM
+ *                          worker and never in check mode.  Its static shared memory comes on top of the GEMM kernel's
+ *                          dynamic shared memory: PB2_ERR_NOT_SUPPORTED, and the engine stays unlinked, when the two do
+ *                          not fit on one SM.  The flag costs link time (four more kernels), so it is opt-in.
+ * PB2_ERR_BAD_PARAM for any other bit. */
+#define PB2_LINK_GEMM_WINDOWS 0x1u
+int  pb2_engine_link_bodies_ex(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
+                               uint32_t checked, uint32_t flags);
 /* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill
  * and stack) bytes per thread, static shared memory per CTA, and the workers a linked window runs (the engine's HBM
  * worker count, or fewer when the linked kernel's occupancy allows fewer).  Any pointer may be NULL.
  * PB2_ERR_NOT_FOUND before pb2_engine_link_bodies. */
 int  pb2_engine_linked_info(pb2_engine_t* engine, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers);
+/* The same for the untraced linked GEMM window kernel of the engine's queue policy; nworkers: the workers a GEMM window
+ * with linked tasks runs (the engine's GEMM worker count, or fewer when the kernel's occupancy allows fewer).
+ * PB2_ERR_NOT_FOUND unless the engine linked with PB2_LINK_GEMM_WINDOWS. */
+int  pb2_engine_linked_gemm_info(pb2_engine_t* engine, int32_t* regs, int32_t* local_bytes, int32_t* static_smem,
+                                 int32_t* nworkers);
 
 /* --- one window of the DAG ---
  * tasks[ntasks], succ[nsucc] (CSR via succ_begin/succ_count), tiles[ntiles] and the ids of
  * the tasks that are ready at submission (startup tasks, parsec.c:1724-1740).
  * 'kind' selects the kernel instantiation: 0 = HBM bodies, 1 = tensor-core GEMM bodies.  An HBM window with a task of
- * a linked body (PB2_BODY_LINKED_0 .. _7) runs the engine's linked kernel (pb2_engine_link_bodies); such a task in a
- * GEMM window, in a shared window or on an engine without an image is refused (PB2_ERR_NOT_SUPPORTED). */
+ * a linked body (PB2_BODY_LINKED_0 .. _7) runs the engine's linked kernel (pb2_engine_link_bodies), and so does a GEMM
+ * window with one when the engine linked with PB2_LINK_GEMM_WINDOWS; such a task in any other GEMM window, in a shared
+ * window or on an engine without an image is refused (PB2_ERR_NOT_SUPPORTED). */
 int  pb2_window_create(pb2_engine_t* engine, pb2_window_t** window, int kind,
                        const pb2_task_t* tasks, int32_t ntasks,
                        const uint32_t* succ, int32_t nsucc,

@@ -151,13 +151,18 @@ int  pb2_device_get_stats(pb2_device_module_t* dev, pb2_device_stats_t* stats);
 /* Link the application's device bodies into the module's engine (pb2_engine_link_bodies: image, format, sliceable as
  * there), before the module's first window.  Afterwards DTD chores may name PB2_BODY_LINKED_0 .. _7 once every GPU
  * module of the context has linked an image, and the module's windows run those tasks in the linked HBM kernel; a window
- * never holds both GEMM tasks and linked-body tasks.  A dry-run module checks the arguments and records the link.
+ * never holds both GEMM tasks and linked-body tasks unless the link set PB2_LINK_GEMM_WINDOWS (pb2_device_link_bodies_ex).  A dry-run module checks the arguments and records the link.
  * PB2_ERR_EXISTS for a second image, PB2_ERR_NOT_SUPPORTED after the module's first window. */
 int  pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable);
 /* pb2_device_link_bodies with the `checked` mask of pb2_engine_link_bodies_checked (pb2_device_link_bodies is this call
  * with checked = 0). */
 int  pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
                                     uint32_t checked);
+/* pb2_device_link_bodies_checked with the link flags of pb2_engine_link_bodies_ex (pb2_device_link_bodies_checked is this
+ * call with flags = 0).  With PB2_LINK_GEMM_WINDOWS a window may hold GEMM tasks and linked-body tasks together: GEMM
+ * chains and the application's bodies around them run in one GEMM window.  A dry-run module records the flag. */
+int  pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
+                               uint32_t checked, uint32_t flags);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes
  * required in / moved H2D and D2D (with the percentage of "required"), bytes required out / written back, evictions --
  * plus the engine's own columns (windows launched, successors released by the device).  Writes a NUL-terminated

@@ -42,6 +42,8 @@ BODY_INCR_F32, BODY_AXPY_F32, BODY_MEMSET_U8, BODY_ADD_AT_I32, BODY_GEMM_BF16 = 
 # application device bodies linked into HBM windows (pb2_engine_link_bodies): BODY_LINKED_0 + i, i < 8
 BODY_LINKED_0, BODY_LINKED_7 = 20, 27
 IMAGE_PTX, IMAGE_CUBIN = 1, 2
+# pb2_engine_link_bodies_ex flags: also link the GEMM window kernel, so linked bodies run in GEMM windows too
+LINK_GEMM_WINDOWS = 0x1
 
 TASK_DEPS_MASK = 0x01
 TILE_INVALID, TILE_STAGING, TILE_VALID = 0, 1, 2
@@ -139,6 +141,7 @@ ENGINE_SYMBOLS = [
     "pb2_partition_create", "pb2_partition_sizes", "pb2_partition_get", "pb2_partition_destroy", "pb2_partition_error",
     "pb2_partition_set_push", "pb2_partition_push_count", "pb2_partition_get_push", "pb2_window_set_push",
     "pb2_engine_link_bodies", "pb2_engine_link_bodies_checked", "pb2_engine_linked_info",
+    "pb2_engine_link_bodies_ex", "pb2_engine_linked_gemm_info",
 ]
 
 
@@ -184,6 +187,8 @@ def load():
     lib.pb2_engine_link_bodies.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32]
     lib.pb2_engine_link_bodies_checked.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32]
     lib.pb2_engine_linked_info.argtypes = [vp, P(i32), P(i32), P(i32), P(i32)]
+    lib.pb2_engine_link_bodies_ex.argtypes = [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32]
+    lib.pb2_engine_linked_gemm_info.argtypes = [vp, P(i32), P(i32), P(i32), P(i32)]
     lib.pb2_window_export.argtypes = [vp, vp]
     lib.pb2_window_set_remote.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32]
     lib.pb2_partition_set_push.argtypes = [vp, C.c_int]

@@ -172,8 +172,9 @@ static bool predicted_on_device(pb2_device_module_t* dev, pb2_htask_t* s) {
 // it touches.  An engine window takes tile GEMMs and HBM bodies together, so that a GEMM chain and the element-wise
 // tasks around it are released on the device instead of through the host; its kind is decided by the closure: 1 (the
 // GEMM kernel, which also runs HBM bodies) when it holds a GEMM task, else 0.  User submit tasks never mix with engine
-// tasks, and tasks of linked bodies (which run in the linked HBM kernel only) never mix with GEMM tasks: the first of
-// the two kinds the closure takes in keeps the other out of this window.
+// tasks.  Unless the module linked its bodies with PB2_LINK_GEMM_WINDOWS, tasks of linked bodies (which then run in the
+// linked HBM kernel only) never mix with GEMM tasks: the first of the two kinds the closure takes in keeps the other out
+// of this window.
 static int take_closure(pb2_device_module_t* dev, pb2_device_window& w, size_t max_roots) {
     if (dev->pending.empty()) return PB2_SUCCESS;
     pb2_taskpool_t* const tp = dev->pending.front()->ec->tp;
@@ -181,7 +182,8 @@ static int take_closure(pb2_device_module_t* dev, pb2_device_window& w, size_t m
     int engine_side = 0;                        // PB2_BODY_GEMM_BF16 or PB2_BODY_LINKED_0 once the window holds one
     auto fits = [&](const pb2_htask_t* t) {
         if ((t->body == PB2_BODY_USER) != want_user) return false;
-        const int side = t->body == PB2_BODY_GEMM_BF16 ? PB2_BODY_GEMM_BF16 : pb2::is_linked_body(t->body) ? PB2_BODY_LINKED_0 : 0;
+        const int side = dev->linked_gemm ? 0 : t->body == PB2_BODY_GEMM_BF16 ? PB2_BODY_GEMM_BF16
+                                              : pb2::is_linked_body(t->body) ? PB2_BODY_LINKED_0 : 0;
         if (side && engine_side && side != engine_side) return false;
         if (side) engine_side = side;
         return true;

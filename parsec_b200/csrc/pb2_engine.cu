@@ -199,6 +199,7 @@ static int encode_tensor_maps(pb2_engine_t* e, const WindowPlan& plan, const pb2
 static PlanParams params_of(const pb2_engine_t* e, int kind) {
     PlanParams p;
     p.kind = kind; p.shared = e->shared_windows; p.trace = e->window_trace; p.linked_image = e->linked_module != nullptr;
+    p.linked_gemm = e->linked_gemm;
     p.queue_policy = e->params.queue_policy; p.gemm_mode = e->params.gemm_mode;
     p.read_groups = e->params.read_groups; p.fuse_readers = e->params.fuse_readers;
     p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
@@ -301,6 +302,7 @@ static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out
 // application's image, linked by the driver's JIT linker
 // ---------------------------------------------------------------------------------------------
 extern "C" const unsigned char pb2_linked_engine_image[], pb2_linked_engine_image_end[];
+extern "C" const unsigned char pb2_linked_gemm_image[], pb2_linked_gemm_image_end[];
 
 // pb2_engine_hbm_kernel<PRIO, TRACE, true> by (PRIO) + 2 * (TRACE)
 static const char* const kLinkedKernels[4] = {
@@ -308,6 +310,13 @@ static const char* const kLinkedKernels[4] = {
     "_ZN3pb221pb2_engine_hbm_kernelILb1ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
     "_ZN3pb221pb2_engine_hbm_kernelILb0ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
     "_ZN3pb221pb2_engine_hbm_kernelILb1ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
+};
+// pb2_engine_gemm2_kernel<PRIO, TRACE, true> (pb2_engine_linked_gemm.cu), the same order
+static const char* const kLinkedGemmKernels[4] = {
+    "_ZN3pb223pb2_engine_gemm2_kernelILb0ELb0ELb1EEEvNS_7Win2DevE",
+    "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb0ELb1EEEvNS_7Win2DevE",
+    "_ZN3pb223pb2_engine_gemm2_kernelILb0ELb1ELb1EEEvNS_7Win2DevE",
+    "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb1ELb1EEEvNS_7Win2DevE",
 };
 
 // The driver calls the linking point needs, fetched through the runtime (as cuTensorMapEncodeTiled is): the library
@@ -321,11 +330,12 @@ struct DriverLink {
     decltype(&cuModuleUnload) module_unload = nullptr;
     decltype(&cuModuleGetFunction) get_function = nullptr;
     decltype(&cuFuncGetAttribute) func_attr = nullptr;
+    decltype(&cuFuncSetAttribute) func_set_attr = nullptr;
     decltype(&cuOccupancyMaxActiveBlocksPerMultiprocessor) occupancy = nullptr;
     decltype(&cuLaunchKernel) launch = nullptr;
     bool complete() const {
         return link_create && link_add && link_complete && link_destroy && module_load && module_unload && get_function &&
-               func_attr && occupancy && launch;
+               func_attr && func_set_attr && occupancy && launch;
     }
 };
 
@@ -341,6 +351,7 @@ static const DriverLink& driver_link() {
         get("cuLinkCreate", r.link_create); get("cuLinkAddData", r.link_add); get("cuLinkComplete", r.link_complete);
         get("cuLinkDestroy", r.link_destroy); get("cuModuleLoadData", r.module_load); get("cuModuleUnload", r.module_unload);
         get("cuModuleGetFunction", r.get_function); get("cuFuncGetAttribute", r.func_attr);
+        get("cuFuncSetAttribute", r.func_set_attr);
         get("cuOccupancyMaxActiveBlocksPerMultiprocessor", r.occupancy); get("cuLaunchKernel", r.launch);
         return r;
     }();
@@ -359,6 +370,27 @@ static int launch_linked(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool tra
     return PB2_SUCCESS;
 }
 
+// The linked GEMM kernel of a window's queue policy and trace on the engine stream, as pb2_gemm2_launch launches the
+// built-in one: 384 threads, the operand ring in dynamic shared memory.
+static int launch_linked_gemm(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool trace) {
+    const int i = (lanes ? 1 : 0) + (trace ? 2 : 0);
+    Win2Dev gd = g;
+    void* args[] = {&gd};
+    const CUresult r = driver_link().launch(e->linked_gemm_fn[i], (unsigned)e->linked_gemm_nworkers[i], 1, 1, gemm::kThreads, 1, 1,
+                                            gemm::kSmemBytes, reinterpret_cast<CUstream>(e->stream), args, nullptr);
+    if (r != CUDA_SUCCESS) { e->last_error = "cuLaunchKernel of the linked GEMM window kernel failed (CUresult " + std::to_string((int)r) + ")"; return PB2_ERR_DEVICE; }
+    return PB2_SUCCESS;
+}
+
+// What the linker made of kernel fn: registers, local bytes per thread, static shared memory.
+static CUresult kernel_resources(CUfunction fn, int32_t* regs, int32_t* local, int32_t* smem) {
+    const DriverLink& d = driver_link();
+    CUresult r = d.func_attr(regs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn);
+    if (r == CUDA_SUCCESS) r = d.func_attr(local, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn);
+    if (r == CUDA_SUCCESS) r = d.func_attr(smem, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, fn);
+    return r;
+}
+
 extern "C" {
 
 int pb2_engine_link_bodies(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable) {
@@ -367,8 +399,14 @@ int pb2_engine_link_bodies(pb2_engine_t* e, const void* image, size_t bytes, int
 
 int pb2_engine_link_bodies_checked(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable,
                                    uint32_t checked) {
+    return pb2_engine_link_bodies_ex(e, image, bytes, format, sliceable, checked, 0);
+}
+
+int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, int format, uint32_t sliceable,
+                              uint32_t checked, uint32_t flags) {
     if (!e) return PB2_ERR_BAD_PARAM;
-    if (const char* why = link_args_error(image, bytes, format, sliceable, checked)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
+    if (const char* why = link_args_error(image, bytes, format, sliceable, checked, flags)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
+    const bool gemm_windows = (flags & PB2_LINK_GEMM_WINDOWS) != 0;
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
     const DriverLink& d = driver_link();
@@ -390,6 +428,9 @@ int pb2_engine_link_bodies_checked(pb2_engine_t* e, const void* image, size_t by
     if (r == CUDA_SUCCESS)
         r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(pb2_linked_engine_image),
                        (size_t)(pb2_linked_engine_image_end - pb2_linked_engine_image), "pb2_engine_linked.cubin", 0, nullptr, nullptr);
+    if (r == CUDA_SUCCESS && gemm_windows)
+        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(pb2_linked_gemm_image),
+                       (size_t)(pb2_linked_gemm_image_end - pb2_linked_gemm_image), "pb2_engine_linked_gemm.cubin", 0, nullptr, nullptr);
     if (r == CUDA_SUCCESS)
         r = d.link_add(st, format == PB2_IMAGE_PTX ? CU_JIT_INPUT_PTX : CU_JIT_INPUT_CUBIN, const_cast<void*>(data), size,
                        "linked bodies", 0, nullptr, nullptr);
@@ -411,19 +452,49 @@ int pb2_engine_link_bodies_checked(pb2_engine_t* e, const void* image, size_t by
         nw[i] = std::max(1, std::min(e->nworkers, e->prop.multiProcessorCount * occ));
     }
     const int mine = e->params.queue_policy == 1 ? 1 : 0;
-    int regs = 0, local = 0, smem = 0;
-    if (r == CUDA_SUCCESS) r = d.func_attr(&regs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn[mine]);
-    if (r == CUDA_SUCCESS) r = d.func_attr(&local, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn[mine]);
-    if (r == CUDA_SUCCESS) r = d.func_attr(&smem, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, fn[mine]);
+    int32_t regs = 0, local = 0, smem = 0;
+    if (r == CUDA_SUCCESS) r = kernel_resources(fn[mine], &regs, &local, &smem);
     if (r != CUDA_SUCCESS) {
         d.module_unload(mod);
         e->last_error = "the linked module has no usable HBM window kernel (CUresult " + std::to_string((int)r) + ")";
         return PB2_ERR_DEVICE;
     }
+    // The GEMM kernels take the operand ring as dynamic shared memory; the bodies' static shared memory comes on top of
+    // it.  A kernel that cannot take the ring beside it (the attribute is refused) or fits no CTA on an SM fails the link.
+    CUfunction gfn[4] = {}, too_big = nullptr;
+    int gnw[4] = {};
+    int32_t gregs = 0, glocal = 0, gsmem = 0;
+    for (int i = 0; gemm_windows && i < 4 && r == CUDA_SUCCESS && !too_big; ++i) {
+        int occ = 0;
+        r = d.get_function(&gfn[i], mod, kLinkedGemmKernels[i]);
+        if (r != CUDA_SUCCESS) break;
+        if (d.func_set_attr(gfn[i], CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, gemm::kSmemBytes) != CUDA_SUCCESS) { too_big = gfn[i]; break; }
+        r = d.occupancy(&occ, gfn[i], gemm::kThreads, gemm::kSmemBytes);
+        if (r == CUDA_SUCCESS && occ == 0) too_big = gfn[i];
+        gnw[i] = std::max(1, std::min(e->nworkers_gemm, e->prop.multiProcessorCount * occ));
+    }
+    if (gemm_windows && r == CUDA_SUCCESS && !too_big) r = kernel_resources(gfn[mine], &gregs, &glocal, &gsmem);
+    if (r != CUDA_SUCCESS) {
+        d.module_unload(mod);
+        e->last_error = "the linked module has no usable GEMM window kernel (CUresult " + std::to_string((int)r) + ")";
+        return PB2_ERR_DEVICE;
+    }
+    if (too_big) {
+        int32_t sm = 0, unused = 0;
+        kernel_resources(too_big, &unused, &unused, &sm);
+        d.module_unload(mod);
+        e->last_error = "the linked GEMM window kernel does not fit on an SM: " + std::to_string(sm) +
+                        " bytes of static shared memory (the kernel's and the bodies') beside its " +
+                        std::to_string(gemm::kSmemBytes) + " bytes of dynamic shared memory";
+        return PB2_ERR_NOT_SUPPORTED;
+    }
     e->linked_module = mod;
     for (int i = 0; i < 4; ++i) { e->linked_fn[i] = fn[i]; e->linked_nworkers[i] = nw[i]; }
     e->linked_regs = regs; e->linked_local = local; e->linked_smem = smem;
     e->linked_sliceable = sliceable; e->linked_checked = checked;
+    e->linked_gemm = gemm_windows;
+    for (int i = 0; i < 4; ++i) { e->linked_gemm_fn[i] = gfn[i]; e->linked_gemm_nworkers[i] = gnw[i]; }
+    e->linked_gemm_regs = gregs; e->linked_gemm_local = glocal; e->linked_gemm_smem = gsmem;
     return PB2_SUCCESS;
 }
 
@@ -434,6 +505,19 @@ int pb2_engine_linked_info(pb2_engine_t* e, int32_t* regs, int32_t* local_bytes,
     if (local_bytes) *local_bytes = e->linked_local;
     if (static_smem) *static_smem = e->linked_smem;
     if (nworkers) *nworkers = e->linked_nworkers[e->params.queue_policy == 1 ? 1 : 0];
+    return PB2_SUCCESS;
+}
+
+int pb2_engine_linked_gemm_info(pb2_engine_t* e, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    if (!e->linked_gemm) {
+        e->last_error = "the engine has not linked the GEMM window kernels (pb2_engine_link_bodies_ex with PB2_LINK_GEMM_WINDOWS)";
+        return PB2_ERR_NOT_FOUND;
+    }
+    if (regs) *regs = e->linked_gemm_regs;
+    if (local_bytes) *local_bytes = e->linked_gemm_local;
+    if (static_smem) *static_smem = e->linked_gemm_smem;
+    if (nworkers) *nworkers = e->linked_gemm_nworkers[e->params.queue_policy == 1 ? 1 : 0];
     return PB2_SUCCESS;
 }
 
@@ -845,6 +929,10 @@ int pb2_window_start(pb2_window_t* w) {
             else if (lanes) PB2_CUDA(e, pb2_hbm_prio_launch(g.w, nw, th, e->stream));
             else pb2_engine_hbm_kernel<false, false><<<nw, th, 0, e->stream>>>(g.w, TraceDev{});
             PB2_CUDA(e, cudaGetLastError());
+        } else if (w->linked) {
+            const int rc = launch_linked_gemm(e, g, lanes, trace);
+            if (rc != PB2_SUCCESS) return rc;
+            w->g.fresh_tmaps = 0;
         } else {
             const int nw = e->nworkers_gemm;
             int rc = trace ? (lanes ? pb2_gemm2_prio_trace_launch(g, nw, e->stream) : pb2_gemm2_trace_launch(g, nw, e->stream))

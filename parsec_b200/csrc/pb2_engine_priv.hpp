@@ -39,11 +39,19 @@ struct pb2_engine_s {
     int linked_nworkers[4] = {};
     int32_t linked_regs = 0, linked_local = 0, linked_smem = 0;
     uint32_t linked_sliceable = 0, linked_checked = 0;
+    // linked with PB2_LINK_GEMM_WINDOWS: the same module's linked GEMM window kernels, their worker counts and what the
+    // linker made of the untraced one of this engine's policy (else linked_gemm is false and the rest stays zero)
+    bool linked_gemm = false;
+    CUfunction linked_gemm_fn[4] = {};
+    int linked_gemm_nworkers[4] = {};
+    int32_t linked_gemm_regs = 0, linked_gemm_local = 0, linked_gemm_smem = 0;
 };
 
-// The argument check of pb2_engine_link_bodies(_checked) and pb2_device_link_bodies(_checked): nullptr, or why the
-// arguments are refused.
-static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable, uint32_t checked) {
+// The argument check of pb2_engine_link_bodies(_checked, _ex) and pb2_device_link_bodies(_checked, _ex): nullptr, or why
+// the arguments are refused.
+static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable, uint32_t checked,
+                                          uint32_t flags = 0) {
+    if (flags & ~(uint32_t)PB2_LINK_GEMM_WINDOWS) return "link flags have an unknown bit (PB2_LINK_GEMM_WINDOWS is the only flag)";
     if (!image || !bytes) return "linked body image is NULL or empty";
     if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
     if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";

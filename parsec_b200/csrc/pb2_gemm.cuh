@@ -294,11 +294,60 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
     }
 }
 
+// Consumer warpgroup `cw` (0 or 1) of a GEMM unit's part: sub-tiles job.part, job.part + nparts, ..., rows m0 + 64 * cw
+// .. of each, the whole chain into one accumulator, added into C at Cbase.  stage / phase: the consumers' place in the
+// smem ring, carried from one part to the next.
+__device__ __forceinline__ void consume_part(const Job& job, uint8_t* smem, uint64_t* full, uint64_t* empty, uint8_t* Cbase,
+                                             uint32_t& stage, uint32_t& phase, int cw) {
+    const int kblocks = (job.K + BK - 1) / BK;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int sub = job.part; sub < job.nsub; sub += job.nparts) {
+        const int m0 = (sub % job.mblocks) * BM, n0 = (sub / job.mblocks) * BN, Nj = min(BN, job.N - n0);
+        {   // pull the sub-tile's C rows into L2 now, so that the read-modify-write after the chain does not pay DRAM latency
+            const int t = threadIdx.x - 128, row = m0 + (t >> 1);
+            if (row < job.M)
+                for (int b = (t & 1) * 128; b < Nj * 2; b += 256)
+                    asm volatile("prefetch.global.L2 [%0];" :: "l"(Cbase + ((size_t)row * job.N + n0) * 2 + b));
+        }
+        mma_kblocks(acc, smem, full, empty, stage, phase, job.seg_count * kblocks, true, cw);
+        epilogue_add(acc, Cbase, job.N, m0 + cw * 64, n0, job.M, n0 + Nj);
+    }
+}
+
+// consume_part out of line, for the LINKED kernels.  In relocatable code ptxas serializes every wgmma of a function that
+// reaches a call it cannot see into (C7509 for the extern pb2_linked_body; silently for an indirect or weak callee),
+// and the kernel reaches the application's body; this function makes no call, so its wgmma groups stay pipelined.
+// Under the standard call ABI it saves the callee-saved registers its 128 contiguous accumulator registers cover (ptxas
+// counts them as spill stores) once per call, outside the k-block loop.  The ring position goes in and comes back by
+// value (stage in the low word, phase in the high word), so nothing of the caller's lives in local memory across the call.
+static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_t* smem, uint8_t* Cbase, uint64_t ring, int cw) {
+    uint32_t stage = (uint32_t)ring, phase = (uint32_t)(ring >> 32);
+    consume_part(sp->job, smem, sp->full, sp->empty, Cbase, stage, phase, cw);
+    return stage | ((uint64_t)phase << 32);
+}
+
+// All 384 threads, in place of a linked body in a GEMM window (LINKED instantiations): the application's body gets this
+// part's slice in the 80-byte block *lp (include/pb2_device_body.h) with check 0, and ts.red as scratch.  GEMM windows
+// have no read groups, so a linked body never runs in check mode here.
+static __device__ __noinline__ unsigned long long run_linked_gemm_body(TaskSmem* sp, pb2_body_check_t* lp) {
+    TaskSmem& s = *sp;
+    if (threadIdx.x < sizeof(BodyArgs) / 4)
+        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&s.args)[threadIdx.x];
+    if (threadIdx.x == 0) { lp->check = 0u; lp->k0 = 0u; }
+    __syncthreads();
+    return pb2_linked_body(s.task.body, &lp->args, s.red);
+}
+
 }  // namespace gemm
 
 // PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: write a record of every part into g.trace (PartSmem,
 // then trace_part); the untraced instantiations never touch it.
-template <bool PRIO, bool TRACE>
+// LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body; built only in
+// pb2_engine_linked_gemm.cu, as relocatable device code that pb2_engine_link_bodies_ex links with the application's
+// image when PB2_LINK_GEMM_WINDOWS is set.  The other instantiations compile as if the flag did not exist.
+template <bool PRIO, bool TRACE, bool LINKED = false>
 __global__ void __launch_bounds__(gemm::kThreads, 1)
 pb2_engine_gemm2_kernel(Win2Dev g) {
     using namespace gemm;
@@ -308,6 +357,8 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
     __shared__ Shared sh;
     PartSmem* rec = nullptr;
     if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
+    pb2_body_check_t* lk = nullptr;          // LINKED: what a linked body is handed (run_linked_gemm_body)
+    if constexpr (LINKED) { __shared__ pb2_body_check_t linked_args; lk = &linked_args; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
@@ -402,21 +453,12 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 }
             } else if (wg >= 1) {
                 // ===== consumers: rows m0 + 64 * cw .. of each sub-tile, the whole chain into one accumulator
-                const int cw = wg - 1;
                 uint8_t* Cbase = reinterpret_cast<uint8_t*>(w.tiles[job.tileC].dev_ptr);
-                float acc[128];
-#pragma unroll
-                for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-                for (int sub = job.part; sub < job.nsub; sub += job.nparts) {
-                    const int m0 = (sub % job.mblocks) * BM, n0 = (sub / job.mblocks) * BN, Nj = min(BN, job.N - n0);
-                    {   // pull the sub-tile's C rows into L2 now, so that the read-modify-write after the chain does not pay DRAM latency
-                        const int t = threadIdx.x - 128, row = m0 + (t >> 1);
-                        if (row < job.M)
-                            for (int b = (t & 1) * 128; b < Nj * 2; b += 256)
-                                asm volatile("prefetch.global.L2 [%0];" :: "l"(Cbase + ((size_t)row * job.N + n0) * 2 + b));
-                    }
-                    mma_kblocks(acc, smem, sh.full, sh.empty, c_stage, c_phase, job.seg_count * kblocks, true, cw);
-                    epilogue_add(acc, Cbase, job.N, m0 + cw * 64, n0, job.M, n0 + Nj);
+                if constexpr (LINKED) {
+                    const uint64_t ring = consume_part_outlined(&sh, smem, Cbase, c_stage | ((uint64_t)c_phase << 32), wg - 1);
+                    c_stage = (uint32_t)ring; c_phase = (uint32_t)(ring >> 32);
+                } else {
+                    consume_part(job, smem, sh.full, sh.empty, Cbase, c_stage, c_phase, wg - 1);
                 }
                 fence_proxy_async();
             }
@@ -430,7 +472,10 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             __syncthreads();
             const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
-                const unsigned long long body_r = run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
+                unsigned long long body_r;
+                if constexpr (LINKED) body_r = is_linked_body(sh.ts.task.body) ? run_linked_gemm_body(&sh.ts, lk)
+                                                                                 : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
+                else body_r = run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
                 fence_proxy_async();
                 return body_r;
             }, rec);

@@ -374,16 +374,21 @@ int pb2_device_link_bodies(pb2_device_module_t* dev, const void* image, size_t b
 }
 int pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
                                    uint32_t checked) {
+    return pb2_device_link_bodies_ex(dev, image, bytes, format, sliceable, checked, 0);
+}
+int pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
+                              uint32_t checked, uint32_t flags) {
     if (!dev || !PB2_DEV_IS_GPU(dev->type)) return PB2_ERR_BAD_PARAM;
     pb2_context_t* ctx = dev->ctx;
-    if (const char* why = link_args_error(image, bytes, format, sliceable, checked)) { ctx->last_error = why; return PB2_ERR_BAD_PARAM; }
+    if (const char* why = link_args_error(image, bytes, format, sliceable, checked, flags)) { ctx->last_error = why; return PB2_ERR_BAD_PARAM; }
     if (dev->linked) { ctx->last_error = "the module has linked an image already (one per module)"; return PB2_ERR_EXISTS; }
     if (dev->st.windows_launched) { ctx->last_error = "linked bodies must be linked before the module's first window"; return PB2_ERR_NOT_SUPPORTED; }
     if (!dev->dry_run) {
-        const int rc = pb2_engine_link_bodies_checked(dev->engine, image, bytes, format, sliceable, checked);
+        const int rc = pb2_engine_link_bodies_ex(dev->engine, image, bytes, format, sliceable, checked, flags);
         if (rc != PB2_SUCCESS) { ctx->last_error = pb2_engine_last_error(dev->engine); return rc; }
     }
     dev->linked = true;
+    dev->linked_gemm = (flags & PB2_LINK_GEMM_WINDOWS) != 0;
     return PB2_SUCCESS;
 }
 

@@ -37,7 +37,7 @@ int validate_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks
         if (kind == 0 && t.body == PB2_BODY_GEMM_BF16) {
             *why = "GEMM body in an HBM-kind window (use kind 1)"; return PB2_ERR_BAD_PARAM; }
         if (is_linked_body(t.body)) {
-            const char* no = kind != 0 ? "linked body in a GEMM window (linked bodies run in HBM windows only)"
+            const char* no = kind != 0 && !p.linked_gemm ? "linked body in a GEMM window (linked bodies run in HBM windows only)"
                            : p.shared ? "linked body in a shared window (not supported)"
                            : !p.linked_image ? "linked body id, but the engine has not linked an image (pb2_engine_link_bodies)"
                            : nullptr;
@@ -183,9 +183,11 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
         const bool g = is_gemm(h);
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
-        // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body
+        // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body; a linked
+        // body whose sliceable bit is clear runs as one part over whole tiles
+        const bool whole = is_linked_body(tasks[h].body) && !((p.linked_sliceable >> (tasks[h].body - PB2_BODY_LINKED_0)) & 1u);
         u.nparts = g ? std::min(((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN), gemm::kMaxParts)
-                     : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
+                 : whole ? 1 : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
             segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});

@@ -14,6 +14,7 @@ struct PlanParams {
     bool shared = false;                  // pb2_engine_set_shared_windows
     bool trace = false;                   // pb2_engine_set_window_trace
     bool linked_image = false;            // the engine has linked an image (pb2_engine_link_bodies)
+    bool linked_gemm = false;             // ... with PB2_LINK_GEMM_WINDOWS: linked bodies may run in GEMM windows too
     int queue_policy = 0, gemm_mode = 0, read_groups = 0, fuse_readers = 0;     // pb2_engine_params_t
     int nworkers = 1, nworkers_gemm = 1;
     int32_t part_bytes = 0, stage_slice_bytes = 0;
@@ -55,7 +56,7 @@ struct WindowPlan {
     RunShape run;
     int32_t slice_bytes = 0;              // stage-in slice size (WinDev::part_bytes)
     int32_t nlanes = 0;                   // queue_policy 1: lanes in use
-    bool linked = false;                  // a task names a linked body: the window runs the engine's linked kernel
+    bool linked = false;                  // a task names a linked body: the window runs the engine's linked kernel of its kind
     std::vector<int32_t> task_entry;      // per task: its ring entry with (parts - 1) in the part field
     std::vector<int32_t> task_unit;       // traced windows, per task: the task that leads its scheduling entity
     std::vector<PartEntity> part_entities;     // traced windows: the ring-entry owners by leading task, their records

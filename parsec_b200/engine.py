@@ -167,20 +167,28 @@ class Engine:
         """Windows created from now on record per-task device time stamps (Window.trace)."""
         _check(self._lib.pb2_engine_set_window_trace(self._h, 1 if on else 0), "set_window_trace", self)
 
-    def link_bodies(self, image, format, sliceable=0, checked=0):
+    def link_bodies(self, image, format, sliceable=0, checked=0, gemm_windows=False):
         """Link the application's device bodies (include/pb2_device_body.h) into this engine's HBM window kernel, once:
         image is PTX text (format L.IMAGE_PTX) or a relocatable sm_90a cubin (L.IMAGE_CUBIN), as bytes; bit i of
         sliceable lets tasks of body L.BODY_LINKED_0 + i be cut into byte-slice parts, and bit i of checked (a subset
-        of sliceable) declares that body's checked form, so that it runs fused with its read group."""
+        of sliceable) declares that body's checked form, so that it runs fused with its read group.  gemm_windows
+        (L.LINK_GEMM_WINDOWS) links the GEMM window kernel too, so that GEMM windows may hold linked tasks."""
         image = bytes(image)
-        _check(self._lib.pb2_engine_link_bodies_checked(self._h, image, len(image), format, sliceable, checked),
-               "pb2_engine_link_bodies_checked", self)
+        flags = L.LINK_GEMM_WINDOWS if gemm_windows else 0
+        _check(self._lib.pb2_engine_link_bodies_ex(self._h, image, len(image), format, sliceable, checked, flags),
+               "pb2_engine_link_bodies_ex", self)
 
     def linked_info(self):
         """What the linker made of the linked kernel: registers and local bytes per thread, static shared memory per
         CTA, and the workers a linked window runs."""
         v = [C.c_int32() for _ in range(4)]
         _check(self._lib.pb2_engine_linked_info(self._h, *[C.byref(x) for x in v]), "pb2_engine_linked_info", self)
+        return dict(zip(("regs", "local_bytes", "static_smem", "nworkers"), (x.value for x in v)))
+
+    def linked_gemm_info(self):
+        """linked_info for the linked GEMM window kernel (link_bodies(..., gemm_windows=True))."""
+        v = [C.c_int32() for _ in range(4)]
+        _check(self._lib.pb2_engine_linked_gemm_info(self._h, *[C.byref(x) for x in v]), "pb2_engine_linked_gemm_info", self)
         return dict(zip(("regs", "local_bytes", "static_smem", "nworkers"), (x.value for x in v)))
 
     def ipc_export(self, dev_ptr):

@@ -29,6 +29,7 @@ PARSEC_SYMBOLS = [
     "pb2_init", "pb2_fini", "pb2_mca_param_set_int", "pb2_mca_param_get_int", "pb2_device_cuda_module_init",
     "pb2_mca_device_registration_complete", "pb2_nb_devices", "pb2_mca_device_get", "pb2_device_get_stats",
     "pb2_devices_statistics_string", "pb2_device_link_bodies", "pb2_device_link_bodies_checked",
+    "pb2_device_link_bodies_ex",
     "pb2_device_index", "pb2_device_type", "pb2_device_memory_register", "pb2_device_memory_unregister",
     "pb2_device_memory_release", "pb2_device_data_advise", "pb2_device_taskpool_register",
     "pb2_device_taskpool_unregister", "pb2_device_kernel_scheduler", "pb2_device_zone_malloc", "pb2_device_zone_free",
@@ -68,6 +69,7 @@ def lib():
         "pb2_device_index": (C.c_int, [vp]), "pb2_device_type": (C.c_int, [vp]),
         "pb2_device_link_bodies": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32]),
         "pb2_device_link_bodies_checked": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32]),
+        "pb2_device_link_bodies_ex": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32]),
         "pb2_device_memory_register": (C.c_int, [vp, vp, vp, C.c_size_t]),
         "pb2_device_memory_unregister": (C.c_int, [vp, vp, vp]), "pb2_device_memory_release": (C.c_int, [vp]),
         "pb2_device_data_advise": (C.c_int, [vp, vp, C.c_int]),
@@ -161,12 +163,13 @@ class Context:
         self.l.pb2_devices_statistics_string(self.h, buf, n)
         return buf.value.decode()
 
-    def link_bodies(self, dev, image, format, sliceable=0, checked=0):
+    def link_bodies(self, dev, image, format, sliceable=0, checked=0, gemm_windows=False):
         """Link the application's device bodies into module dev's engine before its first window (Engine.link_bodies;
-        a dry-run module checks the arguments and records the link)."""
+        a dry-run module checks the arguments and records the link).  gemm_windows: GEMM chains and linked tasks may
+        then share a window."""
         image = bytes(image)
-        _chk(self.l.pb2_device_link_bodies_checked(dev, image, len(image), format, sliceable, checked),
-             "pb2_device_link_bodies_checked")
+        _chk(self.l.pb2_device_link_bodies_ex(dev, image, len(image), format, sliceable, checked, 1 if gemm_windows else 0),
+             "pb2_device_link_bodies_ex")
 
     def stats(self, dev):
         st = DeviceStats()
