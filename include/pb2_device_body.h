@@ -28,7 +28,8 @@
  *
  * Checked bodies (pb2_engine_link_bodies_checked): `a` always points at the `args` member of a pb2_body_check_t, whose
  * `check` and `k0` follow the 72 bytes of pb2_body_args_t; an image compiled against a header without them never reads
- * them, and `check` is 1 only for a body id whose bit is set in the link's `checked` mask, and never in a GEMM window.  The engine then runs the
+ * them, and `check` is 1 only for a body id whose bit is set in the link's `checked` mask (in HBM windows, and in GEMM windows
+ * linked with PB2_LINK_GEMM_WINDOWS, on their 384 threads).  The engine then runs the
  * task fused with the CHECK tasks that read its output tile (one read group), on the same worker, and calls the body in
  * check mode.  A body in check mode
  *   - writes its slice of the output flow (the one flow it writes) exactly as it does with check 0, and stores every

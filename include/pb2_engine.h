@@ -154,10 +154,13 @@ typedef struct pb2_engine_params_s {
     int32_t  part_bytes;       /* HBM bodies: a task whose largest tile exceeds this many bytes is run as up to 512
                                 * parts (byte slices) by different workers (default 256 KiB, <0 = never split);
                                 * pb2_engine_set_part_bytes changes it for the windows created afterwards       */
-    int32_t  read_groups;      /* HBM windows that are not shared: 0 = a run of consecutive out-edges of one task into
-                                * CHECK readers of the same tile (that edge their only input) is executed as one group
-                                * that streams the tile once for all its members (default); < 0 = every task alone  */
-    int32_t  fuse_readers;     /* HBM windows that are not shared, with read groups on and more than one worker:
+    int32_t  read_groups;      /* windows that are not shared: 0 = a run of consecutive out-edges of one task into
+                                * CHECK readers of the same tile (that edge their only input) is executed as one
+                                * group that streams the tile once for all its members (default); < 0 = every task
+                                * alone.  A GEMM task never joins a group; a GEMM window with queue_policy 1 and one
+                                * worker forms none                                                              */
+    int32_t  fuse_readers;     /* windows that are not shared, with read groups on and more than one worker of the
+                                * window's kind (nworkers, nworkers_gemm):
                                 * 0 = a producer that writes the tile its first read group checks runs with that
                                 * group as one unit, each chunk written and then checked while it is still in L2
                                 * (default); < 0 = the producer and the group run one after the other            */
@@ -279,7 +282,7 @@ int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, siz
  *   PB2_LINK_GEMM_WINDOWS  also link the engine's relocatable build of the GEMM window kernel.  GEMM windows (kind 1)
  *                          whose tasks name a linked body then run it beside their GEMM units, and GEMM windows without
  *                          one keep the built-in kernel.  In a GEMM window a body runs on the 384 threads of the GEMM
- *                          worker and never in check mode.  Its static shared memory comes on top of the GEMM kernel's
+ *                          worker, in check mode too when its bit is set in `checked`.  Its static shared memory comes on top of the GEMM kernel's
  *                          dynamic shared memory: PB2_ERR_NOT_SUPPORTED, and the engine stays unlinked, when the two do
  *                          not fit on one SM.  The flag costs link time (four more kernels), so it is opt-in.
  * PB2_ERR_BAD_PARAM for any other bit. */

@@ -18,7 +18,7 @@
 // dependency trace is unchanged); only the intermediate bf16 roundings of C disappear.  Scheduling entities on the
 // device are units (counter-mode dependency words), ring entries are (part, unit).
 // The other tasks of the DAG (HBM bodies: FILL, SCALE, COPY, AXPY, CHECK, ... between the chains) are units of one
-// task; one wider than part_bytes is cut into byte-slice parts like a wide task of an HBM window.  A whole CTA runs each
+// task, or of one read group with the producer that runs with it (as in HBM windows); one wider than part_bytes is cut into byte-slice parts like a wide task of an HBM window.  A whole CTA runs each
 // part with the HBM workers' run_task_part (pb2_worker.cuh), and the last part to finish retires the unit.
 //
 // One CTA per SM is one worker.  Three warpgroups (384 threads):
@@ -222,24 +222,31 @@ struct Job {
 struct Shared {
     alignas(16) Job job;
     TaskSmem ts;                    // non-GEMM units: run_task_part's state; GEMM units stage in with its need / decide
+    GroupSmem gs;                   // non-GEMM units: the read group the unit's first task leads or runs with
     uint64_t full[kStages];
     uint64_t empty[kStages];
 };
 
-// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges.
+// whole warp: the unit is complete (all parts): retire its members in chain order, release its out-edges.  The members
+// of a read group retire in member order, right after the producer that runs with them (flag bit 2), which is the
+// unit's first member: they saw the version it wrote (seen_version of a group led by its first member was stored with
+// each part, group_part_results).
 template <bool PRIO>
 __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& u) {
     const WinDev& w = g.w;
     const int lane = threadIdx.x & 31;
     const int L = u.seg_count;
     unsigned long long ebase = 0, rbase = 0;
+    uint32_t vx = 0;
     if (lane == 0) {
         ebase = atomicAdd(&w.ctl->evt.v, (unsigned long long)(2 * L));
         rbase = atomicAdd(&w.ctl->retired.v, (unsigned long long)L);
         *reinterpret_cast<volatile unsigned long long*>(&w.ctl->progress_ns.v) = globaltimer_ns();
+        if (u.flags & 4) vx = epilog_written_flows(w, w.tasks[g.segs[u.seg_begin].task], w.tasks[g.segs[u.seg_begin + 1].task].tile[0]);
     }
     ebase = __shfl_sync(0xffffffffu, ebase, 0);
     rbase = __shfl_sync(0xffffffffu, rbase, 0);
+    vx = __shfl_sync(0xffffffffu, vx, 0);
     const uint32_t cver = (u.flags & 1) ? *reinterpret_cast<volatile uint32_t*>(&w.tiles[u.tileC].version) : 0u;
     for (int i = lane; i < L; i += 32) {
         const GSeg s = g.segs[u.seg_begin + i];
@@ -252,6 +259,8 @@ __device__ __forceinline__ void retire_unit_warp(const Win2Dev& g, const GUnit& 
             w.seen_version[s.task * PB2_MAX_FLOWS + 1] = *reinterpret_cast<volatile uint32_t*>(&w.tiles[s.tileB].version);
             w.seen_version[s.task * PB2_MAX_FLOWS + 2] = cver + (uint32_t)i;
             w.result[s.task] = 0;
+        } else if (u.flags & 4) {
+            if (i > 0) w.seen_version[s.task * PB2_MAX_FLOWS] = vx;     // the producer's epilog ran above
         } else {
             epilog_written_flows(w, w.tasks[s.task]);      // part 0 stored seen_version (run_task_part)
         }
@@ -328,18 +337,6 @@ static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_
     return stage | ((uint64_t)phase << 32);
 }
 
-// All 384 threads, in place of a linked body in a GEMM window (LINKED instantiations): the application's body gets this
-// part's slice in the 80-byte block *lp (include/pb2_device_body.h) with check 0, and ts.red as scratch.  GEMM windows
-// have no read groups, so a linked body never runs in check mode here.
-static __device__ __noinline__ unsigned long long run_linked_gemm_body(TaskSmem* sp, pb2_body_check_t* lp) {
-    TaskSmem& s = *sp;
-    if (threadIdx.x < sizeof(BodyArgs) / 4)
-        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&s.args)[threadIdx.x];
-    if (threadIdx.x == 0) { lp->check = 0u; lp->k0 = 0u; }
-    __syncthreads();
-    return pb2_linked_body(s.task.body, &lp->args, s.red);
-}
-
 }  // namespace gemm
 
 // PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: write a record of every part into g.trace (PartSmem,
@@ -357,7 +354,7 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
     __shared__ Shared sh;
     PartSmem* rec = nullptr;
     if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
-    pb2_body_check_t* lk = nullptr;          // LINKED: what a linked body is handed (run_linked_gemm_body)
+    pb2_body_check_t* lk = nullptr;          // LINKED: what a linked body is handed (run_linked_part)
     if constexpr (LINKED) { __shared__ pb2_body_check_t linked_args; lk = &linked_args; }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -464,23 +461,29 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             }
         } else {
             // ---------------- an HBM body in the DAG (element-wise task, panel stand-in): the whole CTA runs this
-            // part's byte slice of its flows in place, as a worker of an HBM window does.  Later units read the tiles
-            // through TMA: the generic stores of a stage-in and of the body are followed by fence.proxy.async.
+            // part's byte slice of its flows in place, as a worker of an HBM window does, with the read group its
+            // task leads or runs with (a producer fused with its group: run_fused_part, or run_linked_part in check
+            // mode).  Later units read the tiles through TMA: the generic stores of a stage-in and of the body are
+            // followed by fence.proxy.async.
             const int32_t id = g.segs[job.seg_begin].task;
             if (threadIdx.x < 4) reinterpret_cast<uint4*>(&sh.ts.task)[threadIdx.x] =
                 __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
+            const uint32_t gd = load_group_members(w, id, sh.gs);
+            if (threadIdx.x == 0) { sh.gs.n = (int)(gd & 15u); sh.gs.fused = (gd & PB2_GROUP_FUSED) != 0; }
             __syncthreads();
             const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
                 unsigned long long body_r;
-                if constexpr (LINKED) body_r = is_linked_body(sh.ts.task.body) ? run_linked_gemm_body(&sh.ts, lk)
-                                                                                 : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
-                else body_r = run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
+                if constexpr (LINKED) body_r = is_linked_body(sh.ts.task.body) ? run_linked_part<kThreads>(&sh.ts, &sh.gs, lk)
+                                             : sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs)
+                                                           : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
+                else body_r = sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs) : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
                 fence_proxy_async();
                 return body_r;
             }, rec);
+            if (sh.gs.n && !sh.gs.fused) group_part_results<kThreads, TRACE>(w, sh.ts, sh.gs, id, job.part, r, rec);
             // CHECK parts add their mismatch counts; the first element comes from part 0
-            if (threadIdx.x == 0) store_result(w, sh.ts.task, id, job.part, job.nparts, r);
+            if (threadIdx.x == 0) store_part_results(w, sh.ts.task, id, job.part, job.nparts, r, sh.gs);
         }
         __threadfence();
         __syncthreads();             // every store of the part is done and visible

@@ -1,5 +1,5 @@
-// pb2_hbm.cuh -- the persistent engine kernel of HBM-body windows (pb2_engine_hbm_kernel) and what it runs besides
-// the shared worker code of pb2_worker.cuh: read groups and fused producer units.  Instantiated for the FIFO ready ring
+// pb2_hbm.cuh -- the persistent engine kernel of HBM-body windows (pb2_engine_hbm_kernel); what one worker does with a
+// task, a read group or a fused producer unit is the shared worker code of pb2_worker.cuh.  Instantiated for the FIFO ready ring
 // in pb2_engine.cu and for priority lanes (queue_policy 1) in pb2_engine_prio.cu, and traced (window trace) in
 // pb2_engine_trace.cu and pb2_engine_prio_trace.cu: each translation unit holds one instantiation, because a second
 // kernel calling the same __noinline__ helpers makes ptxas give them the standard call ABI, which costs the kernel a
@@ -33,116 +33,6 @@ constexpr int kHbmWorkersPerSm = 8;
 #ifndef PB2_HBM_THREADS
 #define PB2_HBM_THREADS 64
 #endif
-// A read group in flight on one worker: its members (the leader first), their CHECK constants and out-edges, this
-// part's results.  The retire path takes what it needs of a member from here, not from its descriptor.
-struct GroupSmem {
-    int32_t n;                              // members; 0: the popped task runs alone
-    int32_t fused;                          // the popped task is a producer that runs with this group as one unit
-    int32_t tile;                           // the tile the members read
-    int32_t mem[PB2_GROUP_MAX];
-    uint32_t k[PB2_GROUP_MAX];
-    int32_t succ_begin[PB2_GROUP_MAX];
-    int32_t succ_count[PB2_GROUP_MAX];
-    unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
-};
-
-
-// All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
-// bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
-//  - k equal to the leader's: the leader's result;
-//  - the slice held nothing but the leader's constant: every element mismatches (the first element is the same);
-//  - otherwise the member's slice is counted again, exactly, as a failing CHECK counts it.
-static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
-    TaskSmem& s = *sp;
-    GroupSmem& g = *gp;
-    const unsigned long long r0 = g.res[0];
-#pragma unroll 1
-    for (int i = 1; i < g.n; ++i) {
-        const uint32_t k = g.k[i];
-        if (k == g.k[0] || !(r0 >> 32)) {
-            if (threadIdx.x == 0) g.res[i] = k == g.k[0] ? r0 : ((unsigned long long)(s.args.bytes[0] >> 2) << 32) | (uint32_t)r0;
-            continue;
-        }
-        if (threadIdx.x == 0) s.args.iparam[0] = (int32_t)k;
-        __syncthreads();
-        const unsigned long long r = run_hbm_body(PB2_BODY_CHECK_I32, s.args, s.red);
-        if (threadIdx.x == 0) g.res[i] = r;
-        __syncthreads();
-    }
-    __syncthreads();
-}
-
-// All threads, after the producer of a fused unit stored its slice of output flow fx and one barrier told them whether
-// any element it stored differed from the leader's constant k0: the members' results (run_fused_part).
-static __device__ __forceinline__ void fused_member_results(TaskSmem& s, GroupSmem& g, uint32_t k0, bool mismatch, int fx) {
-    const uint32_t len = s.args.bytes[fx];
-    const uint32_t* const out = static_cast<const uint32_t*>(s.args.flow[fx]);
-    // the slice's first element: k0 if nothing mismatched, else what thread 0 stored there
-    const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && len >= 4 ? (mismatch ? __ldcg(out) : k0) : 0u;
-    if (!mismatch) {
-        if (threadIdx.x == 0)
-            for (int m = 0; m < g.n; ++m) g.res[m] = g.k[m] == k0 ? first : ((unsigned long long)(len >> 2) << 32) | first;
-        return;
-    }
-    unsigned long long r0 = 0;
-#pragma unroll 1
-    for (int m = 0; m < g.n; ++m) {
-        const uint32_t k = g.k[m];
-        unsigned long long rm = r0;
-        if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne(out, len, k, s.red) << 32) | first;
-        if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = rm; }
-    }
-}
-
-// All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
-// producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
-// writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
-// before they leave the SM: the producer's checked body (run_hbm_body<true>) writes its output flow as it would alone,
-// and every thread ORs (element ^ the leader's constant) of each value it stores while the value is still in registers.
-// Its stores carry an L2 evict-first policy: nobody reads the tile back here (the resident Ex05 step is about 3 %
-// shorter than with the default policy, DESIGN.md §8).  One barrier then tells every thread whether the slice held
-// anything but the leader's constant, and the members get group_results' rules:
-//  - nothing else: a member with the leader's constant counts no mismatch, any other member counts every element;
-//  - otherwise the slice is counted again, exactly, from the tile (the barrier made the CTA's stores visible to its
-//    threads, and the loads go through L2), for the leader and every member whose constant differs from the leader's.
-// Returns the producer's result (thread 0); the caller's barrier and __threadfence() order the stores before the release.
-static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp) {
-    TaskSmem& s = *sp;
-    GroupSmem& g = *gp;
-    const int body = s.task.body;
-    const uint32_t k0 = g.k[0];
-    Checked ck{k0, 0u, l2_evict_first()};
-    const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, &ck);
-    const bool mismatch = __syncthreads_or(ck.diff != 0u) != 0;
-    const int fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
-    fused_member_results(s, g, k0, mismatch, fx);
-    return r;
-}
-
-// All threads, in place of a linked body (LINKED instantiations).  The body gets its slice in the 80-byte block *lp
-// (include/pb2_device_body.h), with check 0, unless the task is a checked linked producer fused with its read group:
-// then it runs in check mode against the leader's constant, its threads' return values stand for run_fused_part's
-// Checked::diff, and the members get their results as there.  Its output flow is the flow whose tile is the group's
-// (the one flow it writes, fusable() in form_read_groups).  Its stores carry the body's own cache policy: unlike the
-// built-in producers it writes without the evict-first hint.  A fused producer's own result is 0 (~0 still aborts).
-static __device__ __noinline__ unsigned long long run_linked_part(TaskSmem* sp, GroupSmem* gp, pb2_body_check_t* lp) {
-    TaskSmem& s = *sp;
-    GroupSmem& g = *gp;
-    const bool fused = g.fused != 0;
-    static_assert(sizeof(BodyArgs) % 4 == 0 && sizeof(BodyArgs) / 4 <= PB2_HBM_THREADS, "one word of BodyArgs per thread");
-    if (threadIdx.x < sizeof(BodyArgs) / 4)
-        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&s.args)[threadIdx.x];
-    if (threadIdx.x == 0) { lp->check = fused ? 1u : 0u; lp->k0 = fused ? g.k[0] : 0u; }
-    __syncthreads();
-    const unsigned long long r = pb2_linked_body(s.task.body, &lp->args, s.red);
-    if (!fused) return r;
-    const bool mismatch = __syncthreads_or((uint32_t)r != 0u) != 0;
-    int fx = 0;
-    while (fx + 1 < (int)s.task.nb_flows && !(s.task.tile[fx] == g.tile && (s.task.access[fx] & PB2_FLOW_ACCESS_WRITE))) ++fx;
-    fused_member_results(s, g, lp->k0, mismatch, fx);
-    return threadIdx.x == 0 && r == ~0ull ? ~0ull : 0ull;
-}
-
 // PRIO: queue_policy 1 (priority lanes, pop_prio); the FIFO instantiation is the kernel as it was without them.
 // TRACE: write a record of every part into tr (PartSmem, then trace_part); the untraced instantiations never touch tr.
 // LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body (include/pb2_device_body.h); built
@@ -177,6 +67,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         if (threadIdx.x < 4) reinterpret_cast<uint4*>(&s.task)[threadIdx.x] =
             __ldg(reinterpret_cast<const uint4*>(&w.tasks[id]) + threadIdx.x);
         {
+            // load_group_members, written out: called, it costs this kernel spills at its 80-register budget
             const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
             const int gn = (int)(gd & 15u);
             const uint32_t gb = (gd & ~PB2_GROUP_FUSED) >> 4;
@@ -212,24 +103,11 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
             if constexpr (LINKED) {
-                if (is_linked_body(s.task.body)) return run_linked_part(&s, &g, lk);
+                if (is_linked_body(s.task.body)) return run_linked_part<PB2_HBM_THREADS>(&s, &g, lk);
             }
-            return g.fused ? run_fused_part(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
+            return g.fused ? run_fused_part<PB2_HBM_THREADS>(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         }, rec);
-        if (g.n && !g.fused) {
-            // the leader's part stored the version it saw; every member saw the same one
-            if (threadIdx.x == 0) {
-                g.res[0] = r;
-                if (part == 0) {
-                    const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.seen_version[(size_t)id * PB2_MAX_FLOWS]);
-                    for (int i = 1; i < g.n; ++i) w.seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
-                }
-            }
-            __syncthreads();
-            group_results(&s, &g);
-            // the members' results are part of the body; the readers push nothing out
-            if (TRACE && threadIdx.x == 0) rec->t_exec = rec->t_out = globaltimer_ns();
-        }
+        if (g.n && !g.fused) group_part_results<PB2_HBM_THREADS, TRACE>(w, s, g, id, part, r, rec);
 
         if (threadIdx.x < 32) {
             __threadfence();   // release side: the body's stores (all threads, ordered by the barrier) become
@@ -237,8 +115,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
             if (threadIdx.x == 0) {
                 const pb2_task_t& t = s.task;
                 const int gn = g.n;
-                for (int i = 0; i < gn; ++i) store_check_result(w, g.mem[i], nparts, g.res[i]);   // members are CHECK bodies
-                if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
+                store_part_results(w, t, id, part, nparts, r, g);
                 // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
                 int last = 1;
                 if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }

@@ -56,7 +56,7 @@ struct WinDev {
     int32_t           part_bytes;
     const uint16_t*   nparts;         // HBM windows with wide tasks: parts per task (null: every task is one part)
     int32_t           remote_units;   // remote targets are (parts-1) << 27 | unit of a fused-GEMM window, not << 22 | task
-    // read groups of HBM windows (form_read_groups in pb2_window_plan.cpp; null: none): task id leads the members
+    // read groups (form_read_groups in pb2_window_plan.cpp; null: none): task id leads the members
     // group_mem[group[id] >> 4 .. + (group[id] & 15)), itself first; a count of 0 means the task runs alone.  The other
     // members are never released or popped on their own.  A producer fused with a group (PB2_GROUP_FUSED set in its
     // group word) names that group's members, the leader included, and its edge to the leader is gone from succ[].

@@ -55,7 +55,7 @@ struct GUnit {                  // 48 bytes, read-only
                                     // min(ceil(widest tile / part_bytes), kMaxParts) byte slices (1 in shared windows)
     int32_t tileC;                  // GEMM units: the C tile; -1 otherwise
     int32_t M, N, K;
-    int32_t flags;                  // bit0 is_gemm, bit1 pushout C
+    int32_t flags;                  // bit0 is_gemm, bit1 pushout C, bit2 a producer that runs with its read group
     int32_t pad;
 };
 struct GSeg { int32_t task, tileA, tileB, pad; };

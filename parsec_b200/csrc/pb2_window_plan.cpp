@@ -1,5 +1,5 @@
 // pb2_window_plan.cpp -- the host plan of an engine window (pb2_window_plan.hpp): argument checks, read groups and fused
-// producers of HBM windows, units of GEMM windows, parts, priority lanes and the ring image, part records.
+// producers, units of GEMM windows, parts, priority lanes and the ring image, part records.
 #include <string.h>
 #include <algorithm>
 #include <functional>
@@ -141,8 +141,10 @@ void plan_part_records(const std::vector<int32_t>& lead, const std::vector<int32
 // ---------------------------------------------------------------------------------------------
 // The plan of a GEMM window: its units are the ring-entry owners.  task_lane (queue_policy 1, else empty): a unit's
 // lane is the lane of its first task, for all its parts.  A unit that runs an HBM body is cut into
-// task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.
-int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ, int32_t nsucc,
+// task_parts(..., kMaxParts) byte-slice parts, as HBM windows cut their wide tasks.  The window's read groups
+// (plan.group, formed on plan.tasks and plan.succ before) are units of HBM bodies: a group's members in member order,
+// the leader first, preceded by the producer when one runs with them (flag bit 2); its parts are the first task's.
+int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
                       const int32_t* ready, int32_t nready, bool fuse, const int32_t* rs_begin,
                       const std::vector<uint8_t>& task_lane, const pb2_tile_t* tiles, int32_t part_bytes,
                       WindowPlan& plan, Owners& own, const char** why) {
@@ -172,6 +174,13 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
             if (memcmp(tasks[u].iparam, tasks[t].iparam, sizeof tasks[u].iparam)) continue;
             next[u] = t;
         }
+    // a read group runs as one unit: its members follow its first task (a GEMM task is never in one, see fusable)
+    for (int32_t t = 0; t < (int32_t)plan.group.size(); ++t) {
+        const uint32_t gd = plan.group[(size_t)t];
+        const int32_t* mem = plan.group_mem.data() + ((gd & ~PB2_GROUP_FUSED) >> 4);
+        if (gd & PB2_GROUP_FUSED) next[(size_t)t] = mem[0];             // the producer, then the group it runs with
+        else for (uint32_t i = 1; i < (gd & 15u); ++i) next[(size_t)mem[i - 1]] = mem[i];     // t leads the group
+    }
     std::vector<uint8_t> has_pred((size_t)ntasks, 0);
     for (int32_t u = 0; u < ntasks; ++u) if (next[u] >= 0) has_pred[next[u]] = 1;
     std::vector<GUnit>& units = plan.units;
@@ -188,6 +197,7 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
         const bool whole = is_linked_body(tasks[h].body) && !((p.linked_sliceable >> (tasks[h].body - PB2_BODY_LINKED_0)) & 1u);
         u.nparts = g ? std::min(((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN), gemm::kMaxParts)
                  : whole ? 1 : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
+        if (!plan.group.empty() && (plan.group[(size_t)h] & PB2_GROUP_FUSED)) u.flags |= 4;
         for (int32_t t = h; t >= 0; t = next[t]) {
             unit_of[t] = (int32_t)units.size();
             segs.push_back(GSeg{t, g ? tasks[t].tile[0] : -1, g ? tasks[t].tile[1] : -1, 0});
@@ -203,7 +213,7 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
             const int32_t t = segs[u.seg_begin + i].task;
             for (int32_t e = 0; e < tasks[t].succ_count; ++e) {
                 const int32_t d = PB2_SUCC_TASK(succ[tasks[t].succ_begin + e]);
-                if (d == next[t] && PB2_SUCC_FLOW(succ[tasks[t].succ_begin + e]) == 2) continue;   // the fused link
+                if (is_gemm(t) && d == next[t] && PB2_SUCC_FLOW(succ[tasks[t].succ_begin + e]) == 2) continue;   // the fused link
                 usucc.push_back(unit_of[d]);
             }
         }
@@ -253,12 +263,11 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
         for (size_t u = 0; u < units.size(); ++u) { lead[u] = segs[(size_t)units[u].seg_begin].task; np[u] = units[u].nparts; }
         plan_part_records(lead, np, plan);
     }
-    plan.succ.assign(succ, succ + nsucc);
     return PB2_SUCCESS;
 }
 
 // ---------------------------------------------------------------------------------------------
-// read groups of HBM windows
+// read groups
 // ---------------------------------------------------------------------------------------------
 // A run of >= 2 consecutive out-edges of one task whose targets all
 //   - have that edge as their only input (in-degree 1, not ready at start; counter goal 1, or the edge's one mask bit),
@@ -363,9 +372,24 @@ bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, cons
     return true;
 }
 
+// The read groups and fused producers of a window of either kind (form_read_groups), with the engine's settings:
+// none in a shared window (it is released into by task id from other GPUs and pushes per task: its tasks run alone) or
+// with read_groups < 0, no fusion with fuse_readers < 0 or with one worker of the window's kind (nworkers).  Rewrites
+// the out-edges of plan.tasks and sets plan.succ, and plan.group and group_mem when a group formed (returns true then).
+bool plan_read_groups(const PlanParams& p, int nworkers, const uint32_t* succ, int32_t nsucc, const pb2_tile_t* tiles,
+                      const int32_t* ready, int32_t nready, WindowPlan& plan) {
+    std::vector<uint32_t> gsucc, group;
+    std::vector<int32_t> gmem;
+    const bool grouped = !p.shared && p.read_groups >= 0 &&
+                         form_read_groups(plan.tasks, succ, ready, nready, tiles, p.fuse_readers >= 0 && nworkers > 1,
+                                          p.linked_checked, gsucc, group, gmem);
+    if (grouped) { plan.succ.swap(gsucc); plan.group.swap(group); plan.group_mem.swap(gmem); }
+    else plan.succ.assign(succ, succ + nsucc);
+    return grouped;
+}
+
 // The plan of an HBM window: its tasks (plan.tasks) are the ring-entry owners, each cut into task_parts(...,
-// PB2_MAX_PARTS) parts.  task_lane: as for build_gemm2_units.  Forms the read groups, which rewrites the out-edges of
-// plan.tasks.
+// PB2_MAX_PARTS) parts.  task_lane: as for build_gemm2_units.  Forms the read groups (plan_read_groups).
 void plan_hbm_window(const PlanParams& p, const uint32_t* succ, int32_t nsucc, const pb2_tile_t* tiles, int32_t ntiles,
                      const int32_t* ready, int32_t nready, const std::vector<uint8_t>& task_lane, WindowPlan& plan,
                      Owners& own) {
@@ -396,14 +420,7 @@ void plan_hbm_window(const PlanParams& p, const uint32_t* succ, int32_t nsucc, c
     plan.run.parts = plan.run.claims = extra_parts > 0;
     for (int32_t i = 0; i < ntiles && !plan.run.claims; ++i)
         plan.run.claims = plan.slice_bytes > 0 && tiles[i].state != PB2_TILE_VALID && tiles[i].bytes > (uint32_t)plan.slice_bytes;
-    // shared windows are released into by task id from other GPUs and push per task: their tasks run alone
-    std::vector<uint32_t> gsucc, group;
-    std::vector<int32_t> gmem;
-    const bool grouped = !p.shared && p.read_groups >= 0 &&
-                         form_read_groups(dtasks, succ, ready, nready, tiles, p.fuse_readers >= 0 && p.nworkers > 1,
-                                          p.linked_checked, gsucc, group, gmem);
-    if (grouped) {
-        plan.succ.swap(gsucc); plan.group.swap(group); plan.group_mem.swap(gmem);
+    if (plan_read_groups(p, p.nworkers, succ, nsucc, tiles, ready, nready, plan)) {
         // a read group is led by its leader, unless a producer runs with it: then by the producer
         if (!plan.task_unit.empty())
             for (int pass = 0; pass < 2; ++pass)
@@ -413,7 +430,7 @@ void plan_hbm_window(const PlanParams& p, const uint32_t* succ, int32_t nsucc, c
                     const uint32_t b = (gd & ~PB2_GROUP_FUSED) >> 4;
                     for (uint32_t i = 0; i < (gd & 15u); ++i) plan.task_unit[(size_t)plan.group_mem[b + i]] = t;
                 }
-    } else plan.succ.assign(succ, succ + nsucc);
+    }
     if (!plan.task_unit.empty()) {                // a task owns ring entries unless a group member is led by another task
         std::vector<int32_t> lead((size_t)ntasks), np((size_t)ntasks);
         for (int32_t t = 0; t < ntasks; ++t) { lead[(size_t)t] = t; np[(size_t)t] = plan.task_unit[(size_t)t] == t ? nparts[(size_t)t] : 0; }
@@ -452,7 +469,13 @@ int plan_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, co
         // units only, so shared windows keep one part per HBM unit.
         const int32_t hbm_part_bytes = p.shared ? 0 : p.part_bytes;
         if ((rc = plan_gemm_operands(tasks, ntasks, tiles, ntiles, plan, why)) != PB2_SUCCESS) return rc;
-        if ((rc = build_gemm2_units(p, tasks, ntasks, succ, nsucc, ready, nready, p.gemm_mode == 0,
+        // Read groups as in HBM windows, except with priority lanes and one GEMM worker: such a window retires in the
+        // oracle's priority order (tests/priority_order.py, DESIGN.md §6), and a group runs its members in its leader's
+        // lane, one after the other, where the priority order may run a member of another lane, or a task one member
+        // releases into a higher lane, in between.  An HBM window states that order for DAGs without groups only.
+        if (p.queue_policy == 1 && p.nworkers_gemm == 1) plan.succ.assign(succ, succ + nsucc);
+        else plan_read_groups(p, p.nworkers_gemm, succ, nsucc, tiles, ready, nready, plan);
+        if ((rc = build_gemm2_units(p, plan.tasks.data(), ntasks, plan.succ.data(), ready, nready, p.gemm_mode == 0,
                                     p.shared ? p.next_rs_begin : nullptr, task_lane, tiles, hbm_part_bytes, plan, own, why)) != PB2_SUCCESS)
             return rc;
     }

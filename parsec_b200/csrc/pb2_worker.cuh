@@ -147,4 +147,169 @@ __device__ __forceinline__ void store_result(const WinDev& w, const pb2_task_t& 
     else if (part == 0) w.result[id] = r;
 }
 
+// ---------------------------------------------------------------------------------------------
+// read groups and fused producer units (form_read_groups, pb2_window_plan.cpp), in the HBM window kernel and in the
+// HBM-body units of the GEMM window kernel
+// ---------------------------------------------------------------------------------------------
+// The out-of-line helpers below take NT, the threads of the calling kernel's CTA (PB2_HBM_THREADS or gemm::kThreads):
+// their loops use blockDim.x, and NT gives each kernel its own instantiation, so that no helper has two caller kernels
+// in one translation unit (see stage_in_needed_flows).
+
+// A read group in flight on one worker: its members (the leader first), their CHECK constants and out-edges, this
+// part's results.  The retire path takes what it needs of a member from here, not from its descriptor.
+struct GroupSmem {
+    int32_t n;                              // members; 0: the popped task runs alone
+    int32_t fused;                          // the popped task is a producer that runs with this group as one unit
+    int32_t tile;                           // the tile the members read
+    int32_t mem[PB2_GROUP_MAX];
+    uint32_t k[PB2_GROUP_MAX];
+    int32_t succ_begin[PB2_GROUP_MAX];
+    int32_t succ_count[PB2_GROUP_MAX];
+    unsigned long long res[PB2_GROUP_MAX];  // res[0]: the leader's result, set before group_results
+};
+
+// All threads: the members of the group that task id leads or runs with (w.group) into g, published by the caller's
+// barrier.  Returns id's group word (0: id runs alone); thread 0 of the caller sets g.n and g.fused from it.
+__device__ __forceinline__ uint32_t load_group_members(const WinDev& w, int32_t id, GroupSmem& g) {
+    const uint32_t gd = w.group ? __ldg(&w.group[id]) : 0u;
+    const int gn = (int)(gd & 15u);
+    const uint32_t gb = (gd & ~PB2_GROUP_FUSED) >> 4;
+    if ((int)threadIdx.x < gn) {
+        const int32_t m = __ldg(&w.group_mem[gb + threadIdx.x]);
+        const pb2_task_t& mt = w.tasks[m];
+        g.mem[threadIdx.x] = m;
+        g.k[threadIdx.x] = mt.body == PB2_BODY_CHECK_F32 ? __float_as_uint(__ldg(&mt.fparam)) : (uint32_t)__ldg(&mt.iparam[0]);
+        g.succ_begin[threadIdx.x] = __ldg(&mt.succ_begin);
+        g.succ_count[threadIdx.x] = __ldg(&mt.succ_count);
+        if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
+    }
+    return gd;
+}
+
+// All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
+// bytes with its own constant k (CHECK_F32 compares the bits of fparam, so both bodies are CHECK_I32 on the bits):
+//  - k equal to the leader's: the leader's result;
+//  - the slice held nothing but the leader's constant: every element mismatches (the first element is the same);
+//  - otherwise the member's slice is counted again, exactly, as a failing CHECK counts it.
+template <int NT>
+static __device__ __noinline__ void group_results(TaskSmem* sp, GroupSmem* gp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const unsigned long long r0 = g.res[0];
+#pragma unroll 1
+    for (int i = 1; i < g.n; ++i) {
+        const uint32_t k = g.k[i];
+        if (k == g.k[0] || !(r0 >> 32)) {
+            if (threadIdx.x == 0) g.res[i] = k == g.k[0] ? r0 : ((unsigned long long)(s.args.bytes[0] >> 2) << 32) | (uint32_t)r0;
+            continue;
+        }
+        if (threadIdx.x == 0) s.args.iparam[0] = (int32_t)k;
+        __syncthreads();
+        const unsigned long long r = run_hbm_body(PB2_BODY_CHECK_I32, s.args, s.red);
+        if (threadIdx.x == 0) g.res[i] = r;
+        __syncthreads();
+    }
+    __syncthreads();
+}
+
+// All threads, after run_task_part ran the leader of a read group (not fused) over this part with result r (thread 0):
+// the members' results of the part.  TRACE: the members' results are part of the body; the readers push nothing out.
+template <int NT, bool TRACE>
+__device__ __forceinline__ void group_part_results(const WinDev& w, TaskSmem& s, GroupSmem& g, int32_t id, int part,
+                                                   unsigned long long r, PartSmem* rec) {
+    // the leader's part stored the version it saw; every member saw the same one
+    if (threadIdx.x == 0) {
+        g.res[0] = r;
+        if (part == 0) {
+            const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&w.seen_version[(size_t)id * PB2_MAX_FLOWS]);
+            for (int i = 1; i < g.n; ++i) w.seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
+        }
+    }
+    __syncthreads();
+    group_results<NT>(&s, &g);
+    if (TRACE && threadIdx.x == 0) rec->t_exec = rec->t_out = globaltimer_ns();
+}
+
+// Thread 0, after a part of task id ran with result r: the part's results, the members' of a group first (they are
+// CHECK bodies), then id's own unless id is a group's leader (members[0] has it).
+__device__ __forceinline__ void store_part_results(const WinDev& w, const pb2_task_t& t, int32_t id, int part, int nparts,
+                                                   unsigned long long r, const GroupSmem& g) {
+    const int gn = g.n;
+    for (int i = 0; i < gn; ++i) store_check_result(w, g.mem[i], nparts, g.res[i]);
+    if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
+}
+
+// All threads, after the producer of a fused unit stored its slice of output flow fx and one barrier told them whether
+// any element it stored differed from the leader's constant k0: the members' results (run_fused_part).
+static __device__ __forceinline__ void fused_member_results(TaskSmem& s, GroupSmem& g, uint32_t k0, bool mismatch, int fx) {
+    const uint32_t len = s.args.bytes[fx];
+    const uint32_t* const out = static_cast<const uint32_t*>(s.args.flow[fx]);
+    // the slice's first element: k0 if nothing mismatched, else what thread 0 stored there
+    const uint32_t first = threadIdx.x == 0 && s.args.part == 0 && len >= 4 ? (mismatch ? __ldcg(out) : k0) : 0u;
+    if (!mismatch) {
+        if (threadIdx.x == 0)
+            for (int m = 0; m < g.n; ++m) g.res[m] = g.k[m] == k0 ? first : ((unsigned long long)(len >> 2) << 32) | first;
+        return;
+    }
+    unsigned long long r0 = 0;
+#pragma unroll 1
+    for (int m = 0; m < g.n; ++m) {
+        const uint32_t k = g.k[m];
+        unsigned long long rm = r0;
+        if (m == 0 || k != k0) rm = ((unsigned long long)cta_count_ne(out, len, k, s.red) << 32) | first;
+        if (threadIdx.x == 0) { if (m == 0) r0 = rm; g.res[m] = rm; }
+    }
+}
+
+// All threads, in place of the body of a producer fused with its read group (fuse_readers).  s.args holds the
+// producer's slice of every flow for this part.  Run as separate tasks, the readers of a tile come long after its
+// writer: every other worker writes its own tile in between, far more than L2 holds.  Here the members check the bytes
+// before they leave the SM: the producer's checked body (run_hbm_body<true>) writes its output flow as it would alone,
+// and every thread ORs (element ^ the leader's constant) of each value it stores while the value is still in registers.
+// Its stores carry an L2 evict-first policy: nobody reads the tile back here (the resident Ex05 step is about 3 %
+// shorter than with the default policy, DESIGN.md §8).  One barrier then tells every thread whether the slice held
+// anything but the leader's constant, and the members get group_results' rules:
+//  - nothing else: a member with the leader's constant counts no mismatch, any other member counts every element;
+//  - otherwise the slice is counted again, exactly, from the tile (the barrier made the CTA's stores visible to its
+//    threads, and the loads go through L2), for the leader and every member whose constant differs from the leader's.
+// Returns the producer's result (thread 0); the caller's barrier and __threadfence() order the stores before the release.
+template <int NT>
+static __device__ __noinline__ unsigned long long run_fused_part(TaskSmem* sp, GroupSmem* gp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const int body = s.task.body;
+    const uint32_t k0 = g.k[0];
+    Checked ck{k0, 0u, l2_evict_first()};
+    const unsigned long long r = run_hbm_body<true>(body, s.args, s.red, &ck);
+    const bool mismatch = __syncthreads_or(ck.diff != 0u) != 0;
+    const int fx = (body == PB2_BODY_COPY || body == PB2_BODY_AXPY_F32) ? 1 : 0;     // see fusable() in form_read_groups
+    fused_member_results(s, g, k0, mismatch, fx);
+    return r;
+}
+
+// All threads, in place of a linked body (LINKED instantiations).  The body gets its slice in the 80-byte block *lp
+// (include/pb2_device_body.h), with check 0, unless the task is a checked linked producer fused with its read group:
+// then it runs in check mode against the leader's constant, its threads' return values stand for run_fused_part's
+// Checked::diff, and the members get their results as there.  Its output flow is the flow whose tile is the group's
+// (the one flow it writes, fusable() in form_read_groups).  Its stores carry the body's own cache policy: unlike the
+// built-in producers it writes without the evict-first hint.  A fused producer's own result is 0 (~0 still aborts).
+template <int NT>
+static __device__ __noinline__ unsigned long long run_linked_part(TaskSmem* sp, GroupSmem* gp, pb2_body_check_t* lp) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const bool fused = g.fused != 0;
+    static_assert(sizeof(BodyArgs) % 4 == 0 && sizeof(BodyArgs) / 4 <= NT, "one word of BodyArgs per thread");
+    if (threadIdx.x < sizeof(BodyArgs) / 4)
+        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&s.args)[threadIdx.x];
+    if (threadIdx.x == 0) { lp->check = fused ? 1u : 0u; lp->k0 = fused ? g.k[0] : 0u; }
+    __syncthreads();
+    const unsigned long long r = pb2_linked_body(s.task.body, &lp->args, s.red);
+    if (!fused) return r;
+    const bool mismatch = __syncthreads_or((uint32_t)r != 0u) != 0;
+    int fx = 0;
+    while (fx + 1 < (int)s.task.nb_flows && !(s.task.tile[fx] == g.tile && (s.task.access[fx] & PB2_FLOW_ACCESS_WRITE))) ++fx;
+    fused_member_results(s, g, lp->k0, mismatch, fx);
+    return threadIdx.x == 0 && r == ~0ull ? ~0ull : 0ull;
+}
+
 }  // namespace pb2
