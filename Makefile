@@ -5,10 +5,12 @@ EXTRA     ?=
 NVCCFLAGS := $(EXTRA) -O3 -std=c++17 -lineinfo $(ARCH) -Xcompiler -fPIC,-Wall,-Wno-unused-function -Xptxas -v
 CSRC      := parsec_b200/csrc
 LIB       := parsec_b200/libparsec_b200.so
-CU_SRCS   := $(CSRC)/pb2_engine.cu $(CSRC)/pb2_engine_prio.cu $(CSRC)/pb2_engine_trace.cu $(CSRC)/pb2_engine_prio_trace.cu \
-             $(CSRC)/pb2_stream.cu
+CU_SRCS   := $(CSRC)/pb2_engine.cu $(CSRC)/pb2_stream.cu
 CPP_SRCS  := $(wildcard $(CSRC)/*.cpp)
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) $(wildcard $(CSRC)/*.hpp) $(wildcard include/*.h)
+# the built-in window kernels, one object (and one ptxas log) per variant v = (queue_policy 1) + 2 * (trace)
+WINDOW_OBJS  := $(foreach v,0 1 2 3,build/pb2_window_kernels_$(v).o)
+WINDOW_LOGS  := $(WINDOW_OBJS:.o=.log)
 # the HBM window kernel with application bodies: relocatable device code, linked at run time (pb2_engine_link_bodies)
 LINKED_CUBIN := build/pb2_engine_linked.cubin
 # the GEMM window kernel with application bodies, linked only when asked for (PB2_LINK_GEMM_WINDOWS)
@@ -21,9 +23,14 @@ TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
 
 all: $(LIB) linked_bodies oracle
 
-$(LIB): $(CU_SRCS) $(CPP_SRCS) $(HDRS) $(LINKED_OBJ)
-	$(NVCC) $(NVCCFLAGS) -shared -o $@ $(CU_SRCS) $(CPP_SRCS) $(LINKED_OBJ) -Iinclude 2> build_ptxas.log || (cat build_ptxas.log; exit 1)
+$(LIB): $(CU_SRCS) $(CPP_SRCS) $(HDRS) $(WINDOW_OBJS) $(LINKED_OBJ)
+	$(NVCC) $(NVCCFLAGS) -shared -o $@ $(CU_SRCS) $(CPP_SRCS) $(WINDOW_OBJS) $(LINKED_OBJ) -Iinclude 2> build_ptxas.log || (cat build_ptxas.log; exit 1)
+	@cat $(WINDOW_LOGS) >> build_ptxas.log
 	@grep -E "error|warning" build_ptxas.log | grep -v "ptxas info" || true
+
+build/pb2_window_kernels_%.o: $(CSRC)/pb2_window_kernels.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -DPB2_WINDOW_VARIANT=$* -c -o $@ $< -Iinclude 2> build/pb2_window_kernels_$*.log || (cat build/pb2_window_kernels_$*.log; exit 1)
 
 $(LINKED_CUBIN): $(CSRC)/pb2_engine_linked.cu $(HDRS)
 	@mkdir -p build
@@ -54,7 +61,7 @@ oracle:
 	$(MAKE) -C oracle
 
 clean:
-	rm -f $(LIB) build_ptxas.log $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
+	rm -f $(LIB) build_ptxas.log $(WINDOW_OBJS) $(WINDOW_LOGS) $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
 	      build/linked_gemm_ptxas.log $(TEST_BODIES)
 	$(MAKE) -C oracle clean
 

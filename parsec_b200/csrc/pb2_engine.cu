@@ -120,7 +120,7 @@ struct pb2_window_s {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr;
     bool launched = false;
     bool shared = false;
-    bool linked = false;                // a task names a linked body: the window runs the engine's linked kernel
+    WindowKernel kernel;                // what it launches; the linked kernel when a task names a linked body
     // The per-run state by copy.  pb2_window_create fixes ncopies: 2 for a non-shared HBM window with tasks, else 1
     // (DESIGN.md §5).  Copy 0 is allocated at create, copy 1 at the second arm.  Consecutive runs alternate between
     // the copies, and while a run runs, the reset kernel arms the other copy for the next one on the engine's arm
@@ -199,7 +199,7 @@ static int encode_tensor_maps(pb2_engine_t* e, const WindowPlan& plan, const pb2
 static PlanParams params_of(const pb2_engine_t* e, int kind) {
     PlanParams p;
     p.kind = kind; p.shared = e->shared_windows; p.trace = e->window_trace; p.linked_image = e->linked_module != nullptr;
-    p.linked_gemm = e->linked_gemm;
+    p.linked_gemm = e->kernels[1][1][0].fn != nullptr;
     p.queue_policy = e->params.queue_policy; p.gemm_mode = e->params.gemm_mode;
     p.read_groups = e->params.read_groups; p.fuse_readers = e->params.fuse_readers;
     p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
@@ -298,30 +298,29 @@ static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out
 }
 
 // ---------------------------------------------------------------------------------------------
-// linked bodies: the relocatable linked kernels (pb2_engine_linked.cu, embedded by pb2_linked_image.S) + the
+// window kernels: the engine's kernel table of the built-in kernels (pb2_window_kernels.cu) and the linked ones, the
+// relocatable linked kernels (pb2_engine_linked.cu, pb2_engine_linked_gemm.cu, embedded by pb2_linked_image.S) + the
 // application's image, linked by the driver's JIT linker
 // ---------------------------------------------------------------------------------------------
 extern "C" const unsigned char pb2_linked_engine_image[], pb2_linked_engine_image_end[];
 extern "C" const unsigned char pb2_linked_gemm_image[], pb2_linked_gemm_image_end[];
 
-// pb2_engine_hbm_kernel<PRIO, TRACE, true> by (PRIO) + 2 * (TRACE)
-static const char* const kLinkedKernels[4] = {
-    "_ZN3pb221pb2_engine_hbm_kernelILb0ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
-    "_ZN3pb221pb2_engine_hbm_kernelILb1ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
-    "_ZN3pb221pb2_engine_hbm_kernelILb0ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
-    "_ZN3pb221pb2_engine_hbm_kernelILb1ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
-};
-// pb2_engine_gemm2_kernel<PRIO, TRACE, true> (pb2_engine_linked_gemm.cu), the same order
-static const char* const kLinkedGemmKernels[4] = {
-    "_ZN3pb223pb2_engine_gemm2_kernelILb0ELb0ELb1EEEvNS_7Win2DevE",
-    "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb0ELb1EEEvNS_7Win2DevE",
-    "_ZN3pb223pb2_engine_gemm2_kernelILb0ELb1ELb1EEEvNS_7Win2DevE",
-    "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb1ELb1EEEvNS_7Win2DevE",
+// The linked window kernels by [kind][(PRIO) + 2 * (TRACE)]: pb2_engine_hbm_kernel<PRIO, TRACE, true>
+// (pb2_engine_linked.cu) and pb2_engine_gemm2_kernel<PRIO, TRACE, true> (pb2_engine_linked_gemm.cu)
+static const char* const kLinkedKernels[2][4] = {
+    {"_ZN3pb221pb2_engine_hbm_kernelILb0ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
+     "_ZN3pb221pb2_engine_hbm_kernelILb1ELb0ELb1EEEvNS_6WinDevENS_8TraceDevE",
+     "_ZN3pb221pb2_engine_hbm_kernelILb0ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE",
+     "_ZN3pb221pb2_engine_hbm_kernelILb1ELb1ELb1EEEvNS_6WinDevENS_8TraceDevE"},
+    {"_ZN3pb223pb2_engine_gemm2_kernelILb0ELb0ELb1EEEvNS_7Win2DevE",
+     "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb0ELb1EEEvNS_7Win2DevE",
+     "_ZN3pb223pb2_engine_gemm2_kernelILb0ELb1ELb1EEEvNS_7Win2DevE",
+     "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb1ELb1EEEvNS_7Win2DevE"},
 };
 
-// The driver calls the linking point needs, fetched through the runtime (as cuTensorMapEncodeTiled is): the library
-// gains no link dependency on libcuda.
-struct DriverLink {
+// The driver calls of the linking point and of every window kernel's launch, fetched through the runtime (as
+// cuTensorMapEncodeTiled is): the library gains no link dependency on libcuda.
+struct DriverCalls {
     decltype(&cuLinkCreate) link_create = nullptr;
     decltype(&cuLinkAddData) link_add = nullptr;
     decltype(&cuLinkComplete) link_complete = nullptr;
@@ -339,9 +338,9 @@ struct DriverLink {
     }
 };
 
-static const DriverLink& driver_link() {
-    static const DriverLink d = [] {
-        DriverLink r;
+static const DriverCalls& driver() {
+    static const DriverCalls d = [] {
+        DriverCalls r;
         auto get = [](const char* name, auto& fn) {
             void* p = nullptr;
             cudaDriverEntryPointQueryResult q;
@@ -358,37 +357,71 @@ static const DriverLink& driver_link() {
     return d;
 }
 
-// The linked kernel of a window's queue policy and trace on the engine stream, with the linked worker count.
-static int launch_linked(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool trace) {
-    const int i = (lanes ? 1 : 0) + (trace ? 2 : 0);
-    WinDev wd = g.w;
-    TraceDev tr = trace ? g.trace : TraceDev{};
-    void* args[] = {&wd, &tr};
-    const CUresult r = driver_link().launch(e->linked_fn[i], (unsigned)e->linked_nworkers[i], 1, 1, (unsigned)e->params.threads, 1, 1,
-                                            0, reinterpret_cast<CUstream>(e->stream), args, nullptr);
-    if (r != CUDA_SUCCESS) { e->last_error = "cuLaunchKernel of the linked HBM window kernel failed (CUresult " + std::to_string((int)r) + ")"; return PB2_ERR_DEVICE; }
-    return PB2_SUCCESS;
-}
-
-// The linked GEMM kernel of a window's queue policy and trace on the engine stream, as pb2_gemm2_launch launches the
-// built-in one: 384 threads, the operand ring in dynamic shared memory.
-static int launch_linked_gemm(pb2_engine_t* e, const Win2Dev& g, bool lanes, bool trace) {
-    const int i = (lanes ? 1 : 0) + (trace ? 2 : 0);
-    Win2Dev gd = g;
-    void* args[] = {&gd};
-    const CUresult r = driver_link().launch(e->linked_gemm_fn[i], (unsigned)e->linked_gemm_nworkers[i], 1, 1, gemm::kThreads, 1, 1,
-                                            gemm::kSmemBytes, reinterpret_cast<CUstream>(e->stream), args, nullptr);
-    if (r != CUDA_SUCCESS) { e->last_error = "cuLaunchKernel of the linked GEMM window kernel failed (CUresult " + std::to_string((int)r) + ")"; return PB2_ERR_DEVICE; }
-    return PB2_SUCCESS;
-}
-
-// What the linker made of kernel fn: registers, local bytes per thread, static shared memory.
-static CUresult kernel_resources(CUfunction fn, int32_t* regs, int32_t* local, int32_t* smem) {
-    const DriverLink& d = driver_link();
-    CUresult r = d.func_attr(regs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn);
-    if (r == CUDA_SUCCESS) r = d.func_attr(local, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn);
-    if (r == CUDA_SUCCESS) r = d.func_attr(smem, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, fn);
+// Window kernel fn of `kind` as a kernel table entry k, the same for built-in and linked kernels: its resources, and its
+// launch shape.  A GEMM kernel takes the operand ring as dynamic shared memory beside its static shared memory (the
+// kernel's, and the bodies' when linked); fits is false when it cannot take the ring or fits no CTA on an SM.  A
+// built-in kernel runs on all the engine's workers (nworkers, sized by pb2_engine_create, or nworkers_gemm); a linked
+// one on as many of them as fit on the device at once.
+static CUresult resolve_kernel(const pb2_engine_t* e, CUfunction fn, int kind, bool linked, WindowKernel& k, bool& fits) {
+    const DriverCalls& d = driver();
+    const bool gemm = kind == 1;
+    const int workers = gemm ? e->nworkers_gemm : e->nworkers;
+    k = WindowKernel{};
+    k.fn = fn;
+    k.block = gemm ? gemm::kThreads : (unsigned)e->params.threads;
+    k.dyn_smem = gemm ? gemm::kSmemBytes : 0;
+    fits = true;
+    CUresult r = d.func_attr(&k.regs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn);
+    if (r == CUDA_SUCCESS) r = d.func_attr(&k.local, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn);
+    if (r == CUDA_SUCCESS) r = d.func_attr(&k.static_smem, CU_FUNC_ATTRIBUTE_SHARED_SIZE_BYTES, fn);
+    if (r != CUDA_SUCCESS) return r;
+    if (gemm && d.func_set_attr(fn, CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, gemm::kSmemBytes) != CUDA_SUCCESS) {
+        fits = false;
+        return CUDA_SUCCESS;
+    }
+    int occ = 0;
+    r = d.occupancy(&occ, fn, (int)k.block, k.dyn_smem);
+    if (r == CUDA_SUCCESS && gemm && occ == 0) fits = false;
+    k.grid = (unsigned)(linked ? std::max(1, std::min(workers, e->prop.multiProcessorCount * occ)) : workers);
     return r;
+}
+
+// The kernel table entry of a window that runs linked bodies or not, of `kind` and variant v: a built-in entry is
+// resolved on the current device when a window first needs it.
+static int window_kernel(pb2_engine_t* e, bool linked, int kind, int v, WindowKernel& out) {
+    static WindowKernelSymbols (*const symbols[4])() = {window_kernels_0, window_kernels_1, window_kernels_2, window_kernels_3};
+    std::lock_guard<std::mutex> lk(e->mu);
+    WindowKernel& k = e->kernels[linked ? 1 : 0][kind][v];
+    if (!k.fn && !linked) {
+        if (!driver().complete()) { e->last_error = "the driver's kernel entry points are not available"; return PB2_ERR_NOT_SUPPORTED; }
+        const WindowKernelSymbols s = symbols[v]();
+        cudaFunction_t fn = nullptr;
+        PB2_CUDA(e, cudaGetFuncBySymbol(&fn, kind == 1 ? s.gemm : s.hbm));
+        WindowKernel got;
+        bool fits = true;
+        const CUresult r = resolve_kernel(e, reinterpret_cast<CUfunction>(fn), kind, false, got, fits);
+        if (r != CUDA_SUCCESS || !fits) {
+            e->last_error = std::string("the built-in ") + (kind == 1 ? "GEMM" : "HBM") + " window kernel cannot run (CUresult " +
+                            std::to_string((int)r) + ")";
+            return PB2_ERR_DEVICE;
+        }
+        k = got;
+    }
+    out = k;
+    return PB2_SUCCESS;
+}
+
+// What the linker made of the untraced linked kernel of `kind` of the engine's queue policy, and its worker count.
+static int linked_info(pb2_engine_t* e, int kind, const char* not_linked, int32_t* regs, int32_t* local_bytes,
+                       int32_t* static_smem, int32_t* nworkers) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    const WindowKernel& k = e->kernels[1][kind][e->params.queue_policy == 1 ? 1 : 0];
+    if (!k.fn) { e->last_error = not_linked; return PB2_ERR_NOT_FOUND; }
+    if (regs) *regs = k.regs;
+    if (local_bytes) *local_bytes = k.local;
+    if (static_smem) *static_smem = k.static_smem;
+    if (nworkers) *nworkers = (int32_t)k.grid;
+    return PB2_SUCCESS;
 }
 
 extern "C" {
@@ -409,7 +442,7 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     const bool gemm_windows = (flags & PB2_LINK_GEMM_WINDOWS) != 0;
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
-    const DriverLink& d = driver_link();
+    const DriverCalls& d = driver();
     if (!d.complete()) { e->last_error = "the driver's JIT linker entry points are not available"; return PB2_ERR_NOT_SUPPORTED; }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaFree(nullptr));             // the device's primary context is current: the module is loaded into it
@@ -443,82 +476,39 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
         e->last_error = "linking the application's bodies failed (CUresult " + std::to_string((int)r) + "): " + err.data();
         return PB2_ERR_BAD_PARAM;
     }
-    CUfunction fn[4] = {};
-    int nw[4] = {};
-    for (int i = 0; i < 4 && r == CUDA_SUCCESS; ++i) {
-        int occ = 0;
-        r = d.get_function(&fn[i], mod, kLinkedKernels[i]);
-        if (r == CUDA_SUCCESS) r = d.occupancy(&occ, fn[i], e->params.threads, 0);
-        nw[i] = std::max(1, std::min(e->nworkers, e->prop.multiProcessorCount * occ));
-    }
-    const int mine = e->params.queue_policy == 1 ? 1 : 0;
-    int32_t regs = 0, local = 0, smem = 0;
-    if (r == CUDA_SUCCESS) r = kernel_resources(fn[mine], &regs, &local, &smem);
-    if (r != CUDA_SUCCESS) {
-        d.module_unload(mod);
-        e->last_error = "the linked module has no usable HBM window kernel (CUresult " + std::to_string((int)r) + ")";
-        return PB2_ERR_DEVICE;
-    }
-    // The GEMM kernels take the operand ring as dynamic shared memory; the bodies' static shared memory comes on top of
-    // it.  A kernel that cannot take the ring beside it (the attribute is refused) or fits no CTA on an SM fails the link.
-    CUfunction gfn[4] = {}, too_big = nullptr;
-    int gnw[4] = {};
-    int32_t gregs = 0, glocal = 0, gsmem = 0;
-    for (int i = 0; gemm_windows && i < 4 && r == CUDA_SUCCESS && !too_big; ++i) {
-        int occ = 0;
-        r = d.get_function(&gfn[i], mod, kLinkedGemmKernels[i]);
-        if (r != CUDA_SUCCESS) break;
-        if (d.func_set_attr(gfn[i], CU_FUNC_ATTRIBUTE_MAX_DYNAMIC_SHARED_SIZE_BYTES, gemm::kSmemBytes) != CUDA_SUCCESS) { too_big = gfn[i]; break; }
-        r = d.occupancy(&occ, gfn[i], gemm::kThreads, gemm::kSmemBytes);
-        if (r == CUDA_SUCCESS && occ == 0) too_big = gfn[i];
-        gnw[i] = std::max(1, std::min(e->nworkers_gemm, e->prop.multiProcessorCount * occ));
-    }
-    if (gemm_windows && r == CUDA_SUCCESS && !too_big) r = kernel_resources(gfn[mine], &gregs, &glocal, &gsmem);
-    if (r != CUDA_SUCCESS) {
-        d.module_unload(mod);
-        e->last_error = "the linked module has no usable GEMM window kernel (CUresult " + std::to_string((int)r) + ")";
-        return PB2_ERR_DEVICE;
-    }
-    if (too_big) {
-        int32_t sm = 0, unused = 0;
-        kernel_resources(too_big, &unused, &unused, &sm);
-        d.module_unload(mod);
-        e->last_error = "the linked GEMM window kernel does not fit on an SM: " + std::to_string(sm) +
-                        " bytes of static shared memory (the kernel's and the bodies') beside its " +
-                        std::to_string(gemm::kSmemBytes) + " bytes of dynamic shared memory";
-        return PB2_ERR_NOT_SUPPORTED;
-    }
+    // the linked entries, of GEMM windows only when asked for; a GEMM kernel that does not fit fails the link
+    WindowKernel linked[2][4];
+    for (int kind = 0; kind < (gemm_windows ? 2 : 1); ++kind)
+        for (int v = 0; v < 4; ++v) {
+            CUfunction fn = nullptr;
+            bool fits = true;
+            r = d.get_function(&fn, mod, kLinkedKernels[kind][v]);
+            if (r == CUDA_SUCCESS) r = resolve_kernel(e, fn, kind, true, linked[kind][v], fits);
+            if (r == CUDA_SUCCESS && fits) continue;
+            d.module_unload(mod);
+            if (r != CUDA_SUCCESS) {
+                e->last_error = std::string("the linked module has no usable ") + (kind == 1 ? "GEMM" : "HBM") +
+                                " window kernel (CUresult " + std::to_string((int)r) + ")";
+                return PB2_ERR_DEVICE;
+            }
+            e->last_error = "the linked GEMM window kernel does not fit on an SM: " + std::to_string(linked[kind][v].static_smem) +
+                            " bytes of static shared memory (the kernel's and the bodies') beside its " +
+                            std::to_string(gemm::kSmemBytes) + " bytes of dynamic shared memory";
+            return PB2_ERR_NOT_SUPPORTED;
+        }
     e->linked_module = mod;
-    for (int i = 0; i < 4; ++i) { e->linked_fn[i] = fn[i]; e->linked_nworkers[i] = nw[i]; }
-    e->linked_regs = regs; e->linked_local = local; e->linked_smem = smem;
+    std::copy_n(&linked[0][0], 8, &e->kernels[1][0][0]);
     e->linked_sliceable = sliceable; e->linked_checked = checked;
-    e->linked_gemm = gemm_windows;
-    for (int i = 0; i < 4; ++i) { e->linked_gemm_fn[i] = gfn[i]; e->linked_gemm_nworkers[i] = gnw[i]; }
-    e->linked_gemm_regs = gregs; e->linked_gemm_local = glocal; e->linked_gemm_smem = gsmem;
     return PB2_SUCCESS;
 }
 
 int pb2_engine_linked_info(pb2_engine_t* e, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers) {
-    if (!e) return PB2_ERR_BAD_PARAM;
-    if (!e->linked_module) { e->last_error = "the engine has not linked an image (pb2_engine_link_bodies)"; return PB2_ERR_NOT_FOUND; }
-    if (regs) *regs = e->linked_regs;
-    if (local_bytes) *local_bytes = e->linked_local;
-    if (static_smem) *static_smem = e->linked_smem;
-    if (nworkers) *nworkers = e->linked_nworkers[e->params.queue_policy == 1 ? 1 : 0];
-    return PB2_SUCCESS;
+    return linked_info(e, 0, "the engine has not linked an image (pb2_engine_link_bodies)", regs, local_bytes, static_smem, nworkers);
 }
 
 int pb2_engine_linked_gemm_info(pb2_engine_t* e, int32_t* regs, int32_t* local_bytes, int32_t* static_smem, int32_t* nworkers) {
-    if (!e) return PB2_ERR_BAD_PARAM;
-    if (!e->linked_gemm) {
-        e->last_error = "the engine has not linked the GEMM window kernels (pb2_engine_link_bodies_ex with PB2_LINK_GEMM_WINDOWS)";
-        return PB2_ERR_NOT_FOUND;
-    }
-    if (regs) *regs = e->linked_gemm_regs;
-    if (local_bytes) *local_bytes = e->linked_gemm_local;
-    if (static_smem) *static_smem = e->linked_gemm_smem;
-    if (nworkers) *nworkers = e->linked_gemm_nworkers[e->params.queue_policy == 1 ? 1 : 0];
-    return PB2_SUCCESS;
+    return linked_info(e, 1, "the engine has not linked the GEMM window kernels (pb2_engine_link_bodies_ex with PB2_LINK_GEMM_WINDOWS)",
+                       regs, local_bytes, static_smem, nworkers);
 }
 
 int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_params_t* params) {
@@ -567,7 +557,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
         }
     }
     int occ = 0;
-    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pb2_engine_hbm_kernel<false, false>, p.threads, 0));
+    PB2_CUDA(e, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, window_kernels_0().hbm, p.threads, 0));
     int per_sm = occ < p.workers_per_sm ? occ : p.workers_per_sm;
     if (per_sm < 1) per_sm = 1;
     e->nworkers = e->prop.multiProcessorCount * per_sm;
@@ -587,7 +577,7 @@ int pb2_engine_destroy(pb2_engine_t* e) {
     if (e->dma_stream) cudaStreamDestroy(e->dma_stream);
     if (e->arm_stream) cudaStreamDestroy(e->arm_stream);
     if (e->dma_ev) cudaEventDestroy(e->dma_ev);
-    if (e->linked_module) driver_link().module_unload(e->linked_module);
+    if (e->linked_module) driver().module_unload(e->linked_module);
     delete e;
     return PB2_SUCCESS;
 }
@@ -829,12 +819,14 @@ int pb2_window_create(pb2_engine_t* e, pb2_window_t** window, int kind,
         return rc;
     }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    WindowKernel kernel;
+    if ((rc = window_kernel(e, plan.linked, kind, (plan.run.lanes ? 1 : 0) + (plan.run.trace ? 2 : 0), kernel)) != PB2_SUCCESS) return rc;
     std::vector<CUtensorMap> tmaps;
     if (kind == 1 && (rc = encode_tensor_maps(e, plan, tiles, ntiles, tmaps)) != PB2_SUCCESS) return rc;
     pb2_window_t* w = new pb2_window_s();
+    w->kernel = kernel;
     w->shared = e->shared_windows;
     w->e = e; w->kind = kind; w->ntasks = ntasks; w->ntiles = ntiles;
-    w->linked = plan.linked;
     w->shape = plan.run;
     // shared windows keep one copy (peers hold IPC pointers to it), GEMM windows too (DESIGN.md §5)
     w->ncopies = kind == 0 && !w->shared && ntasks > 0 ? 2 : 1;
@@ -917,29 +909,20 @@ int pb2_window_start(pb2_window_t* w) {
     pb2_engine_t* e = w->e;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     if (w->ntasks > 0) {
-        const Win2Dev g = run_desc(w, w->cur);
-        const bool lanes = w->shape.lanes, trace = w->shape.trace;
-        if (w->kind == 0 && w->linked) {
-            const int rc = launch_linked(e, g, lanes, trace);
-            if (rc != PB2_SUCCESS) return rc;
-        } else if (w->kind == 0) {
-            const int nw = e->nworkers, th = e->params.threads;
-            if (trace) PB2_CUDA(e, lanes ? pb2_hbm_prio_trace_launch(g.w, g.trace, nw, th, e->stream)
-                                         : pb2_hbm_trace_launch(g.w, g.trace, nw, th, e->stream));
-            else if (lanes) PB2_CUDA(e, pb2_hbm_prio_launch(g.w, nw, th, e->stream));
-            else pb2_engine_hbm_kernel<false, false><<<nw, th, 0, e->stream>>>(g.w, TraceDev{});
-            PB2_CUDA(e, cudaGetLastError());
-        } else if (w->linked) {
-            const int rc = launch_linked_gemm(e, g, lanes, trace);
-            if (rc != PB2_SUCCESS) return rc;
-            w->g.fresh_tmaps = 0;
-        } else {
-            const int nw = e->nworkers_gemm;
-            int rc = trace ? (lanes ? pb2_gemm2_prio_trace_launch(g, nw, e->stream) : pb2_gemm2_trace_launch(g, nw, e->stream))
-                           : (lanes ? pb2_gemm2_prio_launch(g, nw, e->stream) : pb2_gemm2_launch<false, false>(g, nw, e->stream));
-            if (rc != PB2_SUCCESS) { e->last_error = "gemm window launch failed"; return rc; }
-            w->g.fresh_tmaps = 0;
+        // an HBM kernel takes (WinDev, TraceDev), the trace empty when the window is untraced; a GEMM kernel takes Win2Dev
+        Win2Dev g = run_desc(w, w->cur);
+        TraceDev tr = w->shape.trace ? g.trace : TraceDev{};
+        void* hbm_args[] = {&g.w, &tr};
+        void* gemm_args[] = {&g};
+        const WindowKernel& k = w->kernel;
+        const CUresult r = driver().launch(k.fn, k.grid, 1, 1, k.block, 1, 1, k.dyn_smem, reinterpret_cast<CUstream>(e->stream),
+                                           w->kind == 1 ? gemm_args : hbm_args, nullptr);
+        if (r != CUDA_SUCCESS) {
+            e->last_error = std::string("cuLaunchKernel of the ") + (w->kind == 1 ? "GEMM" : "HBM") + " window kernel failed (CUresult " +
+                            std::to_string((int)r) + ")";
+            return PB2_ERR_DEVICE;
         }
+        if (w->kind == 1) w->g.fresh_tmaps = 0;
     }
     PB2_CUDA(e, cudaEventRecord(w->ev2, e->stream));
     w->launched = true;

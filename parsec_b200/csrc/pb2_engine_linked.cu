@@ -2,7 +2,7 @@
 // policy x trace instantiations.  Not part of the library's own device code: the Makefile compiles this file with
 // -rdc=true to a relocatable sm_90a cubin, which is embedded in libparsec_b200.so (pb2_linked_image.S) and linked with
 // the application's image by pb2_engine_link_bodies.  pb2_linked_body is resolved there.  The kernels are looked up by
-// the names of kLinkedKernels (pb2_engine.cu).
+// the names of kLinkedKernels[0] (pb2_engine.cu), in the engine's kernel table's order.
 #include <cuda_runtime.h>
 
 #include "pb2_hbm.cuh"

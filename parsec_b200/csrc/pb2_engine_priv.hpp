@@ -1,5 +1,6 @@
 // pb2_engine_priv.hpp -- host-side engine object shared by the translation units of libparsec_b200.so
-// (pb2_engine.cu: windows; pb2_stream.cu: the streaming ring + persistent kernel).
+// (pb2_engine.cu: windows; pb2_window_kernels.cu: the built-in window kernels; pb2_stream.cu: the streaming ring +
+// persistent kernel).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -10,6 +11,22 @@
 #include <utility>
 #include "../../include/pb2_engine.h"
 #include "pb2_window_layout.h"
+
+// One window kernel as the engine launches it: the function, its launch shape, and what the compiler or the linker made
+// of it (registers, local bytes per thread, static shared memory).
+struct WindowKernel {
+    CUfunction fn = nullptr;
+    unsigned grid = 0, block = 0, dyn_smem = 0;
+    int32_t regs = 0, local = 0, static_smem = 0;
+};
+
+// The host symbols of the built-in HBM and GEMM window kernels of variant v = (queue_policy 1) + 2 * (trace):
+// window_kernels_<v> is defined by the object the Makefile compiles from pb2_window_kernels.cu with PB2_WINDOW_VARIANT=v.
+struct WindowKernelSymbols { const void* hbm; const void* gemm; };
+WindowKernelSymbols window_kernels_0();
+WindowKernelSymbols window_kernels_1();
+WindowKernelSymbols window_kernels_2();
+WindowKernelSymbols window_kernels_3();
 
 struct pb2_engine_s {
     int cuda_device = 0;
@@ -31,20 +48,14 @@ struct pb2_engine_s {
     bool window_trace = false;           // windows created from now on record per-task device time stamps
     const int32_t* next_rs_begin = nullptr;   // remote out-degree CSR of the next shared window (not owned)
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
-    // pb2_engine_link_bodies: the module of the linked HBM window kernels, each kernel and its worker count by
-    // (queue_policy 1) + 2 * (trace), what the linker made of the untraced one of this engine's policy, and which
-    // linked body ids may be cut into parts (bit i: PB2_BODY_LINKED_0 + i) and which have a checked form
+    // Every window kernel by [built-in, linked][kind: HBM, GEMM][(queue_policy 1) + 2 * (trace)].  A built-in entry
+    // is resolved when a window first needs it, under mu; pb2_engine_link_bodies_ex resolves the linked HBM entries,
+    // and with PB2_LINK_GEMM_WINDOWS the linked GEMM entries (an entry that is not resolved has a null fn).
+    WindowKernel kernels[2][2][4];
+    // pb2_engine_link_bodies: the module of the linked window kernels, and which linked body ids may be cut into parts
+    // (bit i: PB2_BODY_LINKED_0 + i) and which have a checked form
     CUmodule linked_module = nullptr;
-    CUfunction linked_fn[4] = {};
-    int linked_nworkers[4] = {};
-    int32_t linked_regs = 0, linked_local = 0, linked_smem = 0;
     uint32_t linked_sliceable = 0, linked_checked = 0;
-    // linked with PB2_LINK_GEMM_WINDOWS: the same module's linked GEMM window kernels, their worker counts and what the
-    // linker made of the untraced one of this engine's policy (else linked_gemm is false and the rest stays zero)
-    bool linked_gemm = false;
-    CUfunction linked_gemm_fn[4] = {};
-    int linked_gemm_nworkers[4] = {};
-    int32_t linked_gemm_regs = 0, linked_gemm_local = 0, linked_gemm_smem = 0;
 };
 
 // The argument check of pb2_engine_link_bodies(_checked, _ex) and pb2_device_link_bodies(_checked, _ex): nullptr, or why

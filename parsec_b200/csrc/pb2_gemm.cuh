@@ -340,7 +340,9 @@ static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_
 }  // namespace gemm
 
 // PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: write a record of every part into g.trace (PartSmem,
-// then trace_part); the untraced instantiations never touch it.
+// then trace_part); the untraced instantiations never touch it.  The built-in instantiations are in
+// pb2_window_kernels.cu, one per object, beside the HBM kernel of the same PRIO and TRACE; the engine launches every
+// instantiation with gemm::kThreads threads and the operand ring, gemm::kSmemBytes, as dynamic shared memory.
 // LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body; built only in
 // pb2_engine_linked_gemm.cu, as relocatable device code that pb2_engine_link_bodies_ex links with the application's
 // image when PB2_LINK_GEMM_WINDOWS is set.  The other instantiations compile as if the flag did not exist.
@@ -534,23 +536,5 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
         __syncthreads();             // sh.job is rewritten by the next pop
     }
 }
-
-template <bool PRIO, bool TRACE>
-static inline int pb2_gemm2_launch(const Win2Dev& g, int nworkers, cudaStream_t stream) {
-    static bool attr_set = false;       // one per instantiation
-    if (!attr_set) {
-        if (cudaFuncSetAttribute(pb2_engine_gemm2_kernel<PRIO, TRACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm::kSmemBytes) != cudaSuccess) return PB2_ERR_DEVICE;
-        attr_set = true;
-    }
-    if (nworkers < 1) return PB2_ERR_BAD_PARAM;
-    pb2_engine_gemm2_kernel<PRIO, TRACE><<<nworkers, gemm::kThreads, gemm::kSmemBytes, stream>>>(g);
-    return cudaGetLastError() == cudaSuccess ? PB2_SUCCESS : PB2_ERR_DEVICE;
-}
-
-// pb2_engine_prio.cu: launch the queue_policy 1 instantiation
-int pb2_gemm2_prio_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
-// pb2_engine_trace.cu, pb2_engine_prio_trace.cu: launch the traced FIFO / queue_policy 1 instantiations
-int pb2_gemm2_trace_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
-int pb2_gemm2_prio_trace_launch(const Win2Dev& g, int nworkers, cudaStream_t stream);
 
 }  // namespace pb2

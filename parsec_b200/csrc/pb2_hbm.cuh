@@ -1,9 +1,9 @@
 // pb2_hbm.cuh -- the persistent engine kernel of HBM-body windows (pb2_engine_hbm_kernel); what one worker does with a
-// task, a read group or a fused producer unit is the shared worker code of pb2_worker.cuh.  Instantiated for the FIFO ready ring
-// in pb2_engine.cu and for priority lanes (queue_policy 1) in pb2_engine_prio.cu, and traced (window trace) in
-// pb2_engine_trace.cu and pb2_engine_prio_trace.cu: each translation unit holds one instantiation, because a second
-// kernel calling the same __noinline__ helpers makes ptxas give them the standard call ABI, which costs the kernel a
-// stack frame and spills at its 80-register budget.
+// task, a read group or a fused producer unit is the shared worker code of pb2_worker.cuh.  Instantiated for the FIFO ready
+// ring and for priority lanes (queue_policy 1), untraced and traced (window trace), by pb2_window_kernels.cu, one object
+// per variant: each translation unit holds one instantiation, because a second kernel calling the same __noinline__
+// helpers makes ptxas give them the standard call ABI, which costs the kernel a stack frame and spills at its
+// 80-register budget.
 #pragma once
 #include "pb2_sched.cuh"
 #include "pb2_worker.cuh"
@@ -183,11 +183,5 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         __syncthreads();
     }
 }
-
-// pb2_engine_prio.cu: launch the queue_policy 1 instantiation
-cudaError_t pb2_hbm_prio_launch(const WinDev& w, int nworkers, int threads, cudaStream_t stream);
-// pb2_engine_trace.cu, pb2_engine_prio_trace.cu: launch the traced FIFO / queue_policy 1 instantiations
-cudaError_t pb2_hbm_trace_launch(const WinDev& w, const TraceDev& tr, int nworkers, int threads, cudaStream_t stream);
-cudaError_t pb2_hbm_prio_trace_launch(const WinDev& w, const TraceDev& tr, int nworkers, int threads, cudaStream_t stream);
 
 }  // namespace pb2
