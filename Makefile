@@ -16,10 +16,11 @@ LINKED_CUBIN := build/pb2_engine_linked.cubin
 # the GEMM window kernel with application bodies, linked only when asked for (PB2_LINK_GEMM_WINDOWS)
 LINKED_GEMM_CUBIN := build/pb2_engine_linked_gemm.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
-# the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py), as
-# relocatable cubins and as PTX
+# the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py,
+# tests/test_linked_readers_gpu.py), as relocatable cubins and as PTX
 TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
-                tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx
+                tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx \
+                tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx
 
 all: $(LIB) linked_bodies oracle
 
@@ -55,6 +56,12 @@ tests/cuda/checked_bodies.cubin: tests/cuda/checked_bodies.cu include/pb2_device
 	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -Iinclude -o $@ $<
 
 tests/cuda/checked_bodies.ptx: tests/cuda/checked_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
+
+tests/cuda/reader_bodies.cubin: tests/cuda/reader_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -Iinclude -o $@ $<
+
+tests/cuda/reader_bodies.ptx: tests/cuda/reader_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
 
 oracle:

@@ -19,7 +19,7 @@
  *     the `sliceable` mask of the link call always runs as one part over whole tiles (part 0, elem0 0); a body whose bit
  *     is set may be cut into byte-slice parts like the built-in element-wise bodies, each part run by another worker.
  *   - scratch: 32 words of the worker's shared memory, free for the body's use (32 in GEMM windows too).
- *   - The result is taken from thread 0.  A multi-part task keeps the result of part 0.
+ *   - The result is taken from thread 0.  A multi-part task keeps the result of part 0 (a reader's add up, below).
  *   - Returning ~0ull aborts the window as a bad body (pb2_window_wait: PB2_ERR_BAD_PARAM).
  *   - Static __shared__ variables are allowed; they count against the linked kernel's occupancy, which
  *     pb2_engine_linked_info reports (pb2_engine_linked_gemm_info for GEMM windows, where they come on top of the
@@ -39,6 +39,19 @@
  * Thread 0 returning ~0ull still aborts the window as a bad body.  A fused producer's own result is recorded as 0.  The
  * engine decides the readers' results from one barrier over these values, and counts their mismatches exactly from the
  * tile only when some thread reported one.  The body's stores carry whatever cache policy the body gives them.
+ *
+ * Readers (PB2_LINK_READERS(mask) in the flags of pb2_engine_link_bodies_ex, a subset of `sliceable`): a body whose bit
+ * is set in `mask`
+ *   - only loads from its flows, and stores nothing to them;
+ *   - may be called on any 16-byte-aligned sub-slice of a part (flow, bytes and elem0 describe that sub-slice), and
+ *     several times in a row on one worker, with a barrier between calls; scratch does not survive from one call to
+ *     the next;
+ *   - has its task's result defined as the sum, modulo 2^64, of the values thread 0 returns over all calls and parts.
+ *     ~0ull from any call still aborts the window, and is not added.  A task that runs as one call keeps its value.
+ * The result is then the same whether the engine runs the task alone, cuts it into parts, runs it with the other
+ * readers of the same tile on one worker (a read group, which calls every member on one chunk of the part before the
+ * next), or fuses that group with the task that writes the tile (which then writes each chunk before the members read it
+ * back, with check 0: it needs no checked form).  Reductions that must not depend on that order are integer ones.
  *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */

@@ -285,8 +285,15 @@ int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, siz
  *                          worker, in check mode too when its bit is set in `checked`.  Its static shared memory comes on top of the GEMM kernel's
  *                          dynamic shared memory: PB2_ERR_NOT_SUPPORTED, and the engine stays unlinked, when the two do
  *                          not fit on one SM.  The flag costs link time (four more kernels), so it is opt-in.
+ *   PB2_LINK_READERS(mask) bits 8..15: bit i of `mask` declares that body PB2_BODY_LINKED_0 + i is a reader
+ *                          (include/pb2_device_body.h): it only loads from its flows, and its task's result is the sum
+ *                          of what it returns over all calls.  Consecutive readers of one tile that a task releases run
+ *                          as one read group on one worker, fused with that task when it writes the tile
+ *                          (pb2_engine_params_t::read_groups, fuse_readers), in windows of both kinds.  `mask` must be a
+ *                          subset of `sliceable`: PB2_ERR_BAD_PARAM otherwise.
  * PB2_ERR_BAD_PARAM for any other bit. */
 #define PB2_LINK_GEMM_WINDOWS 0x1u
+#define PB2_LINK_READERS(mask) ((uint32_t)(mask) << 8)
 int  pb2_engine_link_bodies_ex(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
 /* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill

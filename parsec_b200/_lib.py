@@ -45,6 +45,11 @@ IMAGE_PTX, IMAGE_CUBIN = 1, 2
 # pb2_engine_link_bodies_ex flags: also link the GEMM window kernel, so linked bodies run in GEMM windows too
 LINK_GEMM_WINDOWS = 0x1
 
+
+def LINK_READERS(mask):
+    """pb2_engine_link_bodies_ex flags: bit i of mask declares body BODY_LINKED_0 + i a reader (bits 8..15)."""
+    return mask << 8
+
 TASK_DEPS_MASK = 0x01
 TILE_INVALID, TILE_STAGING, TILE_VALID = 0, 1, 2
 SRC_HOST, SRC_PEER = 0, 1

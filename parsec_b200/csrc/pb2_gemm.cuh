@@ -476,16 +476,19 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
                 unsigned long long body_r;
-                if constexpr (LINKED) body_r = is_linked_body(sh.ts.task.body) ? run_linked_part<kThreads>(&sh.ts, &sh.gs, lk)
+                if constexpr (LINKED) body_r = linked_reader_group(w, sh.gs) ? run_linked_group_part<kThreads>(&sh.ts, &sh.gs, lk, w.tasks, w.seen_version)
+                                             : is_linked_body(sh.ts.task.body) ? run_linked_part<kThreads>(&sh.ts, &sh.gs, lk)
                                              : sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs)
                                                            : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
                 else body_r = sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs) : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);
                 fence_proxy_async();
                 return body_r;
             }, rec);
-            if (sh.gs.n && !sh.gs.fused) group_part_results<kThreads, TRACE>(w, sh.ts, sh.gs, id, job.part, r, rec);
-            // CHECK parts add their mismatch counts; the first element comes from part 0
-            if (threadIdx.x == 0) store_part_results(w, sh.ts.task, id, job.part, job.nparts, r, sh.gs);
+            // the leader of a group of linked readers is a reader; run_linked_group_part gave its members their results
+            if (sh.gs.n && !sh.gs.fused && !(LINKED && (sh.ts.task.flags & PB2_TASK_READER)))
+                group_part_results<kThreads, TRACE>(w, sh.ts, sh.gs, id, job.part, r, rec);
+            // CHECK parts add their mismatch counts, linked readers their sums; the first element comes from part 0
+            if (threadIdx.x == 0) store_part_results<LINKED>(w, sh.ts.task, id, job.part, job.nparts, r, sh.gs);
         }
         __threadfence();
         __syncthreads();             // every store of the part is done and visible

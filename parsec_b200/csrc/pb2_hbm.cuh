@@ -103,11 +103,14 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
         const int nparts = task_nparts(w, id);
         const unsigned long long r = run_task_part<true, TRACE>(w, s, &bulk, id, part, nparts, [&] {
             if constexpr (LINKED) {
+                if (linked_reader_group(w, g)) return run_linked_group_part<PB2_HBM_THREADS>(&s, &g, lk, w.tasks, w.seen_version);
                 if (is_linked_body(s.task.body)) return run_linked_part<PB2_HBM_THREADS>(&s, &g, lk);
             }
             return g.fused ? run_fused_part<PB2_HBM_THREADS>(&s, &g) : run_hbm_body(s.task.body, s.args, s.red);
         }, rec);
-        if (g.n && !g.fused) group_part_results<PB2_HBM_THREADS, TRACE>(w, s, g, id, part, r, rec);
+        // the leader of a group of linked readers is a reader; run_linked_group_part gave its members their results
+        if (g.n && !g.fused && !(LINKED && (s.task.flags & PB2_TASK_READER)))
+            group_part_results<PB2_HBM_THREADS, TRACE>(w, s, g, id, part, r, rec);
 
         if (threadIdx.x < 32) {
             __threadfence();   // release side: the body's stores (all threads, ordered by the barrier) become
@@ -115,7 +118,7 @@ pb2_engine_hbm_kernel(WinDev w, TraceDev tr) {
             if (threadIdx.x == 0) {
                 const pb2_task_t& t = s.task;
                 const int gn = g.n;
-                store_part_results(w, t, id, part, nparts, r, g);
+                store_part_results<LINKED>(w, t, id, part, nparts, r, g);
                 // the last part to finish retires the task (fence / RMW chain orders every part's stores before it)
                 int last = 1;
                 if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }

@@ -196,6 +196,7 @@ struct pb2_device_module_s {
     bool trace = false;                      // device_engine_trace at init: windows are created traced
     bool linked = false;                     // pb2_device_link_bodies: windows may run linked bodies
     bool linked_gemm = false;                // ... with PB2_LINK_GEMM_WINDOWS: GEMM windows too
+    uint32_t linked_readers = 0;             // ... PB2_LINK_READERS: bit i, PB2_BODY_LINKED_0 + i is a reader
     pb2_engine_t* engine = nullptr;
     std::deque<pb2_device_window*> inflight; // windows launched and not yet retired (oldest first), pb2_device_module.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up

@@ -35,6 +35,9 @@ struct Lanes {
 
 #define PB2_GROUP_MAX 8     // members per read group (at most 15: the count is 4 bits of group[])
 #define PB2_GROUP_FUSED 0x80000000u   // group[] of a producer that runs with its group as one unit
+// pb2_task_t::flags of a window's device descriptors, set by the planner (the caller's flags keep bits 0..2): the body is
+// a linked reader (PB2_LINK_READERS), whose results add up over parts and calls (store_result)
+#define PB2_TASK_READER 0x80
 
 // A task whose tiles are large is executed as several PARTS (byte slices of its tiles) by different workers: one
 // tile at HBM / NVLink speed needs the whole GPU (a 64-thread CTA keeps 4 KiB in flight; a 4 MiB tile is 1.3 us of

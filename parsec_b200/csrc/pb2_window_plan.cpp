@@ -287,8 +287,15 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
 // knows nothing else of what the body stores (run_linked_part).  The
 // caller turns fusion off with one worker: there the retire order is the FIFO order, in which the members run after
 // every task that was queued when P retired, and a fused unit runs them right after P.
+//
+// Linked readers (a body declared a reader, PB2_LINK_READERS; plan_window marks its tasks PB2_TASK_READER) are members
+// under the same rules, in groups of their own: a run splits where CHECK members and linked readers meet, and a group's
+// linked readers may run different bodies.  Their worker walks each part in chunks and calls every member on a chunk
+// before the next one, so that the members re-read it from the SM's caches (run_linked_group_part).  A producer runs
+// with such a group when it is a built-in fusable body, or a sliceable linked body that writes X and no other tile: it
+// needs no checked form, as it writes each chunk before the members read it back.
 bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, const int32_t* ready, int32_t nready,
-                      const pb2_tile_t* tiles, bool fuse, uint32_t linked_checked,
+                      const pb2_tile_t* tiles, bool fuse, const PlanParams& prm,
                       std::vector<uint32_t>& gsucc, std::vector<uint32_t>& group, std::vector<int32_t>& gmem) {
     const size_t n = tasks.size();
     std::vector<uint8_t> indeg(n, 0);                        // saturates at 2
@@ -298,19 +305,23 @@ bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, cons
             if (d < 2) ++d;
         }
     for (int32_t i = 0; i < nready; ++i) indeg[(size_t)ready[i]] = 2;
+    auto linked_bit = [](uint32_t mask, int body) { return is_linked_body(body) && ((mask >> (body - PB2_BODY_LINKED_0)) & 1u); };
+    // the member kind of edge s's target: 0 none, 1 CHECK, 2 linked reader
     auto reader = [&](uint32_t s) {
         const pb2_task_t& t = tasks[(size_t)PB2_SUCC_TASK(s)];
-        if (indeg[(size_t)PB2_SUCC_TASK(s)] != 1) return false;
-        if (t.dep_goal != ((t.flags & PB2_TASK_DEPS_MASK) ? (int32_t)(1u << PB2_SUCC_FLOW(s)) : 1)) return false;
-        if (t.body != PB2_BODY_CHECK_I32 && t.body != PB2_BODY_CHECK_F32) return false;
-        if (t.nb_flows < 1 || t.tile[0] < 0 || (t.access[0] & (PB2_FLOW_ACCESS_RW | PB2_FLOW_PUSHOUT)) != PB2_FLOW_ACCESS_READ) return false;
-        for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return false;
-        return true;
+        if (indeg[(size_t)PB2_SUCC_TASK(s)] != 1) return 0;
+        if (t.dep_goal != ((t.flags & PB2_TASK_DEPS_MASK) ? (int32_t)(1u << PB2_SUCC_FLOW(s)) : 1)) return 0;
+        const int kind = t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32 ? 1 : (t.flags & PB2_TASK_READER) ? 2 : 0;
+        if (!kind) return 0;
+        if (t.nb_flows < 1 || t.tile[0] < 0 || (t.access[0] & (PB2_FLOW_ACCESS_RW | PB2_FLOW_PUSHOUT)) != PB2_FLOW_ACCESS_READ) return 0;
+        for (int f = 1; f < t.nb_flows; ++f) if (t.tile[f] >= 0) return 0;
+        return kind;
     };
-    // the bodies with a checked form (run_hbm_body<true>), whose output flow `out` writes X
-    auto fusable = [&](const pb2_task_t& p, int32_t x) {
+    // the bodies with a checked form (run_hbm_body<true>), whose output flow `out` writes X; with linked readers
+    // (kind 2) the built-in ones and the sliceable linked ones
+    auto fusable = [&](const pb2_task_t& p, int32_t x, int kind) {
         if (is_linked_body(p.body)) {
-            if (!((linked_checked >> (p.body - PB2_BODY_LINKED_0)) & 1u)) return false;
+            if (!linked_bit(kind == 2 ? prm.linked_sliceable : prm.linked_checked, p.body)) return false;
             int writes = 0;
             for (int f = 0; f < p.nb_flows; ++f) {
                 if (p.tile[f] < 0) continue;
@@ -349,16 +360,17 @@ bool form_read_groups(std::vector<pb2_task_t>& tasks, const uint32_t* succ, cons
         for (int32_t j = 0; j < c;) {
             int32_t r = j + 1;
             int32_t tile = -1;
-            if (reader(out[j])) {
+            const int kind = reader(out[j]);
+            if (kind) {
                 tile = tasks[(size_t)PB2_SUCC_TASK(out[j])].tile[0];
-                while (r < c && r - j < PB2_GROUP_MAX && reader(out[r]) && tasks[(size_t)PB2_SUCC_TASK(out[r])].tile[0] == tile) ++r;
+                while (r < c && r - j < PB2_GROUP_MAX && reader(out[r]) == kind && tasks[(size_t)PB2_SUCC_TASK(out[r])].tile[0] == tile) ++r;
             }
             bool fused = false;
             if (r - j >= 2) {
                 const uint32_t gw = ((uint32_t)gmem.size() << 4) | (uint32_t)(r - j);
                 group[(size_t)PB2_SUCC_TASK(out[j])] = gw;
                 for (int32_t q = j; q < r; ++q) gmem.push_back(PB2_SUCC_TASK(out[q]));
-                fused = fuse && first_group && fusable(tasks[u], tile);
+                fused = fuse && first_group && fusable(tasks[u], tile, kind);
                 if (fused) group[u] = PB2_GROUP_FUSED | gw;
                 first_group = false;
             }
@@ -382,7 +394,7 @@ bool plan_read_groups(const PlanParams& p, int nworkers, const uint32_t* succ, i
     std::vector<int32_t> gmem;
     const bool grouped = !p.shared && p.read_groups >= 0 &&
                          form_read_groups(plan.tasks, succ, ready, nready, tiles, p.fuse_readers >= 0 && nworkers > 1,
-                                          p.linked_checked, gsucc, group, gmem);
+                                          p, gsucc, group, gmem);
     if (grouped) { plan.succ.swap(gsucc); plan.group.swap(group); plan.group_mem.swap(gmem); }
     else plan.succ.assign(succ, succ + nsucc);
     return grouped;
@@ -453,7 +465,13 @@ int plan_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, co
     }
     plan = WindowPlan{};
     plan.tasks.assign(tasks, tasks + ntasks);
-    for (pb2_task_t& t : plan.tasks) { t.flags &= 0x07; plan.linked |= is_linked_body(t.body); }
+    for (pb2_task_t& t : plan.tasks) {
+        t.flags &= 0x07;
+        if (is_linked_body(t.body)) {
+            plan.linked = true;
+            if ((p.linked_readers >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_READER;
+        }
+    }
     std::vector<uint8_t> task_lane;
     if (prio) task_lane = task_priority_lanes(tasks, ntasks, &plan.nlanes);
     if (p.trace) {                              // every task leads itself until a plan groups it

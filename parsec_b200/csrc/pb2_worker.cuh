@@ -139,9 +139,19 @@ __device__ __forceinline__ void store_check_result(const WinDev& w, int32_t id, 
     if (r >> 32) atomicAdd(&w.ctl->body_errors.v, r >> 32);
 }
 
-// Thread 0: store the body result of this part.
+// Thread 0: store a linked reader's result of this part (the sum of its calls): the parts' results add up, modulo 2^64;
+// ~0 aborts the window and is not added.
+__device__ __forceinline__ void store_reader_result(const WinDev& w, int32_t id, int nparts, unsigned long long r) {
+    if (r == ~0ull) st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneBadBody);
+    else if (nparts == 1) w.result[id] = r;
+    else if (r) atomicAdd(&w.result[id], r);
+}
+
+// Thread 0: store the body result of this part.  LINKED (the linked kernels): a task marked PB2_TASK_READER adds it.
+template <bool LINKED = false>
 __device__ __forceinline__ void store_result(const WinDev& w, const pb2_task_t& t, int32_t id, int part, int nparts,
                                              unsigned long long r) {
+    if (LINKED && (t.flags & PB2_TASK_READER)) { store_reader_result(w, id, nparts, r); return; }
     if (r == ~0ull) st_relaxed_gpu(reinterpret_cast<int32_t*>(&w.ctl->done.v), kDoneBadBody);
     if (t.body == PB2_BODY_CHECK_I32 || t.body == PB2_BODY_CHECK_F32) store_check_result(w, id, nparts, r);
     else if (part == 0) w.result[id] = r;
@@ -184,6 +194,12 @@ __device__ __forceinline__ uint32_t load_group_members(const WinDev& w, int32_t 
         if (threadIdx.x == 0) g.tile = __ldg(&mt.tile[0]);
     }
     return gd;
+}
+
+// Whether g, published, is a read group of linked readers (run_linked_group_part): its members are marked
+// PB2_TASK_READER, a CHECK group's never.
+__device__ __forceinline__ bool linked_reader_group(const WinDev& w, const GroupSmem& g) {
+    return g.n && (__ldg(&w.tasks[g.mem[0]].flags) & PB2_TASK_READER);
 }
 
 // All threads, after run_task_part ran the leader's CHECK over this part's slice.  Every member compares the same
@@ -230,13 +246,17 @@ __device__ __forceinline__ void group_part_results(const WinDev& w, TaskSmem& s,
     if (TRACE && threadIdx.x == 0) rec->t_exec = rec->t_out = globaltimer_ns();
 }
 
-// Thread 0, after a part of task id ran with result r: the part's results, the members' of a group first (they are
-// CHECK bodies), then id's own unless id is a group's leader (members[0] has it).
+// Thread 0, after a part of task id ran with result r: the part's results, the members' of a group first (CHECK bodies,
+// or in the LINKED kernels linked readers), then id's own unless id is a group's leader (members[0] has it).
+template <bool LINKED = false>
 __device__ __forceinline__ void store_part_results(const WinDev& w, const pb2_task_t& t, int32_t id, int part, int nparts,
                                                    unsigned long long r, const GroupSmem& g) {
     const int gn = g.n;
-    for (int i = 0; i < gn; ++i) store_check_result(w, g.mem[i], nparts, g.res[i]);
-    if (!gn || g.fused) store_result(w, t, id, part, nparts, r);
+    if (LINKED && linked_reader_group(w, g))
+        for (int i = 0; i < gn; ++i) store_reader_result(w, g.mem[i], nparts, g.res[i]);
+    else
+        for (int i = 0; i < gn; ++i) store_check_result(w, g.mem[i], nparts, g.res[i]);
+    if (!gn || g.fused) store_result<LINKED>(w, t, id, part, nparts, r);
 }
 
 // All threads, after the producer of a fused unit stored its slice of output flow fx and one barrier told them whether
@@ -310,6 +330,98 @@ static __device__ __noinline__ unsigned long long run_linked_part(TaskSmem* sp, 
     while (fx + 1 < (int)s.task.nb_flows && !(s.task.tile[fx] == g.tile && (s.task.access[fx] & PB2_FLOW_ACCESS_WRITE))) ++fx;
     fused_member_results(s, g, lp->k0, mismatch, fx);
     return threadIdx.x == 0 && r == ~0ull ? ~0ull : 0ull;
+}
+
+// The bytes a read group of linked readers walks its part in (run_linked_group_part): half of H100's 50 MB L2 (sm_90a
+// is the only target) over the kernel's workers, in whole 4 KiB, at least 4 KiB.  Every worker keeps one chunk in
+// flight, so the chunks of all workers stay inside L2 while the members re-read them: 24 KiB with the HBM window's
+// 1 056 workers, 192 KiB with the GEMM window's 132.  Chunks that overflow L2 send the re-reads to DRAM, and small
+// ones pay the per-call barriers more often (the sweep is in DESIGN.md §8, *Linked readers*).
+constexpr uint32_t kL2Bytes = 50u << 20;
+__device__ __forceinline__ uint32_t reader_chunk_bytes() {
+    const uint32_t c = (kL2Bytes / 2u / gridDim.x) & ~4095u;
+    return c < 4096u ? 4096u : c;
+}
+
+// Thread 0: a reader's results over its calls, ~0 kept once any call returned it.
+__device__ __forceinline__ unsigned long long add_call_result(unsigned long long acc, unsigned long long r) {
+    return acc == ~0ull || r == ~0ull ? ~0ull : acc + r;
+}
+
+// All threads (LINKED instantiations), in place of the body of a task that leads a read group of linked readers, or
+// of a producer that runs with one (form_read_groups).  Called one after the other over a whole part, the members would
+// each stream it from DRAM: with every worker doing so, far more than L2 holds passes through it between two members'
+// passes.  So the part is walked in chunks of reader_chunk_bytes() (16-byte multiples; the last chunk takes the rest),
+// and every member is called on one chunk before the next: the producer first when one runs with the group (its stores
+// carry the default cache policy, as the members read them back), then each member over the chunk's slice of the tile,
+// a barrier between calls.  Each member's results add up over its calls into g.res (include/pb2_device_body.h); the
+// members of a group led by its first member saw the version the leader saw (as in group_part_results).  Returns the
+// producer's result (thread 0): the sum of its calls when it is itself a reader, else its first chunk's (~0 if any
+// call returned ~0); without a producer, the leader's.
+template <int NT>
+static __device__ __noinline__ unsigned long long run_linked_group_part(TaskSmem* sp, GroupSmem* gp, pb2_body_check_t* lp,
+                                                                        const pb2_task_t* tasks, uint32_t* seen_version) {
+    TaskSmem& s = *sp;
+    GroupSmem& g = *gp;
+    const bool fused = g.fused != 0;
+    const int body = s.task.body;
+    int fx = 0;
+    if (fused)
+        while (fx + 1 < (int)s.task.nb_flows && !(s.task.tile[fx] == g.tile && (s.task.access[fx] & PB2_FLOW_ACCESS_WRITE))) ++fx;
+    const uint32_t len = s.args.bytes[fx], cmax = reader_chunk_bytes();
+    const uint32_t nc = len > cmax ? len / cmax : 1u;
+    uint8_t* const x = static_cast<uint8_t*>(s.args.flow[fx]);
+    // the members' body ids go where a CHECK group keeps its constants
+    if ((int)threadIdx.x < g.n) { g.k[threadIdx.x] = __ldg(&tasks[g.mem[threadIdx.x]].body); g.res[threadIdx.x] = 0; }
+    if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; }
+    const bool psum = (s.task.flags & PB2_TASK_READER) != 0;
+    unsigned long long rp = 0;
+    __syncthreads();
+#pragma unroll 1
+    for (uint32_t c = 0; c < nc; ++c) {
+        const uint32_t off = c * cmax;
+        const bool lastc = c + 1 == nc;
+        if (fused) {
+            if (threadIdx.x < PB2_MAX_FLOWS) {
+                const int f = (int)threadIdx.x;
+                const uint32_t b = s.args.bytes[f], o = off < b ? off : b;
+                lp->args.flow[f] = s.args.flow[f] ? static_cast<uint8_t*>(s.args.flow[f]) + o : nullptr;
+                lp->args.bytes[f] = lastc || b - o < cmax ? b - o : cmax;
+                if (f == 0) {
+                    lp->args.elem0 = s.args.elem0 + (off >> 2); lp->args.part = s.args.part;
+                    lp->args.iparam[0] = s.args.iparam[0]; lp->args.iparam[1] = s.args.iparam[1];
+                    lp->args.iparam[2] = s.args.iparam[2]; lp->args.fparam = s.args.fparam;
+                }
+            }
+            __syncthreads();
+            const unsigned long long r = is_linked_body(body) ? pb2_linked_body(body, &lp->args, s.red)
+                                                              : run_hbm_body(body, *reinterpret_cast<const BodyArgs*>(&lp->args), s.red);
+            if (threadIdx.x == 0) rp = psum ? add_call_result(rp, r) : c == 0 || r == ~0ull ? r : rp;
+            __syncthreads();
+        }
+        const uint32_t cb = lastc ? len - off : cmax;
+#pragma unroll 1
+        for (int i = 0; i < g.n; ++i) {
+            if (threadIdx.x == 0) {
+                const pb2_task_t& mt = tasks[g.mem[i]];
+                pb2_body_args_t& a = lp->args;
+                a.flow[0] = x + off; a.bytes[0] = cb;
+                for (int f = 1; f < PB2_MAX_FLOWS; ++f) { a.flow[f] = nullptr; a.bytes[f] = 0; }
+                a.elem0 = s.args.elem0 + (off >> 2); a.part = s.args.part;
+                a.iparam[0] = __ldg(&mt.iparam[0]); a.iparam[1] = __ldg(&mt.iparam[1]); a.iparam[2] = __ldg(&mt.iparam[2]);
+                a.fparam = __ldg(&mt.fparam);
+            }
+            __syncthreads();
+            const unsigned long long r = pb2_linked_body((int)g.k[i], &lp->args, s.red);
+            if (threadIdx.x == 0) g.res[i] = add_call_result(g.res[i], r);
+            __syncthreads();
+        }
+    }
+    if (threadIdx.x == 0 && !fused && s.args.part == 0) {
+        const uint32_t v = *reinterpret_cast<volatile uint32_t*>(&seen_version[(size_t)g.mem[0] * PB2_MAX_FLOWS]);
+        for (int i = 1; i < g.n; ++i) seen_version[(size_t)g.mem[i] * PB2_MAX_FLOWS] = v;
+    }
+    return fused ? rp : g.res[0];
 }
 
 }  // namespace pb2
