@@ -224,7 +224,8 @@ void* pb2_engine_get_stream(pb2_engine_t* engine);       /* the cudaStream_t eng
 /* n independent copies dst[i][0:bytes[i]] = src[i][..] in ONE kernel launch (workers grid-stride over the list);
  * either side may be HBM, a peer GPU or cudaHostRegister'ed host memory (device-visible alias).  This is what the
  * module uses to write a batch of dirty tiles home (parsec_gpu_create_w2r_task batches <= 20 copies per
- * pseudo-task and pays one cudaMemcpyAsync + event per tile, transfer_gpu.c:224-304).  Stream-ordered. */
+ * pseudo-task and pays one cudaMemcpyAsync + event per tile, transfer_gpu.c:224-304).  Stream-ordered.  Any alignment;
+ * PB2_ERR_VALUE_OUT_OF_BOUNDS, with nothing launched, when a copy is 4 GiB or larger. */
 int  pb2_engine_copy_batch(pb2_engine_t* engine, void* const* dst, const void* const* src, const uint64_t* bytes, int32_t n);
 
 /* --- multi-GPU (one process per GPU): peer-visible memory ---
@@ -241,7 +242,8 @@ int  pb2_engine_enable_peer(pb2_engine_t* engine, int peer_cuda_device);
  * an engine body enqueues when it runs under a device module that is not the engine's (the reference's stream
  * engine drives it then, device_gpu.c:2873-2934).  ptrs/bytes: device address and span of each body argument.
  * CHECK bodies add their mismatch count to a device counter read (and optionally cleared) by
- * pb2_body_launch_errors. */
+ * pb2_body_launch_errors.  PB2_ERR_BAD_PARAM for an argument of bytes > 0 whose pointer is NULL or not 16-byte aligned
+ * (the bodies move 16-byte vectors), PB2_ERR_VALUE_OUT_OF_BOUNDS for one of 4 GiB or more. */
 int  pb2_body_launch(void* cuda_stream, int body, int nb_args, void* const* ptrs, const uint64_t* bytes,
                      const int32_t* iparam3, float fparam);
 int  pb2_body_launch_errors(uint64_t* errors, int reset);
@@ -313,7 +315,9 @@ int  pb2_engine_linked_gemm_info(pb2_engine_t* engine, int32_t* regs, int32_t* l
  * 'kind' selects the kernel instantiation: 0 = HBM bodies, 1 = tensor-core GEMM bodies.  An HBM window with a task of
  * a linked body (PB2_BODY_LINKED_0 .. _7) runs the engine's linked kernel (pb2_engine_link_bodies), and so does a GEMM
  * window with one when the engine linked with PB2_LINK_GEMM_WINDOWS; such a task in any other GEMM window, in a shared
- * window or on an engine without an image is refused (PB2_ERR_NOT_SUPPORTED). */
+ * window or on an engine without an image is refused (PB2_ERR_NOT_SUPPORTED).  The slot (dev_ptr) of a non-empty tile
+ * that a task of any body but NOP names must be 16-byte aligned (PB2_ERR_BAD_PARAM otherwise); host homes (src_ptr) may
+ * have any alignment. */
 int  pb2_window_create(pb2_engine_t* engine, pb2_window_t** window, int kind,
                        const pb2_task_t* tasks, int32_t ntasks,
                        const uint32_t* succ, int32_t nsucc,

@@ -89,7 +89,8 @@ const char* pb2_stream_last_error(pb2_stream_t* stream);
 /* (Re)describe tile `tile` of the device tile table: where the replica lives in HBM, where its source/home copy is,
  * how many bytes, whether it is valid or has to be staged in, and its version.  Takes effect before any task
  * submitted later; the caller must not redescribe a tile that an unretired task uses unless nothing but `src_ptr`
- * of a VALID tile changes. */
+ * of a VALID tile changes.  PB2_ERR_BAD_PARAM for a non-empty tile whose dev_ptr is not 16-byte aligned (the bodies
+ * access slots with 16-byte vectors; src_ptr may have any alignment). */
 int  pb2_stream_set_tile(pb2_stream_t* stream, int32_t tile, const pb2_tile_t* desc);
 
 /* Submit one task.  task->tile[] index the tile table; task->dep_goal is the number of pb2_stream_add_edge calls

@@ -676,6 +676,8 @@ int pb2_engine_memcpy_d2h(pb2_engine_t* e, void* host, const void* dev, size_t b
 int pb2_engine_copy_batch(pb2_engine_t* e, void* const* dst, const void* const* src, const uint64_t* bytes, int32_t n) {
     if (!e || n < 0 || (n && (!dst || !src || !bytes))) return PB2_ERR_BAD_PARAM;
     if (n == 0) return PB2_SUCCESS;
+    for (int32_t i = 0; i < n; ++i)     // the copy loops index bytes with 32 bits, as tiles are below 4 GiB
+        if (bytes[i] >= (1ull << 32)) { e->last_error = "copy of 4 GiB or more"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     std::vector<CopyDesc> h((size_t)n);
     for (int32_t i = 0; i < n; ++i) h[i] = CopyDesc{dst[i], src[i], bytes[i]};
@@ -734,6 +736,8 @@ int pb2_body_launch(void* cuda_stream, int body, int nb_args, void* const* ptrs,
     unsigned long long widest = 0;
     for (int f = 0; f < nb_args; ++f) {
         if (bytes[f] >= (1ull << 32)) return PB2_ERR_VALUE_OUT_OF_BOUNDS;
+        // the bodies load and store 16-byte vectors
+        if (bytes[f] > 0 && (ptrs[f] == nullptr || ((uintptr_t)ptrs[f] & 15))) return PB2_ERR_BAD_PARAM;
         la.ptr[f] = ptrs[f]; la.bytes[f] = bytes[f];
         widest = bytes[f] > widest ? bytes[f] : widest;
     }

@@ -451,10 +451,21 @@ __device__ __forceinline__ int tile_slices_of(int32_t part_bytes, const uint32_t
 }
 __device__ __forceinline__ int tile_slices(const WinDev& w, uint32_t bytes) { return tile_slices_of(w.part_bytes, w.slice_claim, bytes); }
 
-// Stage in the slices [s0, s1) of a tile larger than part_bytes.  Every slice is moved by exactly one CTA (claim
-// bit), so the parts of a wide task -- and the parts of other readers of the same version -- pull the tile in
-// parallel instead of one CTA moving 4 MiB alone; a CTA that finds a slice claimed by someone else only waits
-// for it.  The worker whose slice completes the tile publishes PB2_TILE_VALID.
+// How many of the ns slices of a tile of `bytes` bytes hold bytes.  Slices are ceil16(bytes / ns) long, so when
+// (ns - 1) slices already reach `bytes` the trailing ones are empty (512 x 4097 bytes in 512 slices of 4112: slice 511).  No
+// part's bytes lie in an empty slice (slices_over), so nobody would claim it: the tile is complete once the slices
+// that hold bytes are in.
+__device__ __forceinline__ int live_slices(uint32_t bytes, int ns) {
+    const uint32_t sper = ((bytes / (uint32_t)ns) + 15u) & ~15u;
+    if (sper == 0) return ns;
+    const uint32_t n = bytes / sper + (bytes % sper != 0u);
+    return n < (uint32_t)ns ? (int)n : ns;
+}
+
+// Stage in the slices [s0, s1) of a tile larger than part_bytes, the empty ones (live_slices) left out.  Every slice is
+// moved by exactly one CTA (claim bit), so the parts of a wide task -- and the parts of other readers of the same
+// version -- pull the tile in parallel instead of one CTA moving 4 MiB alone; a CTA that finds a slice claimed by
+// someone else only waits for it.  The worker whose slice completes the tile publishes PB2_TILE_VALID.
 template <bool COUNT>
 static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t tile_id, int nslices, int s0, int s1, int* s_decide,
                                                     BulkSmem* bulk, unsigned long long* moved) {
@@ -466,6 +477,8 @@ static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t ti
     }
     const uint32_t bytes = tile->bytes;
     const uint32_t sper = ((bytes / (uint32_t)nslices) + 15u) & ~15u;
+    const int live = live_slices(bytes, nslices);
+    if (s1 > live) s1 = live;
     uint32_t* claim = w.slice_claim + (size_t)tile_id * PB2_SLICE_WORDS;
     uint32_t* done = w.slice_done + (size_t)tile_id * (PB2_SLICE_WORDS + 1);     // last word: number of staged slices
     for (int sl = s0; sl < s1; ++sl) {
@@ -482,7 +495,7 @@ static __device__ __noinline__ void stage_in_slices(const StageCtx w, int32_t ti
                 atomicOr(&done[sl >> 5], bit);
                 atomicAdd(tile->src_kind == PB2_SRC_PEER ? &w.ctl->bytes_d2d.v : &w.ctl->bytes_h2d.v, (unsigned long long)len);
                 if (COUNT) *moved += len;
-                if ((int)atomicAdd(&done[PB2_SLICE_WORDS], 1u) + 1 == nslices) {
+                if ((int)atomicAdd(&done[PB2_SLICE_WORDS], 1u) + 1 == live) {
                     __threadfence();
                     st_release_gpu(&tile->state, PB2_TILE_VALID);
                     atomicAdd(&w.ctl->stage_ins.v, 1ull);

@@ -308,7 +308,8 @@ pb2_stream_kernel(StreamDev sd) {
             const pb2_task_t& t = s.task;
             store_result(w, t, id, part, nparts, r);
             int last = 1;
-            if (nparts > 1) { last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
+            // the part's result add comes before its count-down: the last part copies w.result into the retire record
+            if (nparts > 1) { __threadfence(); last = atomicSub(&w.parts_left[id], 1) == 1; __threadfence(); }
             if (last) {
                 epilog_written_flows(w, t);
                 // the retire INDEX is taken before the out-edges are released (the host drains records in index
@@ -598,6 +599,8 @@ static void stream_cmd_publish(pb2_stream_t* s, Cmd* c) {
 
 int pb2_stream_set_tile(pb2_stream_t* s, int32_t tile, const pb2_tile_t* desc) {
     if (!s || !desc || tile < 0 || tile >= s->p.max_tiles) return PB2_ERR_BAD_PARAM;
+    if (desc->bytes > 0 && ((uintptr_t)desc->dev_ptr & 15)) {      // the bodies access slots with 16-byte vectors
+        s->last_error = "tile slot not 16-byte aligned"; return PB2_ERR_BAD_PARAM; }
     s->tile_bytes[(size_t)tile] = desc->bytes;
     if (s->dry) { s->dry_tiles[(size_t)tile] = *desc; return PB2_SUCCESS; }
     Cmd* c;

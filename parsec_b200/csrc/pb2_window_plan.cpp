@@ -73,8 +73,22 @@ int plan_gemm_operands(const pb2_task_t* tasks, int32_t ntasks, const pb2_tile_t
         }
         if ((uint64_t)M * N * 2 > tiles[t.tile[2]].bytes) { *why = "GEMM C larger than its tile"; return PB2_ERR_VALUE_OUT_OF_BOUNDS; }
     }
-    for (int32_t i = 0; i < ntiles; ++i)
-        if (rows[i] != 0 && ((uintptr_t)tiles[i].dev_ptr & 15)) { *why = "GEMM tile not 16-byte aligned"; return PB2_ERR_BAD_PARAM; }
+    return PB2_SUCCESS;
+}
+
+// Every body but NOP loads and stores its tiles' slots with 16-byte vectors (GEMM operands through TMA): a slot of such a
+// task must be 16-byte aligned, or the window would fault instead of failing here.  Empty tiles are never accessed.
+int check_slot_alignment(const pb2_task_t* tasks, int32_t ntasks, const pb2_tile_t* tiles, const char** why) {
+    for (int32_t i = 0; i < ntasks; ++i) {
+        const pb2_task_t& t = tasks[i];
+        if (t.body == PB2_BODY_NOP) continue;
+        for (int f = 0; f < t.nb_flows; ++f) {
+            const int32_t id = t.tile[f];
+            if (id < 0 || tiles[id].bytes == 0 || !((uintptr_t)tiles[id].dev_ptr & 15)) continue;
+            *why = t.body == PB2_BODY_GEMM_BF16 ? "GEMM tile not 16-byte aligned" : "tile of a task body not 16-byte aligned";
+            return PB2_ERR_BAD_PARAM;
+        }
+    }
     return PB2_SUCCESS;
 }
 
@@ -458,6 +472,7 @@ int plan_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, co
                 const char** why) {
     int rc = validate_window(p, tasks, ntasks, succ, nsucc, ntiles, ready, nready, why);
     if (rc != PB2_SUCCESS) return rc;
+    if ((rc = check_slot_alignment(tasks, ntasks, tiles, why)) != PB2_SUCCESS) return rc;
     const bool prio = p.queue_policy == 1;
     if (prio && p.shared) {
         *why = "queue_policy 1 (priority lanes) is not supported with shared windows: peers push into one FIFO ring";
