@@ -15,12 +15,16 @@ WINDOW_LOGS  := $(WINDOW_OBJS:.o=.log)
 LINKED_CUBIN := build/pb2_engine_linked.cubin
 # the GEMM window kernel with application bodies, linked only when asked for (PB2_LINK_GEMM_WINDOWS)
 LINKED_GEMM_CUBIN := build/pb2_engine_linked_gemm.cubin
+# both again with the group call of linked readers compiled in, linked instead of them with PB2_LINK_READER_GROUPS
+LINKED_GROUPS_CUBIN := build/pb2_engine_linked_groups.cubin
+LINKED_GEMM_GROUPS_CUBIN := build/pb2_engine_linked_gemm_groups.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
 # the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py,
-# tests/test_linked_readers_gpu.py), as relocatable cubins and as PTX
+# tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py), as relocatable cubins and as PTX
 TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
                 tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx \
-                tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx
+                tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx \
+                tests/cuda/reader_group_bodies.cubin tests/cuda/reader_group_bodies.ptx
 
 all: $(LIB) linked_bodies oracle
 
@@ -41,8 +45,18 @@ $(LINKED_GEMM_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
 	@mkdir -p build
 	$(NVCC) $(NVCCFLAGS) -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_ptxas.log || (cat build/linked_gemm_ptxas.log; exit 1)
 
-$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN)
-	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -DPB2_LINKED_GEMM_CUBIN='"$(abspath $(LINKED_GEMM_CUBIN))"' -o $@ $<
+$(LINKED_GROUPS_CUBIN): $(CSRC)/pb2_engine_linked.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -DPB2_LINKED_READER_GROUPS -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_groups_ptxas.log || (cat build/linked_groups_ptxas.log; exit 1)
+
+$(LINKED_GEMM_GROUPS_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -DPB2_LINKED_READER_GROUPS -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_groups_ptxas.log || (cat build/linked_gemm_groups_ptxas.log; exit 1)
+
+$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN)
+	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -DPB2_LINKED_GEMM_CUBIN='"$(abspath $(LINKED_GEMM_CUBIN))"' \
+	    -DPB2_LINKED_GROUPS_CUBIN='"$(abspath $(LINKED_GROUPS_CUBIN))"' \
+	    -DPB2_LINKED_GEMM_GROUPS_CUBIN='"$(abspath $(LINKED_GEMM_GROUPS_CUBIN))"' -o $@ $<
 
 linked_bodies: $(TEST_BODIES)
 
@@ -64,12 +78,21 @@ tests/cuda/reader_bodies.cubin: tests/cuda/reader_bodies.cu include/pb2_device_b
 tests/cuda/reader_bodies.ptx: tests/cuda/reader_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
 
+# -maxrregcount=80: the group form keeps a count per member in registers; capped, it fits the HBM window kernels'
+# 80-register budget, which the link enforces (the only stack it takes is the call ABI's saved registers)
+tests/cuda/reader_group_bodies.cubin: tests/cuda/reader_group_bodies.cu tests/cuda/reader_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=80 -Iinclude -o $@ $<
+
+tests/cuda/reader_group_bodies.ptx: tests/cuda/reader_group_bodies.cu tests/cuda/reader_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
+
 oracle:
 	$(MAKE) -C oracle
 
 clean:
 	rm -f $(LIB) build_ptxas.log $(WINDOW_OBJS) $(WINDOW_LOGS) $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
-	      build/linked_gemm_ptxas.log $(TEST_BODIES)
+	      build/linked_gemm_ptxas.log $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN) build/linked_groups_ptxas.log \
+	      build/linked_gemm_groups_ptxas.log $(TEST_BODIES)
 	$(MAKE) -C oracle clean
 
 .PHONY: all linked_bodies oracle clean

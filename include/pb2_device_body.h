@@ -53,6 +53,31 @@
  * next), or fuses that group with the task that writes the tile (which then writes each chunk before the members read it
  * back, with check 0: it needs no checked form).  Reductions that must not depend on that order are integer ones.
  *
+ * Reader groups (PB2_LINK_READER_GROUPS(mask), bits 16..23 of the same flags, a subset of the readers mask): the image
+ * also defines
+ *
+ *     extern "C" __device__ unsigned long long pb2_linked_reader_group(const pb2_reader_group_t* g,
+ *                                                                      unsigned long long* results, unsigned int* scratch);
+ *
+ * and a read group calls it once per chunk for all of its members whose bit is set in `mask`, instead of calling
+ * pb2_linked_body once per member; the group's other members are still called one by one.  Contract:
+ *   - All threads of the worker call it together, as pb2_linked_body: 64 in HBM windows, 384 in GEMM windows.
+ *   - g: one chunk of the group's tile (flow, bytes, elem0 and part mean what flow[0], bytes[0], elem0 and part of
+ *     pb2_body_args_t mean for a reader) and the n members of the call, each with its body id and its task's immediates.
+ *   - results[0 .. n): shared memory that the engine zeroes before the call; any thread may atomicAdd into it.  After the
+ *     call results[m] must equal what pb2_linked_body(g->body[m], <the same chunk>) returns from thread 0, so a task's
+ *     result is the same integer on every path: alone, in parts, in a read group called per member or in one call.
+ *     A results[m] of ~0ull marks member m as a bad body, as pb2_linked_body returning ~0 does.
+ *   - scratch: the same 32 words of shared memory as pb2_linked_body gets.
+ *   - ~0ull returned from thread 0 aborts the window as a bad body: every member of the call is then bad, and none of
+ *     their results of the call is added.  Any other return value is ignored.
+ *   - pb2_linked_body must still cover every id: readers that run alone, ungrouped windows (read_groups = -1) and
+ *     members whose bit is clear use it.
+ * An image linked with a nonzero mask must define pb2_linked_reader_group (the link fails otherwise, as any link error
+ * does); with a zero mask the engine links kernels that never call it.  The call runs inside the HBM window kernel's
+ * 80-register budget, which the link enforces: a form that keeps a value per member in registers may need
+ * -maxrregcount=80 (tests/cuda/reader_group_bodies.cu is built so).
+ *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */
 #ifndef PB2_DEVICE_BODY_H
@@ -78,8 +103,24 @@ typedef struct pb2_body_check_s {
     unsigned int    k0;                        /* check mode: the constant every stored element is compared with    */
 } pb2_body_check_t;                            /* 80 bytes on LP64 */
 
+#define PB2_GROUP_MAX 8                        /* members of a read group */
+
+/* What pb2_linked_reader_group is handed: one chunk of the group's tile and the members of the call, in member order. */
+typedef struct pb2_reader_group_s {
+    const void*  flow;                         /* the chunk: device pointer, 16-byte aligned                       */
+    unsigned int bytes;                        /* bytes of the chunk                                               */
+    unsigned int elem0;                        /* index of the chunk's first 4-byte element inside the tile        */
+    unsigned int part;                         /* part index                                                       */
+    unsigned int n;                            /* members in this call, 1 .. PB2_GROUP_MAX                         */
+    int          body[PB2_GROUP_MAX];          /* member m's body id                                               */
+    int          iparam[PB2_GROUP_MAX][3];     /* member m's pb2_task_t::iparam                                    */
+    float        fparam[PB2_GROUP_MAX];        /* member m's pb2_task_t::fparam                                    */
+} pb2_reader_group_t;                          /* 184 bytes on LP64 */
+
 #if defined(__CUDACC__)
 extern "C" __device__ unsigned long long pb2_linked_body(int body, const pb2_body_args_t* a, unsigned int* scratch);
+extern "C" __device__ unsigned long long pb2_linked_reader_group(const pb2_reader_group_t* g, unsigned long long* results,
+                                                                 unsigned int* scratch);
 #endif
 
 #endif /* PB2_DEVICE_BODY_H */

@@ -293,9 +293,16 @@ int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, siz
  *                          as one read group on one worker, fused with that task when it writes the tile
  *                          (pb2_engine_params_t::read_groups, fuse_readers), in windows of both kinds.  `mask` must be a
  *                          subset of `sliceable`: PB2_ERR_BAD_PARAM otherwise.
+ *   PB2_LINK_READER_GROUPS(mask) bits 16..23: bit i of `mask` declares that reader PB2_BODY_LINKED_0 + i has the group
+ *                          form (pb2_linked_reader_group, include/pb2_device_body.h): a read group makes one call of it per
+ *                          chunk for all such members, which then share one pass over the chunk.  `mask` must be a subset
+ *                          of the readers mask (PB2_ERR_BAD_PARAM otherwise).  A nonzero mask links a second build of
+ *                          the window kernels, which makes the call: the image must then define pb2_linked_reader_group
+ *                          (else the link fails as any link error does).  With a zero mask the kernels never call it.
  * PB2_ERR_BAD_PARAM for any other bit. */
 #define PB2_LINK_GEMM_WINDOWS 0x1u
 #define PB2_LINK_READERS(mask) ((uint32_t)(mask) << 8)
+#define PB2_LINK_READER_GROUPS(mask) ((uint32_t)(mask) << 16)
 int  pb2_engine_link_bodies_ex(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
 /* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill

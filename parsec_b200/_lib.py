@@ -50,6 +50,12 @@ def LINK_READERS(mask):
     """pb2_engine_link_bodies_ex flags: bit i of mask declares body BODY_LINKED_0 + i a reader (bits 8..15)."""
     return mask << 8
 
+
+def LINK_READER_GROUPS(mask):
+    """pb2_engine_link_bodies_ex flags: bit i of mask declares that reader BODY_LINKED_0 + i has the group form,
+    pb2_linked_reader_group (bits 16..23, a subset of the readers mask)."""
+    return mask << 16
+
 TASK_DEPS_MASK = 0x01
 TILE_INVALID, TILE_STAGING, TILE_VALID = 0, 1, 2
 SRC_HOST, SRC_PEER = 0, 1

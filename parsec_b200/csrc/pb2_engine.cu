@@ -205,6 +205,7 @@ static PlanParams params_of(const pb2_engine_t* e, int kind) {
     p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
     p.part_bytes = e->params.part_bytes; p.stage_slice_bytes = e->stage_slice_bytes;
     p.linked_sliceable = e->linked_sliceable; p.linked_checked = e->linked_checked; p.linked_readers = e->linked_readers;
+    p.linked_reader_groups = e->linked_reader_groups;
     p.next_rs_begin = e->next_rs_begin;
     return p;
 }
@@ -305,6 +306,9 @@ static int read_part_records(pb2_window_t* w, std::vector<pb2_part_trace_t>& out
 // ---------------------------------------------------------------------------------------------
 extern "C" const unsigned char pb2_linked_engine_image[], pb2_linked_engine_image_end[];
 extern "C" const unsigned char pb2_linked_gemm_image[], pb2_linked_gemm_image_end[];
+// the same two kernels built with PB2_LINKED_READER_GROUPS, which call pb2_linked_reader_group (PB2_LINK_READER_GROUPS)
+extern "C" const unsigned char pb2_linked_engine_groups_image[], pb2_linked_engine_groups_image_end[];
+extern "C" const unsigned char pb2_linked_gemm_groups_image[], pb2_linked_gemm_groups_image_end[];
 
 // The linked window kernels by [kind][(PRIO) + 2 * (TRACE)]: pb2_engine_hbm_kernel<PRIO, TRACE, true>
 // (pb2_engine_linked.cu) and pb2_engine_gemm2_kernel<PRIO, TRACE, true> (pb2_engine_linked_gemm.cu)
@@ -441,6 +445,12 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     if (!e) return PB2_ERR_BAD_PARAM;
     if (const char* why = link_args_error(image, bytes, format, sliceable, checked, flags)) { e->last_error = why; return PB2_ERR_BAD_PARAM; }
     const bool gemm_windows = (flags & PB2_LINK_GEMM_WINDOWS) != 0;
+    // an image without pb2_linked_reader_group links with the plain kernels, which never name it
+    const bool groups = link_reader_groups(flags) != 0;
+    const unsigned char* hbm_image = groups ? pb2_linked_engine_groups_image : pb2_linked_engine_image;
+    const unsigned char* hbm_end = groups ? pb2_linked_engine_groups_image_end : pb2_linked_engine_image_end;
+    const unsigned char* gemm_image = groups ? pb2_linked_gemm_groups_image : pb2_linked_gemm_image;
+    const unsigned char* gemm_end = groups ? pb2_linked_gemm_groups_image_end : pb2_linked_gemm_image_end;
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
     const DriverCalls& d = driver();
@@ -460,11 +470,11 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     CUmodule mod = nullptr;
     CUresult r = d.link_create(5, opt, val, &st);
     if (r == CUDA_SUCCESS)
-        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(pb2_linked_engine_image),
-                       (size_t)(pb2_linked_engine_image_end - pb2_linked_engine_image), "pb2_engine_linked.cubin", 0, nullptr, nullptr);
+        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(hbm_image), (size_t)(hbm_end - hbm_image),
+                       groups ? "pb2_engine_linked_groups.cubin" : "pb2_engine_linked.cubin", 0, nullptr, nullptr);
     if (r == CUDA_SUCCESS && gemm_windows)
-        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(pb2_linked_gemm_image),
-                       (size_t)(pb2_linked_gemm_image_end - pb2_linked_gemm_image), "pb2_engine_linked_gemm.cubin", 0, nullptr, nullptr);
+        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(gemm_image), (size_t)(gemm_end - gemm_image),
+                       groups ? "pb2_engine_linked_gemm_groups.cubin" : "pb2_engine_linked_gemm.cubin", 0, nullptr, nullptr);
     if (r == CUDA_SUCCESS)
         r = d.link_add(st, format == PB2_IMAGE_PTX ? CU_JIT_INPUT_PTX : CU_JIT_INPUT_CUBIN, const_cast<void*>(data), size,
                        "linked bodies", 0, nullptr, nullptr);
@@ -500,6 +510,7 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     e->linked_module = mod;
     std::copy_n(&linked[0][0], 8, &e->kernels[1][0][0]);
     e->linked_sliceable = sliceable; e->linked_checked = checked; e->linked_readers = link_readers(flags);
+    e->linked_reader_groups = link_reader_groups(flags);
     return PB2_SUCCESS;
 }
 

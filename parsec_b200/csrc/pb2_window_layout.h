@@ -38,6 +38,8 @@ struct Lanes {
 // pb2_task_t::flags of a window's device descriptors, set by the planner (the caller's flags keep bits 0..2): the body is
 // a linked reader (PB2_LINK_READERS), whose results add up over parts and calls (store_result)
 #define PB2_TASK_READER 0x80
+// ... and a reader whose read group calls its group form (PB2_LINK_READER_GROUPS, run_linked_group_part)
+#define PB2_TASK_READER_GROUP 0x40
 
 // A task whose tiles are large is executed as several PARTS (byte slices of its tiles) by different workers: one
 // tile at HBM / NVLink speed needs the whole GPU (a 64-thread CTA keeps 4 KiB in flight; a 4 MiB tile is 1.3 us of

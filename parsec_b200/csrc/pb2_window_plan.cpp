@@ -485,6 +485,7 @@ int plan_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, co
         if (is_linked_body(t.body)) {
             plan.linked = true;
             if ((p.linked_readers >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_READER;
+            if ((p.linked_reader_groups >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_READER_GROUP;
         }
     }
     std::vector<uint8_t> task_lane;

@@ -348,6 +348,38 @@ __device__ __forceinline__ unsigned long long add_call_result(unsigned long long
     return acc == ~0ull || r == ~0ull ? ~0ull : acc + r;
 }
 
+#ifdef PB2_LINKED_READER_GROUPS
+static_assert(sizeof(((pb2_reader_group_t*)0)->body) == PB2_GROUP_MAX * sizeof(int), "one group block entry per member");
+
+// Thread 0, before the first chunk of run_linked_group_part: the members of g marked PB2_TASK_READER_GROUP into the
+// group block rg, in member order, their results zeroed, and their bits in mask.
+__device__ __forceinline__ void fill_reader_group(const pb2_task_t* tasks, const GroupSmem& g, pb2_reader_group_t& rg,
+                                                  unsigned long long* res, uint32_t& mask) {
+    uint32_t m = 0, n = 0;
+    for (int i = 0; i < g.n; ++i) {
+        const pb2_task_t& mt = tasks[g.mem[i]];
+        if (!(__ldg(&mt.flags) & PB2_TASK_READER_GROUP)) continue;
+        m |= 1u << i;
+        rg.body[n] = __ldg(&mt.body);
+        rg.iparam[n][0] = __ldg(&mt.iparam[0]); rg.iparam[n][1] = __ldg(&mt.iparam[1]); rg.iparam[n][2] = __ldg(&mt.iparam[2]);
+        rg.fparam[n] = __ldg(&mt.fparam);
+        res[n++] = 0;
+    }
+    rg.n = n;
+    mask = m;
+}
+
+// Thread 0, after a call of pb2_linked_reader_group that returned r: each member of the call adds its result (all of
+// them ~0 when r is), and its result word is zeroed for the next call.
+__device__ __forceinline__ void fold_reader_group(GroupSmem& g, uint32_t mask, unsigned long long r, unsigned long long* res) {
+    for (int i = 0, j = 0; i < g.n; ++i) {
+        if (!((mask >> i) & 1u)) continue;
+        g.res[i] = add_call_result(g.res[i], r == ~0ull ? ~0ull : res[j]);
+        res[j++] = 0;
+    }
+}
+#endif
+
 // All threads (LINKED instantiations), in place of the body of a task that leads a read group of linked readers, or
 // of a producer that runs with one (form_read_groups).  Called one after the other over a whole part, the members would
 // each stream it from DRAM: with every worker doing so, far more than L2 holds passes through it between two members'
@@ -358,6 +390,10 @@ __device__ __forceinline__ unsigned long long add_call_result(unsigned long long
 // members of a group led by its first member saw the version the leader saw (as in group_part_results).  Returns the
 // producer's result (thread 0): the sum of its calls when it is itself a reader, else its first chunk's (~0 if any
 // call returned ~0); without a producer, the leader's.
+// Built with PB2_LINKED_READER_GROUPS (the kernels linked with PB2_LINK_READER_GROUPS), the members marked
+// PB2_TASK_READER_GROUP are not called one by one: one call of pb2_linked_reader_group per chunk gives them all their
+// results, in one pass over the chunk, before the other members are called as above.  Its block and results live in the
+// linked kernels' static shared memory, like *lp.
 template <int NT>
 static __device__ __noinline__ unsigned long long run_linked_group_part(TaskSmem* sp, GroupSmem* gp, pb2_body_check_t* lp,
                                                                         const pb2_task_t* tasks, uint32_t* seen_version) {
@@ -374,9 +410,18 @@ static __device__ __noinline__ unsigned long long run_linked_group_part(TaskSmem
     // the members' body ids go where a CHECK group keeps its constants
     if ((int)threadIdx.x < g.n) { g.k[threadIdx.x] = __ldg(&tasks[g.mem[threadIdx.x]].body); g.res[threadIdx.x] = 0; }
     if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; }
+#ifdef PB2_LINKED_READER_GROUPS
+    __shared__ pb2_reader_group_t rg;
+    __shared__ unsigned long long rg_res[PB2_GROUP_MAX];
+    __shared__ uint32_t rg_mask;
+    if (threadIdx.x == 0) fill_reader_group(tasks, g, rg, rg_res, rg_mask);
+#endif
     const bool psum = (s.task.flags & PB2_TASK_READER) != 0;
     unsigned long long rp = 0;
     __syncthreads();
+#ifdef PB2_LINKED_READER_GROUPS
+    const uint32_t gmask = rg_mask;
+#endif
 #pragma unroll 1
     for (uint32_t c = 0; c < nc; ++c) {
         const uint32_t off = c * cmax;
@@ -400,8 +445,20 @@ static __device__ __noinline__ unsigned long long run_linked_group_part(TaskSmem
             __syncthreads();
         }
         const uint32_t cb = lastc ? len - off : cmax;
+#ifdef PB2_LINKED_READER_GROUPS
+        if (gmask) {
+            if (threadIdx.x == 0) { rg.flow = x + off; rg.bytes = cb; rg.elem0 = s.args.elem0 + (off >> 2); rg.part = s.args.part; }
+            __syncthreads();
+            const unsigned long long r = pb2_linked_reader_group(&rg, rg_res, s.red);
+            __syncthreads();
+            if (threadIdx.x == 0) fold_reader_group(g, gmask, r, rg_res);
+        }
+#endif
 #pragma unroll 1
         for (int i = 0; i < g.n; ++i) {
+#ifdef PB2_LINKED_READER_GROUPS
+            if ((gmask >> i) & 1u) continue;
+#endif
             if (threadIdx.x == 0) {
                 const pb2_task_t& mt = tasks[g.mem[i]];
                 pb2_body_args_t& a = lp->args;

@@ -1,0 +1,29 @@
+// Test-only C entry point to the window planner for tests/test_reader_groups_linked.py: wp_plan_readers of
+// reader_plan_shim.cpp with PlanParams::linked_reader_groups as well (built into one library with window_plan_shim.cpp,
+// which gives wp_array, wp_scalar and wp_free).
+#include "pb2_window_plan.hpp"
+
+using namespace pb2;
+
+extern "C" {
+
+// prm as for wp_plan; linked_checked, linked_readers, linked_reader_groups: bit i, PB2_BODY_LINKED_0 + i has a checked
+// form / is a reader / is a reader with the group form.
+void* wp_plan_reader_groups(const int64_t* prm, uint32_t linked_checked, uint32_t linked_readers,
+                            uint32_t linked_reader_groups, const pb2_task_t* tasks, int32_t ntasks, const uint32_t* succ,
+                            int32_t nsucc, const pb2_tile_t* tiles, int32_t ntiles, const int32_t* ready, int32_t nready,
+                            int* rc, const char** why) {
+    PlanParams p;
+    p.kind = (int)prm[0]; p.shared = prm[1] != 0; p.trace = prm[2] != 0; p.linked_image = p.linked_gemm = prm[3] != 0;
+    p.queue_policy = (int)prm[4]; p.gemm_mode = (int)prm[5]; p.read_groups = (int)prm[6]; p.fuse_readers = (int)prm[7];
+    p.nworkers = (int)prm[8]; p.nworkers_gemm = (int)prm[9];
+    p.part_bytes = (int32_t)prm[10]; p.stage_slice_bytes = (int32_t)prm[11]; p.linked_sliceable = (uint32_t)prm[12];
+    p.linked_checked = linked_checked; p.linked_readers = linked_readers; p.linked_reader_groups = linked_reader_groups;
+    WindowPlan* plan = new WindowPlan();
+    *why = nullptr;
+    *rc = plan_window(p, tasks, ntasks, succ, nsucc, tiles, ntiles, ready, nready, *plan, why);
+    if (*rc != PB2_SUCCESS) { delete plan; return nullptr; }
+    return plan;
+}
+
+}  // extern "C"

@@ -12,9 +12,13 @@ constant), in these windows of one process, alternated run by run:
   - gemm: linked_fused_builtin's DAG beside one small GEMM chain whose C tile four linked readers read, as one GEMM
     window on an engine linked with PB2_LINK_GEMM_WINDOWS (as tools/ab_gemm_groups.py builds it; the chain adds into C
     on every run, so only the Ex05 tasks' results are compared);
-  - gemm_ungrouped: the same GEMM window with read_groups = -1.
+  - gemm_ungrouped: the same GEMM window with read_groups = -1;
+  - group_grouped, group_fused_builtin, group_fused_linked, group_gemm: linked_grouped, linked_fused_builtin,
+    linked_fused_linked and gemm on engines linked with tests/cuda/reader_group_bodies.cubin and its readers declared
+    with the group form (PB2_LINK_READER_GROUPS): each read group calls pb2_linked_reader_group once per chunk.
 Each window runs --runs times after --warmup runs.  Prints one JSON line: the card (name, power limit, maximum SM
-clock), per window the median and min ... max of kernel_ms, and whether every window computed the same results (a
+clock), per window the median and min ... max of kernel_ms, the linked kernels' resources (pb2_engine_linked_info and,
+for the GEMM windows, pb2_engine_linked_gemm_info), and whether every window computed the same results (a
 CHECK reader's mismatch count is the high word of its result) and versions; it fails if they did not.
 
     python tools/ab_linked_readers.py [--runs 30 --warmup 3]
@@ -41,8 +45,10 @@ def windows():
     from parsec_b200 import _lib as L
     from parsec_b200.engine import Engine
     from gemm_chain_dags import ex05_beside_gemm
-    with open(os.path.join(ROOT, "tests", "cuda", "reader_bodies.cubin"), "rb") as f:
-        image = f.read()
+    images = {}
+    for fixture in ("reader_bodies", "reader_group_bodies"):
+        with open(os.path.join(ROOT, "tests", "cuda", fixture + ".cubin"), "rb") as f:
+            images[fixture] = f.read()
     ex = dags.ex05_broadcast(K, 14, TB)
 
     def bodies(dag, producer, reader):
@@ -53,21 +59,27 @@ def windows():
 
     gdag, _, gsizes, ghost = ex05_beside_gemm(K, TB)
     gdag = bodies(gdag, L.BODY_FILL_I32, COUNT_NE)
+    # (name, dag, engine parameters, the fixture linked or None, its group mask)
     cases = [
-        ("builtin_fused", ex, {}, False),
-        ("builtin_ungrouped", ex, dict(read_groups=-1), False),
-        ("linked_ungrouped", bodies(ex, L.BODY_FILL_I32, COUNT_NE), dict(read_groups=-1), True),
-        ("linked_grouped", bodies(ex, L.BODY_FILL_I32, COUNT_NE), dict(fuse_readers=-1), True),
-        ("linked_fused_builtin", bodies(ex, L.BODY_FILL_I32, COUNT_NE), {}, True),
-        ("linked_fused_linked", bodies(ex, FILL, COUNT_NE), {}, True),
-        ("gemm", gdag, {}, True),
-        ("gemm_ungrouped", gdag, dict(read_groups=-1), True),
+        ("builtin_fused", ex, {}, None, 0),
+        ("builtin_ungrouped", ex, dict(read_groups=-1), None, 0),
+        ("linked_ungrouped", bodies(ex, L.BODY_FILL_I32, COUNT_NE), dict(read_groups=-1), "reader_bodies", 0),
+        ("linked_grouped", bodies(ex, L.BODY_FILL_I32, COUNT_NE), dict(fuse_readers=-1), "reader_bodies", 0),
+        ("linked_fused_builtin", bodies(ex, L.BODY_FILL_I32, COUNT_NE), {}, "reader_bodies", 0),
+        ("linked_fused_linked", bodies(ex, FILL, COUNT_NE), {}, "reader_bodies", 0),
+        ("gemm", gdag, {}, "reader_bodies", 0),
+        ("gemm_ungrouped", gdag, dict(read_groups=-1), "reader_bodies", 0),
+        ("group_grouped", bodies(ex, L.BODY_FILL_I32, COUNT_NE), dict(fuse_readers=-1), "reader_group_bodies", READERS),
+        ("group_fused_builtin", bodies(ex, L.BODY_FILL_I32, COUNT_NE), {}, "reader_group_bodies", READERS),
+        ("group_fused_linked", bodies(ex, FILL, COUNT_NE), {}, "reader_group_bodies", READERS),
+        ("group_gemm", gdag, {}, "reader_group_bodies", READERS),
     ]
     out = {}
-    for name, d, kw, link in cases:
+    for name, d, kw, fixture, groups in cases:
         e = Engine(0, **kw)
-        if link:
-            e.link_bodies(image, L.IMAGE_CUBIN, SLICEABLE, 0, gemm_windows=d.kind == 1, readers=READERS)
+        if fixture:
+            e.link_bodies(images[fixture], L.IMAGE_CUBIN, SLICEABLE, 0, gemm_windows=d.kind == 1, readers=READERS,
+                          reader_groups=groups)
         # every tile resident, in 512-byte slots back to back: the Ex05 tiles all -1, the chain's as ex05_beside_gemm
         nb = np.array(gsizes[:d.ntiles], np.int64)
         off = np.concatenate([[0], np.cumsum(nb)[:-1]])
@@ -104,7 +116,8 @@ def main():
             for k, (e, w, _, _) in wins.items():
                 ms[k].append(w.run()["kernel_ms"])
         res = {k: w.results() for k, (e, w, _, _) in wins.items()}
-        infos = {k: e.linked_info() for k, (e, w, _, d) in wins.items() if d.kind == 0 and k.startswith("linked")}
+        infos = {k: e.linked_info() for k, (e, w, _, d) in wins.items() if not k.startswith("builtin")}
+        infos.update({k + "_gemm_kernel": e.linked_gemm_info() for k, (e, w, _, d) in wins.items() if d.kind == 1})
     finally:
         for e, w, slab, _ in wins.values():
             w.close()
