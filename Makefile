@@ -20,11 +20,13 @@ LINKED_GROUPS_CUBIN := build/pb2_engine_linked_groups.cubin
 LINKED_GEMM_GROUPS_CUBIN := build/pb2_engine_linked_gemm_groups.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
 # the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py,
-# tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py), as relocatable cubins and as PTX
+# tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py, tests/test_gemm_worker_bodies_gpu.py), as
+# relocatable cubins and as PTX
 TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
                 tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx \
                 tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx \
-                tests/cuda/reader_group_bodies.cubin tests/cuda/reader_group_bodies.ptx
+                tests/cuda/reader_group_bodies.cubin tests/cuda/reader_group_bodies.ptx \
+                tests/cuda/gemm_worker_bodies.cubin tests/cuda/gemm_worker_bodies.ptx
 
 all: $(LIB) linked_bodies oracle
 
@@ -86,13 +88,20 @@ tests/cuda/reader_group_bodies.cubin: tests/cuda/reader_group_bodies.cu tests/cu
 tests/cuda/reader_group_bodies.ptx: tests/cuda/reader_group_bodies.cu tests/cuda/reader_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -Iinclude -o $@ $<
 
+# -maxrregcount=80: the image is linked into the HBM window kernels as well, whose budget (80) the link enforces
+tests/cuda/gemm_worker_bodies.cubin: tests/cuda/gemm_worker_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=80 -Xptxas -v -Iinclude -o $@ $< 2> tests/cuda/gemm_worker_bodies.log || (cat tests/cuda/gemm_worker_bodies.log; exit 1)
+
+tests/cuda/gemm_worker_bodies.ptx: tests/cuda/gemm_worker_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -maxrregcount=80 -Iinclude -o $@ $<
+
 oracle:
 	$(MAKE) -C oracle
 
 clean:
 	rm -f $(LIB) build_ptxas.log $(WINDOW_OBJS) $(WINDOW_LOGS) $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
 	      build/linked_gemm_ptxas.log $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN) build/linked_groups_ptxas.log \
-	      build/linked_gemm_groups_ptxas.log $(TEST_BODIES)
+	      build/linked_gemm_groups_ptxas.log $(TEST_BODIES) tests/cuda/gemm_worker_bodies.log
 	$(MAKE) -C oracle clean
 
 .PHONY: all linked_bodies oracle clean

@@ -18,7 +18,8 @@
  *     4-byte element inside the tile (elem0), the part index and the task's immediates.  A body whose bit is clear in
  *     the `sliceable` mask of the link call always runs as one part over whole tiles (part 0, elem0 0); a body whose bit
  *     is set may be cut into byte-slice parts like the built-in element-wise bodies, each part run by another worker.
- *   - scratch: 32 words of the worker's shared memory, free for the body's use (32 in GEMM windows too).
+ *   - scratch: 32 words of the worker's shared memory, free for the body's use (32 in GEMM windows too; a GEMM-worker
+ *     body, below, gets the worker's whole operand ring).
  *   - The result is taken from thread 0.  A multi-part task keeps the result of part 0 (a reader's add up, below).
  *   - Returning ~0ull aborts the window as a bad body (pb2_window_wait: PB2_ERR_BAD_PARAM).
  *   - Static __shared__ variables are allowed; they count against the linked kernel's occupancy, which
@@ -78,6 +79,26 @@
  * 80-register budget, which the link enforces: a form that keeps a value per member in registers may need
  * -maxrregcount=80 (tests/cuda/reader_group_bodies.cu is built so).
  *
+ * GEMM-worker bodies (PB2_LINK_GEMM_BODIES(mask), bits 24..31 of the same flags, with PB2_LINK_GEMM_WINDOWS; disjoint
+ * from `sliceable`, and so from `checked` and the readers masks): a body whose bit is set in `mask` runs in GEMM windows
+ * only, and there `scratch` points at the GEMM worker's operand ring instead of the 32 words, so that the application
+ * can stage tensor-core operands (fp64 DMMA, other layouts and precisions) in shared memory.  Contract, on top of the
+ * one above:
+ *   - The ring is PB2_GEMM_BODY_SMEM_BYTES bytes, 1024-byte aligned; its contents are undefined on entry, and the body
+ *     may use all of it.  Nothing of it survives to the next task.
+ *   - The body is called on all 384 threads of the worker (blockDim.x), once per task, over whole tiles (one part,
+ *     elem0 0): such a task is never cut into parts, grouped with readers or fused with a producer.
+ *   - No TMA or bulk copy the body issues may still be in flight when it returns (cp.async copies must be waited on).
+ *   - The engine executes fence.proxy.async before the call and after it, so the body's generic stores to the ring never
+ *     race the wgmma reads and TMA writes of the GEMM units that run on the worker before or after it.
+ *   - scratch is a generic pointer; __cvta_generic_to_shared(scratch) gives its shared-window address, for ld.shared,
+ *     cp.async and ldmatrix.
+ *   - The body is still reached through pb2_linked_body, which the engine links into its HBM window kernels too: the
+ *     image must fit their 80 registers per thread, as every image must (-maxrregcount=80; the link fails otherwise).
+ *     tests/cuda/gemm_worker_bodies.cu runs an fp64 DMMA tile GEMM within that budget.
+ * The 32-word contract is a subset of this one: an image compiled against a header without the mask keeps working.
+ * A task of such a body in an HBM window is refused (PB2_ERR_NOT_SUPPORTED).
+ *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */
 #ifndef PB2_DEVICE_BODY_H
@@ -104,6 +125,10 @@ typedef struct pb2_body_check_s {
 } pb2_body_check_t;                            /* 80 bytes on LP64 */
 
 #define PB2_GROUP_MAX 8                        /* members of a read group */
+
+/* The shared memory a GEMM-worker body gets as `scratch`: the GEMM worker's operand ring, 1024-byte aligned. */
+#define PB2_GEMM_BODY_SMEM_BYTES 196608
+#define PB2_GEMM_BODY_SMEM_ALIGN 1024
 
 /* What pb2_linked_reader_group is handed: one chunk of the group's tile and the members of the call, in member order. */
 typedef struct pb2_reader_group_s {

@@ -299,10 +299,16 @@ int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, siz
  *                          of the readers mask (PB2_ERR_BAD_PARAM otherwise).  A nonzero mask links a second build of
  *                          the window kernels, which makes the call: the image must then define pb2_linked_reader_group
  *                          (else the link fails as any link error does).  With a zero mask the kernels never call it.
+ *   PB2_LINK_GEMM_BODIES(mask) bits 24..31: bit i of `mask` declares that body PB2_BODY_LINKED_0 + i is a GEMM-worker
+ *                          body (include/pb2_device_body.h): in GEMM windows it gets the worker's 192 KiB operand ring
+ *                          as `scratch` and runs as one part, never grouped or fused; HBM windows refuse its tasks
+ *                          (PB2_ERR_NOT_SUPPORTED).  A nonzero mask needs PB2_LINK_GEMM_WINDOWS and must not overlap
+ *                          `sliceable` (so neither `checked` nor the readers masks): PB2_ERR_BAD_PARAM otherwise.
  * PB2_ERR_BAD_PARAM for any other bit. */
 #define PB2_LINK_GEMM_WINDOWS 0x1u
 #define PB2_LINK_READERS(mask) ((uint32_t)(mask) << 8)
 #define PB2_LINK_READER_GROUPS(mask) ((uint32_t)(mask) << 16)
+#define PB2_LINK_GEMM_BODIES(mask) ((uint32_t)(mask) << 24)
 int  pb2_engine_link_bodies_ex(pb2_engine_t* engine, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
 /* What the linker made of the untraced linked kernel of the engine's queue policy: registers per thread, local (spill

@@ -162,7 +162,9 @@ int  pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image,
  * call with flags = 0).  With PB2_LINK_GEMM_WINDOWS a window may hold GEMM tasks and linked-body tasks together: GEMM
  * chains and the application's bodies around them run in one GEMM window.  PB2_LINK_READERS(mask) and
  * PB2_LINK_READER_GROUPS(mask) declare readers and the readers with the group form (pb2_linked_reader_group) as there.
- * A dry-run module checks the flags and records the link. */
+ * PB2_LINK_GEMM_BODIES(mask) declares GEMM-worker bodies as there: a window that holds a task of one is a GEMM window,
+ * as one that holds a GEMM task is, so those tasks never reach an HBM window.  A dry-run module checks the flags and
+ * records the link. */
 int  pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes

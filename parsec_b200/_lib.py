@@ -56,6 +56,12 @@ def LINK_READER_GROUPS(mask):
     pb2_linked_reader_group (bits 16..23, a subset of the readers mask)."""
     return mask << 16
 
+
+def LINK_GEMM_BODIES(mask):
+    """pb2_engine_link_bodies_ex flags: bit i of mask declares body BODY_LINKED_0 + i a GEMM-worker body, which gets the
+    GEMM worker's operand ring as shared memory (bits 24..31; needs LINK_GEMM_WINDOWS, disjoint from sliceable)."""
+    return mask << 24
+
 TASK_DEPS_MASK = 0x01
 TILE_INVALID, TILE_STAGING, TILE_VALID = 0, 1, 2
 SRC_HOST, SRC_PEER = 0, 1

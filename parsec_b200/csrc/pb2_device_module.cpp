@@ -171,7 +171,8 @@ static bool predicted_on_device(pb2_device_module_t* dev, pb2_htask_t* s) {
 // Take the dependency-closed window reachable from the pending tasks of one taskpool, reserving a slot for every tile
 // it touches.  An engine window takes tile GEMMs and HBM bodies together, so that a GEMM chain and the element-wise
 // tasks around it are released on the device instead of through the host; its kind is decided by the closure: 1 (the
-// GEMM kernel, which also runs HBM bodies) when it holds a GEMM task, else 0.  User submit tasks never mix with engine
+// GEMM kernel, which also runs HBM bodies) when it holds a GEMM task -- a bf16 tile GEMM, or a task of a GEMM-worker
+// body (PB2_LINK_GEMM_BODIES), which runs in GEMM windows only -- else 0.  User submit tasks never mix with engine
 // tasks.  Unless the module linked its bodies with PB2_LINK_GEMM_WINDOWS, tasks of linked bodies (which then run in the
 // linked HBM kernel only) never mix with GEMM tasks: the first of the two kinds the closure takes in keeps the other out
 // of this window.
@@ -233,7 +234,8 @@ static int take_closure(pb2_device_module_t* dev, pb2_device_window& w, size_t m
         }
         t->window_index = (int32_t)w.order.size();
         w.order.push_back(t);
-        has_gemm |= t->body == PB2_BODY_GEMM_BF16;
+        has_gemm |= t->body == PB2_BODY_GEMM_BF16 ||
+                    (pb2::is_linked_body(t->body) && ((dev->linked_gemm_bodies >> (t->body - PB2_BODY_LINKED_0)) & 1u));
         for (uint32_t s : t->succ) {
             pb2_htask_t* n = &tp->tasks[PB2_SUCC_TASK(s)];
             if (n->inwin_pred == 0) touched.push_back(n);

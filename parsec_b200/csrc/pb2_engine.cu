@@ -205,7 +205,7 @@ static PlanParams params_of(const pb2_engine_t* e, int kind) {
     p.nworkers = e->nworkers; p.nworkers_gemm = e->nworkers_gemm;
     p.part_bytes = e->params.part_bytes; p.stage_slice_bytes = e->stage_slice_bytes;
     p.linked_sliceable = e->linked_sliceable; p.linked_checked = e->linked_checked; p.linked_readers = e->linked_readers;
-    p.linked_reader_groups = e->linked_reader_groups;
+    p.linked_reader_groups = e->linked_reader_groups; p.linked_gemm_bodies = e->linked_gemm_bodies;
     p.next_rs_begin = e->next_rs_begin;
     return p;
 }
@@ -510,7 +510,7 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     e->linked_module = mod;
     std::copy_n(&linked[0][0], 8, &e->kernels[1][0][0]);
     e->linked_sliceable = sliceable; e->linked_checked = checked; e->linked_readers = link_readers(flags);
-    e->linked_reader_groups = link_reader_groups(flags);
+    e->linked_reader_groups = link_reader_groups(flags); e->linked_gemm_bodies = link_gemm_bodies(flags);
     return PB2_SUCCESS;
 }
 

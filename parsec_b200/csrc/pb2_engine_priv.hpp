@@ -54,9 +54,9 @@ struct pb2_engine_s {
     WindowKernel kernels[2][2][4];
     // pb2_engine_link_bodies: the module of the linked window kernels, and which linked body ids may be cut into parts
     // (bit i: PB2_BODY_LINKED_0 + i), which have a checked form, which are readers (PB2_LINK_READERS) and which readers
-    // have the group form (PB2_LINK_READER_GROUPS)
+    // have the group form (PB2_LINK_READER_GROUPS) and which get the GEMM worker's operand ring (PB2_LINK_GEMM_BODIES)
     CUmodule linked_module = nullptr;
-    uint32_t linked_sliceable = 0, linked_checked = 0, linked_readers = 0, linked_reader_groups = 0;
+    uint32_t linked_sliceable = 0, linked_checked = 0, linked_readers = 0, linked_reader_groups = 0, linked_gemm_bodies = 0;
 };
 
 // The readers mask of link flags (PB2_LINK_READERS): bit i, PB2_BODY_LINKED_0 + i is a reader.
@@ -64,13 +64,17 @@ static inline uint32_t link_readers(uint32_t flags) { return (flags >> 8) & 0xFF
 // The reader groups mask of link flags (PB2_LINK_READER_GROUPS): bit i, reader PB2_BODY_LINKED_0 + i has the group form.
 static inline uint32_t link_reader_groups(uint32_t flags) { return (flags >> 16) & 0xFFu; }
 
+// The GEMM-worker bodies mask of link flags (PB2_LINK_GEMM_BODIES): bit i, PB2_BODY_LINKED_0 + i gets the operand ring.
+static inline uint32_t link_gemm_bodies(uint32_t flags) { return (flags >> 24) & 0xFFu; }
+
 // The argument check of pb2_engine_link_bodies(_checked, _ex) and pb2_device_link_bodies(_checked, _ex): nullptr, or why
 // the arguments are refused.
 static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable, uint32_t checked,
                                           uint32_t flags = 0) {
-    if (flags & ~(uint32_t)(PB2_LINK_GEMM_WINDOWS | PB2_LINK_READERS(0xFFu) | PB2_LINK_READER_GROUPS(0xFFu)))
-        return "link flags have an unknown bit (PB2_LINK_GEMM_WINDOWS, PB2_LINK_READERS(mask), bits 8..15, and "
-               "PB2_LINK_READER_GROUPS(mask), bits 16..23, are the only flags)";
+    if (flags & ~(uint32_t)(PB2_LINK_GEMM_WINDOWS | PB2_LINK_READERS(0xFFu) | PB2_LINK_READER_GROUPS(0xFFu) |
+                            PB2_LINK_GEMM_BODIES(0xFFu)))
+        return "link flags have an unknown bit (PB2_LINK_GEMM_WINDOWS, PB2_LINK_READERS(mask), bits 8..15, "
+               "PB2_LINK_READER_GROUPS(mask), bits 16..23, and PB2_LINK_GEMM_BODIES(mask), bits 24..31, are the only flags)";
     if (!image || !bytes) return "linked body image is NULL or empty";
     if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
     if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";
@@ -82,6 +86,12 @@ static inline const char* link_args_error(const void* image, size_t bytes, int f
     if (link_reader_groups(flags) & ~link_readers(flags))
         return "link flags have an unknown bit: the reader groups mask has a bit that is clear in the readers mask (only a "
                "reader has the group form)";
+    if (link_gemm_bodies(flags) && !(flags & PB2_LINK_GEMM_WINDOWS))
+        return "GEMM-worker bodies mask without PB2_LINK_GEMM_WINDOWS (a GEMM-worker body runs in GEMM windows only)";
+    // the ring is the worker's own: such a body runs whole, never in parts, in a read group or fused with one
+    if (link_gemm_bodies(flags) & sliceable)
+        return "GEMM-worker bodies mask has a bit that is set in the sliceable mask (a GEMM-worker body runs as one part; "
+               "it can be neither checked nor a reader)";
     return nullptr;
 }
 

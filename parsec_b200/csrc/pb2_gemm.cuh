@@ -337,13 +337,34 @@ static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_
     return stage | ((uint64_t)phase << 32);
 }
 
+// All threads (LINKED instantiations), in place of the body of a task marked PB2_TASK_GEMM_BODY: the application's
+// GEMM-worker body gets its task's whole tiles in the 80-byte block *lp, with check 0, as run_linked_part hands them,
+// and the operand ring as scratch (include/pb2_device_body.h).  The ring is idle: the consumers of every GEMM unit that
+// ran on this worker before waited on full[] for each TMA load of the unit and on each of its wgmma groups, before the
+// barrier that ended the unit.  The fences order the body's generic accesses to the ring after those async-proxy
+// accesses, and before the TMA writes of the units after it (the caller's barrier follows the second one).
+static_assert(PB2_GEMM_BODY_SMEM_BYTES == kStages * kStageBytes, "a GEMM-worker body gets the whole operand ring");
+static_assert(kSmemBytes - kStages * kStageBytes == PB2_GEMM_BODY_SMEM_ALIGN, "the ring is aligned up to 1024 bytes");
+static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSmem* sp, pb2_body_check_t* lp, uint8_t* ring) {
+    static_assert(sizeof(BodyArgs) % 4 == 0 && sizeof(BodyArgs) / 4 <= kThreads, "one word of BodyArgs per thread");
+    if (threadIdx.x < sizeof(BodyArgs) / 4)
+        reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&sp->args)[threadIdx.x];
+    if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; }
+    __syncthreads();
+    fence_proxy_async();
+    const unsigned long long r = pb2_linked_body(sp->task.body, &lp->args, reinterpret_cast<unsigned int*>(ring));
+    fence_proxy_async();
+    return r;
+}
+
 }  // namespace gemm
 
 // PRIO: queue_policy 1 (priority lanes of units, pop_prio).  TRACE: write a record of every part into g.trace (PartSmem,
 // then trace_part); the untraced instantiations never touch it.  The built-in instantiations are in
 // pb2_window_kernels.cu, one per object, beside the HBM kernel of the same PRIO and TRACE; the engine launches every
 // instantiation with gemm::kThreads threads and the operand ring, gemm::kSmemBytes, as dynamic shared memory.
-// LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body; built only in
+// LINKED: body ids PB2_BODY_LINKED_0 .. _7 call the application's pb2_linked_body, a task marked PB2_TASK_GEMM_BODY with
+// the operand ring as its scratch (run_gemm_worker_body); built only in
 // pb2_engine_linked_gemm.cu, as relocatable device code that pb2_engine_link_bodies_ex links with the application's
 // image when PB2_LINK_GEMM_WINDOWS is set.  The other instantiations compile as if the flag did not exist.
 template <bool PRIO, bool TRACE, bool LINKED = false>
@@ -476,7 +497,8 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
                 unsigned long long body_r;
-                if constexpr (LINKED) body_r = linked_reader_group(w, sh.gs) ? run_linked_group_part<kThreads>(&sh.ts, &sh.gs, lk, w.tasks, w.seen_version)
+                if constexpr (LINKED) body_r = (sh.ts.task.flags & PB2_TASK_GEMM_BODY) ? run_gemm_worker_body(&sh.ts, lk, smem)
+                                             : linked_reader_group(w, sh.gs) ? run_linked_group_part<kThreads>(&sh.ts, &sh.gs, lk, w.tasks, w.seen_version)
                                              : is_linked_body(sh.ts.task.body) ? run_linked_part<kThreads>(&sh.ts, &sh.gs, lk)
                                              : sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs)
                                                            : run_hbm_body(sh.ts.task.body, sh.ts.args, sh.ts.red);

@@ -40,6 +40,8 @@ struct Lanes {
 #define PB2_TASK_READER 0x80
 // ... and a reader whose read group calls its group form (PB2_LINK_READER_GROUPS, run_linked_group_part)
 #define PB2_TASK_READER_GROUP 0x40
+// ... and a GEMM-worker body (PB2_LINK_GEMM_BODIES): in the linked GEMM kernels it gets the operand ring as scratch
+#define PB2_TASK_GEMM_BODY 0x20
 
 // A task whose tiles are large is executed as several PARTS (byte slices of its tiles) by different workers: one
 // tile at HBM / NVLink speed needs the whole GPU (a 64-thread CTA keeps 4 KiB in flight; a 4 MiB tile is 1.3 us of

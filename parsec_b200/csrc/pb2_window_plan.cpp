@@ -42,6 +42,10 @@ int validate_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks
                            : !p.linked_image ? "linked body id, but the engine has not linked an image (pb2_engine_link_bodies)"
                            : nullptr;
             if (no) { *why = no; return PB2_ERR_NOT_SUPPORTED; }
+            if (kind == 0 && ((p.linked_gemm_bodies >> (t.body - PB2_BODY_LINKED_0)) & 1u)) {
+                *why = "GEMM-worker body in an HBM window (it runs in GEMM windows only, on the worker's operand ring)";
+                return PB2_ERR_NOT_SUPPORTED;
+            }
         }
     }
     for (int32_t i = 0; i < nsucc; ++i)
@@ -486,6 +490,9 @@ int plan_window(const PlanParams& p, const pb2_task_t* tasks, int32_t ntasks, co
             plan.linked = true;
             if ((p.linked_readers >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_READER;
             if ((p.linked_reader_groups >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_READER_GROUP;
+            // a GEMM-worker body is not sliceable (link_args_error): its task runs as one part, is never a reader and
+            // never a fused producer (form_read_groups), so it always runs alone on its worker, with the whole ring
+            if ((p.linked_gemm_bodies >> (t.body - PB2_BODY_LINKED_0)) & 1u) t.flags |= PB2_TASK_GEMM_BODY;
         }
     }
     std::vector<uint8_t> task_lane;

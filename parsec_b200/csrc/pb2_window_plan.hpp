@@ -22,6 +22,8 @@ struct PlanParams {
     uint32_t linked_checked = 0;          // bit i: PB2_BODY_LINKED_0 + i has a checked form (a subset of linked_sliceable)
     uint32_t linked_readers = 0;          // bit i: PB2_BODY_LINKED_0 + i is a reader (a subset of linked_sliceable)
     uint32_t linked_reader_groups = 0;    // bit i: reader PB2_BODY_LINKED_0 + i has the group form (a subset of linked_readers)
+    uint32_t linked_gemm_bodies = 0;      // bit i: PB2_BODY_LINKED_0 + i gets the GEMM worker's operand ring (disjoint from
+                                          // linked_sliceable)
     const int32_t* next_rs_begin = nullptr;     // shared windows: remote out-degree CSR (not owned)
 };
 
@@ -43,7 +45,7 @@ struct PartEntity { int32_t lead, base, nparts; };
 // Everything pb2_window_create uploads or keeps, as host data.  An entry owner is a task of an HBM window or a unit of a
 // GEMM window.
 struct WindowPlan {
-    std::vector<pb2_task_t> tasks;        // the device descriptors: flags masked (+ PB2_TASK_READER, _GROUP), out-edges rewritten by read groups
+    std::vector<pb2_task_t> tasks;        // the device descriptors: flags masked (+ PB2_TASK_READER, _GROUP, PB2_TASK_GEMM_BODY), out-edges rewritten by read groups
     std::vector<uint32_t> succ;           // the device CSR
     std::vector<uint32_t> group;          // HBM windows with read groups (else empty): WinDev::group, group_mem
     std::vector<int32_t> group_mem;
