@@ -176,6 +176,9 @@ typedef struct pb2_engine_info_s {
     int32_t  reserved;
     uint64_t total_mem;
     uint64_t free_mem;
+    int32_t  compression_supported;  /* the device and the driver offer compressible memory (cuMemCreate with
+                                      * CU_MEM_ALLOCATION_COMP_GENERIC)                                            */
+    int32_t  slab_compressible;      /* the engine's last allocation of one granule or more was granted compression */
 } pb2_engine_info_t;
 
 /* What one window run produced; device counters mirror device.h:165-171 statistics. */
@@ -200,7 +203,14 @@ int  pb2_engine_info(pb2_engine_t* engine, pb2_engine_info_t* info);
 const char* pb2_engine_last_error(pb2_engine_t* engine);
 
 /* --- device memory (parsec_device_memory_reserve device_gpu.c:866; cuda memory_allocate/free) --- */
+/* Tile memory.  Where the device supports it, an allocation of one granule (typically 2 MiB) or more is compressible
+ * memory, rounded up to whole granules: the L2 compresses lines on their way to DRAM, so uniform or zero-heavy tiles
+ * cost fewer DRAM bytes, and loads, stores, TMA and copies see ordinary memory.  The device and every peer that
+ * cudaDeviceCanAccessPeer reports may access it.  Smaller requests, and any the driver cannot back with compressed
+ * memory, are cudaMalloc'ed.  pb2_engine_malloc is pb2_engine_malloc_ex with flags 0. */
+#define PB2_MALLOC_IPC 0x1u   /* cudaMalloc memory, which pb2_engine_ipc_export can export to another process */
 int  pb2_engine_malloc(pb2_engine_t* engine, size_t bytes, void** dev_ptr);
+int  pb2_engine_malloc_ex(pb2_engine_t* engine, size_t bytes, uint32_t flags, void** dev_ptr);
 int  pb2_engine_free(pb2_engine_t* engine, void* dev_ptr);
 /* cudaHostRegister(Portable|Mapped) of a whole collection + its device-visible alias
  * (parsec_cuda_memory_register device_cuda_module.c:183-212). Idempotent per ptr. */
@@ -229,7 +239,8 @@ void* pb2_engine_get_stream(pb2_engine_t* engine);       /* the cudaStream_t eng
 int  pb2_engine_copy_batch(pb2_engine_t* engine, void* const* dst, const void* const* src, const uint64_t* bytes, int32_t n);
 
 /* --- multi-GPU (one process per GPU): peer-visible memory ---
- * 64-byte CUDA IPC handles of cudaMalloc'ed memory; a peer process opens them to get a pointer its kernels can
+ * 64-byte CUDA IPC handles of cudaMalloc'ed memory (PB2_MALLOC_IPC; compressible memory is refused with
+ * PB2_ERR_NOT_SUPPORTED); a peer process opens them to get a pointer its kernels can
  * load from / store to over NVLink (parsec_cuda_all_devices_attached enables the same peer access inside one
  * process, device_cuda_module.c:144-181). */
 int  pb2_engine_ipc_export(pb2_engine_t* engine, void* dev_ptr, unsigned char handle[64]);

@@ -44,6 +44,8 @@ BODY_LINKED_0, BODY_LINKED_7 = 20, 27
 IMAGE_PTX, IMAGE_CUBIN = 1, 2
 # pb2_engine_link_bodies_ex flags: also link the GEMM window kernel, so linked bodies run in GEMM windows too
 LINK_GEMM_WINDOWS = 0x1
+# pb2_engine_malloc_ex flags: cudaMalloc memory, which ipc_export can export (compressible memory cannot be)
+MALLOC_IPC = 0x1
 
 
 def LINK_READERS(mask):
@@ -114,7 +116,8 @@ class EngineInfo(C.Structure):
     _fields_ = [("cuda_device", C.c_int32), ("sm_count", C.c_int32), ("cc_major", C.c_int32),
                 ("cc_minor", C.c_int32), ("nworkers", C.c_int32), ("nworkers_gemm", C.c_int32),
                 ("can_map_host", C.c_int32), ("reserved", C.c_int32),
-                ("total_mem", C.c_uint64), ("free_mem", C.c_uint64)]
+                ("total_mem", C.c_uint64), ("free_mem", C.c_uint64),
+                ("compression_supported", C.c_int32), ("slab_compressible", C.c_int32)]
 
 
 class WindowStats(C.Structure):
@@ -149,7 +152,7 @@ _lib = None
 # every extern "C" symbol include/pb2_engine.h declares
 ENGINE_SYMBOLS = [
     "pb2_engine_create", "pb2_engine_destroy", "pb2_engine_info", "pb2_engine_last_error",
-    "pb2_engine_malloc", "pb2_engine_free", "pb2_engine_host_register", "pb2_engine_host_unregister",
+    "pb2_engine_malloc", "pb2_engine_malloc_ex", "pb2_engine_free", "pb2_engine_host_register", "pb2_engine_host_unregister",
     "pb2_engine_memcpy_h2d", "pb2_engine_prefetch_h2d", "pb2_engine_memcpy_d2h", "pb2_engine_synchronize", "pb2_engine_set_stream", "pb2_engine_get_stream", "pb2_engine_copy_batch", "pb2_engine_ipc_export", "pb2_engine_ipc_open",
     "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_window_trace", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
     "pb2_window_arm", "pb2_window_start",
@@ -180,6 +183,7 @@ def load():
     lib.pb2_engine_last_error.argtypes = [vp]
     lib.pb2_engine_last_error.restype = C.c_char_p
     lib.pb2_engine_malloc.argtypes = [vp, C.c_size_t, P(vp)]
+    lib.pb2_engine_malloc_ex.argtypes = [vp, C.c_size_t, C.c_uint32, P(vp)]
     lib.pb2_engine_free.argtypes = [vp, vp]
     lib.pb2_engine_host_register.argtypes = [vp, vp, C.c_size_t, P(vp)]
     lib.pb2_engine_host_unregister.argtypes = [vp, vp]

@@ -323,9 +323,24 @@ static const char* const kLinkedKernels[2][4] = {
      "_ZN3pb223pb2_engine_gemm2_kernelILb1ELb1ELb1EEEvNS_7Win2DevE"},
 };
 
-// The driver calls of the linking point and of every window kernel's launch, fetched through the runtime (as
-// cuTensorMapEncodeTiled is): the library gains no link dependency on libcuda.
+// The driver calls of the linking point, of every window kernel's launch and of compressible tile memory, fetched
+// through the runtime (as cuTensorMapEncodeTiled is): the library gains no link dependency on libcuda.
 struct DriverCalls {
+    decltype(&cuDeviceGet) device_get = nullptr;
+    decltype(&cuDeviceGetAttribute) device_attr = nullptr;
+    decltype(&cuMemCreate) mem_create = nullptr;
+    decltype(&cuMemGetAllocationGranularity) mem_granularity = nullptr;
+    decltype(&cuMemGetAllocationPropertiesFromHandle) mem_props = nullptr;
+    decltype(&cuMemAddressReserve) mem_reserve = nullptr;
+    decltype(&cuMemMap) mem_map = nullptr;
+    decltype(&cuMemSetAccess) mem_set_access = nullptr;
+    decltype(&cuMemUnmap) mem_unmap = nullptr;
+    decltype(&cuMemAddressFree) mem_address_free = nullptr;
+    decltype(&cuMemRelease) mem_release = nullptr;
+    bool vmm() const {
+        return device_get && device_attr && mem_create && mem_granularity && mem_props && mem_reserve && mem_map &&
+               mem_set_access && mem_unmap && mem_address_free && mem_release;
+    }
     decltype(&cuLinkCreate) link_create = nullptr;
     decltype(&cuLinkAddData) link_add = nullptr;
     decltype(&cuLinkComplete) link_complete = nullptr;
@@ -357,9 +372,79 @@ static const DriverCalls& driver() {
         get("cuModuleGetFunction", r.get_function); get("cuFuncGetAttribute", r.func_attr);
         get("cuFuncSetAttribute", r.func_set_attr);
         get("cuOccupancyMaxActiveBlocksPerMultiprocessor", r.occupancy); get("cuLaunchKernel", r.launch);
+        get("cuDeviceGet", r.device_get); get("cuDeviceGetAttribute", r.device_attr); get("cuMemCreate", r.mem_create);
+        get("cuMemGetAllocationGranularity", r.mem_granularity);
+        get("cuMemGetAllocationPropertiesFromHandle", r.mem_props); get("cuMemAddressReserve", r.mem_reserve);
+        get("cuMemMap", r.mem_map); get("cuMemSetAccess", r.mem_set_access); get("cuMemUnmap", r.mem_unmap);
+        get("cuMemAddressFree", r.mem_address_free); get("cuMemRelease", r.mem_release);
         return r;
     }();
     return d;
+}
+
+// Compressible memory on device dev: the L2 compresses its lines on their way to DRAM.
+static CUmemAllocationProp compressible_prop(int dev) {
+    CUmemAllocationProp p{};
+    p.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    p.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    p.location.id = dev;
+    p.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+    return p;
+}
+
+// The granule of compressible memory on device dev, or 0 where the device or the driver offers none.
+static size_t compressible_granule(int dev) {
+    const DriverCalls& d = driver();
+    CUdevice cd = 0;
+    int on = 0;
+    size_t g = 0;
+    if (!d.vmm() || d.device_get(&cd, dev) != CUDA_SUCCESS ||
+        d.device_attr(&on, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, cd) != CUDA_SUCCESS || !on)
+        return 0;
+    const CUmemAllocationProp p = compressible_prop(dev);
+    return d.mem_granularity(&g, &p, CU_MEM_ALLOC_GRANULARITY_MINIMUM) == CUDA_SUCCESS ? g : 0;
+}
+
+static void release_compressible(void* p, CUmemGenericAllocationHandle h, size_t bytes, bool mapped = true) {
+    const DriverCalls& d = driver();
+    const CUdeviceptr ptr = reinterpret_cast<CUdeviceptr>(p);
+    if (mapped) d.mem_unmap(ptr, bytes);
+    if (ptr) d.mem_address_free(ptr, bytes);
+    d.mem_release(h);
+}
+
+// bytes (whole granules) of compressible memory, accessible from the engine's device and from every device that can
+// access it as a peer (cudaDeviceEnablePeerAccess does not cover such a mapping), or nullptr with nothing left behind
+// when any step fails or the driver grants the memory uncompressed (it does when the compression tags run out).
+static void* map_compressible(pb2_engine_t* e, size_t bytes, CUmemGenericAllocationHandle& h) {
+    const DriverCalls& d = driver();
+    const CUmemAllocationProp p = compressible_prop(e->cuda_device);
+    if (d.mem_create(&h, bytes, &p, 0) != CUDA_SUCCESS) return nullptr;
+    CUmemAllocationProp got{};
+    CUdeviceptr ptr = 0;
+    bool mapped = false;
+    bool ok = d.mem_props(&got, h) == CUDA_SUCCESS && got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC;
+    if (ok) ok = d.mem_reserve(&ptr, bytes, e->comp_granule, 0, 0) == CUDA_SUCCESS;
+    if (ok) ok = mapped = d.mem_map(ptr, bytes, 0, h, 0) == CUDA_SUCCESS;
+    if (ok) {
+        int ndev = 0;
+        if (cudaGetDeviceCount(&ndev) != cudaSuccess) { cudaGetLastError(); ndev = 0; }
+        std::vector<CUmemAccessDesc> access;
+        for (int dev = 0; dev < ndev; ++dev) {
+            int can = dev == e->cuda_device;
+            if (!can && cudaDeviceCanAccessPeer(&can, dev, e->cuda_device) != cudaSuccess) { cudaGetLastError(); can = 0; }
+            if (can != 1) continue;
+            CUmemAccessDesc a{};
+            a.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+            a.location.id = dev;
+            a.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+            access.push_back(a);
+        }
+        ok = !access.empty() && d.mem_set_access(ptr, bytes, access.data(), access.size()) == CUDA_SUCCESS;
+    }
+    if (ok) return reinterpret_cast<void*>(ptr);
+    release_compressible(reinterpret_cast<void*>(ptr), h, bytes, mapped);
+    return nullptr;
 }
 
 // Window kernel fn of `kind` as a kernel table entry k, the same for built-in and linked kernels: its resources, and its
@@ -561,6 +646,7 @@ int pb2_engine_create(pb2_engine_t** engine, int cuda_device, const pb2_engine_p
     PB2_CUDA(e, cudaStreamCreateWithFlags(&e->arm_stream, cudaStreamNonBlocking));
     PB2_CUDA(e, cudaEventCreateWithFlags(&e->dma_ev, cudaEventDisableTiming));
     e->stream = e->own_stream;
+    e->comp_granule = compressible_granule(cuda_device);
     {   // keep freed window scratch cached in the default mempool instead of returning it to the driver
         cudaMemPool_t pool;
         if (cudaDeviceGetDefaultMemPool(&pool, cuda_device) == cudaSuccess) {
@@ -590,6 +676,8 @@ int pb2_engine_destroy(pb2_engine_t* e) {
     if (e->arm_stream) cudaStreamDestroy(e->arm_stream);
     if (e->dma_ev) cudaEventDestroy(e->dma_ev);
     if (e->linked_module) driver().module_unload(e->linked_module);
+    if (!e->compressible.empty()) cudaDeviceSynchronize();
+    for (auto& kv : e->compressible) release_compressible(kv.first, kv.second.first, kv.second.second);
     delete e;
     return PB2_SUCCESS;
 }
@@ -606,14 +694,31 @@ int pb2_engine_info(pb2_engine_t* e, pb2_engine_info_t* info) {
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     PB2_CUDA(e, cudaMemGetInfo(&f, &t));
     info->total_mem = t; info->free_mem = f;
+    info->compression_supported = e->comp_granule != 0;
+    info->slab_compressible = e->slab_compressible;
     return PB2_SUCCESS;
 }
 
 const char* pb2_engine_last_error(pb2_engine_t* e) { return e ? e->last_error.c_str() : "null engine"; }
 
-int pb2_engine_malloc(pb2_engine_t* e, size_t bytes, void** dev_ptr) {
-    if (!e || !dev_ptr) return PB2_ERR_BAD_PARAM;
+int pb2_engine_malloc(pb2_engine_t* e, size_t bytes, void** dev_ptr) { return pb2_engine_malloc_ex(e, bytes, 0, dev_ptr); }
+
+int pb2_engine_malloc_ex(pb2_engine_t* e, size_t bytes, uint32_t flags, void** dev_ptr) {
+    if (!e || !dev_ptr || (flags & ~PB2_MALLOC_IPC)) return PB2_ERR_BAD_PARAM;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
+    const size_t g = e->comp_granule;
+    if (g && bytes >= g) {
+        std::lock_guard<std::mutex> lk(e->mu);
+        const size_t mapped = (bytes + g - 1) / g * g;
+        CUmemGenericAllocationHandle h{};
+        void* p = (flags & PB2_MALLOC_IPC) ? nullptr : map_compressible(e, mapped, h);
+        e->slab_compressible = p != nullptr;
+        if (p) {
+            e->compressible[p] = {h, mapped};
+            *dev_ptr = p;
+            return PB2_SUCCESS;
+        }
+    }
     cudaError_t err = cudaMalloc(dev_ptr, bytes ? bytes : 16);
     if (err == cudaErrorMemoryAllocation) { cudaGetLastError(); *dev_ptr = nullptr; return PB2_ERR_OUT_OF_RESOURCE; }
     PB2_CUDA(e, err);
@@ -623,7 +728,18 @@ int pb2_engine_malloc(pb2_engine_t* e, size_t bytes, void** dev_ptr) {
 int pb2_engine_free(pb2_engine_t* e, void* dev_ptr) {
     if (!e) return PB2_ERR_BAD_PARAM;
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
-    PB2_CUDA(e, cudaFree(dev_ptr));
+    std::unique_lock<std::mutex> lk(e->mu);
+    auto it = e->compressible.find(dev_ptr);
+    if (it == e->compressible.end()) {
+        lk.unlock();
+        PB2_CUDA(e, cudaFree(dev_ptr));
+        return PB2_SUCCESS;
+    }
+    const auto [h, bytes] = it->second;
+    e->compressible.erase(it);
+    lk.unlock();
+    PB2_CUDA(e, cudaDeviceSynchronize());       // as cudaFree does: work still using the memory ends first
+    release_compressible(dev_ptr, h, bytes);
     return PB2_SUCCESS;
 }
 
@@ -705,6 +821,16 @@ int pb2_engine_copy_batch(pb2_engine_t* e, void* const* dst, const void* const* 
 
 int pb2_engine_ipc_export(pb2_engine_t* e, void* dev_ptr, unsigned char handle[64]) {
     if (!e || !dev_ptr || !handle) return PB2_ERR_BAD_PARAM;
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        auto it = e->compressible.upper_bound(dev_ptr);     // the allocation that holds dev_ptr is the one before
+        if (it != e->compressible.begin() &&
+            static_cast<char*>(dev_ptr) < static_cast<char*>(std::prev(it)->first) + std::prev(it)->second.second) {
+            e->last_error = "the memory is compressible, which CUDA IPC cannot export: allocate memory for other processes "
+                            "with pb2_engine_malloc_ex(..., PB2_MALLOC_IPC, ...)";
+            return PB2_ERR_NOT_SUPPORTED;
+        }
+    }
     PB2_CUDA(e, cudaSetDevice(e->cuda_device));
     cudaIpcMemHandle_t ih;
     PB2_CUDA(e, cudaIpcGetMemHandle(&ih, dev_ptr));

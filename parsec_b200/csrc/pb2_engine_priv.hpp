@@ -48,6 +48,12 @@ struct pb2_engine_s {
     bool window_trace = false;           // windows created from now on record per-task device time stamps
     const int32_t* next_rs_begin = nullptr;   // remote out-degree CSR of the next shared window (not owned)
     std::map<void*, std::pair<size_t, void*>> registered;   // host ptr -> (bytes, device alias)
+    // Compressible tile memory (pb2_engine_malloc_ex): the granule of such an allocation, 0 where the device or the
+    // driver offers none; every allocation the L2 compresses, base -> (handle, mapped bytes), freed by pb2_engine_free
+    // or with the engine; whether the last allocation of a granule or more was granted compression.
+    size_t comp_granule = 0;
+    std::map<void*, std::pair<CUmemGenericAllocationHandle, size_t>> compressible;
+    bool slab_compressible = false;
     // Every window kernel by [built-in, linked][kind: HBM, GEMM][(queue_policy 1) + 2 * (trace)].  A built-in entry
     // is resolved when a window first needs it, under mu; pb2_engine_link_bodies_ex resolves the linked HBM entries,
     // and with PB2_LINK_GEMM_WINDOWS the linked GEMM entries (an entry that is not resolved has a null fn).

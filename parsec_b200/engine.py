@@ -118,9 +118,11 @@ class Engine:
         _check(self._lib.pb2_engine_info(self._h, C.byref(i)), "pb2_engine_info", self)
         return {f[0]: getattr(i, f[0]) for f in L.EngineInfo._fields_ if f[0] != "reserved"}
 
-    def malloc(self, nbytes):
+    def malloc(self, nbytes, ipc=False):
+        """Device memory, compressible where the device supports it and nbytes is one granule or more (info()'s
+        slab_compressible tells which); ipc=True gives cudaMalloc memory, which ipc_export can export."""
         p = C.c_void_p()
-        _check(self._lib.pb2_engine_malloc(self._h, nbytes, C.byref(p)), "pb2_engine_malloc", self)
+        _check(self._lib.pb2_engine_malloc_ex(self._h, nbytes, L.MALLOC_IPC if ipc else 0, C.byref(p)), "pb2_engine_malloc_ex", self)
         self._allocs.append(p.value)
         return p.value
 

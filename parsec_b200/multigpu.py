@@ -282,7 +282,7 @@ class SharedRun:
         part.set_push(push)
         z = part.sizes(rank)
         self.slab_bytes = max(int(z["slab_bytes"]), 256)
-        self.slab = eng.malloc(self.slab_bytes)
+        self.slab = eng.malloc(self.slab_bytes, ipc=True)
         eng.h2d(self.slab, np.zeros(self.slab_bytes, np.uint8))
         eng.synchronize()
         handles = [None] * world

@@ -29,7 +29,7 @@ from ab_read_groups import TB, card, l2_probe, summary
 class Window:
     """One engine and one resident window of the Ex05 DAG (or of its producers alone) on it."""
 
-    def __init__(self, K, fuse_readers=0, fill_only=False, part_bytes=0, workers_per_sm=0):
+    def __init__(self, K, fuse_readers=0, fill_only=False, part_bytes=0, workers_per_sm=0, ipc=False):
         self.e = Engine(0, workers_per_sm=workers_per_sm, fuse_readers=fuse_readers, part_bytes=part_bytes)
         dag = dags.ex05_broadcast(K, 14, TB)
         tasks, succ = dag.tasks, dag.succ
@@ -38,7 +38,7 @@ class Window:
             tasks["succ_begin"], tasks["succ_count"] = 0, 0
             succ = np.zeros(0, np.uint32)
         self.ntasks = len(tasks)
-        self.slab = self.e.malloc(K * TB)
+        self.slab = self.e.malloc(K * TB, ipc=ipc)       # ipc=True: plain cudaMalloc memory, never compressible
         self.e.h2d(self.slab, np.zeros(K * TB // 4, np.int32))
         tiles = np.zeros(K, L.TILE_DTYPE)
         tiles["dev_ptr"] = self.slab + np.arange(K, dtype=np.uint64) * np.uint64(TB)

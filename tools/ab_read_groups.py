@@ -36,12 +36,13 @@ def card():
     return out
 
 
-def l2_probe():
+def l2_probe(*args):
+    """tools/l2_probe's last JSON line, run with args."""
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     with tempfile.TemporaryDirectory() as d:
         exe = os.path.join(d, "l2_probe")
         subprocess.check_call([nvcc, "-O3", "-gencode", "arch=compute_90a,code=sm_90a", os.path.join(HERE, "l2_probe.cu"), "-o", exe])
-        out = subprocess.run([exe], capture_output=True, text=True, timeout=120).stdout
+        out = subprocess.run([exe, *args], capture_output=True, text=True, timeout=120).stdout
     lines = [l for l in out.splitlines() if l.startswith("{")]
     return json.loads(lines[-1]) if lines else {"error": out[-400:]}
 
