@@ -18,15 +18,21 @@ LINKED_GEMM_CUBIN := build/pb2_engine_linked_gemm.cubin
 # both again with the group call of linked readers compiled in, linked instead of them with PB2_LINK_READER_GROUPS
 LINKED_GROUPS_CUBIN := build/pb2_engine_linked_groups.cubin
 LINKED_GEMM_GROUPS_CUBIN := build/pb2_engine_linked_gemm_groups.cubin
+# the GEMM window kernel that calls GEMM-worker bodies through pb2_linked_gemm_body, with and without the group call,
+# linked instead of the two above with PB2_LINK_GEMM_BODY_ENTRY
+LINKED_GEMM_ENTRY_CUBIN := build/pb2_engine_linked_gemm_entry.cubin
+LINKED_GEMM_ENTRY_GROUPS_CUBIN := build/pb2_engine_linked_gemm_entry_groups.cubin
 LINKED_OBJ   := build/pb2_linked_image.o
 # the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py,
-# tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py, tests/test_gemm_worker_bodies_gpu.py), as
-# relocatable cubins and as PTX
+# tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py, tests/test_gemm_worker_bodies_gpu.py,
+# tests/test_gemm_body_entry_gpu.py), as relocatable cubins and as PTX
 TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
                 tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx \
                 tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx \
                 tests/cuda/reader_group_bodies.cubin tests/cuda/reader_group_bodies.ptx \
-                tests/cuda/gemm_worker_bodies.cubin tests/cuda/gemm_worker_bodies.ptx
+                tests/cuda/gemm_worker_bodies.cubin tests/cuda/gemm_worker_bodies.ptx \
+                tests/cuda/gemm_entry_bodies.cubin tests/cuda/gemm_entry_bodies.ptx \
+                tests/cuda/gemm_entry_group_bodies.cubin
 
 all: $(LIB) linked_bodies oracle
 
@@ -55,10 +61,21 @@ $(LINKED_GEMM_GROUPS_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
 	@mkdir -p build
 	$(NVCC) $(NVCCFLAGS) -DPB2_LINKED_READER_GROUPS -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_groups_ptxas.log || (cat build/linked_gemm_groups_ptxas.log; exit 1)
 
-$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN)
+$(LINKED_GEMM_ENTRY_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -DPB2_LINKED_GEMM_BODY_ENTRY -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_entry_ptxas.log || (cat build/linked_gemm_entry_ptxas.log; exit 1)
+
+$(LINKED_GEMM_ENTRY_GROUPS_CUBIN): $(CSRC)/pb2_engine_linked_gemm.cu $(HDRS)
+	@mkdir -p build
+	$(NVCC) $(NVCCFLAGS) -DPB2_LINKED_GEMM_BODY_ENTRY -DPB2_LINKED_READER_GROUPS -rdc=true -cubin -o $@ $< -Iinclude 2> build/linked_gemm_entry_groups_ptxas.log || (cat build/linked_gemm_entry_groups_ptxas.log; exit 1)
+
+$(LINKED_OBJ): $(CSRC)/pb2_linked_image.S $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN) \
+               $(LINKED_GEMM_ENTRY_CUBIN) $(LINKED_GEMM_ENTRY_GROUPS_CUBIN)
 	gcc -c -DPB2_LINKED_CUBIN='"$(abspath $(LINKED_CUBIN))"' -DPB2_LINKED_GEMM_CUBIN='"$(abspath $(LINKED_GEMM_CUBIN))"' \
 	    -DPB2_LINKED_GROUPS_CUBIN='"$(abspath $(LINKED_GROUPS_CUBIN))"' \
-	    -DPB2_LINKED_GEMM_GROUPS_CUBIN='"$(abspath $(LINKED_GEMM_GROUPS_CUBIN))"' -o $@ $<
+	    -DPB2_LINKED_GEMM_GROUPS_CUBIN='"$(abspath $(LINKED_GEMM_GROUPS_CUBIN))"' \
+	    -DPB2_LINKED_GEMM_ENTRY_CUBIN='"$(abspath $(LINKED_GEMM_ENTRY_CUBIN))"' \
+	    -DPB2_LINKED_GEMM_ENTRY_GROUPS_CUBIN='"$(abspath $(LINKED_GEMM_ENTRY_GROUPS_CUBIN))"' -o $@ $<
 
 linked_bodies: $(TEST_BODIES)
 
@@ -95,13 +112,27 @@ tests/cuda/gemm_worker_bodies.cubin: tests/cuda/gemm_worker_bodies.cu include/pb
 tests/cuda/gemm_worker_bodies.ptx: tests/cuda/gemm_worker_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -maxrregcount=80 -Iinclude -o $@ $<
 
+# -maxrregcount=168: pb2_linked_gemm_body is reached from the GEMM window kernels only, whose budget (168) the link
+# enforces; pb2_linked_body still reaches the HBM kernels too, and ptxas fits it in their 80 (the link checks that)
+tests/cuda/gemm_entry_bodies.cubin: tests/cuda/gemm_entry_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=168 -Xptxas -v -Iinclude -o $@ $< 2> tests/cuda/gemm_entry_bodies.log || (cat tests/cuda/gemm_entry_bodies.log; exit 1)
+
+tests/cuda/gemm_entry_bodies.ptx: tests/cuda/gemm_entry_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 -arch=compute_90a -rdc=true -ptx -maxrregcount=168 -Iinclude -o $@ $<
+
+# the same image with the group form of its reader, pb2_linked_reader_group (PB2_LINK_READER_GROUPS)
+tests/cuda/gemm_entry_group_bodies.cubin: tests/cuda/gemm_entry_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=168 -DGEMM_ENTRY_READER_GROUP -Iinclude -o $@ $<
+
 oracle:
 	$(MAKE) -C oracle
 
 clean:
 	rm -f $(LIB) build_ptxas.log $(WINDOW_OBJS) $(WINDOW_LOGS) $(LINKED_CUBIN) $(LINKED_GEMM_CUBIN) $(LINKED_OBJ) build/linked_ptxas.log \
 	      build/linked_gemm_ptxas.log $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN) build/linked_groups_ptxas.log \
-	      build/linked_gemm_groups_ptxas.log $(TEST_BODIES) tests/cuda/gemm_worker_bodies.log
+	      build/linked_gemm_groups_ptxas.log $(LINKED_GEMM_ENTRY_CUBIN) $(LINKED_GEMM_ENTRY_GROUPS_CUBIN) \
+	      build/linked_gemm_entry_ptxas.log build/linked_gemm_entry_groups_ptxas.log $(TEST_BODIES) \
+	      tests/cuda/gemm_worker_bodies.log tests/cuda/gemm_entry_bodies.log
 	$(MAKE) -C oracle clean
 
 .PHONY: all linked_bodies oracle clean

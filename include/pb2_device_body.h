@@ -93,11 +93,34 @@
  *     race the wgmma reads and TMA writes of the GEMM units that run on the worker before or after it.
  *   - scratch is a generic pointer; __cvta_generic_to_shared(scratch) gives its shared-window address, for ld.shared,
  *     cp.async and ldmatrix.
- *   - The body is still reached through pb2_linked_body, which the engine links into its HBM window kernels too: the
- *     image must fit their 80 registers per thread, as every image must (-maxrregcount=80; the link fails otherwise).
- *     tests/cuda/gemm_worker_bodies.cu runs an fp64 DMMA tile GEMM within that budget.
+ *   - Linked without PB2_LINK_GEMM_BODY_ENTRY, the body is reached through pb2_linked_body, which the engine links into
+ *     its HBM window kernels too: the image must then fit their 80 registers per thread, as every image must
+ *     (-maxrregcount=80; the link fails otherwise).  tests/cuda/gemm_worker_bodies.cu runs an fp64 DMMA tile GEMM within
+ *     that budget.
  * The 32-word contract is a subset of this one: an image compiled against a header without the mask keeps working.
  * A task of such a body in an HBM window is refused (PB2_ERR_NOT_SUPPORTED).
+ *
+ * The GEMM-worker entry point (PB2_LINK_GEMM_BODY_ENTRY, bit 1 of the same flags, with a nonzero GEMM-worker mask): the
+ * image also defines
+ *
+ *     extern "C" __device__ unsigned long long pb2_linked_gemm_body(int body, const pb2_body_args_t* a,
+ *                                                                   unsigned int* scratch);
+ *
+ * and the GEMM window kernels call it, instead of pb2_linked_body, for every task of a body in the GEMM-worker mask.
+ * Its contract is the GEMM-worker contract above (384 threads, once per task over whole tiles, scratch the ring, no bulk
+ * copy in flight on return, the engine's fences around the call, the result from thread 0, ~0ull aborts the window),
+ * with one difference: only the GEMM window kernels reach it, so its budget is theirs, PB2_GEMM_BODY_MAX_REGS (168)
+ * registers per thread, and not the HBM kernels' 80.  Both budgets are enforced when the engine links the image: a
+ * callee that needs more registers than a kernel that reaches it fails the link (PB2_ERR_BAD_PARAM, with the linker's
+ * message), and the engine stays unlinked.  One image holds both entry points, so it is compiled with
+ * -maxrregcount=168; its pb2_linked_body still reaches the HBM kernels and must still fit their 80 registers, which the
+ * HBM link checks: keep the large bodies behind pb2_linked_gemm_body, and pb2_linked_body small.  Other linked
+ * bodies in GEMM windows, and everything in HBM windows, still go through pb2_linked_body.  An image that defines both
+ * and is linked without the flag runs its GEMM-worker bodies through pb2_linked_body; an image linked with the flag
+ * must define pb2_linked_gemm_body (the link fails otherwise, as any link error does).  A PTX image is compiled by the
+ * driver's JIT without any register cap, whatever -maxrregcount it was generated with: a function that then needs more
+ * than a kernel's budget fails the link.  tests/cuda/gemm_entry_bodies.cu runs an fp64 DMMA tile GEMM with 32 x 32 of
+ * C per warp through this entry.
  *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */
@@ -129,6 +152,9 @@ typedef struct pb2_body_check_s {
 /* The shared memory a GEMM-worker body gets as `scratch`: the GEMM worker's operand ring, 1024-byte aligned. */
 #define PB2_GEMM_BODY_SMEM_BYTES 196608
 #define PB2_GEMM_BODY_SMEM_ALIGN 1024
+/* The register budget of pb2_linked_gemm_body (PB2_LINK_GEMM_BODY_ENTRY): that of the GEMM window kernels, which alone
+ * call it (__launch_bounds__(384, 1)); enforced when the engine links the image.  pb2_linked_body's budget is 80. */
+#define PB2_GEMM_BODY_MAX_REGS 168
 
 /* What pb2_linked_reader_group is handed: one chunk of the group's tile and the members of the call, in member order. */
 typedef struct pb2_reader_group_s {
@@ -146,6 +172,7 @@ typedef struct pb2_reader_group_s {
 extern "C" __device__ unsigned long long pb2_linked_body(int body, const pb2_body_args_t* a, unsigned int* scratch);
 extern "C" __device__ unsigned long long pb2_linked_reader_group(const pb2_reader_group_t* g, unsigned long long* results,
                                                                  unsigned int* scratch);
+extern "C" __device__ unsigned long long pb2_linked_gemm_body(int body, const pb2_body_args_t* a, unsigned int* scratch);
 #endif
 
 #endif /* PB2_DEVICE_BODY_H */

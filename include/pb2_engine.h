@@ -315,8 +315,17 @@ int  pb2_engine_link_bodies_checked(pb2_engine_t* engine, const void* image, siz
  *                          as `scratch` and runs as one part, never grouped or fused; HBM windows refuse its tasks
  *                          (PB2_ERR_NOT_SUPPORTED).  A nonzero mask needs PB2_LINK_GEMM_WINDOWS and must not overlap
  *                          `sliceable` (so neither `checked` nor the readers masks): PB2_ERR_BAD_PARAM otherwise.
+ *   PB2_LINK_GEMM_BODY_ENTRY bit 1: the GEMM window kernels call every body of the GEMM-worker mask through
+ *                          pb2_linked_gemm_body, declared in include/pb2_device_body.h, which only they reach: it has
+ *                          their budget of 168 registers per thread and not the HBM kernels' 80; every other call still
+ *                          goes through pb2_linked_body.  Needs a nonzero PB2_LINK_GEMM_BODIES mask (PB2_ERR_BAD_PARAM
+ *                          otherwise, and nothing is recorded).  The flag links another build of the GEMM window
+ *                          kernels, which makes the call: the image must then define pb2_linked_gemm_body, or the link
+ *                          fails as any link error does and the engine stays unlinked.  Without the flag the kernels
+ *                          never call it.
  * PB2_ERR_BAD_PARAM for any other bit. */
 #define PB2_LINK_GEMM_WINDOWS 0x1u
+#define PB2_LINK_GEMM_BODY_ENTRY 0x2u
 #define PB2_LINK_READERS(mask) ((uint32_t)(mask) << 8)
 #define PB2_LINK_READER_GROUPS(mask) ((uint32_t)(mask) << 16)
 #define PB2_LINK_GEMM_BODIES(mask) ((uint32_t)(mask) << 24)

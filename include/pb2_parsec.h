@@ -163,8 +163,9 @@ int  pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image,
  * chains and the application's bodies around them run in one GEMM window.  PB2_LINK_READERS(mask) and
  * PB2_LINK_READER_GROUPS(mask) declare readers and the readers with the group form (pb2_linked_reader_group) as there.
  * PB2_LINK_GEMM_BODIES(mask) declares GEMM-worker bodies as there: a window that holds a task of one is a GEMM window,
- * as one that holds a GEMM task is, so those tasks never reach an HBM window.  A dry-run module checks the flags and
- * records the link. */
+ * as one that holds a GEMM task is, so those tasks never reach an HBM window.  PB2_LINK_GEMM_BODY_ENTRY (with such a
+ * mask) calls them through pb2_linked_gemm_body, at the GEMM kernels' 168 registers, as there.  A dry-run module checks
+ * the flags and records the link. */
 int  pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes

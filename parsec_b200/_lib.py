@@ -44,6 +44,9 @@ BODY_LINKED_0, BODY_LINKED_7 = 20, 27
 IMAGE_PTX, IMAGE_CUBIN = 1, 2
 # pb2_engine_link_bodies_ex flags: also link the GEMM window kernel, so linked bodies run in GEMM windows too
 LINK_GEMM_WINDOWS = 0x1
+# ... and call the GEMM-worker bodies (LINK_GEMM_BODIES) through the image's pb2_linked_gemm_body, at the GEMM kernels'
+# register budget (needs a nonzero GEMM-worker mask)
+LINK_GEMM_BODY_ENTRY = 0x2
 # pb2_engine_malloc_ex flags: cudaMalloc memory, which ipc_export can export (compressible memory cannot be)
 MALLOC_IPC = 0x1
 

@@ -309,6 +309,19 @@ extern "C" const unsigned char pb2_linked_gemm_image[], pb2_linked_gemm_image_en
 // the same two kernels built with PB2_LINKED_READER_GROUPS, which call pb2_linked_reader_group (PB2_LINK_READER_GROUPS)
 extern "C" const unsigned char pb2_linked_engine_groups_image[], pb2_linked_engine_groups_image_end[];
 extern "C" const unsigned char pb2_linked_gemm_groups_image[], pb2_linked_gemm_groups_image_end[];
+// the GEMM kernel built with PB2_LINKED_GEMM_BODY_ENTRY, without and with PB2_LINKED_READER_GROUPS, which calls
+// GEMM-worker bodies through pb2_linked_gemm_body (PB2_LINK_GEMM_BODY_ENTRY)
+extern "C" const unsigned char pb2_linked_gemm_entry_image[], pb2_linked_gemm_entry_image_end[];
+extern "C" const unsigned char pb2_linked_gemm_entry_groups_image[], pb2_linked_gemm_entry_groups_image_end[];
+
+// The GEMM cubin of a link, by [PB2_LINK_GEMM_BODY_ENTRY][reader groups declared]: its bytes, end and name.
+struct LinkedGemmImage { const unsigned char *begin, *end; const char* name; };
+static const LinkedGemmImage kLinkedGemmImages[2][2] = {
+    {{pb2_linked_gemm_image, pb2_linked_gemm_image_end, "pb2_engine_linked_gemm.cubin"},
+     {pb2_linked_gemm_groups_image, pb2_linked_gemm_groups_image_end, "pb2_engine_linked_gemm_groups.cubin"}},
+    {{pb2_linked_gemm_entry_image, pb2_linked_gemm_entry_image_end, "pb2_engine_linked_gemm_entry.cubin"},
+     {pb2_linked_gemm_entry_groups_image, pb2_linked_gemm_entry_groups_image_end, "pb2_engine_linked_gemm_entry_groups.cubin"}},
+};
 
 // The linked window kernels by [kind][(PRIO) + 2 * (TRACE)]: pb2_engine_hbm_kernel<PRIO, TRACE, true>
 // (pb2_engine_linked.cu) and pb2_engine_gemm2_kernel<PRIO, TRACE, true> (pb2_engine_linked_gemm.cu)
@@ -534,8 +547,9 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     const bool groups = link_reader_groups(flags) != 0;
     const unsigned char* hbm_image = groups ? pb2_linked_engine_groups_image : pb2_linked_engine_image;
     const unsigned char* hbm_end = groups ? pb2_linked_engine_groups_image_end : pb2_linked_engine_image_end;
-    const unsigned char* gemm_image = groups ? pb2_linked_gemm_groups_image : pb2_linked_gemm_image;
-    const unsigned char* gemm_end = groups ? pb2_linked_gemm_groups_image_end : pb2_linked_gemm_image_end;
+    // an image without pb2_linked_gemm_body links with GEMM kernels that never name it
+    const bool entry = (flags & PB2_LINK_GEMM_BODY_ENTRY) != 0;
+    const LinkedGemmImage& gemm_image = kLinkedGemmImages[entry][groups];
     std::lock_guard<std::mutex> lk(e->mu);
     if (e->linked_module) { e->last_error = "the engine has linked an image already (one per engine)"; return PB2_ERR_EXISTS; }
     const DriverCalls& d = driver();
@@ -558,8 +572,8 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
         r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(hbm_image), (size_t)(hbm_end - hbm_image),
                        groups ? "pb2_engine_linked_groups.cubin" : "pb2_engine_linked.cubin", 0, nullptr, nullptr);
     if (r == CUDA_SUCCESS && gemm_windows)
-        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(gemm_image), (size_t)(gemm_end - gemm_image),
-                       groups ? "pb2_engine_linked_gemm_groups.cubin" : "pb2_engine_linked_gemm.cubin", 0, nullptr, nullptr);
+        r = d.link_add(st, CU_JIT_INPUT_CUBIN, const_cast<unsigned char*>(gemm_image.begin),
+                       (size_t)(gemm_image.end - gemm_image.begin), gemm_image.name, 0, nullptr, nullptr);
     if (r == CUDA_SUCCESS)
         r = d.link_add(st, format == PB2_IMAGE_PTX ? CU_JIT_INPUT_PTX : CU_JIT_INPUT_CUBIN, const_cast<void*>(data), size,
                        "linked bodies", 0, nullptr, nullptr);
@@ -596,6 +610,7 @@ int pb2_engine_link_bodies_ex(pb2_engine_t* e, const void* image, size_t bytes, 
     std::copy_n(&linked[0][0], 8, &e->kernels[1][0][0]);
     e->linked_sliceable = sliceable; e->linked_checked = checked; e->linked_readers = link_readers(flags);
     e->linked_reader_groups = link_reader_groups(flags); e->linked_gemm_bodies = link_gemm_bodies(flags);
+    e->linked_gemm_body_entry = entry;
     return PB2_SUCCESS;
 }
 

@@ -60,9 +60,11 @@ struct pb2_engine_s {
     WindowKernel kernels[2][2][4];
     // pb2_engine_link_bodies: the module of the linked window kernels, and which linked body ids may be cut into parts
     // (bit i: PB2_BODY_LINKED_0 + i), which have a checked form, which are readers (PB2_LINK_READERS) and which readers
-    // have the group form (PB2_LINK_READER_GROUPS) and which get the GEMM worker's operand ring (PB2_LINK_GEMM_BODIES)
+    // have the group form (PB2_LINK_READER_GROUPS) and which get the GEMM worker's operand ring (PB2_LINK_GEMM_BODIES),
+    // and whether the GEMM kernels call those through pb2_linked_gemm_body (PB2_LINK_GEMM_BODY_ENTRY)
     CUmodule linked_module = nullptr;
     uint32_t linked_sliceable = 0, linked_checked = 0, linked_readers = 0, linked_reader_groups = 0, linked_gemm_bodies = 0;
+    bool linked_gemm_body_entry = false;
 };
 
 // The readers mask of link flags (PB2_LINK_READERS): bit i, PB2_BODY_LINKED_0 + i is a reader.
@@ -77,10 +79,11 @@ static inline uint32_t link_gemm_bodies(uint32_t flags) { return (flags >> 24) &
 // the arguments are refused.
 static inline const char* link_args_error(const void* image, size_t bytes, int format, uint32_t sliceable, uint32_t checked,
                                           uint32_t flags = 0) {
-    if (flags & ~(uint32_t)(PB2_LINK_GEMM_WINDOWS | PB2_LINK_READERS(0xFFu) | PB2_LINK_READER_GROUPS(0xFFu) |
-                            PB2_LINK_GEMM_BODIES(0xFFu)))
-        return "link flags have an unknown bit (PB2_LINK_GEMM_WINDOWS, PB2_LINK_READERS(mask), bits 8..15, "
-               "PB2_LINK_READER_GROUPS(mask), bits 16..23, and PB2_LINK_GEMM_BODIES(mask), bits 24..31, are the only flags)";
+    if (flags & ~(uint32_t)(PB2_LINK_GEMM_WINDOWS | PB2_LINK_GEMM_BODY_ENTRY | PB2_LINK_READERS(0xFFu) |
+                            PB2_LINK_READER_GROUPS(0xFFu) | PB2_LINK_GEMM_BODIES(0xFFu)))
+        return "link flags have an unknown bit (PB2_LINK_GEMM_WINDOWS, PB2_LINK_GEMM_BODY_ENTRY, PB2_LINK_READERS(mask), "
+               "bits 8..15, PB2_LINK_READER_GROUPS(mask), bits 16..23, and PB2_LINK_GEMM_BODIES(mask), bits 24..31, are "
+               "the only flags)";
     if (!image || !bytes) return "linked body image is NULL or empty";
     if (format != PB2_IMAGE_PTX && format != PB2_IMAGE_CUBIN) return "linked body image format must be PB2_IMAGE_PTX or PB2_IMAGE_CUBIN";
     if (sliceable >> 8) return "sliceable mask has bits above bit 7 (there are 8 linked body ids)";
@@ -98,6 +101,9 @@ static inline const char* link_args_error(const void* image, size_t bytes, int f
     if (link_gemm_bodies(flags) & sliceable)
         return "GEMM-worker bodies mask has a bit that is set in the sliceable mask (a GEMM-worker body runs as one part; "
                "it can be neither checked nor a reader)";
+    if ((flags & PB2_LINK_GEMM_BODY_ENTRY) && !link_gemm_bodies(flags))
+        return "PB2_LINK_GEMM_BODY_ENTRY without a PB2_LINK_GEMM_BODIES mask (the entry point is called for GEMM-worker "
+               "bodies only)";
     return nullptr;
 }
 

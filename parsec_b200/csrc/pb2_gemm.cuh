@@ -343,6 +343,8 @@ static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_
 // ran on this worker before waited on full[] for each TMA load of the unit and on each of its wgmma groups, before the
 // barrier that ended the unit.  The fences order the body's generic accesses to the ring after those async-proxy
 // accesses, and before the TMA writes of the units after it (the caller's barrier follows the second one).
+// Built with PB2_LINKED_GEMM_BODY_ENTRY (the kernels linked with PB2_LINK_GEMM_BODY_ENTRY), the call goes to the
+// application's pb2_linked_gemm_body instead, which only these kernels reach, so it has their register budget.
 static_assert(PB2_GEMM_BODY_SMEM_BYTES == kStages * kStageBytes, "a GEMM-worker body gets the whole operand ring");
 static_assert(kSmemBytes - kStages * kStageBytes == PB2_GEMM_BODY_SMEM_ALIGN, "the ring is aligned up to 1024 bytes");
 static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSmem* sp, pb2_body_check_t* lp, uint8_t* ring) {
@@ -352,7 +354,11 @@ static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSm
     if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; }
     __syncthreads();
     fence_proxy_async();
+#ifdef PB2_LINKED_GEMM_BODY_ENTRY
+    const unsigned long long r = pb2_linked_gemm_body(sp->task.body, &lp->args, reinterpret_cast<unsigned int*>(ring));
+#else
     const unsigned long long r = pb2_linked_body(sp->task.body, &lp->args, reinterpret_cast<unsigned int*>(ring));
+#endif
     fence_proxy_async();
     return r;
 }

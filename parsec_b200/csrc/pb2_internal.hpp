@@ -198,6 +198,7 @@ struct pb2_device_module_s {
     bool linked_gemm = false;                // ... with PB2_LINK_GEMM_WINDOWS: GEMM windows too
     uint32_t linked_readers = 0;             // ... PB2_LINK_READERS: bit i, PB2_BODY_LINKED_0 + i is a reader
     uint32_t linked_gemm_bodies = 0;         // ... PB2_LINK_GEMM_BODIES: bit i, PB2_BODY_LINKED_0 + i runs in GEMM windows only
+    bool linked_gemm_body_entry = false;     // ... PB2_LINK_GEMM_BODY_ENTRY: those run through pb2_linked_gemm_body
     pb2_engine_t* engine = nullptr;
     std::deque<pb2_device_window*> inflight; // windows launched and not yet retired (oldest first), pb2_device_module.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up

@@ -391,6 +391,7 @@ int pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_
     dev->linked_gemm = (flags & PB2_LINK_GEMM_WINDOWS) != 0;
     dev->linked_readers = link_readers(flags);
     dev->linked_gemm_bodies = link_gemm_bodies(flags);
+    dev->linked_gemm_body_entry = (flags & PB2_LINK_GEMM_BODY_ENTRY) != 0;
     return PB2_SUCCESS;
 }
 

@@ -170,7 +170,7 @@ class Engine:
         _check(self._lib.pb2_engine_set_window_trace(self._h, 1 if on else 0), "set_window_trace", self)
 
     def link_bodies(self, image, format, sliceable=0, checked=0, gemm_windows=False, readers=0, reader_groups=0,
-                    gemm_bodies=0):
+                    gemm_bodies=0, gemm_body_entry=False):
         """Link the application's device bodies (include/pb2_device_body.h) into this engine's HBM window kernel, once:
         image is PTX text (format L.IMAGE_PTX) or a relocatable sm_90a cubin (L.IMAGE_CUBIN), as bytes; bit i of
         sliceable lets tasks of body L.BODY_LINKED_0 + i be cut into byte-slice parts, and bit i of checked (a subset
@@ -181,10 +181,12 @@ class Engine:
         readers) declares that reader's group form, which the image then defines: a read group calls it once per chunk
         for all such members.  Bit i of gemm_bodies (L.LINK_GEMM_BODIES, with gemm_windows, disjoint from sliceable)
         declares that body a GEMM-worker body: it runs in GEMM windows only, as one part, with the GEMM worker's
-        operand ring (PB2_GEMM_BODY_SMEM_BYTES) as its scratch."""
+        operand ring (PB2_GEMM_BODY_SMEM_BYTES) as its scratch.  gemm_body_entry (L.LINK_GEMM_BODY_ENTRY, with a nonzero
+        gemm_bodies) calls those bodies through the image's pb2_linked_gemm_body, which only the GEMM window kernels
+        reach, so it has their 168 registers per thread instead of the HBM kernels' 80."""
         image = bytes(image)
         flags = ((L.LINK_GEMM_WINDOWS if gemm_windows else 0) | L.LINK_READERS(readers) | L.LINK_READER_GROUPS(reader_groups)
-                 | L.LINK_GEMM_BODIES(gemm_bodies))
+                 | L.LINK_GEMM_BODIES(gemm_bodies) | (L.LINK_GEMM_BODY_ENTRY if gemm_body_entry else 0))
         _check(self._lib.pb2_engine_link_bodies_ex(self._h, image, len(image), format, sliceable, checked, flags),
                "pb2_engine_link_bodies_ex", self)
 

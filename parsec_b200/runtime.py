@@ -164,15 +164,15 @@ class Context:
         return buf.value.decode()
 
     def link_bodies(self, dev, image, format, sliceable=0, checked=0, gemm_windows=False, readers=0, reader_groups=0,
-                    gemm_bodies=0):
+                    gemm_bodies=0, gemm_body_entry=False):
         """Link the application's device bodies into module dev's engine before its first window (Engine.link_bodies;
         a dry-run module checks the arguments and records the link).  gemm_windows: GEMM chains and linked tasks may
         then share a window.  readers, reader_groups: the bodies declared readers, and the readers declared with the
         group form (Engine.link_bodies).  gemm_bodies: the GEMM-worker bodies (Engine.link_bodies), whose tasks then
-        always run in GEMM windows."""
+        always run in GEMM windows.  gemm_body_entry: call them through pb2_linked_gemm_body (Engine.link_bodies)."""
         image = bytes(image)
         flags = ((L.LINK_GEMM_WINDOWS if gemm_windows else 0) | L.LINK_READERS(readers) | L.LINK_READER_GROUPS(reader_groups)
-                 | L.LINK_GEMM_BODIES(gemm_bodies))
+                 | L.LINK_GEMM_BODIES(gemm_bodies) | (L.LINK_GEMM_BODY_ENTRY if gemm_body_entry else 0))
         _chk(self.l.pb2_device_link_bodies_ex(dev, image, len(image), format, sliceable, checked, flags),
              "pb2_device_link_bodies_ex")
 
