@@ -25,14 +25,15 @@ LINKED_GEMM_ENTRY_GROUPS_CUBIN := build/pb2_engine_linked_gemm_entry_groups.cubi
 LINKED_OBJ   := build/pb2_linked_image.o
 # the device bodies the GPU tests link (tests/test_linked_bodies_gpu.py, tests/test_checked_linked_gpu.py,
 # tests/test_linked_readers_gpu.py, tests/test_reader_groups_linked_gpu.py, tests/test_gemm_worker_bodies_gpu.py,
-# tests/test_gemm_body_entry_gpu.py), as relocatable cubins and as PTX
+# tests/test_gemm_body_entry_gpu.py, tests/test_gemm_body_parts_gpu.py), as relocatable cubins and as PTX
 TEST_BODIES  := tests/cuda/linked_bodies.cubin tests/cuda/linked_bodies.ptx \
                 tests/cuda/checked_bodies.cubin tests/cuda/checked_bodies.ptx \
                 tests/cuda/reader_bodies.cubin tests/cuda/reader_bodies.ptx \
                 tests/cuda/reader_group_bodies.cubin tests/cuda/reader_group_bodies.ptx \
                 tests/cuda/gemm_worker_bodies.cubin tests/cuda/gemm_worker_bodies.ptx \
                 tests/cuda/gemm_entry_bodies.cubin tests/cuda/gemm_entry_bodies.ptx \
-                tests/cuda/gemm_entry_group_bodies.cubin
+                tests/cuda/gemm_entry_group_bodies.cubin \
+                tests/cuda/gemm_part_bodies.cubin tests/cuda/gemm_part_group_bodies.cubin
 
 all: $(LIB) linked_bodies oracle
 
@@ -124,6 +125,14 @@ tests/cuda/gemm_entry_bodies.ptx: tests/cuda/gemm_entry_bodies.cu include/pb2_de
 tests/cuda/gemm_entry_group_bodies.cubin: tests/cuda/gemm_entry_bodies.cu include/pb2_device_body.h
 	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=168 -DGEMM_ENTRY_READER_GROUP -Iinclude -o $@ $<
 
+# GEMM-worker bodies that split their tasks by part (pb2_engine_set_gemm_body_parts), at the GEMM kernels' 168
+# registers, and with the group form of their reader
+tests/cuda/gemm_part_bodies.cubin: tests/cuda/gemm_part_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=168 -Xptxas -v -Iinclude -o $@ $< 2> tests/cuda/gemm_part_bodies.log || (cat tests/cuda/gemm_part_bodies.log; exit 1)
+
+tests/cuda/gemm_part_group_bodies.cubin: tests/cuda/gemm_part_bodies.cu include/pb2_device_body.h
+	$(NVCC) -O3 -std=c++17 $(ARCH) -rdc=true -cubin -maxrregcount=168 -DGEMM_PART_READER_GROUP -Iinclude -o $@ $<
+
 oracle:
 	$(MAKE) -C oracle
 
@@ -132,7 +141,7 @@ clean:
 	      build/linked_gemm_ptxas.log $(LINKED_GROUPS_CUBIN) $(LINKED_GEMM_GROUPS_CUBIN) build/linked_groups_ptxas.log \
 	      build/linked_gemm_groups_ptxas.log $(LINKED_GEMM_ENTRY_CUBIN) $(LINKED_GEMM_ENTRY_GROUPS_CUBIN) \
 	      build/linked_gemm_entry_ptxas.log build/linked_gemm_entry_groups_ptxas.log $(TEST_BODIES) \
-	      tests/cuda/gemm_worker_bodies.log tests/cuda/gemm_entry_bodies.log
+	      tests/cuda/gemm_worker_bodies.log tests/cuda/gemm_entry_bodies.log tests/cuda/gemm_part_bodies.log
 	$(MAKE) -C oracle clean
 
 .PHONY: all linked_bodies oracle clean

@@ -87,7 +87,8 @@
  *   - The ring is PB2_GEMM_BODY_SMEM_BYTES bytes, 1024-byte aligned; its contents are undefined on entry, and the body
  *     may use all of it.  Nothing of it survives to the next task.
  *   - The body is called on all 384 threads of the worker (blockDim.x), once per task, over whole tiles (one part,
- *     elem0 0): such a task is never cut into parts, grouped with readers or fused with a producer.
+ *     elem0 0): such a task is never cut into byte slices, grouped with readers or fused with a producer.  It runs as
+ *     several parts only when the application declares so (below, "in parts").
  *   - No TMA or bulk copy the body issues may still be in flight when it returns (cp.async copies must be waited on).
  *   - The engine executes fence.proxy.async before the call and after it, so the body's generic stores to the ring never
  *     race the wgmma reads and TMA writes of the GEMM units that run on the worker before or after it.
@@ -122,6 +123,26 @@
  * than a kernel's budget fails the link.  tests/cuda/gemm_entry_bodies.cu runs an fp64 DMMA tile GEMM with 32 x 32 of
  * C per warp through this entry.
  *
+ * GEMM-worker bodies in parts (pb2_engine_set_gemm_body_parts(engine, body, nparts), pb2_device_set_gemm_body_parts):
+ * every task of a body declared with nparts > 1 runs as nparts parts, through either entry point.  The default, 1, is
+ * the contract above unchanged.  With nparts > 1:
+ *   - The body is called once per part, on all 384 threads of a worker.  Parts may run at the same time on different
+ *     workers, or one after another on one worker.
+ *   - Every part gets the task's whole tiles: flow / bytes as for one part, elem0 0, and args.part = its part index p.
+ *     `a` points at the `args` member of a pb2_gemm_body_args_t, whose `nparts` gives the count (1 for a task that
+ *     runs as one part; check and k0 are 0).  An image compiled against a header without it never reads it.
+ *   - The body splits the work by (p, nparts) itself: the parts store disjoint bytes of the flows the task writes, and
+ *     no part reads bytes that another part of the same task writes.
+ *   - Every part gets its own worker's ring as scratch, with the fences above; nothing passes from one part to another.
+ *   - The task's result is part 0's; ~0ull from any part aborts the window.
+ *   - The part that finishes last retires the task: successors are released and versions bumped once, after every
+ *     part's stores.
+ *   - A written flow marked PB2_FLOW_PUSHOUT is copied home whole and once, by the worker that retires the task, after
+ *     the last part's stores; bytes_d2h and that part's record count it once.  The parts push nothing themselves:
+ *     they are not byte slices of the tile.
+ * Parts of a task that runs alone on a wide machine put more SMs on it; when the window has more independent tasks than
+ * workers they only add operand traffic, so the count is the application's choice.
+ *
  * Plain C types only: the header compiles under gcc, nvcc and NVRTC without any other header.
  */
 #ifndef PB2_DEVICE_BODY_H
@@ -146,6 +167,16 @@ typedef struct pb2_body_check_s {
     unsigned int    check;                     /* 1: check mode (only for ids in the link's `checked` mask), else 0 */
     unsigned int    k0;                        /* check mode: the constant every stored element is compared with    */
 } pb2_body_check_t;                            /* 80 bytes on LP64 */
+
+/* The block a GEMM-worker body's `a` points into (at args) in GEMM windows: pb2_body_check_t's words, then the parts
+ * its task runs as (pb2_engine_set_gemm_body_parts).  Read it through ((const pb2_gemm_body_args_t*)a). */
+typedef struct pb2_gemm_body_args_s {
+    pb2_body_args_t args;
+    unsigned int    check;                     /* 0                                                                 */
+    unsigned int    k0;                        /* 0                                                                 */
+    unsigned int    nparts;                    /* the task's parts (args.part is this part's index, 0 .. nparts - 1) */
+    unsigned int    reserved;                  /* 0                                                                 */
+} pb2_gemm_body_args_t;                        /* 88 bytes on LP64 */
 
 #define PB2_GROUP_MAX 8                        /* members of a read group */
 

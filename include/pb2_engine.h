@@ -341,6 +341,15 @@ int  pb2_engine_linked_info(pb2_engine_t* engine, int32_t* regs, int32_t* local_
  * PB2_ERR_NOT_FOUND unless the engine linked with PB2_LINK_GEMM_WINDOWS. */
 int  pb2_engine_linked_gemm_info(pb2_engine_t* engine, int32_t* regs, int32_t* local_bytes, int32_t* static_smem,
                                  int32_t* nworkers);
+/* Parts per task of GEMM-worker body `body` (PB2_BODY_LINKED_0 .. _7, its bit set in the link's PB2_LINK_GEMM_BODIES
+ * mask) in the GEMM windows created from now on: every task of the body then runs as `nparts` parts, each on a worker of
+ * its own where workers are free, each handed the task's whole tiles and its part index (include/pb2_device_body.h,
+ * pb2_gemm_body_args_t); the body splits the work by part itself.  The default is 1 for every body: one part on one
+ * worker.  PB2_ERR_NOT_FOUND before pb2_engine_link_bodies_ex; PB2_ERR_BAD_PARAM for any other id, or one that is not a
+ * GEMM-worker body of the link; PB2_ERR_VALUE_OUT_OF_BOUNDS for nparts < 1 or > PB2_GEMM_BODY_MAX_PARTS.  Every refusal
+ * leaves the counts as they were and says why in pb2_engine_last_error. */
+#define PB2_GEMM_BODY_MAX_PARTS 32             /* the 5-bit part field of a GEMM window's ring entry */
+int  pb2_engine_set_gemm_body_parts(pb2_engine_t* engine, int body, int32_t nparts);
 
 /* --- one window of the DAG ---
  * tasks[ntasks], succ[nsucc] (CSR via succ_begin/succ_count), tiles[ntiles] and the ids of

@@ -168,6 +168,13 @@ int  pb2_device_link_bodies_checked(pb2_device_module_t* dev, const void* image,
  * the flags and records the link. */
 int  pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_t bytes, int format, uint32_t sliceable,
                                uint32_t checked, uint32_t flags);
+/* pb2_engine_set_gemm_body_parts for the module's engine: the tasks of GEMM-worker body `body` run as `nparts` parts in
+ * the windows the module builds afterwards.  The same refusals, with PB2_ERR_NOT_FOUND before
+ * pb2_device_link_bodies_ex; the message is in the context's last error.  A dry-run module checks the arguments and
+ * records the count (pb2_device_gemm_body_parts). */
+int  pb2_device_set_gemm_body_parts(pb2_device_module_t* dev, int body, int32_t nparts);
+/* The part count the module holds for GEMM-worker body `body` (1 unless set), or a negative error code. */
+int  pb2_device_gemm_body_parts(pb2_device_module_t* dev, int body);
 /* parsec_devices_print_statistics (device.c:499-590): one row per device -- kernels run and their share, bytes
  * required in / moved H2D and D2D (with the percentage of "required"), bytes required out / written back, evictions --
  * plus the engine's own columns (windows launched, successors released by the device).  Writes a NUL-terminated

@@ -47,6 +47,8 @@ LINK_GEMM_WINDOWS = 0x1
 # ... and call the GEMM-worker bodies (LINK_GEMM_BODIES) through the image's pb2_linked_gemm_body, at the GEMM kernels'
 # register budget (needs a nonzero GEMM-worker mask)
 LINK_GEMM_BODY_ENTRY = 0x2
+# the most parts a task of a GEMM-worker body runs as (pb2_engine_set_gemm_body_parts): a GEMM ring entry's part field
+GEMM_BODY_MAX_PARTS = 32
 # pb2_engine_malloc_ex flags: cudaMalloc memory, which ipc_export can export (compressible memory cannot be)
 MALLOC_IPC = 0x1
 
@@ -157,7 +159,7 @@ ENGINE_SYMBOLS = [
     "pb2_engine_create", "pb2_engine_destroy", "pb2_engine_info", "pb2_engine_last_error",
     "pb2_engine_malloc", "pb2_engine_malloc_ex", "pb2_engine_free", "pb2_engine_host_register", "pb2_engine_host_unregister",
     "pb2_engine_memcpy_h2d", "pb2_engine_prefetch_h2d", "pb2_engine_memcpy_d2h", "pb2_engine_synchronize", "pb2_engine_set_stream", "pb2_engine_get_stream", "pb2_engine_copy_batch", "pb2_engine_ipc_export", "pb2_engine_ipc_open",
-    "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_window_trace", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
+    "pb2_engine_ipc_close", "pb2_engine_enable_peer", "pb2_body_launch", "pb2_body_launch_errors", "pb2_engine_set_shared_windows", "pb2_engine_set_part_bytes", "pb2_engine_set_gemm_body_parts", "pb2_engine_set_window_trace", "pb2_engine_set_stage_slice_bytes", "pb2_window_export", "pb2_window_set_remote", "pb2_window_task_entries",
     "pb2_window_arm", "pb2_window_start",
     "pb2_window_create", "pb2_window_destroy", "pb2_window_launch", "pb2_window_wait",
     "pb2_window_results", "pb2_window_trace", "pb2_window_part_trace",
@@ -204,6 +206,7 @@ def load():
     lib.pb2_engine_set_shared_windows.argtypes = [vp, C.c_int, vp]
     lib.pb2_window_task_entries.argtypes = [vp, vp]
     lib.pb2_engine_set_part_bytes.argtypes = [vp, i32]
+    lib.pb2_engine_set_gemm_body_parts.argtypes = [vp, C.c_int, i32]
     lib.pb2_engine_set_window_trace.argtypes = [vp, C.c_int]
     lib.pb2_window_trace.argtypes = [vp, vp, vp, vp, vp]
     lib.pb2_window_part_trace.argtypes = [vp, vp, i32, P(i32)]

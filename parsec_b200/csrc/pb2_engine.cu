@@ -206,6 +206,7 @@ static PlanParams params_of(const pb2_engine_t* e, int kind) {
     p.part_bytes = e->params.part_bytes; p.stage_slice_bytes = e->stage_slice_bytes;
     p.linked_sliceable = e->linked_sliceable; p.linked_checked = e->linked_checked; p.linked_readers = e->linked_readers;
     p.linked_reader_groups = e->linked_reader_groups; p.linked_gemm_bodies = e->linked_gemm_bodies;
+    std::copy_n(e->gemm_body_parts, 8, p.gemm_body_parts);
     p.next_rs_begin = e->next_rs_begin;
     return p;
 }
@@ -920,6 +921,16 @@ int pb2_engine_set_stage_slice_bytes(pb2_engine_t* e, int32_t bytes) {
 int pb2_engine_set_part_bytes(pb2_engine_t* e, int32_t part_bytes) {
     if (!e) return PB2_ERR_BAD_PARAM;
     e->params.part_bytes = part_bytes == 0 ? kDefaultPartBytes : part_bytes;
+    return PB2_SUCCESS;
+}
+int pb2_engine_set_gemm_body_parts(pb2_engine_t* e, int body, int32_t nparts) {
+    if (!e) return PB2_ERR_BAD_PARAM;
+    int rc;
+    if (const char* why = gemm_body_parts_error(e->linked_module != nullptr, e->linked_gemm_bodies, body, nparts, &rc)) {
+        e->last_error = why;
+        return rc;
+    }
+    e->gemm_body_parts[body - PB2_BODY_LINKED_0] = nparts;
     return PB2_SUCCESS;
 }
 int pb2_engine_set_window_trace(pb2_engine_t* e, int on) {

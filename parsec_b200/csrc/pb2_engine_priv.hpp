@@ -65,6 +65,8 @@ struct pb2_engine_s {
     CUmodule linked_module = nullptr;
     uint32_t linked_sliceable = 0, linked_checked = 0, linked_readers = 0, linked_reader_groups = 0, linked_gemm_bodies = 0;
     bool linked_gemm_body_entry = false;
+    // pb2_engine_set_gemm_body_parts: parts per task of GEMM-worker body PB2_BODY_LINKED_0 + i
+    int32_t gemm_body_parts[8] = {1, 1, 1, 1, 1, 1, 1, 1};
 };
 
 // The readers mask of link flags (PB2_LINK_READERS): bit i, PB2_BODY_LINKED_0 + i is a reader.
@@ -104,6 +106,21 @@ static inline const char* link_args_error(const void* image, size_t bytes, int f
     if ((flags & PB2_LINK_GEMM_BODY_ENTRY) && !link_gemm_bodies(flags))
         return "PB2_LINK_GEMM_BODY_ENTRY without a PB2_LINK_GEMM_BODIES mask (the entry point is called for GEMM-worker "
                "bodies only)";
+    return nullptr;
+}
+
+// The argument check of pb2_engine_set_gemm_body_parts and pb2_device_set_gemm_body_parts: nullptr, or why the call is
+// refused with the code in *rc.  linked: an image is linked; gemm_bodies: the link's GEMM-worker mask.
+static inline const char* gemm_body_parts_error(bool linked, uint32_t gemm_bodies, int body, int32_t nparts, int* rc) {
+    *rc = PB2_ERR_NOT_FOUND;
+    if (!linked) return "no image is linked yet: part counts are declared for the GEMM-worker bodies of a link";
+    *rc = PB2_ERR_BAD_PARAM;
+    if (body < PB2_BODY_LINKED_0 || body > PB2_BODY_LINKED_7) return "body is not a linked body id (PB2_BODY_LINKED_0 .. _7)";
+    if (!((gemm_bodies >> (body - PB2_BODY_LINKED_0)) & 1u))
+        return "body is not a GEMM-worker body of the link (its bit is clear in the PB2_LINK_GEMM_BODIES mask)";
+    *rc = PB2_ERR_VALUE_OUT_OF_BOUNDS;
+    if (nparts < 1 || nparts > PB2_GEMM_BODY_MAX_PARTS) return "nparts must be 1 .. PB2_GEMM_BODY_MAX_PARTS (32)";
+    *rc = PB2_SUCCESS;
     return nullptr;
 }
 

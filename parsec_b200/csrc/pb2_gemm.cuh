@@ -347,11 +347,14 @@ static __device__ __noinline__ uint64_t consume_part_outlined(Shared* sp, uint8_
 // application's pb2_linked_gemm_body instead, which only these kernels reach, so it has their register budget.
 static_assert(PB2_GEMM_BODY_SMEM_BYTES == kStages * kStageBytes, "a GEMM-worker body gets the whole operand ring");
 static_assert(kSmemBytes - kStages * kStageBytes == PB2_GEMM_BODY_SMEM_ALIGN, "the ring is aligned up to 1024 bytes");
-static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSmem* sp, pb2_body_check_t* lp, uint8_t* ring) {
+// A task of a body declared in parts (pb2_engine_set_gemm_body_parts) calls it once per part, each over whole tiles
+// (run_task_part<..., GEMM_BODY_PARTS>) with its part index in args.part and the count in lp->nparts.
+static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSmem* sp, pb2_gemm_body_args_t* lp, uint8_t* ring,
+                                                                          int nparts) {
     static_assert(sizeof(BodyArgs) % 4 == 0 && sizeof(BodyArgs) / 4 <= kThreads, "one word of BodyArgs per thread");
     if (threadIdx.x < sizeof(BodyArgs) / 4)
         reinterpret_cast<uint32_t*>(&lp->args)[threadIdx.x] = reinterpret_cast<const uint32_t*>(&sp->args)[threadIdx.x];
-    if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; }
+    if (threadIdx.x == 0) { lp->check = 0; lp->k0 = 0; lp->nparts = (unsigned)nparts; lp->reserved = 0; }
     __syncthreads();
     fence_proxy_async();
 #ifdef PB2_LINKED_GEMM_BODY_ENTRY
@@ -361,6 +364,21 @@ static __device__ __forceinline__ unsigned long long run_gemm_worker_body(TaskSm
 #endif
     fence_proxy_async();
     return r;
+}
+
+// All threads, on the worker whose part of a GEMM-worker task in parts retires it: every written flow marked PUSHOUT,
+// copied home whole.  Its parts wrote it on other SMs; their stores are visible (each part's __threadfence before it
+// counted parts_left down) and the copy reads through L2.
+template <bool TRACE>
+__device__ __forceinline__ void push_out_whole_flows(const WinDev& w, const pb2_task_t& t, PartSmem* rec) {
+#pragma unroll 1
+    for (int f = 0; f < (int)t.nb_flows; ++f) {
+        if (t.tile[f] < 0 || !(t.access[f] & PB2_FLOW_PUSHOUT) || !(t.access[f] & PB2_FLOW_ACCESS_WRITE)) continue;
+        const pb2_tile_t* tile = &w.tiles[t.tile[f]];
+        cta_copy<false>(tile->src_ptr, tile->dev_ptr, tile->bytes);
+        if (threadIdx.x == 0) atomicAdd(&w.ctl->bytes_d2h.v, (unsigned long long)tile->bytes);
+        if (TRACE && threadIdx.x == 0) rec->out_bytes += tile->bytes;
+    }
 }
 
 }  // namespace gemm
@@ -384,7 +402,11 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
     PartSmem* rec = nullptr;
     if constexpr (TRACE) { __shared__ PartSmem part_rec; rec = &part_rec; }
     pb2_body_check_t* lk = nullptr;          // LINKED: what a linked body is handed (run_linked_part)
-    if constexpr (LINKED) { __shared__ pb2_body_check_t linked_args; lk = &linked_args; }
+    pb2_gemm_body_args_t* lg = nullptr;      // ... the same block, as a GEMM-worker body reads it (run_gemm_worker_body)
+    if constexpr (LINKED) {
+        __shared__ pb2_gemm_body_args_t linked_args;
+        lg = &linked_args; lk = reinterpret_cast<pb2_body_check_t*>(&linked_args);
+    }
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
@@ -500,10 +522,10 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
             const uint32_t gd = load_group_members(w, id, sh.gs);
             if (threadIdx.x == 0) { sh.gs.n = (int)(gd & 15u); sh.gs.fused = (gd & PB2_GROUP_FUSED) != 0; }
             __syncthreads();
-            const unsigned long long r = run_task_part<false, TRACE>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
+            const unsigned long long r = run_task_part<false, TRACE, LINKED>(w, sh.ts, nullptr, id, job.part, job.nparts, [&] {
                 if (sh.ts.need) fence_proxy_async();
                 unsigned long long body_r;
-                if constexpr (LINKED) body_r = (sh.ts.task.flags & PB2_TASK_GEMM_BODY) ? run_gemm_worker_body(&sh.ts, lk, smem)
+                if constexpr (LINKED) body_r = (sh.ts.task.flags & PB2_TASK_GEMM_BODY) ? run_gemm_worker_body(&sh.ts, lg, smem, job.nparts)
                                              : linked_reader_group(w, sh.gs) ? run_linked_group_part<kThreads>(&sh.ts, &sh.gs, lk, w.tasks, w.seen_version)
                                              : is_linked_body(sh.ts.task.body) ? run_linked_part<kThreads>(&sh.ts, &sh.gs, lk)
                                              : sh.gs.fused ? run_fused_part<kThreads>(&sh.ts, &sh.gs)
@@ -555,6 +577,30 @@ pb2_engine_gemm2_kernel(Win2Dev g) {
                 if (TRACE && threadIdx.x == 0) rec->out_bytes += (unsigned long long)(tile->bytes - c_bytes);
             }
             __syncthreads();
+        }
+        if constexpr (LINKED) {
+            // ---------------- a part of a GEMM-worker task in parts: the worker that counts the last part pushes the
+            // task's flows out whole, after every part's stores, then records its part and retires the unit
+            if (!job.is_gemm && job.nparts > 1 && (sh.ts.task.flags & PB2_TASK_GEMM_BODY)) {
+                if (threadIdx.x == 0) { __threadfence(); sh.ts.last = atomicSub(&g.parts_left[job.unit], 1) == 1; }
+                __syncthreads();
+                const bool last = sh.ts.last != 0;
+                if (last) {
+                    __threadfence();
+                    push_out_whole_flows<TRACE>(w, sh.ts.task, rec);
+                    __threadfence();
+                    __syncthreads();
+                }
+                if (warp == 0) {
+                    if (TRACE && lane == 0) {
+                        if (last) rec->t_out = globaltimer_ns();
+                        trace_part(g.trace, job.unit, job.part, *rec, last);
+                    }
+                    if (last) retire_unit_warp<PRIO>(g, g.units[job.unit]);
+                }
+                __syncthreads();     // sh.job is rewritten by the next pop
+                continue;
+            }
         }
         if (warp == 0) {
             int last = 0;

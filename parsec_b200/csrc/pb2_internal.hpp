@@ -199,6 +199,7 @@ struct pb2_device_module_s {
     uint32_t linked_readers = 0;             // ... PB2_LINK_READERS: bit i, PB2_BODY_LINKED_0 + i is a reader
     uint32_t linked_gemm_bodies = 0;         // ... PB2_LINK_GEMM_BODIES: bit i, PB2_BODY_LINKED_0 + i runs in GEMM windows only
     bool linked_gemm_body_entry = false;     // ... PB2_LINK_GEMM_BODY_ENTRY: those run through pb2_linked_gemm_body
+    int32_t gemm_body_parts[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // pb2_device_set_gemm_body_parts, per GEMM-worker body
     pb2_engine_t* engine = nullptr;
     std::deque<pb2_device_window*> inflight; // windows launched and not yet retired (oldest first), pb2_device_module.cpp
     size_t pipe_chunk = 0;                   // roots per window while a large batch of pending tasks is being cut up

@@ -395,6 +395,27 @@ int pb2_device_link_bodies_ex(pb2_device_module_t* dev, const void* image, size_
     return PB2_SUCCESS;
 }
 
+// The module's windows are planned by its engine, which holds the counts; the module keeps them too, so that a dry-run
+// module records them.
+int pb2_device_set_gemm_body_parts(pb2_device_module_t* dev, int body, int32_t nparts) {
+    if (!dev || !PB2_DEV_IS_GPU(dev->type)) return PB2_ERR_BAD_PARAM;
+    int rc;
+    if (const char* why = gemm_body_parts_error(dev->linked, dev->linked_gemm_bodies, body, nparts, &rc)) {
+        dev->ctx->last_error = why;
+        return rc;
+    }
+    if (!dev->dry_run && (rc = pb2_engine_set_gemm_body_parts(dev->engine, body, nparts)) != PB2_SUCCESS) {
+        dev->ctx->last_error = pb2_engine_last_error(dev->engine);
+        return rc;
+    }
+    dev->gemm_body_parts[body - PB2_BODY_LINKED_0] = nparts;
+    return PB2_SUCCESS;
+}
+int pb2_device_gemm_body_parts(pb2_device_module_t* dev, int body) {
+    if (!dev || !PB2_DEV_IS_GPU(dev->type) || body < PB2_BODY_LINKED_0 || body > PB2_BODY_LINKED_7) return PB2_ERR_BAD_PARAM;
+    return dev->gemm_body_parts[body - PB2_BODY_LINKED_0];
+}
+
 int pb2_device_get_stats(pb2_device_module_t* dev, pb2_device_stats_t* st) { if (!dev || !st) return PB2_ERR_BAD_PARAM; *st = dev->st; return PB2_SUCCESS; }
 static void best_unit(uint64_t bytes, double* v, const char** unit) {       // parsec_compute_best_unit: 1024-based
     static const char* units[] = {"B", "KB", "MB", "GB", "TB", "PB"};

@@ -70,6 +70,8 @@ struct GSeg { int32_t task, tileA, tileB, pad; };
 namespace gemm {
 constexpr int BM = 128, BN = 256;  // a C sub-tile: one part of a GEMM unit runs every nparts-th of them
 constexpr int kMaxParts = 32;      // the part index travels in the 5-bit flow field of a ring entry
+// a task of a GEMM-worker body runs as up to PB2_GEMM_BODY_MAX_PARTS parts (pb2_engine_set_gemm_body_parts)
+static_assert(PB2_GEMM_BODY_MAX_PARTS == kMaxParts, "a GEMM-worker body's part index travels in a ring entry's part field");
 }  // namespace gemm
 
 // Application device bodies linked into HBM windows (pb2_engine_link_bodies).

@@ -211,9 +211,11 @@ int build_gemm2_units(const PlanParams& p, const pb2_task_t* tasks, int32_t ntas
         u.flags = g ? 1 : 0; u.tileC = g ? tasks[h].tile[2] : -1;
         u.M = tasks[h].iparam[0]; u.N = tasks[h].iparam[1]; u.K = tasks[h].iparam[2];
         // a part runs every nparts-th 128 x 256 sub-tile of C, or one byte slice of the tiles of an HBM body; a linked
-        // body whose sliceable bit is clear runs as one part over whole tiles
+        // body whose sliceable bit is clear runs as one part over whole tiles, and a GEMM-worker body as the parts its
+        // count declares, each over whole tiles (the body splits the work by part index itself)
         const bool whole = is_linked_body(tasks[h].body) && !((p.linked_sliceable >> (tasks[h].body - PB2_BODY_LINKED_0)) & 1u);
         u.nparts = g ? std::min(((u.M + gemm::BM - 1) / gemm::BM) * ((u.N + gemm::BN - 1) / gemm::BN), gemm::kMaxParts)
+                 : (tasks[h].flags & PB2_TASK_GEMM_BODY) ? p.gemm_body_parts[tasks[h].body - PB2_BODY_LINKED_0]
                  : whole ? 1 : task_parts(tasks[h], [&](int32_t id) { return tiles[id].bytes; }, part_bytes, gemm::kMaxParts);
         if (!plan.group.empty() && (plan.group[(size_t)h] & PB2_GROUP_FUSED)) u.flags |= 4;
         for (int32_t t = h; t >= 0; t = next[t]) {

@@ -24,6 +24,7 @@ struct PlanParams {
     uint32_t linked_reader_groups = 0;    // bit i: reader PB2_BODY_LINKED_0 + i has the group form (a subset of linked_readers)
     uint32_t linked_gemm_bodies = 0;      // bit i: PB2_BODY_LINKED_0 + i gets the GEMM worker's operand ring (disjoint from
                                           // linked_sliceable)
+    int32_t gemm_body_parts[8] = {1, 1, 1, 1, 1, 1, 1, 1};   // parts per task of GEMM-worker body PB2_BODY_LINKED_0 + i
     const int32_t* next_rs_begin = nullptr;     // shared windows: remote out-degree CSR (not owned)
 };
 

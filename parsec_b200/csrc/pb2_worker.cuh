@@ -56,11 +56,15 @@ static __device__ __noinline__ void stage_in_needed_flows(const StageCtx c, Task
 // threads) and returns its result in thread 0.  Returns the body result (thread 0).  BULK as for
 // stage_in_needed_flows; without it `bulk` is not used.  TRACE (traced window kernels): thread 0 stamps the end of the
 // stage-in, of the body and of the pushout into *rec, and counts the bytes this CTA moved in and pushed out there.
-template <bool BULK, bool TRACE = false, class Exec>
+// GEMM_BODY_PARTS (the linked GEMM window kernels): a part of a GEMM-worker task that runs in parts
+// (pb2_engine_set_gemm_body_parts) covers the task's whole tiles, whose stage-in the parts share through the slice
+// claims, and pushes nothing out: the part that retires the task pushes its flows out whole (pb2_gemm.cuh).
+template <bool BULK, bool TRACE = false, bool GEMM_BODY_PARTS = false, class Exec>
 __device__ __forceinline__ unsigned long long
 run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part, int nparts, Exec exec,
               PartSmem* rec = nullptr) {
     const pb2_task_t& t = s.task;
+    const bool whole = GEMM_BODY_PARTS && nparts > 1 && (t.flags & PB2_TASK_GEMM_BODY);
     // ---- push: one thread per flow works out its slice and whether the tile has to be staged in -----------------
     if (threadIdx.x < 32) {
         const int f = (int)threadIdx.x;
@@ -74,7 +78,7 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
             widest = v > widest ? v : widest;
         }
         uint32_t off, len;
-        part_slice(widest, (uint32_t)nparts, (uint32_t)part, bytes, off, len);
+        part_slice(widest, whole ? 1u : (uint32_t)nparts, whole ? 0u : (uint32_t)part, bytes, off, len);
         const bool need = mine && (t.access[f] & PB2_FLOW_ACCESS_READ) && ld_acquire_gpu(&tile->state) != PB2_TILE_VALID;
         const unsigned needmask = __ballot_sync(0xffffffffu, need);
         if (f < PB2_MAX_FLOWS) {
@@ -104,7 +108,7 @@ run_task_part(const WinDev& w, TaskSmem& s, BulkSmem* bulk, int32_t id, int part
     // ---- pop: pushout of written flows to their home copy (parsec_device_kernel_pop stage_out) ----
 #pragma unroll
     for (int f = 0; f < PB2_MAX_FLOWS; ++f) {
-        if (f < (int)t.nb_flows && t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
+        if (!whole && f < (int)t.nb_flows && t.tile[f] >= 0 && (t.access[f] & PB2_FLOW_PUSHOUT) && (t.access[f] & PB2_FLOW_ACCESS_WRITE)) {
             const pb2_tile_t* tile = &w.tiles[t.tile[f]];
             cta_copy<false>(reinterpret_cast<uint8_t*>(tile->src_ptr) + s.off[f], s.args.flow[f], s.args.bytes[f],
                             BULK ? bulk : nullptr);

@@ -190,6 +190,12 @@ class Engine:
         _check(self._lib.pb2_engine_link_bodies_ex(self._h, image, len(image), format, sliceable, checked, flags),
                "pb2_engine_link_bodies_ex", self)
 
+    def set_gemm_body_parts(self, body, nparts):
+        """Run every task of GEMM-worker body `body` (a bit of link_bodies' gemm_bodies) as nparts parts, 1 ..
+        L.GEMM_BODY_MAX_PARTS, in the GEMM windows created from now on.  Each part gets the task's whole tiles and its
+        part index, and the body splits the work by it (include/pb2_device_body.h).  The default is 1."""
+        _check(self._lib.pb2_engine_set_gemm_body_parts(self._h, body, nparts), "set_gemm_body_parts", self)
+
     def linked_info(self):
         """What the linker made of the linked kernel: registers and local bytes per thread, static shared memory per
         CTA, and the workers a linked window runs."""

@@ -29,7 +29,7 @@ PARSEC_SYMBOLS = [
     "pb2_init", "pb2_fini", "pb2_mca_param_set_int", "pb2_mca_param_get_int", "pb2_device_cuda_module_init",
     "pb2_mca_device_registration_complete", "pb2_nb_devices", "pb2_mca_device_get", "pb2_device_get_stats",
     "pb2_devices_statistics_string", "pb2_device_link_bodies", "pb2_device_link_bodies_checked",
-    "pb2_device_link_bodies_ex",
+    "pb2_device_link_bodies_ex", "pb2_device_set_gemm_body_parts", "pb2_device_gemm_body_parts",
     "pb2_device_index", "pb2_device_type", "pb2_device_memory_register", "pb2_device_memory_unregister",
     "pb2_device_memory_release", "pb2_device_data_advise", "pb2_device_taskpool_register",
     "pb2_device_taskpool_unregister", "pb2_device_kernel_scheduler", "pb2_device_zone_malloc", "pb2_device_zone_free",
@@ -70,6 +70,8 @@ def lib():
         "pb2_device_link_bodies": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32]),
         "pb2_device_link_bodies_checked": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32]),
         "pb2_device_link_bodies_ex": (C.c_int, [vp, C.c_char_p, C.c_size_t, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32]),
+        "pb2_device_set_gemm_body_parts": (C.c_int, [vp, C.c_int, C.c_int32]),
+        "pb2_device_gemm_body_parts": (C.c_int, [vp, C.c_int]),
         "pb2_device_memory_register": (C.c_int, [vp, vp, vp, C.c_size_t]),
         "pb2_device_memory_unregister": (C.c_int, [vp, vp, vp]), "pb2_device_memory_release": (C.c_int, [vp]),
         "pb2_device_data_advise": (C.c_int, [vp, vp, C.c_int]),
@@ -175,6 +177,17 @@ class Context:
                  | L.LINK_GEMM_BODIES(gemm_bodies) | (L.LINK_GEMM_BODY_ENTRY if gemm_body_entry else 0))
         _chk(self.l.pb2_device_link_bodies_ex(dev, image, len(image), format, sliceable, checked, flags),
              "pb2_device_link_bodies_ex")
+
+    def set_gemm_body_parts(self, dev, body, nparts):
+        """Run every task of GEMM-worker body `body` as nparts parts in the windows module dev builds afterwards
+        (Engine.set_gemm_body_parts; a dry-run module checks the arguments and records the count)."""
+        _chk(self.l.pb2_device_set_gemm_body_parts(dev, body, nparts), "pb2_device_set_gemm_body_parts")
+
+    def gemm_body_parts(self, dev, body):
+        """The part count module dev holds for GEMM-worker body `body` (1 unless set)."""
+        n = self.l.pb2_device_gemm_body_parts(dev, body)
+        _chk(min(n, 0), "pb2_device_gemm_body_parts")
+        return n
 
     def stats(self, dev):
         st = DeviceStats()
